@@ -62,6 +62,8 @@ SIGNATURES = {
     'cfb_adain_nhwc': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, _P]),
     'cfb_debug_time_conv': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P, c_int64,
                                    _P, _P, _P, c_int32, POINTER(c_float)]),
+    'cfb_debug_conv_tc': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                 _P, _P, c_int32, _P, _P, _P, c_float, _P, _P, _P, c_int64, _P, POINTER(c_int32)]),
     'cfb_rrdb_create': (c_void_p, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32]),
     'cfb_rrdb_destroy': (None, [_P]),
     'cfb_rrdb_set_param': (c_int, [_P, c_char_p, _P, c_int64]),

@@ -3,8 +3,8 @@
 // Computes the 3x3 / 1x1 convolutions and linears of the CodeFormer hot path
 //   nn.Conv2d call sites      /root/reference/basicsr/archs/vqgan_arch.py:120,132,147-151,173-200,243,266,292,314
 //   Fuse_sft convs, Linear    /root/reference/basicsr/archs/codeformer_arch.py:104-106,141-149,183,192
-// as GEMMs  D[M = 128 output pixels, N = 64 output channels] += A[M, K] * B[N, K]^T  with K = taps * Cin, on the
-// Hopper tensor cores:
+// as GEMMs  D[M = 128 output pixels, N = 64 or 128 output channels (TcCfg)] += A[M, K] * B[N, K]^T  with K = taps * Cin, on
+// the Hopper tensor cores:
 //   * operands are error-compensated fp16 pairs  x = hi + lo  (hi = fp16(x), lo = fp16(x - hi)); the products
 //     lo*hi + hi*lo + hi*hi are three wgmma.mma_async m64n64k16 per 64-row half and k-step, fp32 accumulation in registers
 //     (>= 21 effective mantissa bits; the 1e-3 parity bar needs >= 16, SURVEY.md Appendix B);
@@ -261,6 +261,11 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// arrive when `pred` holds (a predicated instruction, no branch)
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+               ::"r"(bar), "r"((uint32_t)pred) : "memory");
+}
 // Bounded wait without a trap.  A protocol bug (or an injected fault) must surface as a Python exception, never as a hung
 // GPU and never as a sticky context error (SURVEY.md section 8(b) "Errors": the reference's callers catch RuntimeError and
 // fall back to the input face, inference_codeformer.py:209-211).  On time-out the waiting thread raises the device-wide
@@ -372,18 +377,42 @@ __device__ __forceinline__ void wg_mma_64x64(float (&d)[32], uint64_t da, uint64
       : "memory");
 }
 
-// Warpgroup-uniform decision (named barrier 2, the 128 threads of physical warps 0..3): true when `v` holds in any thread.
-// The wgmma instructions are .sync.aligned over the warpgroup, so after a barrier wait that may have been abandoned (time-out /
-// device-wide abort flag) the four warps must agree before any of them issues the next one.
-__device__ __forceinline__ bool wg_any(bool v) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T: same register layout with j = 0..15
+__device__ __forceinline__ void wg_mma_64x128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accum)
+      : "memory");
+}
+__device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// Warpgroup-uniform decision (named barrier `bar_id` over the 128 threads of one MMA warpgroup: 2 for physical warps 0..3, 3
+// for warps 4..7): true when `v` holds in any thread.  The wgmma instructions are .sync.aligned over the warpgroup, so after a
+// barrier wait that may have been abandoned (time-out / device-wide abort flag) the four warps must agree before any of them
+// issues the next one.
+__device__ __forceinline__ bool wg_any(bool v, uint32_t bar_id = 2) {
   uint32_t r;
   asm volatile(
       "{\n\t.reg .pred p, q;\n\t"
       "setp.ne.u32 p, %1, 0;\n\t"
-      "bar.red.or.pred q, 2, 128, p;\n\t"
+      "bar.red.or.pred q, %2, 128, p;\n\t"
       "selp.u32 %0, 1, 0, q;\n\t}"
       : "=r"(r)
-      : "r"((uint32_t)v)
+      : "r"((uint32_t)v), "r"(bar_id)
       : "memory");
   return r != 0;
 }
@@ -558,28 +587,37 @@ struct TcParams {
 #define TC_STAMP(i) do { } while (0)
 #endif
 
-constexpr int TC_EPI_WARPS = 8;                       // 4 row quadrants x 2 column halves
-constexpr int TC_MMA_WARPS = 4;                       // one warpgroup issues the wgmma of the whole 128-row tile
-constexpr int TC_THREADS = 32 * (TC_MMA_WARPS + 1 + TC_EPI_WARPS);   // MMA warpgroup, TMA warp, epilogue warps
-// XF (fused operand transform): warps 10.. transform the A patches, the warp after them loads the raw patches.
+// XF (fused operand transform): the warps after the epilogue warps transform the A patches, the warp after them loads the raw
+// patches.
 constexpr int XF_SKEW = 128;                          // byte skew of the second patch plane (see the transform warps)
 constexpr int TC_A_BYTES = 128 * 128;                 // 128 pixels x 64 fp16
 
-// Every tile is 128 output pixels x BN = 64 output channels: the accumulator of a 128 x 64 tile is 64 fp32 registers per
-// thread of the MMA warpgroup, which leaves room for the 18 warps of the transform variants.
+// Tiles are 128 output pixels x BN output channels.
+//   BN = 64 (every engine): one MMA warpgroup issues the wgmma of the whole 128-row tile into 2 x 32 fp32 registers per thread
+//     and hands every partial sum to 8 epilogue warps (4 row quadrants x 2 column halves), which fold it into registers.
+//   BN = 128 (halo engine, 3x3 and Upsample convs with Cout % 128 == 0): two MMA warpgroups, one per 64-pixel half, issue
+//     m64n128k16 into 64 fp32 registers per thread and fold their partial sums themselves into the shared fp32 tile slot;
+//     4 epilogue warps (one per row quadrant, all 128 columns) read the finished tile from the slot.  A 64-channel patch is
+//     transformed once per 128 output channels instead of once per 64, and each A byte read from shared memory feeds twice
+//     the MACs.  16 warps (8 MMA, TMA, 4 epilogue, 2 transform, patch loader) leave 128 registers per thread.
 template <int BN>
 struct TcCfg {
-  static_assert(BN == 64, "the wgmma engine runs 64-wide n-tiles");
+  static_assert(BN == 64 || BN == 128, "the wgmma engine runs 64- or 128-wide n-tiles");
+  static constexpr bool WIDE = BN == 128;
+  static constexpr int MMA_WARPS = WIDE ? 8 : 4;
+  static constexpr int EPI_WARPS = WIDE ? 4 : 8;
+  static constexpr int THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS);   // MMA warpgroup(s), TMA warp, epilogue warps
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * TC_A_BYTES + 2 * B_BYTES;
   static constexpr int STAGES = 3;
-  // Partial-sum hand-off: the MMA warpgroup accumulates `chunk` k-blocks in registers, then stores the fp32 partial sum into
-  // this shared-memory slot (128 rows, padded by 4 floats against bank conflicts) and goes on with the next chunk while the
-  // epilogue warps fold the slot into their fp32 registers with round-to-nearest adds.
+  // Partial-sum hand-off (128 rows, padded by 4 floats against bank conflicts).  BN = 64: the MMA warpgroup stores each
+  // partial sum here and goes on with the next chunk while the epilogue warps fold the slot into their fp32 registers with
+  // round-to-nearest adds.  BN = 128: the MMA warpgroups keep the running sum here (first chunk stored, later chunks added with
+  // round-to-nearest adds: the same sums in the same order), the epilogue reads the tile once.
   static constexpr int SLOT_PITCH = BN + 4;
   static constexpr int SLOT_BYTES = 128 * SLOT_PITCH * 4;
   static constexpr int SLOTS = 1;
-  static constexpr int STG_BYTES = 8 * 4096;               // per-epilogue-warp 32x32-float transpose patches
+  static constexpr int STG_BYTES = WIDE ? 0 : 8 * 4096;    // per-epilogue-warp 32x32-float transpose patches
   static constexpr int TAIL_BYTES = SLOT_BYTES + 1024 /*align slack*/ + 512 /*barriers*/ + STG_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + TAIL_BYTES;
   // halo engine: 16x8-pixel tiles; the (16+2)x(8+2) input patch of one 64-channel block is fetched ONCE (hi and lo
@@ -588,15 +626,15 @@ struct TcCfg {
   static constexpr int H_A_SLOT = 2 * H_A_PLANE;
   static constexpr int H_A_SLOTS = 2;
   static constexpr int H_B_SLOT = 2 * B_BYTES;
-  static constexpr int H_B_SLOTS = 4;
+  static constexpr int H_B_SLOTS = WIDE ? 2 : 4;           // 2 x 32 KB: a refill has one k-block (1536 MMA clocks) to land
   static constexpr int H_SMEM_BYTES = H_A_SLOTS * H_A_SLOT + H_B_SLOTS * H_B_SLOT + TAIL_BYTES;
   // fused operand transform (XF, halo engine only): the A patches arrive as the RAW fp32 activation (two 32-channel planes per
   // slot) and the transform warps apply GroupNorm-affine + SiLU + the hi/lo split in place before the MMAs read them
-  static constexpr int XF_WARPS = 4;                       // 18 warps: <= 112 registers per thread, no spills
-  static constexpr int XF_THREADS = TC_THREADS + 32 * XF_WARPS + 32;
+  static constexpr int XF_WARPS = WIDE ? 2 : 4;             // a BN = 128 patch feeds twice the MMA time of a BN = 64 one
+  static constexpr int XF_THREADS = THREADS + 32 * XF_WARPS + 32;
   static constexpr int X_A_SLOTS = 2;
   static constexpr int X_A_PLANE2 = H_A_PLANE + XF_SKEW;   // second plane of an XF slot (ends at 46720 <= H_A_SLOT)
-  static constexpr int X_B_SLOTS = 4;
+  static constexpr int X_B_SLOTS = H_B_SLOTS;
   static constexpr int X_SMEM_BYTES = X_A_SLOTS * H_A_SLOT + X_B_SLOTS * H_B_SLOT + TAIL_BYTES;
 };
 
@@ -607,13 +645,16 @@ struct TcCfg {
 // registers with round-to-nearest adds.
 // CPG > 0: the epilogue also emits GroupNorm(32) partial sums of the stored tile (CPG = Cout/32 channels per group).
 template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false>
-__global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TC_THREADS, 1)
+__global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
   static_assert(!XF || HALO, "the fused operand transform exists for the halo engine only");
   static_assert(!GEN || (XF && CPG == 0), "the generalised addressing exists for the fused-transform engine only");
   static_assert(!K1 || (XF && !GEN && CPG == 0), "K1 = fused transform of a 1x1 conv (patch = tile): its own instantiation");
   using Cfg = TcCfg<BN>;
+  constexpr bool WIDE = Cfg::WIDE;
+  static_assert(!WIDE || (HALO && !GEN && !K1 && CPG != 2), "128-wide tiles exist for the 3x3 / Upsample halo engine");
+  constexpr int MMA_WARPS = Cfg::MMA_WARPS, EPI_WARPS = Cfg::EPI_WARPS;
   constexpr int A_SLOTS = XF ? Cfg::X_A_SLOTS : Cfg::H_A_SLOTS;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -636,32 +677,32 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   uint64_t* araw = aempty + 3;                       // XF: raw patch landed (TMA -> transform warps)
   uint8_t* stage_buf = reinterpret_cast<uint8_t*>(bars) + 512;      // epilogue transpose patches (16-byte aligned)
 
-  // Roles are numbered logically (0 TMA, 1 MMA, 2..9 epilogue, 10.. transform, then the patch loader).  The MMA role is the
-  // warpgroup of physical warps 0..3 (wgmma needs an aligned warpgroup); the other roles sit on the remaining warp ids in
-  // REVERSE order: the sub-partition arbiter favours the highest warp id among its eligible warps, and the TMA producer must
-  // never wait for an issue slot, then the epilogue; the instruction-heavy transform warps come last.
-  constexpr int NWARPS = (XF ? TcCfg<BN>::XF_THREADS : TC_THREADS) / 32;
+  // Roles are numbered logically (0 TMA, 1 MMA, 2.. epilogue, then transform, then the patch loader).  The MMA role is the
+  // warpgroup(s) of physical warps 0..MMA_WARPS-1 (wgmma needs aligned warpgroups); the other roles sit on the remaining warp
+  // ids in REVERSE order: the sub-partition arbiter favours the highest warp id among its eligible warps, and the TMA producer
+  // must never wait for an issue slot, then the epilogue; the instruction-heavy transform warps come last.
+  constexpr int NWARPS = (XF ? Cfg::XF_THREADS : Cfg::THREADS) / 32;
   const int pwarp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform
   const int ridx = NWARPS - 1 - pwarp;
-  const int warp = pwarp < TC_MMA_WARPS ? 1 : (ridx == 0 ? 0 : ridx + 1);
+  const int warp = pwarp < MMA_WARPS ? 1 : (ridx == 0 ? 0 : ridx + 1);
   const int lane = threadIdx.x & 31;
   bool aborted = false;      // set when a barrier wait timed out anywhere on the device: leave the role loop (see mbar_wait)
   if (threadIdx.x == 0) TC_STAMP(0);
 
   if (warp == 0 && lane == 0) {
     for (int a = 0; a < 3; ++a) {
-      mbar_init(smem_u32(afull + a), XF ? TcCfg<BN>::XF_WARPS : 1);      // XF: every transform warp arrives
-      mbar_init(smem_u32(aempty + a), TC_MMA_WARPS);
+      mbar_init(smem_u32(afull + a), XF ? Cfg::XF_WARPS : 1);      // XF: every transform warp arrives
+      mbar_init(smem_u32(aempty + a), MMA_WARPS);
       mbar_init(smem_u32(araw + a), 1);
     }
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA_lo) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB_lo) : "memory");
-    for (int s = 0; s < NRING; ++s) { mbar_init(smem_u32(full + s), 1); mbar_init(smem_u32(empty + s), TC_MMA_WARPS); }
+    for (int s = 0; s < NRING; ++s) { mbar_init(smem_u32(full + s), 1); mbar_init(smem_u32(empty + s), MMA_WARPS); }
     for (int a = 0; a < Cfg::SLOTS; ++a) {
-      mbar_init(smem_u32(cfull + a), TC_MMA_WARPS);
-      mbar_init(smem_u32(cempty + a), TC_EPI_WARPS);
+      mbar_init(smem_u32(cfull + a), MMA_WARPS);
+      mbar_init(smem_u32(cempty + a), EPI_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -754,17 +795,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       }
     }
   } else if (warp == 1) {
-    // ============================ MMA warpgroup (physical warps 0..3) ============================
-    // Per k-block (64 K-elements) and 64-row half of the tile: 4 k-steps x {A_lo B_hi, A_hi B_lo, A_hi B_hi}.
+    // ============================ MMA warpgroup(s) (physical warps 0..MMA_WARPS-1) ============================
+    // Per k-block (64 K-elements) and 64-row half of the tile: 4 k-steps x {A_lo B_hi, A_hi B_lo, A_hi B_hi}.  BN = 64: one
+    // warpgroup issues both halves (m64n64k16); BN = 128: warpgroup `wg` issues half `wg` (m64n128k16).
     // A descriptors: per-tap engine = 128 rows of 128 B in 8-row groups 1024 B apart (rows 64..127 start 8 KB in).  Halo
     // engine: rows of the tile are pixels (h, w) of a 16x8 patch; patch row h is one 8-row core-matrix group that starts
     // (h + r) * PW + s rows into the halo buffer => group stride PW*128 B and a start address that is only 128-byte
     // aligned.  The tensor core applies the 128B swizzle on absolute shared-memory address bits, i.e. exactly the pattern
     // the TMA unit used when it wrote the buffer.
     {
+      constexpr int MH = WIDE ? 1 : 2;                  // 64-row halves issued by this warpgroup
       const uint32_t a_sbo = HALO ? (uint32_t)(p.PW * 128) : 1024u;
       const uint32_t a_half = HALO ? (uint32_t)(8 * p.PW * 128) : 8192u;
-      const int wq = (int)(threadIdx.x >> 5);          // 16-row group of this warp inside each 64-row half
+      const int wq = (int)(threadIdx.x >> 5) & 3;      // 16-row group of this warp inside each 64-row half
+      const int wg = (int)(threadIdx.x >> 7);          // BN = 128: the 64-row half of this warpgroup
+      const uint32_t bar_id = 2u + (uint32_t)wg;       // named barrier of this warpgroup's abort decision
       const uint32_t slot_base = smem_u32(acc_slot);
       int stage = 0;
       uint32_t phase = 0;
@@ -772,7 +817,83 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       uint32_t slot_phase = 0;
       int aslot = 0;
       uint32_t aphase = 0;
-      float acc[2][32];
+      float acc[MH][WIDE ? 64 : 32];
+      if constexpr (WIDE) {
+        // BN = 128: per chunk of k-blocks, every k-block's group is committed with one earlier group still in flight
+        // (wait_group 1, a fixed depth), after which the weight slot (and, after its last tap, the patch) of the PREVIOUS
+        // k-block is released; wait_group 0 only after the chunk's last k-block, where the partial sum is folded.
+        for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
+          const int par = p.up4 ? ((tile / p.n_tiles) & 3) : 0;    // output parity of this tile
+          const int par_y = par >> 1, par_x = par & 1;
+          for (int c0 = 0; c0 < nk; c0 += p.chunk) {
+            const int c1 = min(c0 + p.chunk, nk);
+            uint32_t prev_empty = 0, prev_aempty = 0;                // barriers the previous k-block releases (0: none)
+            for (int it = c0; it < c1; ++it) {
+              const int kb = it / p.taps;
+              const int tap = it - kb * p.taps;
+              if (tap == 0) {
+                mbar_wait(smem_u32(afull + aslot), aphase, aborted);
+                if (wg_any(aborted, bar_id)) { wg_wait_all(); aborted = true; goto teardown; }
+              }
+              int r = (p.taps == 9) ? tap / 3 : 0;
+              int sft = (p.taps == 9) ? tap - r * 3 : 0;
+              if (p.up4) { r = (tap >> 1) + par_y; sft = (tap & 1) + par_x; }
+              const uint32_t a_hi0 = smem_u32(smem + aslot * Cfg::H_A_SLOT) + (uint32_t)((r * p.PW + sft) * 128) +
+                                     (uint32_t)wg * a_half;
+              const uint32_t a_lo0 = a_hi0 + (uint32_t)(XF ? Cfg::X_A_PLANE2 : Cfg::H_A_PLANE);
+              const uint32_t bsm = smem_u32(ring_base + stage * RING_BYTES);
+              mbar_wait(smem_u32(full + stage), phase, aborted);
+              if (wg_any(aborted, bar_id)) { wg_wait_all(); aborted = true; goto teardown; }
+              wg_fence();
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const uint64_t db_hi = wg_desc(bsm + 32 * k, 1024u), db_lo = wg_desc(bsm + Cfg::B_BYTES + 32 * k, 1024u);
+                const uint64_t da_hi = wg_desc(a_hi0 + 32 * k, a_sbo), da_lo = wg_desc(a_lo0 + 32 * k, a_sbo);
+                wg_mma_64x128(acc[0], da_lo, db_hi, (it == c0 && k == 0) ? 0u : 1u);
+                wg_mma_64x128(acc[0], da_hi, db_lo, 1u);
+                wg_mma_64x128(acc[0], da_hi, db_hi, 1u);
+              }
+              wg_commit();
+              wg_wait_1();
+              __syncwarp();
+              mbar_arrive_if(prev_empty, lane == 0 && prev_empty != 0);
+              mbar_arrive_if(prev_aempty, lane == 0 && prev_aempty != 0);
+              prev_empty = smem_u32(empty + stage);
+              prev_aempty = tap == p.taps - 1 ? smem_u32(aempty + aslot) : 0u;
+              if (++stage == NRING) { stage = 0; phase ^= 1; }
+              if (tap == p.taps - 1 && ++aslot == A_SLOTS) { aslot = 0; aphase ^= 1; }
+            }
+            wg_wait_all();
+            __syncwarp();
+            mbar_arrive_if(prev_empty, lane == 0);
+            mbar_arrive_if(prev_aempty, lane == 0 && prev_aempty != 0);
+            // fold into the tile slot: the first chunk of a tile waits until the epilogue has read the previous tile and
+            // stores 0 + sum (the epilogue's fold starts from 0), later chunks add with round-to-nearest
+            const bool first_chunk = c0 == 0;
+            if (first_chunk) {
+              mbar_wait(smem_u32(cempty + slot), slot_phase ^ 1, aborted);
+              if (wg_any(aborted, bar_id)) { aborted = true; goto teardown; }
+            }
+            const uint32_t sbase = slot_base + (uint32_t)(slot * Cfg::SLOT_BYTES);
+            const int row = wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+#pragma unroll
+              for (int h8 = 0; h8 < 2; ++h8) {
+                const uint32_t e = sbase + (uint32_t)(((row + 8 * h8) * Cfg::SLOT_PITCH + 8 * j + 2 * (lane & 3)) * 4);
+                float x = 0.f, y = 0.f;
+                if (!first_chunk) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x), "=f"(y) : "r"(e) : "memory");
+                x = __fadd_rn(x, acc[0][4 * j + 2 * h8]);
+                y = __fadd_rn(y, acc[0][4 * j + 2 * h8 + 1]);
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(e), "f"(x), "f"(y) : "memory");
+              }
+            }
+          }
+          __syncwarp();                                              // tile complete -> epilogue warps
+          if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
+          if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+        }
+      } else {
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
         const int par = p.up4 ? ((tile / p.n_tiles) & 3) : 0;      // output parity of this tile
         const int par_y = par >> 1, par_x = par & 1;
@@ -842,8 +963,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           }
         }
       }
+      }
     }
-  } else if (XF && warp == 2 + TC_EPI_WARPS + TcCfg<BN>::XF_WARPS) {
+  } else if (XF && warp == 2 + EPI_WARPS + Cfg::XF_WARPS) {
     // ============================ XF: A-patch loader (own warp: patches must be requested a whole patch ahead) ==========
     // The patch of one 64-channel block arrives as RAW fp32 NHWC values of the producing conv's output: two TMA boxes of
     // 32 channels (128 B rows, 128B swizzle) into the two planes of the slot.  tmA_hi / tmA_lo are the fp32 tensor maps of
@@ -878,7 +1000,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
       }
     }
-  } else if (XF && warp >= 2 + TC_EPI_WARPS) {
+  } else if (XF && warp >= 2 + EPI_WARPS) {
     // ============================ XF: operand transform (warps 10..) ============================
     // raw fp32 patch (zero outside the image: TMA out-of-bounds fill) -> y = act(x * scale[n,c] + shift[n,c]) (GroupNorm folded
     // into scale/shift, vqgan_arch.py:14-20,153-160) -> fp16 hi = rn(y), lo = rn(y - hi), written back IN PLACE in the
@@ -890,12 +1012,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // fall on different banks: each warp-wide LDS.128 / STS.128 is 4 conflict-free wavefronts.  Pixels outside the image
     // stay exactly zero (the conv pads the NORMALISED tensor).  fence.proxy.async publishes the writes to the tensor core.
     if constexpr (XF) {
-      constexpr int XFW = TcCfg<BN>::XF_WARPS;
+      constexpr int XFW = Cfg::XF_WARPS;
       constexpr int RPP = 4 * XFW;                                  // patch rows per pass (8 lanes per row)
       constexpr int XF_PW = 10, XF_PH = 18, XF_ROWS = XF_PW * XF_PH;   // halo patch of an 8 x 16 tile and a 3 x 3 filter
       constexpr int NPASS = (XF_ROWS + RPP - 1) / RPP;
       constexpr int NPASS1 = (128 + RPP - 1) / RPP;                     // 1x1 convs: the patch is the 8 x 16 tile itself
-      const int t = (warp - (2 + TC_EPI_WARPS)) * 32 + lane;
+      const int t = (warp - (2 + EPI_WARPS)) * 32 + lane;
       const int j = t & 7, rsub = t >> 3;
       const int pl = j >> 2, c0 = 2 * (j & 3);                      // source plane and first 16-byte chunk of this lane's 8 channels
       const int mode = p.in_scale ? (p.in_act == IN_SILU ? 2 : 1) : 0;   // 2: affine + SiLU, 1: affine, 0: raw split
@@ -981,10 +1103,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       if (amax > 65504.f) report_overflow();      // an operand left the fp16 range: the host turns the status word into an error
     }
   } else {
-    // ============================ epilogue (warps 2..9) ============================
-    constexpr int HC = BN / 2;               // columns owned by this thread
+    // ============================ epilogue (warps 2..EPI_WARPS+1) ============================
+    constexpr int HC = BN * 4 / EPI_WARPS;   // columns owned by this warp: 32 (BN = 64), all 128 (BN = 128)
     const int lg = (warp - 2) & 3;           // row quadrant of this warp: rows [32*lg, 32*lg+32) of the tile
-    const int half = (warp - 2) >> 2;        // which half of the tile's columns (logical warps e and e+4 share a quadrant)
+    const int half = (warp - 2) >> 2;        // BN = 64: which half of the tile's columns (logical warps e and e+4 share a quadrant)
     const int row = lg * 32 + lane;          // pixel row of the tile
     const int cbase = half * HC;
     const float wsi = __ldg(p.wscale_inv);
@@ -1033,30 +1155,35 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           asm volatile("prefetch.global.L2 [%0];" ::"l"(p.sft_scale + off0 + j));
         }
       }
-      float acc[HC];
-#pragma unroll
-      for (int j = 0; j < HC; ++j) acc[j] = 0.f;
-      for (int it0 = 0; it0 < nk; it0 += p.chunk) {
+      float acc[WIDE ? 1 : HC];
+      if constexpr (WIDE) {
+        // the MMA warpgroups have folded every partial sum of this tile into the slot; it is read by the store loop below
         mbar_wait<250>(smem_u32(cfull + slot), slot_phase, aborted); if (aborted) goto teardown;
-        const uint32_t srow = smem_u32(acc_slot) + (uint32_t)(slot * Cfg::SLOT_BYTES) + (uint32_t)((row * Cfg::SLOT_PITCH + cbase) * 4);
+      } else {
 #pragma unroll
-        for (int c0 = 0; c0 < HC; c0 += 4) {          // round-to-nearest adds of the partial sum
-          const float4 v = lds128f(srow + (uint32_t)(c0 * 4));
-          acc[c0] += v.x; acc[c0 + 1] += v.y; acc[c0 + 2] += v.z; acc[c0 + 3] += v.w;
+        for (int j = 0; j < HC; ++j) acc[j] = 0.f;
+        for (int it0 = 0; it0 < nk; it0 += p.chunk) {
+          mbar_wait<250>(smem_u32(cfull + slot), slot_phase, aborted); if (aborted) goto teardown;
+          const uint32_t srow = smem_u32(acc_slot) + (uint32_t)(slot * Cfg::SLOT_BYTES) + (uint32_t)((row * Cfg::SLOT_PITCH + cbase) * 4);
+#pragma unroll
+          for (int c0 = 0; c0 < HC; c0 += 4) {          // round-to-nearest adds of the partial sum
+            const float4 v = lds128f(srow + (uint32_t)(c0 * 4));
+            acc[c0] += v.x; acc[c0 + 1] += v.y; acc[c0 + 2] += v.z; acc[c0 + 3] += v.w;
+          }
+          asm volatile("" ::: "memory");
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(cempty + slot));
+          if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
         }
-        asm volatile("" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(cempty + slot));
-        if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
       }
       if (warp == 2 && lane == 0 && tile == first_tile) TC_STAMP(7);
       if (warp == 2 && lane == 0 && tile == first_tile + tile_step) TC_STAMP(17);
       // ---- finalize this tile: scale, bias, residual, activation, SFT, store (fp32 NHWC), GroupNorm partials.
       // A thread owns a pixel ROW, so storing straight from registers would touch 32 different 128-byte lines per
-      // instruction.  Each warp instead transposes 32x32-float blocks through a private 4 KB XOR-swizzled smem patch:
-      // afterwards lane l holds the 16-byte chunk (l & 7) of row (l >> 3) + 4*it, i.e. 8 lanes cover one full 128-byte
-      // line and every global access (residual / SFT loads, the store) is a fully used line.
-      if (!HALO && !GEN && p.vq_cand) {
+      // instruction.  Each warp instead transposes 32x32-float blocks through a private 4 KB XOR-swizzled smem patch (BN = 128:
+      // reads the tile slot directly): afterwards lane l holds the 16-byte chunk (l & 7) of row (l >> 3) + 4*it, i.e. 8 lanes
+      // cover one full 128-byte line and every global access (residual / SFT loads, the store) is a fully used line.
+      if constexpr (!HALO && !GEN) if (p.vq_cand) {
         // VectorQuantizer.forward (vqgan_arch.py:40-46): this thread owns token row `pix` and HC codes; d = (|z|^2 + |e|^2) - 2 z.e
         // in the reference's operation order, first minimum of the slice (ascending index, strict <); no staging, no store of
         // the [tokens, codes] matrix.  The candidates of a token (2 per n-tile) are reduced by vq_select_cand.
@@ -1132,19 +1259,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           __syncwarp();
         }
       } else {
+      // BN = 128: this warp's 32 rows of the tile slot, 16-byte chunk (lane & 7) of row (lane >> 3) + 4*it
+      const uint32_t slot_q = smem_u32(acc_slot) + (uint32_t)(slot * Cfg::SLOT_BYTES) +
+                              (uint32_t)(((lg * 32 + rsub) * Cfg::SLOT_PITCH + cbase + cch * 4) * 4);
 #pragma unroll
       for (int q = 0; q < HC; q += 32) {
+        if constexpr (!WIDE) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          sts128f(stg_w + (uint32_t)((j ^ (lane & 7)) << 4), acc[q + 4 * j] * wsi, acc[q + 4 * j + 1] * wsi, acc[q + 4 * j + 2] * wsi,
-                  acc[q + 4 * j + 3] * wsi);
-        __syncwarp();
+          for (int j = 0; j < 8; ++j)
+            sts128f(stg_w + (uint32_t)((j ^ (lane & 7)) << 4), acc[q + 4 * j] * wsi, acc[q + 4 * j + 1] * wsi, acc[q + 4 * j + 2] * wsi,
+                    acc[q + 4 * j + 3] * wsi);
+          __syncwarp();
+        }
         const int colq = col0 + q + cch * 4;                  // first of this lane's 4 channels
         float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
         if (p.bias) bv = __ldg(reinterpret_cast<const float4*>(p.bias + colq));
         // global offsets of the (row, chunk) items of this lane, then their residual loads in flight at once: all 8 rows, or two
-        // batches of 4 in the register-capped transform variants
-        constexpr int RB = XF ? 4 : 8;
+        // batches of 4 in the register-capped (96-register) BN = 64 transform variants
+        constexpr int RB = (XF && !WIDE) ? 4 : 8;
         float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
 #pragma unroll
         for (int ib = 0; ib < 8; ib += RB) {
@@ -1166,7 +1298,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         for (int k = 0; k < RB; ++k) {
           const int it = ib + k;
           const int r = it * 4 + rsub;                        // row within this warp's 32-row quadrant
-          float4 v = lds128f(stg + (uint32_t)(r * 128 + ((cch ^ (r & 7)) << 4)));
+          float4 v;
+          if constexpr (WIDE) {      // scaled here as the BN = 64 path scales before its transpose (__fmul_rn: never contracted)
+            v = lds128f(slot_q + (uint32_t)((it * 4 * Cfg::SLOT_PITCH + q) * 4));
+            v.x = __fmul_rn(v.x, wsi); v.y = __fmul_rn(v.y, wsi); v.z = __fmul_rn(v.z, wsi); v.w = __fmul_rn(v.w, wsi);
+          } else {
+            v = lds128f(stg + (uint32_t)(r * 128 + ((cch ^ (r & 7)) << 4)));
+          }
           const int64_t off = offs[k];
           v.x += bv.x + rres[k].x; v.y += bv.y + rres[k].y; v.z += bv.z + rres[k].z; v.w += bv.w + rres[k].w;
           if (p.out_act == OUT_LRELU) {
@@ -1229,6 +1367,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
         __syncwarp();
       }
+      }
+      if constexpr (WIDE) {          // every read of the tile slot is done: the MMA warpgroups may store the next tile
+        if (lane == 0) mbar_arrive(smem_u32(cempty + slot));
+        if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
       }
       if (warp == 2 && lane == 0 && tile == first_tile) TC_STAMP(16);
       if (warp == 2 && lane == 0 && tile == first_tile + tile_step) TC_STAMP(18);
@@ -1388,7 +1530,7 @@ template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1
 static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int SMEM = XF ? Cfg::X_SMEM_BYTES : (HALO ? Cfg::H_SMEM_BYTES : Cfg::SMEM_BYTES);
-  constexpr int THREADS = XF ? TcCfg<BN>::XF_THREADS : TC_THREADS;
+  constexpr int THREADS = XF ? Cfg::XF_THREADS : Cfg::THREADS;
   static_assert(SMEM <= 232448, "shared memory budget");
   // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE property of the function: remember it per device
   // (one process may drive several GPUs from several threads)
@@ -1407,7 +1549,16 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
   return 0;
 }
 template <int CPG>
-static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false) {
+static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, bool wide = false) {
+  if (wide) {            // 128-wide n-tiles: conv_tc() only asks for them where tc_wide_tiles() holds
+    if constexpr (CPG != 2) {
+      CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: 128-wide tiles need the 3x3 / Upsample halo engine");
+      if (p.xform) return launch_tc2<128, CPG, true, true>(m, p, sm_count, st);
+      return launch_tc2<128, CPG, true>(m, p, sm_count, st);
+    } else {
+      CFB_REQUIRE(false, "conv_tc: 128-wide tiles need Cout % 128 == 0");
+    }
+  }
   if constexpr (CPG == 0) {
     if (gen) {
       CFB_REQUIRE(p.xform && p.PW == 10 && p.PH == 18, "conv_tc: generalised variant needs the halo + transform engine");
@@ -1426,6 +1577,15 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   if (p.PW > 0) return launch_tc2<64, CPG, true>(m, p, sm_count, st);
   return launch_tc2<64, CPG, false>(m, p, sm_count, st);
 }
+
+// 128-output-channel tiles (two MMA warpgroups, see TcCfg) for the 3x3 and Upsample convs of the halo engine with
+// Cout % 128 == 0.  CFB_TC_BN=64 keeps every conv on 64-wide tiles (same results bit for bit: A/B comparisons in one build).
+static bool tc_wide_tiles(const ConvArgs& a, const TcGeom& g) {
+  static const bool on = [] { const char* e = getenv("CFB_TC_BN"); return !(e && atoi(e) == 64); }();
+  return on && g.halo && !a.gen && a.ksize == 3 && (a.mode == CONV_SAME || a.mode == CONV_UP) && a.Cout % 128 == 0;
+}
+
+int tc_tile_n(const ConvArgs& a) { return tc_wide_tiles(a, tc_geometry(a)) ? 128 : TC_TILE_N; }
 
 // GroupNorm partial sums can be emitted for Cout in {64, 128, 256, 512} (2 .. 16 channels per group inside a 64-wide n-tile)
 bool tc_can_emit_stats(const ConvArgs& a) {
@@ -1465,7 +1625,8 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   const TcGeom geo = tc_geometry(a);
   const int BW = geo.BW, BH = geo.BH;
   const int PW = geo.halo ? BW + a.ksize - 1 : 0, PH = geo.halo ? BH + a.ksize - 1 : 0;
-  constexpr int BN = TC_TILE_N;
+  const bool wide = tc_wide_tiles(a, geo);
+  const int BN = wide ? 128 : TC_TILE_N;
   TcMaps mp;
   CUtensorMap &mA_hi = mp.a_hi, &mA_lo = mp.a_lo, &mB_hi = mp.b_hi, &mB_lo = mp.b_lo;
   if (a.xform) {
@@ -1559,11 +1720,11 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   CFB_REQUIRE(!a.gn_part || tc_can_emit_stats(a), "conv_tc: GroupNorm partials are not available for this Cout");
   if (a.gen) return launch_tc<0>(mp, p, sm_count, st, true);
   switch (cpg) {
-    case 0: return launch_tc<0>(mp, p, sm_count, st);
-    case 2: return launch_tc<2>(mp, p, sm_count, st);
-    case 4: return launch_tc<4>(mp, p, sm_count, st);
-    case 8: return launch_tc<8>(mp, p, sm_count, st);
-    case 16: return launch_tc<16>(mp, p, sm_count, st);
+    case 0: return launch_tc<0>(mp, p, sm_count, st, false, wide);
+    case 2: return launch_tc<2>(mp, p, sm_count, st, false, wide);
+    case 4: return launch_tc<4>(mp, p, sm_count, st, false, wide);
+    case 8: return launch_tc<8>(mp, p, sm_count, st, false, wide);
+    case 16: return launch_tc<16>(mp, p, sm_count, st, false, wide);
   }
   CFB_REQUIRE(false, "conv_tc: no kernel variant for this configuration");
   return 1;

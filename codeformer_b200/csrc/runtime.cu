@@ -2171,6 +2171,47 @@ int cfb_conv2d_nhwc(const float* in, const float* weight_oihw, const float* bias
   API_END(1)
 }
 
+int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias, float* out,
+                      int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                      const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                      const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
+                      void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n) {
+  API_BEGIN
+  CFB_REQUIRE(in && weight_oihw && out && workspace && tile_n, "cfb_debug_conv_tc: NULL argument");
+  CFB_REQUIRE(mode == cfb::CONV_SAME || mode == cfb::CONV_UP, "cfb_debug_conv_tc: mode must be 0 or 2");
+  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, 3, mode), "cfb_debug_conv_tc: workspace too small");
+  CFB_CHECK(cfb::async_status_init(nullptr));
+  cudaStream_t st = (cudaStream_t)stream;
+  cfb::ConvArgs a;
+  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = 3; a.mode = mode;
+  a.Ho = mode == cfb::CONV_UP ? h * 2 : h;
+  a.Wo = mode == cfb::CONV_UP ? w * 2 : w;
+  a.bias = bias; a.in_scale = in_scale; a.in_shift = in_shift; a.in_act = in_act; a.residual = residual; a.out = out;
+  a.sft_dec = sft_dec; a.sft_scale = sft_scale; a.sft_w = sft_w; a.out_planes = out_planes; a.gn_part = gn_part;
+  a.in2 = in2; a.Cin1 = in2 ? cin1 : 0;
+  CFB_REQUIRE(cfb::tc_supported(a), "cfb_debug_conv_tc: shape not on the wgmma engine");
+  const size_t wn = (size_t)cout * cin * 9;
+  const size_t wsplit = mode == cfb::CONV_UP ? (size_t)16 * cout * cin : wn;
+  char* p = (char*)workspace + align256(wn * 4);
+  __half* whi = (__half*)p; p += align256(wsplit * 2);
+  __half* wlo = (__half*)p; p += align256(wsplit * 2);
+  float* wsc = (float*)p; p += 256;
+  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
+  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1;
+  if (xform) {
+    CFB_REQUIRE(cfb::tc_can_xform(a), "cfb_debug_conv_tc: no fused operand transform for this conv");
+    a.xform = true; a.skip_prep = true;
+  }
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (mode == cfb::CONV_UP) CFB_CHECK(cfb::tc_split_weights_up4(weight_oihw, whi, wlo, cout, cin, wsc, st));
+  else CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, 3, wsc, st));
+  *tile_n = cfb::tc_tile_n(a);
+  CFB_CHECK(cfb::conv_tc(a, p, sms, st));
+  return 0;
+  API_END(1)
+}
 int cfb_debug_time_conv(const float* in, const float* weight_oihw, float* out, int32_t n, int32_t h, int32_t w, int32_t cin,
                         int32_t cout, int32_t ksize, int32_t mode, int32_t reps, void* workspace, int64_t workspace_bytes,
                         void* stream, const float* in_scale, const float* in_shift, int32_t in_act, float* ms_per_launch) {
