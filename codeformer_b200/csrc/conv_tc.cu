@@ -3,7 +3,8 @@
 // Computes the 3x3 / 1x1 convolutions and linears of the CodeFormer hot path
 //   nn.Conv2d call sites      /root/reference/basicsr/archs/vqgan_arch.py:120,132,147-151,173-200,243,266,292,314
 //   Fuse_sft convs, Linear    /root/reference/basicsr/archs/codeformer_arch.py:104-106,141-149,183,192
-// as GEMMs  D[M = 128 output pixels, N = 64 or 128 output channels (TcCfg)] += A[M, K] * B[N, K]^T  with K = taps * Cin, on
+// as GEMMs  D[M = 128 output pixels, N = 64 or 128 output channels (TcCfg; 64-channel halo tiles are computed transposed, CM)]
+// += A[M, K] * B[N, K]^T  with K = taps * Cin, on
 // the Hopper tensor cores:
 //   * operands are error-compensated fp16 pairs  x = hi + lo  (hi = fp16(x), lo = fp16(x - hi)); the products
 //     lo*hi + hi*lo + hi*hi are three wgmma.mma_async m64n64k16 per 64-row half and k-step, fp32 accumulation in registers
@@ -644,7 +645,10 @@ struct TcCfg {
 // cross terms (lo*hi, hi*lo) of every k-step before hi*hi, and the epilogue warps fold every finished partial sum into fp32
 // registers with round-to-nearest adds.
 // CPG > 0: the epilogue also emits GroupNorm(32) partial sums of the stored tile (CPG = Cout/32 channels per group).
-template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false>
+// CM (channel-major, BN = 64 only): the MMA warpgroup computes the tile transposed, D^T[64 channels x 128 pixels] =
+// W[64 x K] * X[128 x K]^T, as one m64n128k16 per product and k-step (weights = A operand, halo patch = B operand), and stores
+// each partial sum into the slot as [pixel][channel]: the epilogue is that of the pixel-major 128 x 64 tile.
+template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false>
 __global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
@@ -654,6 +658,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   using Cfg = TcCfg<BN>;
   constexpr bool WIDE = Cfg::WIDE;
   static_assert(!WIDE || (HALO && !GEN && !K1 && CPG != 2), "128-wide tiles exist for the 3x3 / Upsample halo engine");
+  static_assert(!CM || (BN == 64 && HALO && !GEN && !K1), "channel-major tiles exist for the 64-channel 3x3 / Upsample halo convs");
   constexpr int MMA_WARPS = Cfg::MMA_WARPS, EPI_WARPS = Cfg::EPI_WARPS;
   constexpr int A_SLOTS = XF ? Cfg::X_A_SLOTS : Cfg::H_A_SLOTS;
   constexpr int STAGES = Cfg::STAGES;
@@ -797,14 +802,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   } else if (warp == 1) {
     // ============================ MMA warpgroup(s) (physical warps 0..MMA_WARPS-1) ============================
     // Per k-block (64 K-elements) and 64-row half of the tile: 4 k-steps x {A_lo B_hi, A_hi B_lo, A_hi B_hi}.  BN = 64: one
-    // warpgroup issues both halves (m64n64k16); BN = 128: warpgroup `wg` issues half `wg` (m64n128k16).
+    // warpgroup issues both halves (m64n64k16); BN = 128: warpgroup `wg` issues half `wg` (m64n128k16); CM: one warpgroup
+    // issues the whole transposed tile (m64n128k16, weights as A: W_hi X_lo, W_lo X_hi, W_hi X_hi -- the same products in
+    // the same order).
     // A descriptors: per-tap engine = 128 rows of 128 B in 8-row groups 1024 B apart (rows 64..127 start 8 KB in).  Halo
     // engine: rows of the tile are pixels (h, w) of a 16x8 patch; patch row h is one 8-row core-matrix group that starts
     // (h + r) * PW + s rows into the halo buffer => group stride PW*128 B and a start address that is only 128-byte
     // aligned.  The tensor core applies the 128B swizzle on absolute shared-memory address bits, i.e. exactly the pattern
     // the TMA unit used when it wrote the buffer.
+    // CM: the same descriptor is the B operand and spans the whole 128-pixel tile: its 16 core-matrix groups are the 16 patch
+    // rows, PW*128 B apart, and the second 64-row half starts a_half = 8 groups in.
     {
-      constexpr int MH = WIDE ? 1 : 2;                  // 64-row halves issued by this warpgroup
+      constexpr bool N128 = WIDE || CM;                 // m64n128k16 issue: one accumulator of 64 fp32 per thread
+      constexpr int MH = N128 ? 1 : 2;                  // 64-row halves issued by this warpgroup
       const uint32_t a_sbo = HALO ? (uint32_t)(p.PW * 128) : 1024u;
       const uint32_t a_half = HALO ? (uint32_t)(8 * p.PW * 128) : 8192u;
       const int wq = (int)(threadIdx.x >> 5) & 3;      // 16-row group of this warp inside each 64-row half
@@ -817,11 +827,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       uint32_t slot_phase = 0;
       int aslot = 0;
       uint32_t aphase = 0;
-      float acc[MH][WIDE ? 64 : 32];
-      if constexpr (WIDE) {
-        // BN = 128: per chunk of k-blocks, every k-block's group is committed with one earlier group still in flight
+      float acc[MH][N128 ? 64 : 32];
+      if constexpr (N128) {
+        // BN = 128 and CM: per chunk of k-blocks, every k-block's group is committed with one earlier group still in flight
         // (wait_group 1, a fixed depth), after which the weight slot (and, after its last tap, the patch) of the PREVIOUS
-        // k-block is released; wait_group 0 only after the chunk's last k-block, where the partial sum is folded.
+        // k-block is released; wait_group 0 only after the chunk's last k-block, where the partial sum is folded (BN = 128)
+        // or handed to the epilogue warps (CM).
         for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
           const int par = p.up4 ? ((tile / p.n_tiles) & 3) : 0;    // output parity of this tile
           const int par_y = par >> 1, par_x = par & 1;
@@ -849,9 +860,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               for (int k = 0; k < 4; ++k) {
                 const uint64_t db_hi = wg_desc(bsm + 32 * k, 1024u), db_lo = wg_desc(bsm + Cfg::B_BYTES + 32 * k, 1024u);
                 const uint64_t da_hi = wg_desc(a_hi0 + 32 * k, a_sbo), da_lo = wg_desc(a_lo0 + 32 * k, a_sbo);
-                wg_mma_64x128(acc[0], da_lo, db_hi, (it == c0 && k == 0) ? 0u : 1u);
-                wg_mma_64x128(acc[0], da_hi, db_lo, 1u);
-                wg_mma_64x128(acc[0], da_hi, db_hi, 1u);
+                if constexpr (CM) {
+                  wg_mma_64x128(acc[0], db_hi, da_lo, (it == c0 && k == 0) ? 0u : 1u);
+                  wg_mma_64x128(acc[0], db_lo, da_hi, 1u);
+                  wg_mma_64x128(acc[0], db_hi, da_hi, 1u);
+                } else {
+                  wg_mma_64x128(acc[0], da_lo, db_hi, (it == c0 && k == 0) ? 0u : 1u);
+                  wg_mma_64x128(acc[0], da_hi, db_lo, 1u);
+                  wg_mma_64x128(acc[0], da_hi, db_hi, 1u);
+                }
               }
               wg_commit();
               wg_wait_1();
@@ -867,6 +884,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             __syncwarp();
             mbar_arrive_if(prev_empty, lane == 0);
             mbar_arrive_if(prev_aempty, lane == 0 && prev_aempty != 0);
+            if constexpr (CM) {
+              // partial sum -> slot[pixel][channel], folded by the epilogue warps as on the pixel-major tile.  Thread t holds
+              // channels 16*(t/32) + (t%32)/4 (+8) and pixels 8j + 2(t%4) (+1); with SLOT_PITCH = 68 the 32 scalar stores of
+              // one instruction fall on 32 distinct banks, (4*pixel + channel) mod 32.
+              mbar_wait(smem_u32(cempty + slot), slot_phase ^ 1, aborted);
+              if (wg_any(aborted, bar_id)) { aborted = true; goto teardown; }
+              const uint32_t st0 = slot_base + (uint32_t)(slot * Cfg::SLOT_BYTES) +
+                                   (uint32_t)((2 * (lane & 3) * Cfg::SLOT_PITCH + wq * 16 + (lane >> 2)) * 4);
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                for (int h8 = 0; h8 < 2; ++h8) {
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    const uint32_t a = st0 + (uint32_t)(((8 * j + e) * Cfg::SLOT_PITCH + 8 * h8) * 4);
+                    asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(acc[0][4 * j + 2 * h8 + e]) : "memory");
+                  }
+                }
+              }
+              __syncwarp();
+              if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
+              if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+              continue;
+            }
             // fold into the tile slot: the first chunk of a tile waits until the epilogue has read the previous tile and
             // stores 0 + sum (the epilogue's fold starts from 0), later chunks add with round-to-nearest
             const bool first_chunk = c0 == 0;
@@ -889,9 +930,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               }
             }
           }
-          __syncwarp();                                              // tile complete -> epilogue warps
-          if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
-          if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+          if constexpr (!CM) {
+            __syncwarp();                                            // tile complete -> epilogue warps
+            if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
+            if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+          }
         }
       } else {
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
@@ -1526,7 +1569,7 @@ size_t tc_scratch_bytes(const ConvArgs& a) {
 
 struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
 
-template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false>
+template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false>
 static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int SMEM = XF ? Cfg::X_SMEM_BYTES : (HALO ? Cfg::H_SMEM_BYTES : Cfg::SMEM_BYTES);
@@ -1539,18 +1582,27 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
   CFB_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count ? total : sm_count;
-  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st, m.a_hi, m.a_lo,
-                 m.b_hi, m.b_lo, p);
+  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st, m.a_hi,
+                 m.a_lo, m.b_hi, m.b_lo, p);
   return 0;
 }
 template <int CPG>
-static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, bool wide = false) {
-  if (wide) {            // 128-wide n-tiles: conv_tc() only asks for them where tc_wide_tiles() holds
+static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, int tile = TC_TILE_N) {
+  if (tile == TC_TILE_CM) {    // channel-major 128 x 64 tiles: conv_tc() only asks for them where tc_tile_kind() says so
+    if constexpr (CPG <= 2) {
+      CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: channel-major tiles need the 3x3 / Upsample halo engine");
+      if (p.xform) return launch_tc2<64, CPG, true, true, false, false, true>(m, p, sm_count, st);
+      return launch_tc2<64, CPG, true, false, false, false, true>(m, p, sm_count, st);
+    } else {
+      CFB_REQUIRE(false, "conv_tc: channel-major tiles need Cout % 128 == 64");
+    }
+  }
+  if (tile == 128) {     // 128-wide n-tiles: conv_tc() only asks for them where tc_tile_kind() says so
     if constexpr (CPG != 2) {
       CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: 128-wide tiles need the 3x3 / Upsample halo engine");
       if (p.xform) return launch_tc2<128, CPG, true, true>(m, p, sm_count, st);
@@ -1578,14 +1630,17 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   return launch_tc2<64, CPG, false>(m, p, sm_count, st);
 }
 
-// 128-output-channel tiles (two MMA warpgroups, see TcCfg) for the 3x3 and Upsample convs of the halo engine with
-// Cout % 128 == 0.  CFB_TC_BN=64 keeps every conv on 64-wide tiles (same results bit for bit: A/B comparisons in one build).
-static bool tc_wide_tiles(const ConvArgs& a, const TcGeom& g) {
+// Tile of the 3x3 and Upsample convs of the halo engine (not GEN): 128-output-channel tiles (two MMA warpgroups, see TcCfg)
+// when Cout % 128 == 0, channel-major 128 x 64 tiles (TC_TILE_CM, see conv_tc_kernel) otherwise; every other conv runs on
+// pixel-major 128 x 64 tiles.  CFB_TC_BN=64 keeps every conv on the pixel-major 128 x 64 tiles (same results bit for bit:
+// A/B comparisons in one build).
+static int tc_tile_kind(const ConvArgs& a, const TcGeom& g) {
   static const bool on = [] { const char* e = getenv("CFB_TC_BN"); return !(e && atoi(e) == 64); }();
-  return on && g.halo && !a.gen && a.ksize == 3 && (a.mode == CONV_SAME || a.mode == CONV_UP) && a.Cout % 128 == 0;
+  if (!(on && g.halo && !a.gen && a.ksize == 3 && (a.mode == CONV_SAME || a.mode == CONV_UP))) return TC_TILE_N;
+  return a.Cout % 128 == 0 ? 128 : TC_TILE_CM;
 }
 
-int tc_tile_n(const ConvArgs& a) { return tc_wide_tiles(a, tc_geometry(a)) ? 128 : TC_TILE_N; }
+int tc_tile_n(const ConvArgs& a) { return tc_tile_kind(a, tc_geometry(a)); }
 
 // GroupNorm partial sums can be emitted for Cout in {64, 128, 256, 512} (2 .. 16 channels per group inside a 64-wide n-tile)
 bool tc_can_emit_stats(const ConvArgs& a) {
@@ -1625,8 +1680,8 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   const TcGeom geo = tc_geometry(a);
   const int BW = geo.BW, BH = geo.BH;
   const int PW = geo.halo ? BW + a.ksize - 1 : 0, PH = geo.halo ? BH + a.ksize - 1 : 0;
-  const bool wide = tc_wide_tiles(a, geo);
-  const int BN = wide ? 128 : TC_TILE_N;
+  const int tile = tc_tile_kind(a, geo);
+  const int BN = tile == 128 ? 128 : TC_TILE_N;
   TcMaps mp;
   CUtensorMap &mA_hi = mp.a_hi, &mA_lo = mp.a_lo, &mB_hi = mp.b_hi, &mB_lo = mp.b_lo;
   if (a.xform) {
@@ -1720,11 +1775,11 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   CFB_REQUIRE(!a.gn_part || tc_can_emit_stats(a), "conv_tc: GroupNorm partials are not available for this Cout");
   if (a.gen) return launch_tc<0>(mp, p, sm_count, st, true);
   switch (cpg) {
-    case 0: return launch_tc<0>(mp, p, sm_count, st, false, wide);
-    case 2: return launch_tc<2>(mp, p, sm_count, st, false, wide);
-    case 4: return launch_tc<4>(mp, p, sm_count, st, false, wide);
-    case 8: return launch_tc<8>(mp, p, sm_count, st, false, wide);
-    case 16: return launch_tc<16>(mp, p, sm_count, st, false, wide);
+    case 0: return launch_tc<0>(mp, p, sm_count, st, false, tile);
+    case 2: return launch_tc<2>(mp, p, sm_count, st, false, tile);
+    case 4: return launch_tc<4>(mp, p, sm_count, st, false, tile);
+    case 8: return launch_tc<8>(mp, p, sm_count, st, false, tile);
+    case 16: return launch_tc<16>(mp, p, sm_count, st, false, tile);
   }
   CFB_REQUIRE(false, "conv_tc: no kernel variant for this configuration");
   return 1;

@@ -21,7 +21,10 @@ size_t tc_scratch_bytes(const ConvArgs& a);   // operand (hi/lo fp16 activation 
 bool tc_can_emit_stats(const ConvArgs& a);    // GroupNorm(32) partial sums available from the epilogue for this shape
 int tc_tiles_per_image(const ConvArgs& a);    // 128-pixel tiles per image (GroupNorm partial slots = 4x this)
 int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st);
-int tc_tile_n(const ConvArgs& a);             // output channels per tile conv_tc() uses for this conv: 128 or 64
+// channel-major 128 x 64 tile (the MMAs compute the tile transposed, weights as the A operand): the tile kind tc_tile_n()
+// reports for it, distinct from the 64 of the pixel-major 128 x 64 tile
+constexpr int TC_TILE_CM = -64;
+int tc_tile_n(const ConvArgs& a);             // tile conv_tc() uses for this conv: 128, 64 or TC_TILE_CM (64 channels)
 // batched GEMM over 16x16-token images on fp16 hi/lo operand planes (attention cores); see conv_tc.cu
 struct BmmArgs {
   const void* a_planes = nullptr; int a_pitch = 0, a_c0 = 0;   // A: [N][256][a_pitch] hi | lo

@@ -187,8 +187,10 @@ int cfb_debug_time_conv(const float* in, const float* weight_oihw, float* out, i
  * (Upsample); xform 1 = fused operand transform (in_scale/in_shift optional: null = plain hi/lo split of the raw values), with
  * in2 != null channels [cin1, cin) read from in2 (torch.cat of Fuse_sft_block); residual, SFT (out = sft_dec + sft_w *
  * (sft_dec * sft_scale + conv)), out_planes (fp16 hi | lo planes of out, each align1024(n*Ho*Wo*cout*2) bytes) and gn_part
- * (GroupNorm(32) partial sums, 4 * 2 * 32 floats per 128-pixel tile) optional.  *tile_n receives the output channels per tile
- * of the launched kernel (128 or 64).  workspace >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, 3, mode). */
+ * (GroupNorm(32) partial sums, 4 * 2 * 32 floats per 128-pixel tile) optional.  *tile_n receives the tile of the launched
+ * kernel: 128 (128 pixels x 128 channels), 64 (128 pixels x 64 channels, pixel-major) or -64 (128 pixels x 64 channels,
+ * channel-major: computed transposed with the weights as the wgmma A operand).
+ * workspace >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, 3, mode). */
 int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias, float* out,
                       int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
                       const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,

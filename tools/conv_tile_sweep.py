@@ -1,7 +1,8 @@
-"""Per-shape time of the halo conv kernels of CodeFormer.forward on 128-wide (default) vs 64-wide (CFB_TC_BN=64) n-tiles.
+"""Per-shape time of the halo conv kernels of CodeFormer.forward on their default tiles vs 128 x 64 pixel-major tiles (CFB_TC_BN=64).
 
-Every distinct 3x3 stride-1 / Upsample conv shape of the forward with Cout % 128 == 0 (the convs the tile width applies to) is
-timed alone with CUDA events by cfb_debug_time_conv at batch 32.  CFB_TC_BN is read once per process, so the two settings run
+Every distinct 3x3 stride-1 / Upsample conv shape of the forward with Cout % 128 == 0 (128 x 128 tiles by default) and the
+Cout = 64 shapes at 512^2 (channel-major 128 x 64 tiles by default; the raw-plane row times the kernel without the fused
+transform) is timed alone with CUDA events by cfb_debug_time_conv at batch 32.  CFB_TC_BN is read once per process, so the two settings run
 in separate processes, alternating A/B/A/B (--rounds), and the median per setting is reported.  Nominal FLOPs are the conv's
 2*M*N*K (Upsample: of the 3x3 conv at the output resolution, as the forward's FLOP count has them); the fraction is of the
 H100 SXM data-sheet dense bf16/fp16 rate.  The card name and power limit are read in the same run.
@@ -25,6 +26,7 @@ SHAPES = [
     (32, 512, 256, 0, True), (128, 256, 128, 0, True), (256, 256, 128, 0, True),
     (16, 512, 512, 2, False), (32, 256, 256, 2, False), (64, 256, 256, 2, False), (128, 128, 128, 2, False),
     (256, 128, 128, 2, False),
+    (512, 64, 64, 0, True), (512, 128, 64, 0, True), (512, 64, 64, 0, False),
 ]
 
 CHILD = r'''
@@ -84,9 +86,9 @@ def main():
     ap.add_argument('--reps', type=int, default=10, help='launches per CUDA-event timing')
     args = ap.parse_args()
     card = gpu_info()
-    times = {64: [], 128: []}
+    times = {64: [], None: []}           # 64: CFB_TC_BN=64; None: default tiles
     for _ in range(args.rounds):
-        for bn in (64, 128):
+        for bn in (64, None):
             times[bn].append(run_side(bn, args.batch, args.reps))
     print(json.dumps({'gpu': card, 'batch': args.batch, 'rounds': args.rounds}))
     for i, (H, Cin, Cout, mode, xf) in enumerate(SHAPES):
@@ -94,13 +96,13 @@ def main():
         flops = 2.0 * args.batch * Ho * Ho * Cout * Cin * 9
         row = {'shape': f'{"up" if mode == 2 else "conv"} {Cin}->{Cout} @{Ho}^2{" gn+silu" if xf else " raw"}',
                'gflop': round(flops / 1e9, 1)}
-        for bn in (64, 128):
+        for bn, key in ((64, 'bn64'), (None, 'default')):
             ms = [t[i] for t in times[bn]]
             med = statistics.median(ms)
             tf = flops / (med * 1e-3) / 1e12
-            row[f'bn{bn}'] = {'ms': round(med, 4), 'ms_min': round(min(ms), 4), 'ms_max': round(max(ms), 4),
-                              'tflops': round(tf, 1), 'frac': round(tf / PEAK_TFLOPS, 4)}
-        row['speedup'] = round(row['bn64']['ms'] / row['bn128']['ms'], 3)
+            row[key] = {'ms': round(med, 4), 'ms_min': round(min(ms), 4), 'ms_max': round(max(ms), 4),
+                        'tflops': round(tf, 1), 'frac': round(tf / PEAK_TFLOPS, 4)}
+        row['speedup'] = round(row['bn64']['ms'] / row['default']['ms'], 3)
         print(json.dumps(row))
 
 
