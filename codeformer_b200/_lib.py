@@ -7,7 +7,7 @@ module raises, and every forward raises ``RuntimeError(cfb_last_error())`` on a 
 """
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libcfb200.so')
@@ -86,6 +86,10 @@ SIGNATURES = {
     'cfb_debug_set_stamps': (c_int, [_P]),
     'cfb_nchw_to_nhwc': (c_int, [_P, _P, c_int32, c_int32, c_int32, _P]),
     'cfb_nhwc_to_nchw': (c_int, [_P, _P, c_int32, c_int32, c_int32, _P]),
+    'cfb_warp_affine_u8': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
+    'cfb_resize_linear_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'cfb_paste_faces_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
+    'cfb_paste_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, c_double, _P, _P, _P, c_int64, _P]),
 }
 
 _lib = None

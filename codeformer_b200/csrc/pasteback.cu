@@ -1,0 +1,613 @@
+// Whole-image paste-back on the GPU: the face crop warp and FaceRestoreHelper.paste_faces_to_input_image
+// (/root/reference/facelib/utils/face_restoration_helper.py:319-349, 372-516) with cv2's arithmetic.
+//
+//   warpAffine    M is inverted in double; destination pixels map to the source in 1/32 fixed point (AB_BITS 10,
+//                 INTER_BITS 5).  u8: 15-bit integer weights (32-fy)(32-fx)*32 ..., (sum + 2^14) >> 15.  f32 / f64:
+//                 the same weights as exact dyadic floats, ((v0 w0 + v1 w1) + v2 w2) + v3 w3.  The parse mask's flags=3
+//                 is INTER_AREA, which warpAffine runs as INTER_LINEAR.
+//   resize        INTER_LINEAR, 11-bit weights (horizontal clamped, vertical not); an exact halving is the 2x2 mean.
+//   erode         rectangular k x k, anchor k/2, pixels outside the image never erode, k == 0 means 3x3.
+//   GaussianBlur  separable, BORDER_REFLECT_101, taps summed in order (the float kernel is cv2.getGaussianKernel).
+//
+// Every per-face step works on the face's ROI: the bounding box of the face square grown by 2 source pixels, mapped
+// to the canvas, grown by 2 pixels and clipped.  Outside it every warp of the face is exactly 0, so the soft mask is 0
+// and the blend m*a + (1-m)*b returns b unchanged: restricting to the ROI is exact.  Values outside the ROI but inside
+// the canvas are 0, so erosion ignores them (a 0 inside the window already gives the minimum) and the blur reads them as
+// 0; at the canvas border both follow cv2 (no erosion, reflect-101).
+//
+// The steps that do not depend on the blend order run for all faces at once (blockIdx.z = face).  The areas of the first
+// erosion are read back once per image (they fix the kernel sizes); then one composite launch per face, in face order.
+// Arithmetic that cv2 does unfused is written with _rn intrinsics so nvcc cannot contract it into FMAs.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <algorithm>
+#include <cmath>
+#include <string>
+#include <vector>
+
+#include "../../include/cfb200.h"
+#include "kernels.cuh"
+
+namespace cfb {
+namespace {
+
+constexpr int kParse = 512;           // the parsing network's resolution
+constexpr int kParseK = 101;          // GaussianBlur(parse_mask, (101, 101), 11), applied twice
+constexpr int kRoiPad = 2;
+
+struct PbFace {
+  double A[6];        // destination (canvas / crop) -> source (face) map: cv2's inverse of the given matrix
+  int x0, y0, rw, rh; // ROI on the canvas
+  int k2;             // second erosion kernel (0 -> 3x3)
+  int r;              // blur radius (w_edge)
+  int goff;           // offset of the blur kernel in the coefficient array
+  int pad_;
+  long long off;      // offset of the face's ROI planes (floats)
+};
+
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+void invert_affine(const double* M, double* A) {      // cv2.invertAffineTransform / warpAffine's own inversion
+  double D = M[0] * M[4] - M[1] * M[3];
+  D = D != 0. ? 1. / D : 0.;
+  const double A11 = M[4] * D, A22 = M[0] * D, A12 = -M[1] * D, A21 = -M[3] * D;
+  A[0] = A11; A[1] = A12; A[2] = -A11 * M[2] - A12 * M[5];
+  A[3] = A21; A[4] = A22; A[5] = -A21 * M[2] - A22 * M[5];
+}
+
+void face_roi(const double* inv, int S, int H, int W, int* roi) {
+  double xmn = 1e300, xmx = -1e300, ymn = 1e300, ymx = -1e300;
+  const double c[4][2] = {{-2., -2.}, {S + 2., -2.}, {-2., S + 2.}, {S + 2., S + 2.}};
+  for (int i = 0; i < 4; ++i) {
+    const double x = c[i][0] * inv[0] + c[i][1] * inv[1] + inv[2];
+    const double y = c[i][0] * inv[3] + c[i][1] * inv[4] + inv[5];
+    xmn = std::min(xmn, x); xmx = std::max(xmx, x); ymn = std::min(ymn, y); ymx = std::max(ymx, y);
+  }
+  auto clampd = [](double v, int lo, int hi) { return (int)std::max<double>(lo, std::min<double>(hi, v)); };
+  const int x0 = clampd(std::floor(xmn) - kRoiPad, 0, W), y0 = clampd(std::floor(ymn) - kRoiPad, 0, H);
+  const int x1 = clampd(std::ceil(xmx) + kRoiPad + 1, 0, W), y1 = clampd(std::ceil(ymx) + kRoiPad + 1, 0, H);
+  roi[0] = x0; roi[1] = y0; roi[2] = std::max(x1 - x0, 0); roi[3] = std::max(y1 - y0, 0);
+}
+
+// cv2.getGaussianKernel(n, sigma): fixed tables for n <= 9 and sigma <= 0, else the normalised exp
+void gaussian_kernel(int n, double sigma, std::vector<double>& k) {
+  static const double t3[] = {0.25, 0.5, 0.25}, t5[] = {0.0625, 0.25, 0.375, 0.25, 0.0625},
+      t7[] = {0.03125, 0.109375, 0.21875, 0.28125, 0.21875, 0.109375, 0.03125},
+      t9[] = {0.015625, 0.05078125, 0.1171875, 0.19921875, 0.234375, 0.19921875, 0.1171875, 0.05078125, 0.015625};
+  k.assign(n, 0.);
+  if (sigma <= 0 && n <= 9) {
+    const double* t = n == 1 ? nullptr : n == 3 ? t3 : n == 5 ? t5 : n == 7 ? t7 : t9;
+    for (int i = 0; i < n; ++i) k[i] = t ? t[i] : 1.;
+    return;
+  }
+  const double sig = sigma > 0 ? sigma : n * 0.15 + 0.35;
+  const double scale2 = -0.125 / (sig * sig);
+  const int n2 = (n - 1) / 2;
+  std::vector<double> v(n2);
+  double sum = 0.;
+  for (int i = 0, x = 1 - n; i < n2; ++i, x += 2) { v[i] = std::exp((double)(x * x) * scale2); sum += v[i]; }
+  sum = sum * 2 + 1.;
+  const double mul = 1. / sum;
+  for (int i = 0; i < n2; ++i) k[i] = k[n - 1 - i] = v[i] * mul;
+  k[n2] = mul;
+}
+
+// ---- device helpers ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void warp_coord(const double* A, int x, int y, int& ix, int& iy, int& fx, int& fy) {
+  const int ad = __double2int_rn(__dmul_rn(__dmul_rn(A[0], (double)x), 1024.));
+  const int bd = __double2int_rn(__dmul_rn(__dmul_rn(A[3], (double)x), 1024.));
+  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(A[1], (double)y), A[2]), 1024.)) + 16;
+  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(A[4], (double)y), A[5]), 1024.)) + 16;
+  const int X = (X0 + ad) >> 5, Y = (Y0 + bd) >> 5;
+  ix = X >> 5; iy = Y >> 5; fx = X & 31; fy = Y & 31;
+}
+
+__device__ __forceinline__ int border_idx(int p, int n, int mode) {
+  if (p >= 0 && p < n) return p;
+  if (mode == 0) return -1;
+  if (mode == 4) {                         // reflect-101
+    if (n == 1) return 0;
+    const int per = 2 * (n - 1);
+    int q = p % per; if (q < 0) q += per;
+    return q >= n ? per - q : q;
+  }
+  const int per = 2 * n;                   // reflect
+  int q = p % per; if (q < 0) q += per;
+  return q >= n ? per - 1 - q : q;
+}
+
+// bilinear u8 HWC 3-channel sample, cv2 fixed point; mode 0 = constant cval
+__device__ __forceinline__ void sample_u8(const uint8_t* src, int h, int w, int ix, int iy, int fx, int fy, int mode,
+                                          const int* cval, int* out) {
+  const int wt[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+  int acc[3] = {0, 0, 0};
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int yy = border_idx(iy + (t >> 1), h, mode), xx = border_idx(ix + (t & 1), w, mode);
+    if (yy >= 0 && xx >= 0) {
+      const uint8_t* p = src + ((size_t)yy * w + xx) * 3;
+      acc[0] += p[0] * wt[t]; acc[1] += p[1] * wt[t]; acc[2] += p[2] * wt[t];
+    } else {
+      acc[0] += cval[0] * wt[t]; acc[1] += cval[1] * wt[t]; acc[2] += cval[2] * wt[t];
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) out[c] = min(max((acc[c] + (1 << 14)) >> 15, 0), 255);
+}
+
+// ---- kernels ----------------------------------------------------------------------------------------------------
+__global__ void k_warp_crop(const uint8_t* __restrict__ src, int h, int w, const double* __restrict__ maps, int n,
+                            uint8_t* __restrict__ out, int oh, int ow, int mode, int c0, int c1, int c2) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh || f >= n) return;
+  int ix, iy, fx, fy, v[3];
+  const int cval[3] = {c0, c1, c2};
+  warp_coord(maps + 6 * f, x, y, ix, iy, fx, fy);
+  sample_u8(src, h, w, ix, iy, fx, fy, mode, cval, v);
+  uint8_t* o = out + (((size_t)f * oh + y) * ow + x) * 3;
+  o[0] = (uint8_t)v[0]; o[1] = (uint8_t)v[1]; o[2] = (uint8_t)v[2];
+}
+
+// INTER_LINEAR taps of one output coordinate (cv2 resize): source index and float fraction
+__device__ __forceinline__ void lin_tap(int d, double scale, int& s, float& f) {
+  f = __double2float_rn(__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5));
+  const float fl = floorf(f);
+  s = (int)fl;
+  f = __fsub_rn(f, fl);
+}
+
+__global__ void k_resize_u8(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst, int oh, int ow,
+                            double sx_scale, double sy_scale, int n) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh || f >= n) return;
+  src += (size_t)f * h * w * 3;
+  uint8_t* o = dst + (((size_t)f * oh + y) * ow + x) * 3;
+  if (w == 2 * ow && h == 2 * oh) {        // cv2 runs an exact halving as INTER_AREA
+    const uint8_t* p = src + ((size_t)(2 * y) * w + 2 * x) * 3;
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)((p[c] + p[c + 3] + p[(size_t)w * 3 + c] + p[(size_t)w * 3 + c + 3] + 2) >> 2);
+    return;
+  }
+  int sx, sy;
+  float fx, fy;
+  lin_tap(x, sx_scale, sx, fx);
+  if (sx < 0) { sx = 0; fx = 0.f; }
+  if (sx >= w - 1) { sx = w - 1; fx = 0.f; }
+  const int a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fx), 2048.f)), a1 = __float2int_rn(__fmul_rn(fx, 2048.f));
+  const int sx1 = min(sx + 1, w - 1);
+  lin_tap(y, sy_scale, sy, fy);
+  const int b0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fy), 2048.f)), b1 = __float2int_rn(__fmul_rn(fy, 2048.f));
+  const int y0 = min(max(sy, 0), h - 1), y1 = min(max(sy + 1, 0), h - 1);
+  const uint8_t* r0 = src + (size_t)y0 * w * 3;
+  const uint8_t* r1 = src + (size_t)y1 * w * 3;
+  for (int c = 0; c < 3; ++c) {
+    const int s0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1, s1 = r1[sx * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
+    const int v = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
+    o[c] = (uint8_t)min(max(v, 0), 255);
+  }
+}
+
+__global__ void k_resize_f64(const double* __restrict__ src, int h, int w, double* __restrict__ dst, int oh, int ow,
+                             double sx_scale, double sy_scale) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh) return;
+  src += (size_t)f * h * w;
+  int sx, sy;
+  float fx, fy;
+  lin_tap(x, sx_scale, sx, fx);
+  bool hi = false;
+  if (sx < 0) { sx = 0; fx = 0.f; }
+  if (sx >= w - 1) { sx = w - 1; fx = 0.f; hi = true; }
+  const double a0 = (double)__fsub_rn(1.f, fx), a1 = (double)fx;
+  lin_tap(y, sy_scale, sy, fy);
+  const double b0 = (double)__fsub_rn(1.f, fy), b1 = (double)fy;
+  const int yy[2] = {min(max(sy, 0), h - 1), min(max(sy + 1, 0), h - 1)};
+  double r[2];
+  for (int i = 0; i < 2; ++i) {
+    const double* row = src + (size_t)yy[i] * w;
+    r[i] = hi ? row[sx] : __dadd_rn(__dmul_rn(row[sx], a0), __dmul_rn(row[min(sx + 1, w - 1)], a1));
+  }
+  dst[((size_t)f * oh + y) * ow + x] = __dadd_rn(__dmul_rn(r[0], b0), __dmul_rn(r[1], b1));
+}
+
+// ones(S x S) warped to the ROI, f32 bilinear with constant 0: the in-bounds weights, exact multiples of 1/1024
+__global__ void k_mask_warp(const PbFace* __restrict__ faces, int S, float* __restrict__ ws) {
+  const PbFace& F = faces[blockIdx.z];
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= F.rw || y >= F.rh) return;
+  int ix, iy, fx, fy;
+  warp_coord(F.A, F.x0 + x, F.y0 + y, ix, iy, fx, fy);
+  const int wt[4] = {(32 - fy) * (32 - fx), (32 - fy) * fx, fy * (32 - fx), fy * fx};
+  int acc = 0;
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int yy = iy + (t >> 1), xx = ix + (t & 1);
+    if (yy >= 0 && yy < S && xx >= 0 && xx < S) acc += wt[t];
+  }
+  ws[F.off + (size_t)y * F.rw + x] = (float)acc * (1.f / 1024.f);
+}
+
+// one pass of a rectangular erosion on the ROI planes: plane `in` -> plane `out` (0/1/2 within the face's planes)
+__global__ void k_erode(const PbFace* __restrict__ faces, float* __restrict__ ws, int in, int out, int k1, bool cols) {
+  const PbFace& F = faces[blockIdx.z];
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= F.rw || y >= F.rh) return;
+  int k = k1 >= 0 ? k1 : F.k2;
+  if (k == 0) k = 3;
+  const int a = k / 2;
+  const size_t plane = (size_t)F.rw * F.rh;
+  const float* src = ws + F.off + in * plane;
+  float m = INFINITY;
+  if (!cols) {
+    const int lo = max(x - a, 0), hi = min(x - a + k, F.rw);
+    for (int j = lo; j < hi; ++j) m = fminf(m, src[(size_t)y * F.rw + j]);
+  } else {
+    const int lo = max(y - a, 0), hi = min(y - a + k, F.rh);
+    for (int i = lo; i < hi; ++i) m = fminf(m, src[(size_t)i * F.rw + x]);
+  }
+  ws[F.off + out * plane + (size_t)y * F.rw + x] = m;
+}
+
+// sum of each face's first erosion in fp64: one block per face, fixed-order strided partials and tree
+__global__ void k_area(const PbFace* __restrict__ faces, const float* __restrict__ ws, int plane_idx, double* __restrict__ area) {
+  const PbFace& F = faces[blockIdx.x];
+  const size_t plane = (size_t)F.rw * F.rh;
+  const float* p = ws + F.off + plane_idx * plane;
+  double s = 0.;
+  for (size_t i = threadIdx.x; i < plane; i += blockDim.x) s += (double)p[i];
+  __shared__ double red[1024];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) area[blockIdx.x] = red[0];
+}
+
+// f32 Gaussian pass on the ROI planes: reflect-101 at the canvas border, 0 outside the ROI inside the canvas
+__global__ void k_blur_roi(const PbFace* __restrict__ faces, float* __restrict__ ws, const float* __restrict__ gk, int in,
+                           int out, bool cols, int H, int W) {
+  const PbFace& F = faces[blockIdx.z];
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= F.rw || y >= F.rh) return;
+  const size_t plane = (size_t)F.rw * F.rh;
+  const float* src = ws + F.off + in * plane;
+  const float* k = gk + F.goff;
+  const int r = F.r;
+  float acc = 0.f;
+  for (int t = 0; t <= 2 * r; ++t) {
+    float v = 0.f;
+    if (!cols) {
+      const int gx = border_idx(F.x0 + x + t - r, W, 4) - F.x0;
+      if (gx >= 0 && gx < F.rw) v = src[(size_t)y * F.rw + gx];
+    } else {
+      const int gy = border_idx(F.y0 + y + t - r, H, 4) - F.y0;
+      if (gy >= 0 && gy < F.rh) v = src[(size_t)gy * F.rw + x];
+    }
+    acc = t == 0 ? __fmul_rn(v, k[0]) : __fadd_rn(acc, __fmul_rn(v, k[t]));
+  }
+  ws[F.off + out * plane + (size_t)y * F.rw + x] = acc;
+}
+
+__global__ void k_u8_to_f64(const uint8_t* __restrict__ src, double* __restrict__ dst, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (double)src[i];
+}
+
+// f64 Gaussian pass over whole 512 x 512 parse masks (blockIdx.z = face), reflect-101
+__global__ void k_blur_f64(const double* __restrict__ src, double* __restrict__ dst, const double* __restrict__ k, int ks, bool cols) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= kParse || y >= kParse) return;
+  const size_t base = (size_t)blockIdx.z * kParse * kParse;
+  src += base;
+  const int r = ks / 2;
+  double acc = 0.;
+  for (int t = 0; t < ks; ++t) {
+    const double v = cols ? src[(size_t)border_idx(y + t - r, kParse, 4) * kParse + x]
+                          : src[(size_t)y * kParse + border_idx(x + t - r, kParse, 4)];
+    acc = t == 0 ? __dmul_rn(v, k[0]) : __dadd_rn(acc, __dmul_rn(v, k[t]));
+  }
+  dst[base + (size_t)y * kParse + x] = acc;
+}
+
+// parse_mask[:10] = ... = 0; parse_mask / 255.
+__global__ void k_parse_finish(double* __restrict__ p, int nfaces) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)nfaces * kParse * kParse) return;
+  const int x = (int)(i % kParse), y = (int)((i / kParse) % kParse);
+  const bool edge = x < 10 || y < 10 || x >= kParse - 10 || y >= kParse - 10;
+  p[i] = __ddiv_rn(edge ? 0. : p[i], 255.);
+}
+
+template <typename T>
+__global__ void k_canvas_in(const uint8_t* __restrict__ src, T* __restrict__ dst, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (T)src[i];
+}
+
+// astype(np.uint8) as numpy does it on x86: truncate toward zero, keep the low byte
+template <typename T>
+__global__ void k_canvas_out(const T* __restrict__ src, uint8_t* __restrict__ dst, float* __restrict__ dbg, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const T v = src[i];
+  dst[i] = (uint8_t)((long long)v & 255);
+  if (dbg) dbg[i] = (float)v;
+}
+
+// one face into the canvas: inv_restored (u8 warp), the parse warp (f64 bilinear), min(parse, soft), the blend
+template <typename T>
+__global__ void k_composite(const PbFace* __restrict__ faces, int fi, const uint8_t* __restrict__ face, int S,
+                            const double* __restrict__ parse, const float* __restrict__ ws, T* __restrict__ canvas, int W) {
+  const PbFace& F = faces[fi];
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= F.rw || y >= F.rh) return;
+  int ix, iy, fx, fy, v[3];
+  warp_coord(F.A, F.x0 + x, F.y0 + y, ix, iy, fx, fy);
+  const int zero[3] = {0, 0, 0};
+  sample_u8(face, S, S, ix, iy, fx, fy, 0, zero, v);
+  const size_t plane = (size_t)F.rw * F.rh, p = (size_t)y * F.rw + x;
+  const float ero = ws[F.off + 2 * plane + p], soft = ws[F.off + 1 * plane + p];
+  T* c = canvas + ((size_t)(F.y0 + y) * W + F.x0 + x) * 3;
+  if constexpr (sizeof(T) == 8) {
+    double m = (double)soft;
+    if (parse) {
+      const float a = fx * (1.f / 32.f), b = fy * (1.f / 32.f);
+      const float wt[4] = {__fmul_rn(1.f - b, 1.f - a), __fmul_rn(1.f - b, a), __fmul_rn(b, 1.f - a), __fmul_rn(b, a)};
+      double acc = 0.;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const int yy = iy + (t >> 1), xx = ix + (t & 1);
+        const double s = (yy >= 0 && yy < S && xx >= 0 && xx < S) ? parse[(size_t)yy * S + xx] : 0.;
+        acc = t == 0 ? __dmul_rn(s, (double)wt[0]) : __dadd_rn(acc, __dmul_rn(s, (double)wt[t]));
+      }
+      if (acc < m) m = acc;
+    }
+    const double om = __dsub_rn(1., m);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const double pasted = (double)__fmul_rn(ero, (float)v[ch]);
+      c[ch] = __dadd_rn(__dmul_rn(m, pasted), __dmul_rn(om, (double)c[ch]));
+    }
+  } else {
+    const float om = __fsub_rn(1.f, soft);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const float pasted = __fmul_rn(ero, (float)v[ch]);
+      c[ch] = __fadd_rn(__fmul_rn(soft, pasted), __fmul_rn(om, (float)c[ch]));
+    }
+  }
+}
+
+inline dim3 grid2(int w, int h, int z, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y, z); }
+
+struct Plan {
+  std::vector<PbFace> faces;
+  size_t roi_floats = 0;
+  int max_rw = 0, max_rh = 0;
+};
+
+int make_plan(int H, int W, int n, int S, const double* inv, Plan& P) {
+  P.faces.assign(n, PbFace{});
+  size_t off = 0;
+  for (int i = 0; i < n; ++i) {
+    PbFace& F = P.faces[i];
+    invert_affine(inv + 6 * i, F.A);
+    int roi[4];
+    face_roi(inv + 6 * i, S, H, W, roi);
+    F.x0 = roi[0]; F.y0 = roi[1]; F.rw = roi[2]; F.rh = roi[3];
+    F.off = (long long)off;
+    off += align256((size_t)F.rw * F.rh * 3 * 4) / 4;
+    P.max_rw = std::max(P.max_rw, F.rw);
+    P.max_rh = std::max(P.max_rh, F.rh);
+  }
+  P.roi_floats = off;
+  return 0;
+}
+
+struct Layout {
+  size_t canvas, roi, parse0, parse1, parse_rs, faces, area, pgauss, gauss, total;
+};
+
+Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gauss_floats) {
+  Layout L{};
+  size_t o = 0;
+  auto take = [&](size_t b) { const size_t r = o; o += align256(b); return r; };
+  L.canvas = take((size_t)H * W * 3 * (use_parse ? 8 : 4));
+  L.roi = take(P.roi_floats * 4);
+  const size_t pm = (size_t)n * kParse * kParse * 8;
+  L.parse0 = take(use_parse ? pm : 0);
+  L.parse1 = take(use_parse ? pm : 0);
+  L.parse_rs = take(use_parse && S != kParse ? (size_t)n * S * S * 8 : 0);
+  L.faces = take((size_t)std::max(n, 1) * sizeof(PbFace));
+  L.area = take((size_t)std::max(n, 1) * 8);
+  L.pgauss = take(kParseK * 8);
+  L.gauss = take((size_t)gauss_floats * 4);
+  L.total = o;
+  return L;
+}
+
+// the largest w_edge a face can get: the first erosion is <= 1 on its ROI
+int max_gauss_floats(const Plan& P) {
+  int s = 0;
+  for (const PbFace& F : P.faces) s += 2 * ((int)std::sqrt((double)F.rw * F.rh) / 20) + 1;
+  return s;
+}
+
+template <typename T>
+int paste_impl(uint8_t* canvas_u8, int H, int W, const uint8_t* faces, int n, int S, const uint8_t* parse_u8,
+               const double* inv, double upscale, float* dbg, int32_t* w_edge_out, char* ws, int64_t ws_bytes,
+               cudaStream_t st) {
+  const bool use_parse = parse_u8 != nullptr;
+  Plan P;
+  CFB_CHECK(make_plan(H, W, n, S, inv, P));
+  const Layout L = layout(H, W, n, S, use_parse, P, max_gauss_floats(P));
+  CFB_REQUIRE((int64_t)L.total <= ws_bytes, "cfb_paste_faces: workspace too small");
+  T* canvas = (T*)(ws + L.canvas);
+  float* roi = (float*)(ws + L.roi);
+  PbFace* dfaces = (PbFace*)(ws + L.faces);
+  double* darea = (double*)(ws + L.area);
+  float* dgauss = (float*)(ws + L.gauss);
+  double* dpk = (double*)(ws + L.pgauss);
+  const size_t npx = (size_t)H * W * 3;
+  k_canvas_in<T><<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(canvas_u8, canvas, npx);
+  CFB_LAUNCH_CHECK();
+  const dim3 b(32, 8);
+  std::vector<double> gk;
+  const double* parse_src = nullptr;
+  if (n > 0) {
+    const int k1 = (int)(2 * upscale);
+    CFB_CUDA(cudaMemcpyAsync(dfaces, P.faces.data(), n * sizeof(PbFace), cudaMemcpyHostToDevice, st));
+    const dim3 g = grid2(P.max_rw, P.max_rh, n, b);
+    k_mask_warp<<<g, b, 0, st>>>(dfaces, S, roi);
+    CFB_LAUNCH_CHECK();
+    k_erode<<<g, b, 0, st>>>(dfaces, roi, 0, 1, k1, false);
+    CFB_LAUNCH_CHECK();
+    k_erode<<<g, b, 0, st>>>(dfaces, roi, 1, 2, k1, true);          // plane 2: inv_mask_erosion
+    CFB_LAUNCH_CHECK();
+    k_area<<<n, 1024, 0, st>>>(dfaces, roi, 2, darea);
+    CFB_LAUNCH_CHECK();
+    if (use_parse) {                        // independent of the areas: enqueue before the read-back
+      double* p0 = (double*)(ws + L.parse0);
+      double* p1 = (double*)(ws + L.parse1);
+      gaussian_kernel(kParseK, 11., gk);
+      CFB_CUDA(cudaMemcpyAsync(dpk, gk.data(), kParseK * 8, cudaMemcpyHostToDevice, st));
+      const size_t pn = (size_t)n * kParse * kParse;
+      k_u8_to_f64<<<(unsigned)((pn + 255) / 256), 256, 0, st>>>(parse_u8, p0, pn);
+      CFB_LAUNCH_CHECK();
+      const dim3 gp = grid2(kParse, kParse, n, b);
+      for (int rep = 0; rep < 2; ++rep) {
+        k_blur_f64<<<gp, b, 0, st>>>(p0, p1, dpk, kParseK, false);
+        CFB_LAUNCH_CHECK();
+        k_blur_f64<<<gp, b, 0, st>>>(p1, p0, dpk, kParseK, true);
+        CFB_LAUNCH_CHECK();
+      }
+      k_parse_finish<<<(unsigned)((pn + 255) / 256), 256, 0, st>>>(p0, n);
+      CFB_LAUNCH_CHECK();
+      parse_src = p0;
+      if (S != kParse) {
+        double* rs = (double*)(ws + L.parse_rs);
+        const double sc = 1. / ((double)S / kParse);
+        k_resize_f64<<<grid2(S, S, n, b), b, 0, st>>>(p0, kParse, kParse, rs, S, S, sc, sc);
+        CFB_LAUNCH_CHECK();
+        parse_src = rs;
+      }
+    }
+    std::vector<double> area(n);
+    CFB_CUDA(cudaMemcpyAsync(area.data(), darea, n * 8, cudaMemcpyDeviceToHost, st));
+    CFB_CUDA(cudaStreamSynchronize(st));
+    std::vector<float> gauss;
+    for (int i = 0; i < n; ++i) {
+      const int w_edge = (int)std::sqrt(area[i]) / 20;
+      PbFace& F = P.faces[i];
+      F.k2 = 2 * w_edge;
+      F.r = w_edge;
+      F.goff = (int)gauss.size();
+      gaussian_kernel(2 * w_edge + 1, 0., gk);
+      for (double v : gk) gauss.push_back((float)v);
+      if (w_edge_out) w_edge_out[i] = w_edge;
+    }
+    CFB_REQUIRE(gauss.size() <= (size_t)max_gauss_floats(P), "cfb_paste_faces: blur kernel larger than its ROI bound");
+    CFB_CUDA(cudaMemcpyAsync(dgauss, gauss.data(), gauss.size() * 4, cudaMemcpyHostToDevice, st));
+    CFB_CUDA(cudaMemcpyAsync(dfaces, P.faces.data(), n * sizeof(PbFace), cudaMemcpyHostToDevice, st));
+    k_erode<<<g, b, 0, st>>>(dfaces, roi, 2, 0, -1, false);
+    CFB_LAUNCH_CHECK();
+    k_erode<<<g, b, 0, st>>>(dfaces, roi, 0, 1, -1, true);           // plane 1: inv_mask_center
+    CFB_LAUNCH_CHECK();
+    k_blur_roi<<<g, b, 0, st>>>(dfaces, roi, dgauss, 1, 0, false, H, W);
+    CFB_LAUNCH_CHECK();
+    k_blur_roi<<<g, b, 0, st>>>(dfaces, roi, dgauss, 0, 1, true, H, W);   // plane 1: inv_soft_mask
+    CFB_LAUNCH_CHECK();
+    for (int i = 0; i < n; ++i) {
+      const PbFace& F = P.faces[i];
+      if (F.rw == 0 || F.rh == 0) continue;
+      k_composite<T><<<grid2(F.rw, F.rh, 1, b), b, 0, st>>>(dfaces, i, faces + (size_t)i * S * S * 3, S,
+                                                             parse_src ? parse_src + (size_t)i * S * S : nullptr, roi, canvas, W);
+      CFB_LAUNCH_CHECK();
+    }
+  }
+  k_canvas_out<T><<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(canvas, canvas_u8, dbg, npx);
+  CFB_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+}  // namespace cfb
+
+#define API_BEGIN try {
+#define API_END(ret)                                                                                        \
+  } catch (const std::exception& e) { cfb::set_error(std::string("exception: ") + e.what()); return ret; } \
+  catch (...) { cfb::set_error("unknown exception"); return ret; }
+
+extern "C" {
+
+int cfb_warp_affine_u8(const uint8_t* img, int32_t h, int32_t w, const double* affines, int32_t n, uint8_t* out,
+                       int32_t out_h, int32_t out_w, int32_t border_mode, int32_t v0, int32_t v1, int32_t v2, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_warp_affine_u8: bad size");
+  CFB_REQUIRE(n == 0 || (img && affines && out), "cfb_warp_affine_u8: NULL argument");
+  CFB_REQUIRE(border_mode == 0 || border_mode == 2 || border_mode == 4, "cfb_warp_affine_u8: border mode must be 0 (constant), 2 (reflect) or 4 (reflect-101)");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<double> maps(6 * (size_t)n);
+  for (int i = 0; i < n; ++i) cfb::invert_affine(affines + 6 * i, maps.data() + 6 * i);
+  double* dmaps = nullptr;
+  CFB_CUDA(cudaMallocAsync((void**)&dmaps, maps.size() * 8, st));
+  CFB_CUDA(cudaMemcpyAsync(dmaps, maps.data(), maps.size() * 8, cudaMemcpyHostToDevice, st));
+  const dim3 b(32, 8);
+  cfb::k_warp_crop<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(img, h, w, dmaps, n, out, out_h, out_w, border_mode, v0, v1, v2);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(dmaps, st));
+  return 0;
+  API_END(1)
+}
+
+int cfb_resize_linear_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_resize_linear_u8: bad size");
+  CFB_REQUIRE(n == 0 || (src && dst), "cfb_resize_linear_u8: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h == out_h && w == out_w) {                  // cv2.resize to the same size is a copy
+    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  const dim3 b(32, 8);
+  cfb::k_resize_u8<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(src, h, w, dst, out_h, out_w, 1. / ((double)out_w / w),
+                                                                  1. / ((double)out_h / h), n);
+  CFB_LAUNCH_CHECK();
+  return 0;
+  API_END(1)
+}
+
+int64_t cfb_paste_faces_workspace_bytes(int32_t h_up, int32_t w_up, int32_t n, int32_t face_size, int32_t use_parse,
+                                        const double* inverse_affines) {
+  if (h_up <= 0 || w_up <= 0 || n < 0 || face_size <= 0 || (n > 0 && !inverse_affines)) {
+    cfb::set_error("cfb_paste_faces_workspace_bytes: bad argument");
+    return -1;
+  }
+  cfb::Plan P;
+  cfb::make_plan(h_up, w_up, n, face_size, inverse_affines, P);
+  const cfb::Layout L = cfb::layout(h_up, w_up, n, face_size, use_parse != 0, P, cfb::max_gauss_floats(P));
+  return (int64_t)L.total;
+}
+
+int cfb_paste_faces(uint8_t* canvas, int32_t h_up, int32_t w_up, const uint8_t* faces, int32_t n, int32_t face_size,
+                    const uint8_t* parse_masks, const double* inverse_affines, double upscale, float* debug_canvas,
+                    int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(h_up > 0 && w_up > 0 && n >= 0 && face_size > 0 && upscale > 0, "cfb_paste_faces: bad size");
+  CFB_REQUIRE(canvas && workspace && (n == 0 || (faces && inverse_affines)), "cfb_paste_faces: NULL argument");
+  const int64_t need = cfb_paste_faces_workspace_bytes(h_up, w_up, n, face_size, parse_masks != nullptr, inverse_affines);
+  CFB_REQUIRE(need > 0 && workspace_bytes >= need, "cfb_paste_faces: workspace too small (cfb_paste_faces_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (parse_masks)
+    return cfb::paste_impl<double>(canvas, h_up, w_up, faces, n, face_size, parse_masks, inverse_affines, upscale,
+                                   debug_canvas, w_edge_out, (char*)workspace, workspace_bytes, st);
+  return cfb::paste_impl<float>(canvas, h_up, w_up, faces, n, face_size, nullptr, inverse_affines, upscale, debug_canvas,
+                                w_edge_out, (char*)workspace, workspace_bytes, st);
+  API_END(1)
+}
+
+}  // extern "C"

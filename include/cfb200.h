@@ -264,6 +264,28 @@ int cfb_debug_set_stamps(int64_t* stamps);
 int cfb_nchw_to_nhwc(const float* in, float* out, int32_t n, int32_t c, int32_t hw, void* stream);
 int cfb_nhwc_to_nchw(const float* in, float* out, int32_t n, int32_t c, int32_t hw, void* stream);
 
+/* ---- whole-image paste-back (face_restoration_helper.py:319-349, 372-516; pasteback.cu) ----
+ * cv2 arithmetic throughout (fixed-point warpAffine coordinates, 11-bit INTER_LINEAR resize, rect erosion, reflect-101
+ * Gaussian blur).  All images are uint8 HWC, 3 channels, device memory; matrices are host double[6] (row-major 2x3).
+ * cfb_warp_affine_u8: n crops [n,out_h,out_w,3] of one image with cv2.warpAffine(img, affines[i], (out_w, out_h), INTER_LINEAR,
+ *   border_mode, (v0, v1, v2)); border_mode 0 = constant, 2 = reflect, 4 = reflect-101 (cv2's numbering).
+ * cfb_resize_linear_u8: cv2.resize(src[i], (out_w, out_h), INTER_LINEAR) for n images [n,h,w,3].
+ * cfb_paste_faces: pastes n restored faces [n,S,S,3] into `canvas` [h_up,w_up,3] (the resized background; overwritten with the
+ *   result) in face order.  inverse_affines are the matrices paste_faces_to_input_image passes to warpAffine (after its offset
+ *   adjustments); upscale sets the first erosion (int(2*upscale)).  parse_masks [n,512,512] (0/255, MASK_COLORMAP of the
+ *   parsing network's argmax) selects use_parse (float64 blend); NULL blends in float32.  debug_canvas (optional, device
+ *   [h_up,w_up,3] f32) receives the canvas before the uint8 cast; w_edge_out (optional, host int32[n]) the fusion edge per
+ *   face.  The areas that fix the kernel sizes are read back once, so the call synchronises `stream`. */
+int cfb_warp_affine_u8(const uint8_t* img, int32_t h, int32_t w, const double* affines, int32_t n, uint8_t* out,
+                       int32_t out_h, int32_t out_w, int32_t border_mode, int32_t v0, int32_t v1, int32_t v2, void* stream);
+int cfb_resize_linear_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
+                         void* stream);
+int64_t cfb_paste_faces_workspace_bytes(int32_t h_up, int32_t w_up, int32_t n, int32_t face_size, int32_t use_parse,
+                                        const double* inverse_affines);
+int cfb_paste_faces(uint8_t* canvas, int32_t h_up, int32_t w_up, const uint8_t* faces, int32_t n, int32_t face_size,
+                    const uint8_t* parse_masks, const double* inverse_affines, double upscale, float* debug_canvas,
+                    int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
