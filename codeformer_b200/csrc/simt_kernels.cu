@@ -359,7 +359,16 @@ int conv_first_u8(const unsigned char* x_bgr_hwc, const float* wgt, const float*
   return 0;
 }
 
-// 4 horizontally adjacent output pixels per thread: every weight read from shared memory feeds 4 pixels.
+// One output pixel per thread, tiles of 4 x 64 pixels.  The GroupNorm-affine input patch of a tile, 6 x 66 pixels x all Cin
+// channels, is read once with coalesced loads (a pixel's Cin floats are contiguous) and normalised into shared memory; the
+// 9-tap loop then reads it there.  Reading each thread's taps straight from global memory instead (4 pixels 1 KB apart per
+// lane and 16 B at a time) fetched every input byte several times over and left the conv far from its DRAM bound.
+// The per-pixel sums run in the same order as the plain definition: rows, then channels, then columns, bias first.
+constexpr int CL_TH = 4, CL_TW = 64;                 // output tile
+constexpr int CL_PH = CL_TH + 2, CL_PW = CL_TW + 2;  // input patch
+constexpr int CL_MAX_CIN = 128;                      // shared memory: 9*Cin*16 + 6*66*Cin*4 bytes <= 227 KB
+static size_t conv_last_smem(int Cin) { return (size_t)(9 * Cin * 4 + CL_PH * CL_PW * Cin) * sizeof(float); }
+
 template <bool U8>
 __global__ void __launch_bounds__(256) conv_last_kernel(const float* __restrict__ in, const float* __restrict__ in_scale,
                                                         const float* __restrict__ in_shift, const float* __restrict__ wgt,
@@ -367,100 +376,101 @@ __global__ void __launch_bounds__(256) conv_last_kernel(const float* __restrict_
                                                         int H, int W, int Cin) {
   extern __shared__ __align__(16) float sm[];
   float* ws = sm;                 // [9][Cin][3] padded -> [9][Cin][4]
-  float* sc = ws + 9 * Cin * 4;   // [Cin]
-  float* sh = sc + Cin;
-  const int64_t HW = (int64_t)H * W;
-  const int64_t pix0 = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
-  const int n = (int)(((int64_t)blockIdx.x * 1024) / HW);  // HW % 1024 == 0: whole CTA in one image
+  // [CL_PH][CL_PW][Cin/4] float4: normalised patch, zero outside the image.  Channel quad q of patch column pc is stored at
+  // q ^ (pc & 7): the 8 lanes of one LDS.128 phase read 8 adjacent columns at the same q and hit 8 distinct bank quads.
+  float* xs = ws + 9 * Cin * 4;
+  const int Q = Cin / 4;
+  const int tiles_x = (W + CL_TW - 1) / CL_TW, tiles_y = (H + CL_TH - 1) / CL_TH;
+  const int n = (int)(blockIdx.x / (unsigned)(tiles_x * tiles_y));
+  const int trem = (int)blockIdx.x - n * tiles_x * tiles_y;
+  const int y0 = (trem / tiles_x) * CL_TH, x0 = (trem % tiles_x) * CL_TW;
   pdl_launch_dependents();
   pdl_wait();
   for (int i = threadIdx.x; i < 9 * Cin; i += 256) {
     ws[i * 4 + 0] = wgt[i * 3 + 0]; ws[i * 4 + 1] = wgt[i * 3 + 1]; ws[i * 4 + 2] = wgt[i * 3 + 2]; ws[i * 4 + 3] = 0.f;
   }
-  for (int i = threadIdx.x; i < Cin; i += 256) {
-    sc[i] = in_scale ? in_scale[(int64_t)n * Cin + i] : 1.f;
-    sh[i] = in_shift ? in_shift[(int64_t)n * Cin + i] : 0.f;
+  for (int i = threadIdx.x; i < CL_PH * CL_PW * Q; i += 256) {
+    const int q = i % Q, pix = i / Q;
+    const int pr = pix / CL_PW, pc = pix - pr * CL_PW;
+    const int iy = y0 - 1 + pr, ix = x0 - 1 + pc;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);       // zero padding of the *normalised* tensor
+    if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(in + (((int64_t)n * H + iy) * W + ix) * Cin) + q);
+      const float4 s4 = in_scale ? __ldg(reinterpret_cast<const float4*>(in_scale + (int64_t)n * Cin) + q) : make_float4(1.f, 1.f, 1.f, 1.f);
+      const float4 h4 = in_shift ? __ldg(reinterpret_cast<const float4*>(in_shift + (int64_t)n * Cin) + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+      v = make_float4(fmaf(t.x, s4.x, h4.x), fmaf(t.y, s4.y, h4.y), fmaf(t.z, s4.z, h4.z), fmaf(t.w, s4.w, h4.w));
+    }
+    reinterpret_cast<float4*>(xs)[pix * Q + (q ^ (pc & 7))] = v;
   }
   __syncthreads();
-  const int rem = (int)(pix0 - (int64_t)n * HW);
-  const int y = rem / W, x0 = rem - y * W;     // W % 4 == 0: the 4 pixels share a row
-  float acc[4][3];
-#pragma unroll
-  for (int p = 0; p < 4; ++p) { acc[p][0] = bias ? bias[0] : 0.f; acc[p][1] = bias ? bias[1] : 0.f; acc[p][2] = bias ? bias[2] : 0.f; }
+  const int tr = threadIdx.x / CL_TW, tc = threadIdx.x % CL_TW;
+  const int y = y0 + tr, x = x0 + tc;
+  float acc[3];
+  acc[0] = bias ? bias[0] : 0.f; acc[1] = bias ? bias[1] : 0.f; acc[2] = bias ? bias[2] : 0.f;
   for (int r = 0; r < 3; ++r) {
     const int iy = y + r - 1;
     if (iy < 0 || iy >= H) continue;
-    const float* rowp = in + ((int64_t)n * H + iy) * W * Cin;
+    const float4* prow = reinterpret_cast<const float4*>(xs) + (tr + r) * CL_PW * Q;
     for (int c = 0; c < Cin; c += 4) {
-      const float4 s4 = *reinterpret_cast<const float4*>(sc + c);
-      const float4 h4 = *reinterpret_cast<const float4*>(sh + c);
-      float v[6][4];
+      float4 v[3];
 #pragma unroll
-      for (int q = 0; q < 6; ++q) {
-        const int ix = x0 + q - 1;
-        if (ix >= 0 && ix < W) {
-          const float4 t = __ldg(reinterpret_cast<const float4*>(rowp + (int64_t)ix * Cin + c));
-          v[q][0] = fmaf(t.x, s4.x, h4.x); v[q][1] = fmaf(t.y, s4.y, h4.y);
-          v[q][2] = fmaf(t.z, s4.z, h4.z); v[q][3] = fmaf(t.w, s4.w, h4.w);
-        } else {
-          v[q][0] = v[q][1] = v[q][2] = v[q][3] = 0.f;      // zero padding of the *normalised* tensor
-        }
-      }
+      for (int s = 0; s < 3; ++s) v[s] = prow[(tc + s) * Q + ((c >> 2) ^ ((tc + s) & 7))];
 #pragma unroll
       for (int s = 0; s < 3; ++s) {
         const float* wt = ws + ((r * 3 + s) * Cin + c) * 4;
+        const float vj[4] = {v[s].x, v[s].y, v[s].z, v[s].w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float4 w4 = *reinterpret_cast<const float4*>(wt + j * 4);
-#pragma unroll
-          for (int p = 0; p < 4; ++p) {
-            acc[p][0] = fmaf(v[p + s][j], w4.x, acc[p][0]);
-            acc[p][1] = fmaf(v[p + s][j], w4.y, acc[p][1]);
-            acc[p][2] = fmaf(v[p + s][j], w4.z, acc[p][2]);
-          }
+          acc[0] = fmaf(vj[j], w4.x, acc[0]);
+          acc[1] = fmaf(vj[j], w4.y, acc[1]);
+          acc[2] = fmaf(vj[j], w4.z, acc[2]);
         }
       }
     }
   }
+  if (y >= H || x >= W) return;
+  const int64_t HW = (int64_t)H * W, pix = (int64_t)y * W + x;
   if constexpr (U8) {
-    // uint8 HWC BGR: 4 pixels = 12 contiguous bytes
-    unsigned b[12];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      b[p * 3 + 0] = model_output_to_u8(acc[p][2]); b[p * 3 + 1] = model_output_to_u8(acc[p][1]); b[p * 3 + 2] = model_output_to_u8(acc[p][0]);
-    }
-    unsigned* o8 = reinterpret_cast<unsigned*>(reinterpret_cast<unsigned char*>(out) + ((int64_t)n * HW + rem) * 3);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) o8[k] = b[k * 4] | (b[k * 4 + 1] << 8) | (b[k * 4 + 2] << 16) | (b[k * 4 + 3] << 24);
+    // uint8 HWC BGR
+    unsigned char* o8 = reinterpret_cast<unsigned char*>(out) + ((int64_t)n * HW + pix) * 3;
+    o8[0] = (unsigned char)model_output_to_u8(acc[2]); o8[1] = (unsigned char)model_output_to_u8(acc[1]);
+    o8[2] = (unsigned char)model_output_to_u8(acc[0]);
   } else {
-    float* o = out + (int64_t)n * 3 * HW + rem;
+    float* o = out + (int64_t)n * 3 * HW + pix;
 #pragma unroll
-    for (int k = 0; k < 3; ++k)
-      *reinterpret_cast<float4*>(o + k * HW) = make_float4(acc[0][k], acc[1][k], acc[2][k], acc[3][k]);
+    for (int k = 0; k < 3; ++k) o[k * HW] = acc[k];
   }
+}
+
+template <bool U8>
+static int launch_conv_last(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
+                            float* out, int N, int H, int W, int Cin, cudaStream_t st) {
+  CFB_REQUIRE(Cin % 32 == 0 && Cin <= CL_MAX_CIN, "conv_last: Cin must be a multiple of 32 and at most 128");
+  if (N == 0 || H == 0 || W == 0) return 0;
+  // the patch needs more than the default 48 KB of dynamic shared memory: a per-device property of the function
+  static std::atomic<uint64_t> attr_done{0};
+  int dev = 0;
+  CFB_CUDA(cudaGetDevice(&dev));
+  const uint64_t bit = 1ull << (dev & 63);
+  if (!(attr_done.load(std::memory_order_acquire) & bit)) {
+    CFB_CUDA(cudaFuncSetAttribute(conv_last_kernel<U8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_last_smem(CL_MAX_CIN)));
+    attr_done.fetch_or(bit, std::memory_order_release);
+  }
+  const int64_t tiles = (int64_t)N * ((H + CL_TH - 1) / CL_TH) * ((W + CL_TW - 1) / CL_TW);
+  CFB_REQUIRE(tiles <= 0x7fffffffLL, "conv_last: too many tiles");
+  CFB_LAUNCH_PDL(conv_last_kernel<U8>, dim3((unsigned)tiles), dim3(256), conv_last_smem(Cin), st, in, in_scale, in_shift, wgt, bias,
+                 out, N, H, W, Cin);
+  return 0;
 }
 
 int conv_last(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
               float* out, int N, int H, int W, int Cin, cudaStream_t st) {
-  const int64_t HW = (int64_t)H * W;
-  CFB_REQUIRE(HW % 1024 == 0 && W % 4 == 0 && Cin % 4 == 0, "conv_last: H*W must be a multiple of 1024, W and Cin of 4");
-  if (N == 0) return 0;
-  const size_t smem = (size_t)(9 * Cin * 4 + 2 * Cin) * sizeof(float);
-  CFB_REQUIRE(smem <= 48 * 1024, "conv_last: Cin too large");
-  CFB_LAUNCH_PDL(conv_last_kernel<false>, dim3((unsigned)(N * HW / 1024)), dim3(256), smem, st, in, in_scale, in_shift, wgt, bias, out, N, H,
-                 W, Cin);
-  return 0;
+  return launch_conv_last<false>(in, in_scale, in_shift, wgt, bias, out, N, H, W, Cin, st);
 }
 int conv_last_u8(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
                  unsigned char* out_bgr_hwc, int N, int H, int W, int Cin, cudaStream_t st) {
-  const int64_t HW = (int64_t)H * W;
-  CFB_REQUIRE(HW % 1024 == 0 && W % 4 == 0 && Cin % 4 == 0, "conv_last: H*W must be a multiple of 1024, W and Cin of 4");
-  if (N == 0) return 0;
-  const size_t smem = (size_t)(9 * Cin * 4 + 2 * Cin) * sizeof(float);
-  CFB_REQUIRE(smem <= 48 * 1024, "conv_last: Cin too large");
-  CFB_LAUNCH_PDL(conv_last_kernel<true>, dim3((unsigned)(N * HW / 1024)), dim3(256), smem, st, in, in_scale, in_shift, wgt, bias,
-                 reinterpret_cast<float*>(out_bgr_hwc), N, H, W, Cin);
-  return 0;
+  return launch_conv_last<true>(in, in_scale, in_shift, wgt, bias, reinterpret_cast<float*>(out_bgr_hwc), N, H, W, Cin, st);
 }
 
 // stand-alone plumbing (unit parity + callers that want the fp32 tensor): uint8 HWC BGR <-> fp32 NCHW RGB in [-1,1]
