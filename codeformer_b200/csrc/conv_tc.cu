@@ -1286,9 +1286,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             const int r = it * 4 + rsub;
             float4 v = lds128f(stg + (uint32_t)(r * 128 + ((cch ^ (r & 7)) << 4)));
             v.x += bv.x + rres[it].x; v.y += bv.y + rres[it].y; v.z += bv.z + rres[it].z; v.w += bv.w + rres[it].w;
-            if (p.out_act == OUT_LRELU) {
-              v.x = v.x > 0.f ? v.x : 0.2f * v.x; v.y = v.y > 0.f ? v.y : 0.2f * v.y;
-              v.z = v.z > 0.f ? v.z : 0.2f * v.z; v.w = v.w > 0.f ? v.w : 0.2f * v.w;
+            if (p.out_act == OUT_LRELU || p.out_act == OUT_RELU) {      // ReLU = slope 0 (a negative value becomes -0.0)
+              const float sl = p.out_act == OUT_LRELU ? 0.2f : 0.f;
+              v.x = v.x > 0.f ? v.x : sl * v.x; v.y = v.y > 0.f ? v.y : sl * v.y;
+              v.z = v.z > 0.f ? v.z : sl * v.z; v.w = v.w > 0.f ? v.w : sl * v.w;
             }
             if (pixs[it] >= 0) {
               if (p.residual2) {
@@ -1358,6 +1359,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             v.y = 0.5f * v.y * (1.f + erff(v.y * 0.70710678118654752440f));
             v.z = 0.5f * v.z * (1.f + erff(v.z * 0.70710678118654752440f));
             v.w = 0.5f * v.w * (1.f + erff(v.w * 0.70710678118654752440f));
+          } else if (p.out_act == OUT_RELU) {
+            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
           }
           if (p.sft_dec && inside[k]) {
             const float4 d = __ldg(reinterpret_cast<const float4*>(p.sft_dec + off));
@@ -1531,7 +1534,8 @@ int tc_tiles_per_image(const ConvArgs& a) {
 bool tc_supported(const ConvArgs& a) {
   if (a.Cin % 64 != 0 || a.Cout % 64 != 0) return false;
   if (!(a.ksize == 1 || a.ksize == 3)) return false;
-  if (a.mode == CONV_DOWN && a.ksize != 3) return false;
+  if (a.mode == CONV_DOWN && a.ksize != 3 && !(a.ksize == 1 && a.down_pad == 0 && a.Ho == (a.H + 1) / 2)) return false;
+  if (a.mode == CONV_DOWN && a.down_pad != 0 && !(a.down_pad == 1 && a.ksize == 3)) return false;
   if (a.Wo < 1 || a.Ho < 1) return false;
   const TcGeom g = tc_geometry(a);
   if (a.gen) return g.halo && a.ksize == 3;
@@ -1724,7 +1728,7 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   }
   TcParams p;
   p.N = a.N; p.Ho = a.Ho; p.Wo = a.Wo; p.Cout = a.Cout;
-  p.taps = a.ksize * a.ksize; p.pad = a.mode == CONV_DOWN ? 0 : a.ksize / 2; p.stride = a.mode == CONV_DOWN ? 2 : 1;
+  p.taps = a.ksize * a.ksize; p.pad = a.mode == CONV_DOWN ? a.down_pad : a.ksize / 2; p.stride = a.mode == CONV_DOWN ? 2 : 1;
   p.up4 = a.mode == CONV_UP ? 1 : 0;
   p.a_c0 = 0; p.b_c0 = 0; p.b_batched = 0;
   p.heads = 1; p.a_c_head = 0; p.b_c_head = 0; p.a_img_per_head = 0; p.b_r_head = 0; p.out_per_head = 1; p.o_c_head = 0;
@@ -1747,7 +1751,8 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.cout_valid % 4 == 0 && p.res_pitch % 4 == 0 && p.res2_pitch % 4 == 0,
                 "conv_tc: channel pitches / offsets must be multiples of 4");
     CFB_REQUIRE(!a.subsample || (a.mode == CONV_SAME && a.Ho % 2 == 0 && a.Wo % 2 == 0), "conv_tc: subsampling needs even sizes");
-    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU, "conv_tc: generalised variant has bias / residual / LeakyReLU epilogues");
+    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU,
+                "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU epilogues");
   }
   if (p.taps * p.kblocks <= 12) p.chunk = p.taps * p.kblocks;   // short K (Cin = 64): one partial sum, no 8+1 split
   p.in_scale = nullptr; p.in_shift = nullptr; p.in_act = IN_NONE; p.xform = a.xform ? 1 : 0;

@@ -101,7 +101,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 #endif
 
 enum InAct { IN_NONE = 0, IN_SILU = 1 };
-enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2 };
+enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2, OUT_RELU = 3 };
 enum ConvMode { CONV_SAME = 0, CONV_DOWN = 1, CONV_UP = 2 };
 
 // Convolution / linear layer as an implicit GEMM over NHWC fp32 activations.
@@ -112,6 +112,8 @@ struct ConvArgs {
   int Ho = 0, Wo = 0, Cout = 0;
   int ksize = 3;                    // 1 | 3
   int mode = CONV_SAME;
+  int down_pad = 0;                 // CONV_DOWN (per-tap engine): zero padding before the window; 0 = the Downsample's (0,1,0,1)
+                                    // padding (Ho = H/2), 1 = a torchvision-style 3x3 stride-2 pad-1 conv (Ho = ceil(H/2))
   const float* wgt_f32 = nullptr;   // [taps][Cin][Cout] fp32 (CUDA-core engine)
   const void* wgt_hi = nullptr;     // [taps][Cout][Cin] fp16 hi   (tensor-core engine)
   const void* wgt_lo = nullptr;     // [taps][Cout][Cin] fp16 lo
@@ -184,6 +186,15 @@ int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bia
 int relayout_thin_out(const float* oihw, float* out, int Cout, cudaStream_t st);
 int fold_bn(const float* w, const float* gamma, const float* beta, const float* mean, const float* var, float eps, float* wout,
             float* bout, int Cout, int per_out, cudaStream_t st);
+// RetinaFace-ResNet50 (detection.cu): stem conv + max-pool, FPN top-down add, head gather, candidate compaction
+int rf_stem(const float* x_nchw, const unsigned char* img_bgr_hwc, const float* wt, const float* bias, float* out, int N, int H,
+            int W, cudaStream_t st);
+int rf_maxpool(const float* in, float* out, int N, int H, int W, cudaStream_t st);
+int rf_add_nearest(float* fine, const float* coarse, int N, int Hf, int Wf, int Hc, int Wc, int C, cudaStream_t st);
+int rf_heads(const float* const h[3], const int hh[3], const int ww[3], float* loc, float* conf, float* landms, int N, int P,
+             cudaStream_t st);
+int rf_candidates(const float* loc, const float* conf, const float* landms, int N, int H, int W, float thr, float* rows, int* counts,
+                  cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

@@ -1525,6 +1525,290 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
 }  // namespace cfb
 
 // =========================================================================================================
+// RetinaFace-ResNet50: the face detector of whole-image mode
+//   /root/reference/facelib/detection/retinaface/retinaface.py:77-145 (RetinaFace, cfg_re50), retinaface_net.py (FPN, SSH,
+//   heads), torchvision resnet50 conv1 .. layer4 (body, return layers layer2/3/4).
+// Eval-mode BatchNorm is folded into every conv at prepare.  Engines per conv form:
+//   stem (7x7 s2 + max-pool)            SIMT (detection.cu), fp32 or uint8 BGR input
+//   3x3 stride 1 (layer conv2, FPN merge, SSH)   generalised fused-transform halo engine (ragged tiles, destination slices
+//                                        of the SSH concat, ReLU epilogue)
+//   1x1 (bottleneck conv1 / conv3 + residual, downsample, FPN output_k, heads), 3x3 stride 2 pad 1
+//                                        per-tap engine on operand planes (ragged tiles; stride 2 computes only the output
+//                                        positions: element-strided TMA boxes, ceil(H/2) outputs)
+//   FPN top-down add (after the ReLU)   SIMT, torch's nearest index
+// =========================================================================================================
+namespace cfb {
+struct RfConv { GenConv c; std::string bn; int k = 3, stride = 1; bool gen = false; };
+}
+struct cfb_retinaface {
+  std::mutex mu;
+  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
+  std::vector<cfb::RfConv> convs;        // body blocks (conv1, conv2, conv3[, downsample]), fpn, ssh, heads: see rf_build
+  int blocks[4] = {3, 4, 6, 3};
+  float *stem_w = nullptr, *stem_b = nullptr;
+  float* slab = nullptr; size_t slab_bytes = 0;
+  int device = -1, sm_count = 148;
+  bool prepared = false;
+  cfb::Arena arena;
+};
+namespace cfb {
+
+static void rf_build(cfb_retinaface* n) {
+  n->convs.clear();
+  auto add = [&](const std::string& w, const std::string& bn, int cin, int cout, int k, int stride, bool gen) {
+    RfConv r; r.c.name = w; r.bn = bn; r.c.cin = cin; r.c.cout = cout; r.k = k; r.stride = stride; r.gen = gen;
+    n->convs.push_back(r);
+  };
+  const int widths[4] = {64, 128, 256, 512};
+  int cin = 64;
+  for (int l = 0; l < 4; ++l) {
+    const int wd = widths[l];
+    for (int b = 0; b < n->blocks[l]; ++b) {
+      const std::string p = "body.layer" + std::to_string(l + 1) + "." + std::to_string(b) + ".";
+      const int s = (b == 0 && l > 0) ? 2 : 1;
+      add(p + "conv1.weight", p + "bn1.", cin, wd, 1, 1, false);
+      add(p + "conv2.weight", p + "bn2.", wd, wd, 3, s, s == 1);
+      add(p + "conv3.weight", p + "bn3.", wd, 4 * wd, 1, 1, false);
+      if (b == 0) add(p + "downsample.0.weight", p + "downsample.1.", cin, 4 * wd, 1, s, false);
+      cin = 4 * wd;
+    }
+  }
+  const int ins[3] = {512, 1024, 2048};
+  for (int k = 0; k < 3; ++k) {
+    const std::string p = "fpn.output" + std::to_string(k + 1) + ".";
+    add(p + "0.weight", p + "1.", ins[k], 256, 1, 1, false);
+  }
+  add("fpn.merge1.0.weight", "fpn.merge1.1.", 256, 256, 3, 1, true);
+  add("fpn.merge2.0.weight", "fpn.merge2.1.", 256, 256, 3, 1, true);
+  for (int k = 0; k < 3; ++k) {
+    const std::string p = "ssh" + std::to_string(k + 1) + ".";
+    add(p + "conv3X3.0.weight", p + "conv3X3.1.", 256, 128, 3, 1, true);
+    add(p + "conv5X5_1.0.weight", p + "conv5X5_1.1.", 256, 64, 3, 1, true);
+    add(p + "conv5X5_2.0.weight", p + "conv5X5_2.1.", 64, 64, 3, 1, true);
+    add(p + "conv7X7_2.0.weight", p + "conv7X7_2.1.", 64, 64, 3, 1, true);
+    add(p + "conv7x7_3.0.weight", p + "conv7x7_3.1.", 64, 64, 3, 1, true);
+  }
+  for (int k = 0; k < 3; ++k) add("heads." + std::to_string(k), "", 256, 64, 1, 1, false);   // bbox 8 | class 4 | landmark 20 | 0
+}
+
+static const float* rf_param(cfb_retinaface* n, const std::string& name, int64_t numel) {
+  auto it = n->raw.find(name);
+  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
+  if (it->second.second != numel) {
+    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
+    return nullptr;
+  }
+  return it->second.first;
+}
+
+static int rf_prepare(cfb_retinaface* n, cudaStream_t st) {
+  int dev = 0, major = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CFB_REQUIRE(major == 9, "RetinaFace: the wgmma engine needs an sm_90 device (there is no other path)");
+  CFB_CHECK(async_status_init(st));
+  rf_build(n);
+  size_t total = 0, padmax = 0;
+  for (RfConv& r : n->convs) {
+    r.c.cin_p = r.c.cin; r.c.cout_p = r.c.cout;
+    const size_t wn = (size_t)r.c.cout * r.c.cin * r.k * r.k;
+    total += 2 * align256(wn * 2) + align256((size_t)r.c.cout * 4) + 256;
+    padmax = std::max(padmax, wn * 4);
+  }
+  total += 2 * align256(padmax) + align256(2048 * 4) + align256((size_t)64 * 147 * 4) + align256(256);
+  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
+    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
+    else cudaFree(n->slab);
+    n->slab = nullptr; n->slab_bytes = 0;
+  }
+  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
+  n->device = dev; n->sm_count = sms;
+  char* p = (char*)n->slab;
+  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
+  float* pad_scratch = (float*)take(padmax);
+  float* fold_w = (float*)take(padmax);
+  float* fold_b = (float*)take(2048 * 4);
+  auto fold = [&](const std::string& w_name, const std::string& bn, int cout, int per_out) -> int {
+    const float* w = rf_param(n, w_name, (int64_t)cout * per_out);
+    const float* g = rf_param(n, bn + "weight", cout);
+    const float* be = rf_param(n, bn + "bias", cout);
+    const float* mu = rf_param(n, bn + "running_mean", cout);
+    const float* var = rf_param(n, bn + "running_var", cout);
+    if (!w || !g || !be || !mu || !var) return 1;
+    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
+  };
+  for (RfConv& r : n->convs) {
+    GenConv& c = r.c;
+    const size_t wn = (size_t)c.cout * c.cin * r.k * r.k;
+    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
+    c.bias = (float*)take((size_t)c.cout * 4); c.wscale = (float*)take(8);
+    if (r.bn.empty()) {        // heads: [bbox 8 | class 4 | landmark 20 | zero 32] x 256, with their biases
+      CFB_CUDA(cudaMemsetAsync(fold_w, 0, wn * 4, st));
+      CFB_CUDA(cudaMemsetAsync(fold_b, 0, 64 * 4, st));
+      const std::string lv = c.name.substr(6);
+      const struct { const char* head; int rows, row0; } parts[3] = {{"BboxHead.", 8, 0}, {"ClassHead.", 4, 8}, {"LandmarkHead.", 20, 12}};
+      for (const auto& h : parts) {
+        const std::string base = std::string(h.head) + lv + ".conv1x1.";
+        const float* w = rf_param(n, base + "weight", (int64_t)h.rows * 256);
+        const float* b = rf_param(n, base + "bias", h.rows);
+        if (!w || !b) return 1;
+        CFB_CUDA(cudaMemcpyAsync(fold_w + (size_t)h.row0 * 256, w, (size_t)h.rows * 256 * 4, cudaMemcpyDeviceToDevice, st));
+        CFB_CUDA(cudaMemcpyAsync(fold_b + h.row0, b, (size_t)h.rows * 4, cudaMemcpyDeviceToDevice, st));
+      }
+    } else {
+      CFB_CHECK(fold(c.name, r.bn, c.cout, c.cin * r.k * r.k));
+    }
+    if (r.gen) {
+      CFB_CHECK(gen_conv_prepare(c, fold_w, fold_b, pad_scratch, st));
+    } else {
+      CFB_CHECK(tc_split_weights(fold_w, c.w_hi, c.w_lo, c.cout, c.cin, r.k, c.wscale, st));
+      CFB_CUDA(cudaMemcpyAsync(c.bias, fold_b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  n->stem_w = (float*)take((size_t)64 * 147 * 4); n->stem_b = (float*)take(256);
+  CFB_CHECK(fold("body.conv1.weight", "body.bn1.", 64, 147));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, fold_w, (size_t)64 * 147 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaStreamSynchronize(st));
+  n->prepared = true;
+  return 0;
+}
+
+// number of priors of an h x w input (PriorBox: two anchors per cell of the /8, /16, /32 maps, ceil-divided)
+static int64_t rf_priors(int H, int W) {
+  int64_t P = 0;
+  for (int s : {8, 16, 32}) P += 2 * (int64_t)((H + s - 1) / s) * ((W + s - 1) / s);
+  return P;
+}
+
+static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* img, float* loc, float* conf, float* landms, int N,
+                      int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
+  CFB_REQUIRE(dry || n->prepared, "cfb_retinaface_prepare has not been called");
+  if (!dry) {
+    int dev = -1;
+    CFB_CUDA(cudaGetDevice(&dev));
+    CFB_REQUIRE(dev == n->device, "RetinaFace was prepared on another CUDA device");
+    CFB_CHECK(async_status_check("cfb_retinaface_forward"));
+  }
+  CFB_REQUIRE(H >= 1 && W >= 1 && N >= 0, "RetinaFace: empty image");
+  CFB_REQUIRE(rf_priors(H, W) * N < ((int64_t)1 << 31) / 16, "RetinaFace: image too large");
+  if (N == 0) return 0;
+  if (n->convs.empty()) rf_build(n);
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  auto alloc = [&](float** p, size_t elems) -> int {
+    *p = (float*)ar.alloc(elems * sizeof(float));
+    CFB_REQUIRE(*p != nullptr, "workspace too small (cfb_retinaface_workspace_bytes)");
+    return 0;
+  };
+  // one conv of the plan: 3x3 stride 1 on the generalised engine, everything else on the per-tap engine
+  auto conv = [&](const RfConv& r, const float* in, int h, int w, float* out, int act, const float* res, int out_pitch = 0,
+                  int out_c0 = 0) -> int {
+    if (r.gen) {
+      GenLaunch g{&r.c, in, r.c.cin, h, w, N, out, out_pitch ? out_pitch : r.c.cout, out_c0, act};
+      g.res = res; g.res_pitch = r.c.cout;
+      return dry ? 0 : gen_conv(g, n->sm_count, st);
+    }
+    ConvArgs a;
+    a.in = in; a.N = N; a.H = h; a.W = w; a.Cin = r.c.cin; a.Cout = r.c.cout; a.ksize = r.k;
+    a.Ho = r.stride == 2 ? (h + 1) / 2 : h; a.Wo = r.stride == 2 ? (w + 1) / 2 : w;
+    a.mode = r.stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = (r.stride == 2 && r.k == 3) ? 1 : 0;
+    a.wgt_hi = r.c.w_hi; a.wgt_lo = r.c.w_lo; a.wscale_inv = r.c.wscale + 1; a.bias = r.c.bias;
+    a.residual = res; a.out_act = act; a.out = out;
+    CFB_REQUIRE(tc_supported(a), "RetinaFace: conv not supported by the wgmma engine: " + r.c.name);
+    void* scratch = ar.alloc(tc_scratch_bytes(a));
+    CFB_REQUIRE(scratch != nullptr, "workspace too small (cfb_retinaface_workspace_bytes)");
+    if (!dry) CFB_CHECK(conv_tc(a, scratch, n->sm_count, st));
+    ar.release(scratch);
+    return 0;
+  };
+  const int H2 = (H - 1) / 2 + 1, W2 = (W - 1) / 2 + 1;
+  int h = (H2 - 1) / 2 + 1, w = (W2 - 1) / 2 + 1;
+  float *s0 = nullptr, *cur = nullptr;
+  CFB_CHECK(alloc(&s0, (size_t)N * H2 * W2 * 64));
+  if (!dry) CFB_CHECK(rf_stem(x, img, n->stem_w, n->stem_b, s0, N, H, W, st));
+  CFB_CHECK(alloc(&cur, (size_t)N * h * w * 64));
+  if (!dry) CFB_CHECK(rf_maxpool(s0, cur, N, H2, W2, st));
+  ar.release(s0);
+  size_t ci = 0;
+  float* C[3] = {nullptr, nullptr, nullptr};
+  int ch[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
+  for (int l = 0; l < 4; ++l) {
+    for (int b = 0; b < n->blocks[l]; ++b) {
+      const RfConv& c1 = n->convs[ci++];
+      const RfConv& c2 = n->convs[ci++];
+      const RfConv& c3 = n->convs[ci++];
+      const RfConv* ds = b == 0 ? &n->convs[ci++] : nullptr;
+      const int ho = c2.stride == 2 ? (h + 1) / 2 : h, wo = c2.stride == 2 ? (w + 1) / 2 : w;
+      float *t1 = nullptr, *t2 = nullptr, *res = cur, *y = nullptr;
+      CFB_CHECK(alloc(&t1, (size_t)N * h * w * c1.c.cout));
+      CFB_CHECK(conv(c1, cur, h, w, t1, OUT_RELU, nullptr));
+      CFB_CHECK(alloc(&t2, (size_t)N * ho * wo * c2.c.cout));
+      CFB_CHECK(conv(c2, t1, h, w, t2, OUT_RELU, nullptr));
+      ar.release(t1);
+      if (ds) {
+        CFB_CHECK(alloc(&res, (size_t)N * ho * wo * ds->c.cout));
+        CFB_CHECK(conv(*ds, cur, h, w, res, OUT_NONE, nullptr));
+      }
+      CFB_CHECK(alloc(&y, (size_t)N * ho * wo * c3.c.cout));
+      CFB_CHECK(conv(c3, t2, ho, wo, y, OUT_RELU, res));          // relu(bn3(conv3(.)) + identity)
+      ar.release(t2);
+      if (res != cur) ar.release(res);
+      if (l < 2 || b > 0) ar.release(cur);       // the input of layer3.0 / layer4.0 is a kept pyramid level (C3 / C4)
+      cur = y; h = ho; w = wo;
+    }
+    if (l >= 1) { C[l - 1] = cur; ch[l - 1] = h; cw[l - 1] = w; }      // layer2/3/4 outputs; still the next layer's input
+  }
+  // FPN (retinaface_net.py:76-96): output_k = relu(bn(conv1x1(C_k))); output_2 += nearest(output_3); merge2; output_1 += ...
+  float* O[3];
+  for (int k = 0; k < 3; ++k) {
+    CFB_CHECK(alloc(&O[k], (size_t)N * ch[k] * cw[k] * 256));
+    CFB_CHECK(conv(n->convs[ci + k], C[k], ch[k], cw[k], O[k], OUT_RELU, nullptr));
+    ar.release(C[k]);
+  }
+  const RfConv& merge1 = n->convs[ci + 3];
+  const RfConv& merge2 = n->convs[ci + 4];
+  ci += 5;
+  float *m2 = nullptr, *m1 = nullptr;
+  if (!dry) CFB_CHECK(rf_add_nearest(O[1], O[2], N, ch[1], cw[1], ch[2], cw[2], 256, st));
+  CFB_CHECK(alloc(&m2, (size_t)N * ch[1] * cw[1] * 256));
+  CFB_CHECK(conv(merge2, O[1], ch[1], cw[1], m2, OUT_RELU, nullptr));
+  ar.release(O[1]);
+  if (!dry) CFB_CHECK(rf_add_nearest(O[0], m2, N, ch[0], cw[0], ch[1], cw[1], 256, st));
+  CFB_CHECK(alloc(&m1, (size_t)N * ch[0] * cw[0] * 256));
+  CFB_CHECK(conv(merge1, O[0], ch[0], cw[0], m1, OUT_RELU, nullptr));
+  ar.release(O[0]);
+  float* fpn[3] = {m1, m2, O[2]};
+  // SSH (retinaface_net.py:47-59): relu(cat[conv3X3, conv5X5, conv7X7]) written as three destination slices with ReLU
+  // epilogues; then the three 1x1 heads of the level in one conv
+  float* hd[3];
+  for (int k = 0; k < 3; ++k) {
+    const RfConv* s = &n->convs[ci + 5 * k];
+    const int hk = ch[k], wk = cw[k];
+    float *f = nullptr, *t5 = nullptr, *t7 = nullptr;
+    CFB_CHECK(alloc(&f, (size_t)N * hk * wk * 256));
+    CFB_CHECK(conv(s[0], fpn[k], hk, wk, f, OUT_RELU, nullptr, 256, 0));
+    CFB_CHECK(alloc(&t5, (size_t)N * hk * wk * 64));
+    CFB_CHECK(conv(s[1], fpn[k], hk, wk, t5, OUT_RELU, nullptr));
+    CFB_CHECK(conv(s[2], t5, hk, wk, f, OUT_RELU, nullptr, 256, 128));
+    CFB_CHECK(alloc(&t7, (size_t)N * hk * wk * 64));
+    CFB_CHECK(conv(s[3], t5, hk, wk, t7, OUT_RELU, nullptr));
+    CFB_CHECK(conv(s[4], t7, hk, wk, f, OUT_RELU, nullptr, 256, 192));
+    ar.release(t5); ar.release(t7);
+    ar.release(fpn[k]);
+    CFB_CHECK(alloc(&hd[k], (size_t)N * hk * wk * 64));
+    CFB_CHECK(conv(n->convs[ci + 15 + k], f, hk, wk, hd[k], OUT_NONE, nullptr));
+    ar.release(f);
+  }
+  if (!dry) CFB_CHECK(rf_heads(hd, ch, cw, loc, conf, landms, N, (int)rf_priors(H, W), st));
+  for (int k = 0; k < 3; ++k) ar.release(hd[k]);
+  return 0;
+}
+
+}  // namespace cfb
+
+// =========================================================================================================
 // C ABI
 // =========================================================================================================
 #define API_BEGIN try {
@@ -1728,6 +2012,117 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
   g.res = residual; g.res_pitch = res_pitch; g.res2 = residual2; g.res2_pitch = res2_pitch; g.post = post_scale;
   g.pad_mode = pad_mode; g.sub = subsample != 0;
   return cfb::gen_conv(g, sms, st);
+  API_END(1)
+}
+
+int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h, int32_t w,
+                           int32_t cin, int32_t cout, int32_t ksize, int32_t stride, int32_t out_act, const float* residual,
+                           void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(in && weight_oihw && out && workspace, "cfb_conv2d_pertap_nhwc: NULL argument");
+  CFB_REQUIRE(stride == 1 || stride == 2, "cfb_conv2d_pertap_nhwc: stride must be 1 or 2");
+  CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_RELU, "cfb_conv2d_pertap_nhwc: activation must be none or ReLU");
+  cudaStream_t st = (cudaStream_t)stream;
+  CFB_CHECK(cfb::async_status_init(st));
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  cfb::ConvArgs a;
+  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
+  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
+  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
+  CFB_REQUIRE(cfb::tc_supported(a), "cfb_conv2d_pertap_nhwc: shape not supported by the wgmma engine");
+  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_pertap_workspace_bytes(n, h, w, cin, cout, ksize, stride),
+              "cfb_conv2d_pertap_nhwc: workspace too small");
+  const size_t wn = (size_t)cout * cin * ksize * ksize;
+  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+  __half* whi = (__half*)p; p += align256(wn * 2);
+  __half* wlo = (__half*)p; p += align256(wn * 2);
+  float* wsc = (float*)p; p += 256;
+  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
+  CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, ksize, wsc, st));
+  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.bias = bias; a.residual = residual; a.out_act = out_act; a.out = out;
+  return cfb::conv_tc(a, p, sms, st);
+  API_END(1)
+}
+
+int64_t cfb_conv2d_pertap_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride) {
+  if (n < 0 || h < 1 || w < 1 || cin < 1 || cout < 1 || !(ksize == 1 || ksize == 3) || !(stride == 1 || stride == 2)) return -1;
+  cfb::ConvArgs a;
+  a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
+  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
+  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
+  const size_t wn = (size_t)cout * cin * ksize * ksize;
+  return (int64_t)(2 * align256(wn * 2) + 256 + cfb::tc_scratch_bytes(a) + 4096);
+}
+
+int64_t cfb_retinaface_priors(int32_t h, int32_t w) { return h < 1 || w < 1 ? -1 : cfb::rf_priors(h, w); }
+
+cfb_retinaface* cfb_retinaface_create(void) {
+  API_BEGIN
+  cfb_retinaface* n = new cfb_retinaface();
+  cfb::rf_build(n);
+  return n;
+  API_END(nullptr)
+}
+void cfb_retinaface_destroy(cfb_retinaface* n) {
+  if (!n) return;
+  if (n->slab) {
+    int cur = -1;
+    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
+    if (sw) cudaSetDevice(n->device);
+    cudaFree(n->slab);
+    if (sw) cudaSetDevice(cur);
+  }
+  delete n;
+}
+int cfb_retinaface_set_param(cfb_retinaface* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_retinaface_set_param: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  n->raw[name] = {dev_ptr, numel};
+  n->prepared = false;
+  return 0;
+  API_END(1)
+}
+int cfb_retinaface_prepare(cfb_retinaface* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_retinaface_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::rf_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_retinaface_workspace_bytes(cfb_retinaface* n, int32_t batch, int32_t h, int32_t w) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_retinaface_workspace_bytes: NULL net"); return -1; }
+  std::lock_guard<std::mutex> lk(n->mu);
+  if (cfb::rf_forward(n, (const float*)0x1000, nullptr, nullptr, nullptr, nullptr, batch, h, w, nullptr, 0, nullptr, true) != 0) return -1;
+  return (int64_t)n->arena.high() + 4096;
+  API_END(-1)
+}
+int cfb_retinaface_forward(cfb_retinaface* n, const float* x_nchw, float* loc, float* conf, float* landms, int32_t batch, int32_t h,
+                           int32_t w, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (x_nchw && loc && conf && landms && workspace)), "cfb_retinaface_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::rf_forward(n, x_nchw, nullptr, loc, conf, landms, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_retinaface_forward_u8(cfb_retinaface* n, const uint8_t* img_bgr_hwc, float* loc, float* conf, float* landms, int32_t batch,
+                              int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (img_bgr_hwc && loc && conf && landms && workspace)), "cfb_retinaface_forward_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::rf_forward(n, nullptr, img_bgr_hwc, loc, conf, landms, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream,
+                         false);
+  API_END(1)
+}
+int cfb_retinaface_candidates(const float* loc, const float* conf, const float* landms, int32_t batch, int32_t h, int32_t w,
+                              float conf_threshold, float* rows, int32_t* counts, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(batch == 0 || (loc && conf && landms && rows && counts), "cfb_retinaface_candidates: NULL argument");
+  CFB_REQUIRE(h >= 1 && w >= 1 && batch >= 0, "cfb_retinaface_candidates: empty image");
+  return cfb::rf_candidates(loc, conf, landms, batch, h, w, conf_threshold, rows, counts, (cudaStream_t)stream);
   API_END(1)
 }
 

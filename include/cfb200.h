@@ -243,6 +243,34 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
                         int32_t res_pitch, const float* residual2, int32_t res2_pitch, float post_scale, void* workspace,
                         int64_t workspace_bytes, void* stream);
 
+/* One 1x1 or 3x3 conv of the per-tap engine on any h x w (test entry point for the detector's conv forms).  stride 2 computes
+ * only the output positions, ceil(h/2) x ceil(w/2): 3x3 with padding 1, 1x1 without.  in / out / residual NHWC, cin and cout
+ * multiples of 64.  out = act(conv + bias + residual), act 0 none / 3 ReLU. */
+int64_t cfb_conv2d_pertap_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride);
+int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h, int32_t w,
+                           int32_t cin, int32_t cout, int32_t ksize, int32_t stride, int32_t out_act, const float* residual,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- RetinaFace-ResNet50 face detector (facelib/detection/retinaface; detection.cu + the conv engine) ----
+ * Parameters by the reference's state-dict names (BatchNorm folded at prepare).  forward: x fp32 NCHW [batch,3,h,w] (the
+ * mean-subtracted image) -> loc [batch,P,4], conf [batch,P,2] (softmaxed), landms [batch,P,10], P = cfb_retinaface_priors(h, w).
+ * forward_u8: uint8 HWC BGR images [batch,h,w,3] with the (104,117,123) mean subtraction fused.
+ * candidates: per image, the rows [x1,y1,x2,y2,score,10 landmark coordinates] (pixels) of the priors whose score is
+ * > conf_threshold, in prior order, into rows [batch,P,15]; counts [batch] (device int32). */
+typedef struct cfb_retinaface cfb_retinaface;
+int64_t   cfb_retinaface_priors(int32_t h, int32_t w);
+cfb_retinaface* cfb_retinaface_create(void);
+void      cfb_retinaface_destroy(cfb_retinaface* net);
+int       cfb_retinaface_set_param(cfb_retinaface* net, const char* name, const float* dev_ptr, int64_t numel);
+int       cfb_retinaface_prepare(cfb_retinaface* net, void* stream);
+int64_t   cfb_retinaface_workspace_bytes(cfb_retinaface* net, int32_t batch, int32_t h, int32_t w);
+int       cfb_retinaface_forward(cfb_retinaface* net, const float* x_nchw, float* loc, float* conf, float* landms, int32_t batch,
+                                 int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int       cfb_retinaface_forward_u8(cfb_retinaface* net, const uint8_t* img_bgr_hwc, float* loc, float* conf, float* landms,
+                                    int32_t batch, int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int       cfb_retinaface_candidates(const float* loc, const float* conf, const float* landms, int32_t batch, int32_t h, int32_t w,
+                                    float conf_threshold, float* rows, int32_t* counts, void* stream);
+
 /* Asynchronous failures.  Kernels never trap and never leave a sticky CUDA error behind (the reference's callers catch
  * RuntimeError and fall back to the input face, inference_codeformer.py:209-211; web-demos/hugging_face/app.py:176): a
  * barrier time-out of the tensor-core pipeline or an activation outside the fp16 operand range (|x| > 65504) sets a bit

@@ -1,0 +1,85 @@
+"""RetinaFace-ResNet50 timing on one GPU: detect_faces per image (host uint8 in, numpy out), the forward alone (CUDA events),
+and the oracle's torch module (cuDNN) on the same card as a comparison point.  --profile prints the kernel shares of one
+forward under torch.profiler instead (run it separately: tracing slows the host).
+
+    python tools/detection_bench.py [--sizes 640x853,1080x1440] [--iters 20] [--profile]
+"""
+import argparse
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import codeformer_b200 as cb                                   # noqa: E402
+from codeformer_b200 import detection as D                      # noqa: E402
+from oracle import retinaface_oracle as RO                      # noqa: E402
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        pl = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm', '--format=csv,noheader'],
+                            capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:                                        # noqa: BLE001
+        pl = f'unknown ({e})'
+    return f'{name}, power limit / max SM clock: {pl}'
+
+
+def timed(fn, iters, warmup=3):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        ts.append(a.elapsed_time(b))
+    return float(np.median(ts))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--sizes', default='640x853,1080x1440')
+    ap.add_argument('--iters', type=int, default=20)
+    ap.add_argument('--profile', action='store_true')
+    args = ap.parse_args()
+    torch.set_grad_enabled(False)
+    dev = 'cuda:0'
+    print(card())
+    sd = D.random_retinaface_state_dict(1)
+    net = cb.RetinaFace().to(dev)
+    net.load_state_dict(sd, strict=True)
+    sd_dev = {k: v.to(dev) for k, v in sd.items()}
+    for s in args.sizes.split(','):
+        h, w = (int(v) for v in s.split('x'))
+        img = np.random.default_rng(0).integers(0, 256, (h, w, 3), dtype=np.uint8)
+        x = RO.input_from_u8(img).to(dev)
+        if args.profile:
+            net(x)
+            torch.cuda.synchronize()
+            from torch.profiler import ProfilerActivity, profile
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                net(x)
+                torch.cuda.synchronize()
+            print(f'--- {h}x{w}: kernel shares of one forward')
+            print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=15))
+            continue
+        det_ms = timed(lambda: net.detect_faces(img), args.iters)
+        fwd_ms = timed(lambda: net(x), args.iters)
+        torch.backends.cudnn.allow_tf32 = False
+        torch.backends.cuda.matmul.allow_tf32 = False
+        ref_fp32 = timed(lambda: RO.forward(sd_dev, x), args.iters)
+        torch.backends.cudnn.allow_tf32 = True
+        ref_tf32 = timed(lambda: RO.forward(sd_dev, x), args.iters)
+        print(f'{h}x{w}: detect_faces {det_ms:.2f} ms/image (host uint8 in, numpy out), forward {fwd_ms:.2f} ms; '
+              f'oracle torch module on cuDNN: {ref_fp32:.2f} ms (allow_tf32=False), {ref_tf32:.2f} ms (default, TF32 convs)')
+
+
+if __name__ == '__main__':
+    main()
