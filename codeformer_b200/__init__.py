@@ -11,6 +11,7 @@ from .upsampler import RRDBNet, RealESRGANer                   # noqa: F401
 from .parsing import ParseNet, face_parse_mask, init_parsing_model   # noqa: F401
 from .pasteback import warp_faces, paste_faces, align_warp_face, paste_faces_to_input_image   # noqa: F401
 from .detection import RetinaFace, init_detection_model   # noqa: F401
+from .yolov5face import YOLOv5lFace, YoloDetector   # noqa: F401
 
 
 def check_async_status():
@@ -23,4 +24,5 @@ def check_async_status():
 
 __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQuantizer', 'RRDBNet', 'RealESRGANer', 'ParseNet', 'face_parse_mask', 'init_parsing_model',
            'warp_faces', 'paste_faces', 'align_warp_face', 'paste_faces_to_input_image', 'RetinaFace', 'init_detection_model',
+           'YOLOv5lFace', 'YoloDetector',
            'check_async_status']

@@ -83,6 +83,8 @@ SIGNATURES = {
     'cfb_conv2d_pertap_workspace_bytes': (c_int64, [c_int32] * 7),
     'cfb_conv2d_pertap_nhwc': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P,
                                        _P, c_int64, _P]),
+    'cfb_conv2d_pertap_slice_nhwc': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                             c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_priors': (c_int64, [c_int32, c_int32]),
     'cfb_retinaface_create': (c_void_p, []),
     'cfb_retinaface_destroy': (None, [_P]),
@@ -92,6 +94,16 @@ SIGNATURES = {
     'cfb_retinaface_forward': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_forward_u8': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_candidates': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, _P, _P]),
+    'cfb_yolov5face_predictions': (c_int64, [c_int32, c_int32]),
+    'cfb_yolov5face_create': (c_void_p, []),
+    'cfb_yolov5face_destroy': (None, [_P]),
+    'cfb_yolov5face_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
+    'cfb_yolov5face_prepare': (c_int, [_P, _P]),
+    'cfb_yolov5face_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32]),
+    'cfb_yolov5face_forward': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_yolov5face_forward_u8': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32,
+                                          _P, c_int64, _P]),
+    'cfb_yolov5face_candidates': (c_int, [_P, c_int32, c_int32, c_int32, c_float, _P, _P, _P]),
     'cfb_check_async_status': (c_int, []),
     'cfb_debug_set_wait_limit': (c_int, [c_int64]),
     'cfb_debug_inject_fault': (c_int, [c_int32]),

@@ -154,6 +154,9 @@ __device__ void report_overflow();       // status word, defined with the barrie
 // operand preparation: fp32 NHWC (+ fused GroupNorm affine, SiLU, nearest x2) -> fp16 hi / lo NHWC planes
 // ------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float tc_silu(float x) { return x / (1.f + expf(-x)); }
+// output SiLU of the epilogues (YOLOv5 Conv): the fast exponential and division keep the epilogue's register budget; __expf
+// is within 2 + 1.173 |x| ulp, far inside the fp32 parity bars of the detector
+__device__ __forceinline__ float tc_silu_out(float x) { return __fdividef(x, 1.f + __expf(-x)); }
 
 // One block = PB consecutive output pixels of ONE image; a thread keeps the same 8-channel slice for all its pixels, so
 // the per-(n,c) GroupNorm scale/shift is loaded once per block instead of once per element.
@@ -648,7 +651,7 @@ struct TcCfg {
 // CM (channel-major, BN = 64 only): the MMA warpgroup computes the tile transposed, D^T[64 channels x 128 pixels] =
 // W[64 x K] * X[128 x K]^T, as one m64n128k16 per product and k-step (weights = A operand, halo patch = B operand), and stores
 // each partial sum into the slot as [pixel][channel]: the epilogue is that of the pixel-major 128 x 64 tile.
-template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false>
+template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false>
 __global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
@@ -1156,8 +1159,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // tile geometry: 8 x 16 pixels on the halo engine (compile-time), else BW = 2^bw_shift columns (or any BW: division)
     const int BW = HALO ? 8 : p.BW, BH = HALO ? 16 : p.BH;
     const int bw_shift = HALO ? 3 : ((BW & (BW - 1)) == 0 ? __ffs(BW) - 1 : -1);   // log2(BW) when BW is a power of two
-    // element strides of one tile row / column in `out` (Upsample tiles write every second pixel of the output)
-    const int64_t SW = (int64_t)(p.up4 ? 2 : 1) * p.Cout, SH = SW * p.Wo;
+    // element strides of one tile row / column in `out` (Upsample tiles write every second pixel of the output).  On the
+    // per-tap engine out_pitch is Cout unless the conv writes a channel slice of a wider buffer (then residual, SFT, planes and
+    // statistics are off, and the host has moved p.out to the slice's first channel)
+    const int64_t SW = (int64_t)(p.up4 ? 2 : 1) * (HALO ? p.Cout : p.out_pitch), SH = SW * p.Wo;
     // every tile lies inside the image unless the image size is not a multiple of the tile (per-tap engine only): then the
     // outside rows / columns of the last tiles are neither stored nor counted in the GroupNorm partials
     const int ts = p.up4 ? 2 : 1;
@@ -1182,9 +1187,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       const int64_t pix = ((int64_t)n * p.Ho + oy) * p.Wo + ox;
       // first pixel of the tile in `out` (elements); the (row, chunk) items of the store loop are hh * SH + ww * SW away
       const int64_t off_tile = (((int64_t)n * p.Ho + (p.up4 ? 2 * ty * BH + ((mt & 3) >> 1) : ty * BH)) * p.Wo +
-                                (p.up4 ? 2 * tx * BW + (mt & 1) : tx * BW)) * p.Cout;
+                                (p.up4 ? 2 * tx * BW + (mt & 1) : tx * BW)) * (HALO ? p.Cout : p.out_pitch);
       const int col0 = nt * BN + cbase + (hsplit ? (nb % p.heads) * p.o_c_head : 0);
-      const int64_t off0 = pix * p.Cout + col0;
+      const int64_t off0 = pix * (HALO ? p.Cout : p.out_pitch) + col0;
       // pull this thread's residual / SFT row slices towards L2 now: they are consumed only after the whole K loop
       const bool row_in = whole_tiles || (oy < p.Ho && ox < p.Wo);
       if (!GEN && p.residual && row_in) {
@@ -1290,6 +1295,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               const float sl = p.out_act == OUT_LRELU ? 0.2f : 0.f;
               v.x = v.x > 0.f ? v.x : sl * v.x; v.y = v.y > 0.f ? v.y : sl * v.y;
               v.z = v.z > 0.f ? v.z : sl * v.z; v.w = v.w > 0.f ? v.w : sl * v.w;
+            } else if (SILU) {
+              v.x = tc_silu_out(v.x); v.y = tc_silu_out(v.y); v.z = tc_silu_out(v.z); v.w = tc_silu_out(v.w);
             }
             if (pixs[it] >= 0) {
               if (p.residual2) {
@@ -1361,6 +1368,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             v.w = 0.5f * v.w * (1.f + erff(v.w * 0.70710678118654752440f));
           } else if (p.out_act == OUT_RELU) {
             v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+          } else if (SILU) {
+            v.x = tc_silu_out(v.x); v.y = tc_silu_out(v.y); v.z = tc_silu_out(v.z); v.w = tc_silu_out(v.w);
           }
           if (p.sft_dec && inside[k]) {
             const float4 d = __ldg(reinterpret_cast<const float4*>(p.sft_dec + off));
@@ -1573,7 +1582,7 @@ size_t tc_scratch_bytes(const ConvArgs& a) {
 
 struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
 
-template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false>
+template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false>
 static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int SMEM = XF ? Cfg::X_SMEM_BYTES : (HALO ? Cfg::H_SMEM_BYTES : Cfg::SMEM_BYTES);
@@ -1586,17 +1595,20 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
   CFB_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count ? total : sm_count;
-  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st, m.a_hi,
+  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st, m.a_hi,
                  m.a_lo, m.b_hi, m.b_lo, p);
   return 0;
 }
 template <int CPG>
 static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, int tile = TC_TILE_N) {
+  // the SiLU epilogue (YOLOv5) is built into two variants only, so the others keep their register budgets
+  CFB_REQUIRE(p.out_act != OUT_SILU || (CPG == 0 && (gen || (!p.xform && p.PW == 0))),
+              "conv_tc: the SiLU epilogue is built for the per-tap and generalised engines without statistics");
   if (tile == TC_TILE_CM) {    // channel-major 128 x 64 tiles: conv_tc() only asks for them where tc_tile_kind() says so
     if constexpr (CPG <= 2) {
       CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: channel-major tiles need the 3x3 / Upsample halo engine");
@@ -1618,8 +1630,10 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   if constexpr (CPG == 0) {
     if (gen) {
       CFB_REQUIRE(p.xform && p.PW == 10 && p.PH == 18, "conv_tc: generalised variant needs the halo + transform engine");
+      if (p.out_act == OUT_SILU) return launch_tc2<64, 0, true, true, true, false, false, true>(m, p, sm_count, st);
       return launch_tc2<64, 0, true, true, true>(m, p, sm_count, st);
     }
+    if (p.out_act == OUT_SILU) return launch_tc2<64, 0, false, false, false, false, false, true>(m, p, sm_count, st);
   }
   if (p.xform) {         // fused operand transform: conv_tc() only asks for it when tc_can_xform() holds
     CFB_REQUIRE((p.PW == 10 && p.PH == 18) || (p.PW == 8 && p.PH == 16 && p.taps == 1),
@@ -1751,8 +1765,14 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.cout_valid % 4 == 0 && p.res_pitch % 4 == 0 && p.res2_pitch % 4 == 0,
                 "conv_tc: channel pitches / offsets must be multiples of 4");
     CFB_REQUIRE(!a.subsample || (a.mode == CONV_SAME && a.Ho % 2 == 0 && a.Wo % 2 == 0), "conv_tc: subsampling needs even sizes");
-    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU,
-                "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU epilogues");
+    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU || a.out_act == OUT_SILU,
+                "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU / SiLU epilogues");
+  } else if (p.out_pitch != a.Cout || p.out_c0 != 0) {
+    // per-tap engine writing a channel slice: the tile offsets use the destination pitch, which only the plain store follows
+    CFB_REQUIRE(!geo.halo && p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.out_c0 + a.Cout <= p.out_pitch,
+                "conv_tc: a destination slice needs the per-tap engine, 4-aligned and inside the pitch");
+    CFB_REQUIRE(!a.residual && !a.sft_dec && !a.out_planes && !a.gn_part && !a.vq_cand && !a.residual2 && a.cout_valid == 0,
+                "conv_tc: a destination slice of the per-tap engine takes bias and activation only");
   }
   if (p.taps * p.kblocks <= 12) p.chunk = p.taps * p.kblocks;   // short K (Cin = 64): one partial sum, no 8+1 split
   p.in_scale = nullptr; p.in_shift = nullptr; p.in_act = IN_NONE; p.xform = a.xform ? 1 : 0;
@@ -1772,7 +1792,8 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(a.in2 == nullptr, "conv_tc: a two-source input needs the fused operand transform");
   }
   p.bias = a.bias; p.residual = a.residual; p.out_act = a.out_act;
-  p.sft_dec = a.sft_dec; p.sft_scale = a.sft_scale; p.sft_w = a.sft_w; p.wscale_inv = a.wscale_inv; p.out = a.out;
+  p.sft_dec = a.sft_dec; p.sft_scale = a.sft_scale; p.sft_w = a.sft_w; p.wscale_inv = a.wscale_inv;
+  p.out = a.gen || !a.out ? a.out : a.out + a.out_c0;      // per-tap engine: the slice offset is folded into the base pointer
   p.gn_part = a.gn_part; p.gn_cpg = a.Cout / 32;
   p.pl_hi = (__half*)a.out_planes;
   p.pl_lo = a.out_planes ? (__half*)((char*)a.out_planes + (((size_t)a.N * a.Ho * a.Wo * a.Cout * 2 + 1023) / 1024 * 1024)) : nullptr;

@@ -101,7 +101,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 #endif
 
 enum InAct { IN_NONE = 0, IN_SILU = 1 };
-enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2, OUT_RELU = 3 };
+enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2, OUT_RELU = 3, OUT_SILU = 4 };
 enum ConvMode { CONV_SAME = 0, CONV_DOWN = 1, CONV_UP = 2 };
 
 // Convolution / linear layer as an implicit GEMM over NHWC fp32 activations.
@@ -195,6 +195,16 @@ int rf_heads(const float* const h[3], const int hh[3], const int ww[3], float* l
              cudaStream_t st);
 int rf_candidates(const float* loc, const float* conf, const float* landms, int N, int H, int W, float thr, float* rows, int* counts,
                   cudaStream_t st);
+// YOLOv5l-face (yolo.cu): stem conv, StemBlock / SPP max pools, concat-slice copy, Detect decode, candidate compaction
+int yolo_stem(const float* x_nchw, const unsigned char* img_bgr_hwc, const float* wt, const float* bias, float* out, int N, int H,
+              int W, int ih, int iw, int top, int left, cudaStream_t st);
+int yolo_maxpool2(const float* in, float* out, int N, int H, int W, int C, int out_pitch, int out_c0, cudaStream_t st);
+int yolo_spp(float* buf, int N, int H, int W, int C, cudaStream_t st);
+int yolo_copy(const float* src, int src_pitch, int src_c0, float* dst, int dst_pitch, int dst_c0, int N, int Hs, int Ws, int C,
+              bool up2, cudaStream_t st);
+int yolo_decode(const float* const h[3], float* const raw[3], const int ny[3], const int nx[3], const float* anchor_grid, float* pred,
+                int N, int P, cudaStream_t st);
+int yolo_candidates(const float* pred, int N, int P, float thr, float* rows, int* counts, cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

@@ -10,6 +10,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <algorithm>
 #include <array>
 #include <atomic>
 #include <cmath>
@@ -1809,6 +1810,322 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
 }  // namespace cfb
 
 // =========================================================================================================
+// YOLOv5l-face: the other large detector of whole-image mode (--detection_model YOLOv5l)
+//   facelib/detection/yolov5face/models/yolov5l.yaml, common.py (Conv, StemBlock, C3, Bottleneck, SPP), yolo.py (Detect).
+// Every Conv is conv (no bias) + BatchNorm2d (folded at prepare) + SiLU.  Engines per conv form:
+//   stem_1 (3x3 s2, 3 -> 64)                      SIMT (yolo.cu), fp32 or uint8 BGR input with the letterbox fused
+//   3x3 stride 1 (Bottleneck cv2)                 generalised halo engine, SiLU epilogue; the shortcut enters as residual2
+//                                                 after the activation (x + silu(bn(conv)))
+//   1x1, 3x3 stride 2 pad 1, Detect (48 -> 64)   per-tap engine, SiLU epilogue (none for Detect), destination slices
+// The concatenations never run as copies of both halves: C3's m-chain and cv2 write the two halves of cv3's input, the stem's
+// stem_2b and max pool the two halves of stem_3's input, SPP's cv1 and pools the four quarters of cv2's input, and the head's
+// convs 9 / 13 / 17 / 20 write into the concat buffers of layers 21 / 18 / 18 / 21.  The copy kernel fills the rest: the
+// nearest x2 upsamples (layers 10, 14) and the backbone features of layers 11 and 15.
+// =========================================================================================================
+namespace cfb {
+struct YoConv { GenConv c; int k = 1, stride = 1; bool gen = false, bn = true; };
+}
+struct cfb_yolov5face {
+  std::mutex mu;
+  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
+  std::unordered_map<std::string, cfb::YoConv> convs;     // by module prefix, e.g. "model.1.m.0.cv2"
+  float *stem_w = nullptr, *stem_b = nullptr, *anchor_grid = nullptr;
+  float* slab = nullptr; size_t slab_bytes = 0;
+  int device = -1, sm_count = 148;
+  bool prepared = false;
+  cfb::Arena arena;
+};
+namespace cfb {
+
+// (layer, c1, c2, bottlenecks, shortcut) of the eight C3 blocks of yolov5l.yaml
+struct YoC3 { int i, c1, c2, n; bool sc; };
+static const YoC3 kYoC3[8] = {{1, 64, 128, 3, true},     {3, 256, 256, 9, true},
+                                                               {5, 512, 512, 9, true},    {8, 1024, 1024, 3, false},
+                                                               {12, 1024, 512, 3, false}, {16, 512, 256, 3, false},
+                                                               {19, 512, 512, 3, false},  {22, 1024, 1024, 3, false}};
+
+static void yo_build(cfb_yolov5face* n) {
+  n->convs.clear();
+  auto add = [&](const std::string& name, int cin, int cout, int k, int stride, bool bn = true) {
+    YoConv r; r.c.name = name; r.c.cin = cin; r.c.cout = cout; r.k = k; r.stride = stride; r.gen = k == 3 && stride == 1; r.bn = bn;
+    r.c.cin_p = (cin + 63) / 64 * 64; r.c.cout_p = (cout + 63) / 64 * 64;
+    n->convs[name] = r;
+  };
+  add("model.0.stem_2a", 64, 32, 1, 1);
+  add("model.0.stem_2b", 32, 64, 3, 2);
+  add("model.0.stem_3", 128, 64, 1, 1);
+  for (const auto& b : kYoC3) {
+    const std::string p = "model." + std::to_string(b.i) + ".";
+    const int c_ = b.c2 / 2;
+    add(p + "cv1", b.c1, c_, 1, 1);
+    add(p + "cv2", b.c1, c_, 1, 1);
+    add(p + "cv3", 2 * c_, b.c2, 1, 1);
+    for (int j = 0; j < b.n; ++j) {
+      add(p + "m." + std::to_string(j) + ".cv1", c_, c_, 1, 1);
+      add(p + "m." + std::to_string(j) + ".cv2", c_, c_, 3, 1);
+    }
+  }
+  add("model.2", 128, 256, 3, 2);
+  add("model.4", 256, 512, 3, 2);
+  add("model.6", 512, 1024, 3, 2);
+  add("model.7.cv1", 1024, 512, 1, 1);
+  add("model.7.cv2", 2048, 1024, 1, 1);
+  add("model.9", 1024, 512, 1, 1);
+  add("model.13", 512, 256, 1, 1);
+  add("model.17", 256, 256, 3, 2);
+  add("model.20", 512, 512, 3, 2);
+  const int ch[3] = {256, 512, 1024};
+  for (int l = 0; l < 3; ++l) add("model.23.m." + std::to_string(l), ch[l], 48, 1, 1, false);
+}
+
+static const float* yo_param(cfb_yolov5face* n, const std::string& name, int64_t numel) {
+  auto it = n->raw.find(name);
+  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
+  if (it->second.second != numel) {
+    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
+    return nullptr;
+  }
+  return it->second.first;
+}
+
+static int yo_prepare(cfb_yolov5face* n, cudaStream_t st) {
+  int dev = 0, major = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CFB_REQUIRE(major == 9, "YOLOv5-face: the wgmma engine needs an sm_90 device (there is no other path)");
+  CFB_CHECK(async_status_init(st));
+  yo_build(n);
+  size_t total = 0, padmax = 0;
+  for (auto& kv : n->convs) {
+    const GenConv& c = kv.second.c;
+    const size_t wn = (size_t)c.cout_p * c.cin_p * kv.second.k * kv.second.k;
+    total += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
+    padmax = std::max(padmax, wn * 4);
+  }
+  total += 2 * align256(padmax) + align256(1024 * 4) + align256((size_t)64 * 27 * 4) + align256(256) + align256(18 * 4);
+  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
+    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
+    else cudaFree(n->slab);
+    n->slab = nullptr; n->slab_bytes = 0;
+  }
+  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
+  n->device = dev; n->sm_count = sms;
+  char* p = (char*)n->slab;
+  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
+  float* pad_scratch = (float*)take(padmax);
+  float* fold_w = (float*)take(padmax);
+  float* fold_b = (float*)take(1024 * 4);
+  auto fold = [&](const std::string& m, int cout, int per_out) -> int {   // Conv m: m.conv.weight + m.bn.*
+    const float* w = yo_param(n, m + ".conv.weight", (int64_t)cout * per_out);
+    const float* g = yo_param(n, m + ".bn.weight", cout);
+    const float* be = yo_param(n, m + ".bn.bias", cout);
+    const float* mu = yo_param(n, m + ".bn.running_mean", cout);
+    const float* var = yo_param(n, m + ".bn.running_var", cout);
+    if (!w || !g || !be || !mu || !var) return 1;
+    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
+  };
+  for (auto& kv : n->convs) {
+    YoConv& r = kv.second;
+    GenConv& c = r.c;
+    const int taps = r.k * r.k;
+    const size_t wn = (size_t)c.cout_p * c.cin_p * taps;
+    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
+    c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
+    if (r.bn) {
+      CFB_CHECK(fold(c.name, c.cout, c.cin * taps));
+    } else {                 // Detect: plain conv with bias
+      const float* w = yo_param(n, c.name + ".weight", (int64_t)c.cout * c.cin);
+      const float* b = yo_param(n, c.name + ".bias", c.cout);
+      if (!w || !b) return 1;
+      CFB_CUDA(cudaMemcpyAsync(fold_w, w, (size_t)c.cout * c.cin * 4, cudaMemcpyDeviceToDevice, st));
+      CFB_CUDA(cudaMemcpyAsync(fold_b, b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    if (r.gen) {
+      CFB_CHECK(gen_conv_prepare(c, fold_w, fold_b, pad_scratch, st));
+    } else {                 // zero-padded [cout_p][cin_p][k][k] (stem_2a / stem_2b / Detect), then the fp16 hi/lo split
+      CFB_CUDA(cudaMemsetAsync(pad_scratch, 0, wn * 4, st));
+      CFB_CUDA(cudaMemcpy2DAsync(pad_scratch, (size_t)c.cin_p * taps * 4, fold_w, (size_t)c.cin * taps * 4, (size_t)c.cin * taps * 4,
+                                 c.cout, cudaMemcpyDeviceToDevice, st));
+      CFB_CHECK(tc_split_weights(pad_scratch, c.w_hi, c.w_lo, c.cout_p, c.cin_p, r.k, c.wscale, st));
+      CFB_CUDA(cudaMemsetAsync(c.bias, 0, (size_t)c.cout_p * 4, st));
+      CFB_CUDA(cudaMemcpyAsync(c.bias, fold_b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  n->stem_w = (float*)take((size_t)64 * 27 * 4); n->stem_b = (float*)take(256);
+  CFB_CHECK(fold("model.0.stem_1", 64, 27));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, fold_w, (size_t)64 * 27 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  const float* ag = yo_param(n, "model.23.anchor_grid", 18);
+  if (!ag) return 1;
+  n->anchor_grid = (float*)take(18 * 4);
+  CFB_CUDA(cudaMemcpyAsync(n->anchor_grid, ag, 18 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaStreamSynchronize(st));
+  n->prepared = true;
+  return 0;
+}
+
+// predictions of an h x w input: 3 anchors per cell of the /8, /16, /32 maps
+static int64_t yo_predictions(int H, int W) {
+  return 3 * ((int64_t)(H / 8) * (W / 8) + (int64_t)(H / 16) * (W / 16) + (int64_t)(H / 32) * (W / 32));
+}
+
+static int yo_forward(cfb_yolov5face* n, const float* x, const unsigned char* img, int ih, int iw, int top, int left, float* pred,
+                      float* const raw[3], int N, int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
+  CFB_REQUIRE(dry || n->prepared, "cfb_yolov5face_prepare has not been called");
+  if (!dry) {
+    int dev = -1;
+    CFB_CUDA(cudaGetDevice(&dev));
+    CFB_REQUIRE(dev == n->device, "YOLOv5-face was prepared on another CUDA device");
+    CFB_CHECK(async_status_check("cfb_yolov5face_forward"));
+  }
+  CFB_REQUIRE(H >= 32 && W >= 32 && H % 32 == 0 && W % 32 == 0 && N >= 0, "YOLOv5-face: H and W must be positive multiples of 32");
+  CFB_REQUIRE(!img || (ih >= 1 && iw >= 1 && top >= 0 && left >= 0 && top + ih <= H && left + iw <= W),
+              "YOLOv5-face: the image must lie inside the letterbox canvas");
+  CFB_REQUIRE(yo_predictions(H, W) * N < ((int64_t)1 << 31) / 16 && (int64_t)H * W <= ((int64_t)1 << 26), "YOLOv5-face: image too large");
+  if (N == 0) return 0;
+  if (n->convs.empty()) yo_build(n);
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  auto alloc = [&](float** p, int h, int w, int c) -> int {
+    *p = (float*)ar.alloc((size_t)N * h * w * c * sizeof(float));
+    CFB_REQUIRE(*p != nullptr, "workspace too small (cfb_yolov5face_workspace_bytes)");
+    return 0;
+  };
+  // one conv: 3x3 stride 1 on the generalised engine (res2: the Bottleneck shortcut), everything else on the per-tap engine
+  auto conv = [&](const std::string& name, const float* in, int h, int w, float* out, int out_pitch, int out_c0, int act,
+                  const float* res2 = nullptr, int res2_pitch = 0) -> int {
+    const YoConv& r = n->convs.at(name);
+    if (r.gen) {
+      GenLaunch g{&r.c, in, r.c.cin_p, h, w, N, out, out_pitch, out_c0, act};
+      g.res2 = res2; g.res2_pitch = res2_pitch;
+      return dry ? 0 : gen_conv(g, n->sm_count, st);
+    }
+    ConvArgs a;
+    a.in = in; a.N = N; a.H = h; a.W = w; a.Cin = r.c.cin_p; a.Cout = r.c.cout_p; a.ksize = r.k;
+    a.Ho = r.stride == 2 ? (h + 1) / 2 : h; a.Wo = r.stride == 2 ? (w + 1) / 2 : w;
+    a.mode = r.stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = r.stride == 2 ? 1 : 0;
+    a.wgt_hi = r.c.w_hi; a.wgt_lo = r.c.w_lo; a.wscale_inv = r.c.wscale + 1; a.bias = r.c.bias;
+    a.out_act = act; a.out = out; a.out_pitch = out_pitch == r.c.cout_p ? 0 : out_pitch; a.out_c0 = out_c0;
+    CFB_REQUIRE(tc_supported(a), "YOLOv5-face: conv not supported by the wgmma engine: " + name);
+    void* scratch = ar.alloc(tc_scratch_bytes(a));
+    CFB_REQUIRE(scratch != nullptr, "workspace too small (cfb_yolov5face_workspace_bytes)");
+    if (!dry) CFB_CHECK(conv_tc(a, scratch, n->sm_count, st));
+    ar.release(scratch);
+    return 0;
+  };
+  // C3 (common.py): cv3(cat(m(cv1(x)), cv2(x))) with the cat as one [2c_] buffer; out: a dense [c2] buffer
+  auto c3 = [&](int i, const float* in, int h, int w, float** out) -> int {
+    const YoC3& b = *std::find_if(std::begin(kYoC3), std::end(kYoC3), [&](const YoC3& e) { return e.i == i; });
+    const std::string p = "model." + std::to_string(i) + ".";
+    const int c_ = b.c2 / 2;
+    float *cat = nullptr, *a = nullptr, *t = nullptr;
+    CFB_CHECK(alloc(&cat, h, w, 2 * c_));
+    CFB_CHECK(conv(p + "cv2", in, h, w, cat, 2 * c_, c_, OUT_SILU));
+    CFB_CHECK(alloc(&a, h, w, c_));
+    CFB_CHECK(conv(p + "cv1", in, h, w, a, c_, 0, OUT_SILU));
+    CFB_CHECK(alloc(&t, h, w, c_));
+    for (int j = 0; j < b.n; ++j) {
+      const std::string m = p + "m." + std::to_string(j) + ".";
+      CFB_CHECK(conv(m + "cv1", a, h, w, t, c_, 0, OUT_SILU));
+      float* dst = nullptr;
+      if (j == b.n - 1) dst = cat;
+      else CFB_CHECK(alloc(&dst, h, w, c_));
+      CFB_CHECK(conv(m + "cv2", t, h, w, dst, j == b.n - 1 ? 2 * c_ : c_, 0, OUT_SILU, b.sc ? a : nullptr, c_));
+      ar.release(a);
+      a = dst;
+    }
+    ar.release(t);
+    CFB_CHECK(alloc(out, h, w, b.c2));
+    CFB_CHECK(conv(p + "cv3", cat, h, w, *out, b.c2, 0, OUT_SILU));
+    ar.release(cat);
+    return 0;
+  };
+  const int H2 = H / 2, W2 = W / 2, H4 = H / 4, W4 = W / 4, H8 = H / 8, W8 = W / 8, H16 = H / 16, W16 = W / 16, H32 = H / 32,
+            W32 = W / 32;
+  // StemBlock
+  float *s1 = nullptr, *t = nullptr, *sc = nullptr, *x0 = nullptr;
+  CFB_CHECK(alloc(&s1, H2, W2, 64));
+  if (!dry) CFB_CHECK(yolo_stem(x, img, n->stem_w, n->stem_b, s1, N, H, W, ih, iw, top, left, st));
+  CFB_CHECK(alloc(&t, H2, W2, 64));
+  CFB_CHECK(conv("model.0.stem_2a", s1, H2, W2, t, 64, 0, OUT_SILU));          // 32 channels + 32 zero channels
+  CFB_CHECK(alloc(&sc, H4, W4, 128));
+  CFB_CHECK(conv("model.0.stem_2b", t, H2, W2, sc, 128, 0, OUT_SILU));
+  ar.release(t);
+  if (!dry) CFB_CHECK(yolo_maxpool2(s1, sc, N, H2, W2, 64, 128, 64, st));
+  ar.release(s1);
+  CFB_CHECK(alloc(&x0, H4, W4, 64));
+  CFB_CHECK(conv("model.0.stem_3", sc, H4, W4, x0, 64, 0, OUT_SILU));
+  ar.release(sc);
+  // backbone
+  float *x1 = nullptr, *x2 = nullptr, *x3 = nullptr, *x4 = nullptr, *x5 = nullptr, *x6 = nullptr, *sp = nullptr, *x7 = nullptr,
+        *x8 = nullptr;
+  CFB_CHECK(c3(1, x0, H4, W4, &x1));
+  ar.release(x0);
+  CFB_CHECK(alloc(&x2, H8, W8, 256));
+  CFB_CHECK(conv("model.2", x1, H4, W4, x2, 256, 0, OUT_SILU));
+  ar.release(x1);
+  CFB_CHECK(c3(3, x2, H8, W8, &x3));
+  ar.release(x2);
+  CFB_CHECK(alloc(&x4, H16, W16, 512));
+  CFB_CHECK(conv("model.4", x3, H8, W8, x4, 512, 0, OUT_SILU));
+  CFB_CHECK(c3(5, x4, H16, W16, &x5));
+  ar.release(x4);
+  CFB_CHECK(alloc(&x6, H32, W32, 1024));
+  CFB_CHECK(conv("model.6", x5, H16, W16, x6, 1024, 0, OUT_SILU));
+  CFB_CHECK(alloc(&sp, H32, W32, 2048));                                   // SPP: [cv1 | mp3 | mp5 | mp7]
+  CFB_CHECK(conv("model.7.cv1", x6, H32, W32, sp, 2048, 0, OUT_SILU));
+  ar.release(x6);
+  if (!dry) CFB_CHECK(yolo_spp(sp, N, H32, W32, 512, st));
+  CFB_CHECK(alloc(&x7, H32, W32, 1024));
+  CFB_CHECK(conv("model.7.cv2", sp, H32, W32, x7, 1024, 0, OUT_SILU));
+  ar.release(sp);
+  CFB_CHECK(c3(8, x7, H32, W32, &x8));
+  ar.release(x7);
+  // head: cat21 = [20 | 9] at /32, cat11 = [up(9) | 5] at /16, cat18 = [17 | 13] at /16, cat15 = [up(13) | 3] at /8
+  float *cat21 = nullptr, *cat11 = nullptr, *cat18 = nullptr, *cat15 = nullptr, *x12 = nullptr, *p3 = nullptr, *p4 = nullptr,
+        *p5 = nullptr;
+  CFB_CHECK(alloc(&cat21, H32, W32, 1024));
+  CFB_CHECK(conv("model.9", x8, H32, W32, cat21, 1024, 512, OUT_SILU));
+  ar.release(x8);
+  CFB_CHECK(alloc(&cat11, H16, W16, 1024));
+  if (!dry) CFB_CHECK(yolo_copy(cat21, 1024, 512, cat11, 1024, 0, N, H32, W32, 512, true, st));
+  if (!dry) CFB_CHECK(yolo_copy(x5, 512, 0, cat11, 1024, 512, N, H16, W16, 512, false, st));
+  ar.release(x5);
+  CFB_CHECK(c3(12, cat11, H16, W16, &x12));
+  ar.release(cat11);
+  CFB_CHECK(alloc(&cat18, H16, W16, 512));
+  CFB_CHECK(conv("model.13", x12, H16, W16, cat18, 512, 256, OUT_SILU));
+  ar.release(x12);
+  CFB_CHECK(alloc(&cat15, H8, W8, 512));
+  if (!dry) CFB_CHECK(yolo_copy(cat18, 512, 256, cat15, 512, 0, N, H16, W16, 256, true, st));
+  if (!dry) CFB_CHECK(yolo_copy(x3, 256, 0, cat15, 512, 256, N, H8, W8, 256, false, st));
+  ar.release(x3);
+  CFB_CHECK(c3(16, cat15, H8, W8, &p3));
+  ar.release(cat15);
+  CFB_CHECK(conv("model.17", p3, H8, W8, cat18, 512, 0, OUT_SILU));
+  CFB_CHECK(c3(19, cat18, H16, W16, &p4));
+  ar.release(cat18);
+  CFB_CHECK(conv("model.20", p4, H16, W16, cat21, 1024, 0, OUT_SILU));
+  CFB_CHECK(c3(22, cat21, H32, W32, &p5));
+  ar.release(cat21);
+  // Detect
+  const float* P[3] = {p3, p4, p5};
+  const int ny[3] = {H8, H16, H32}, nx[3] = {W8, W16, W32};
+  float* hd[3];
+  for (int l = 0; l < 3; ++l) {
+    CFB_CHECK(alloc(&hd[l], ny[l], nx[l], 64));
+    CFB_CHECK(conv("model.23.m." + std::to_string(l), P[l], ny[l], nx[l], hd[l], 64, 0, OUT_NONE));
+  }
+  if (!dry) CFB_CHECK(yolo_decode(hd, raw, ny, nx, n->anchor_grid, pred, N, (int)yo_predictions(H, W), st));
+  for (int l = 0; l < 3; ++l) ar.release(hd[l]);
+  ar.release(p3); ar.release(p4); ar.release(p5);
+  return 0;
+}
+
+}  // namespace cfb
+
+// =========================================================================================================
 // C ABI
 // =========================================================================================================
 #define API_BEGIN try {
@@ -2046,6 +2363,39 @@ int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const floa
   API_END(1)
 }
 
+int cfb_conv2d_pertap_slice_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h,
+                                 int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride, int32_t out_act,
+                                 int32_t out_pitch, int32_t out_c0, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(in && weight_oihw && out && workspace, "cfb_conv2d_pertap_slice_nhwc: NULL argument");
+  CFB_REQUIRE(stride == 1 || stride == 2, "cfb_conv2d_pertap_slice_nhwc: stride must be 1 or 2");
+  CFB_REQUIRE(ksize == 1 || stride == 2, "cfb_conv2d_pertap_slice_nhwc: 3x3 convs run stride 2 on the per-tap engine");
+  CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_SILU, "cfb_conv2d_pertap_slice_nhwc: activation must be none or SiLU");
+  cudaStream_t st = (cudaStream_t)stream;
+  CFB_CHECK(cfb::async_status_init(st));
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  cfb::ConvArgs a;
+  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
+  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
+  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
+  CFB_REQUIRE(cfb::tc_supported(a), "cfb_conv2d_pertap_slice_nhwc: shape not supported by the wgmma engine");
+  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_pertap_workspace_bytes(n, h, w, cin, cout, ksize, stride),
+              "cfb_conv2d_pertap_slice_nhwc: workspace too small");
+  const size_t wn = (size_t)cout * cin * ksize * ksize;
+  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+  __half* whi = (__half*)p; p += align256(wn * 2);
+  __half* wlo = (__half*)p; p += align256(wn * 2);
+  float* wsc = (float*)p; p += 256;
+  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
+  CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, ksize, wsc, st));
+  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.bias = bias; a.out_act = out_act; a.out = out;
+  a.out_pitch = out_pitch == cout ? 0 : out_pitch; a.out_c0 = out_c0;
+  return cfb::conv_tc(a, p, sms, st);
+  API_END(1)
+}
+
 int64_t cfb_conv2d_pertap_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride) {
   if (n < 0 || h < 1 || w < 1 || cin < 1 || cout < 1 || !(ksize == 1 || ksize == 3) || !(stride == 1 || stride == 2)) return -1;
   cfb::ConvArgs a;
@@ -2123,6 +2473,84 @@ int cfb_retinaface_candidates(const float* loc, const float* conf, const float* 
   CFB_REQUIRE(batch == 0 || (loc && conf && landms && rows && counts), "cfb_retinaface_candidates: NULL argument");
   CFB_REQUIRE(h >= 1 && w >= 1 && batch >= 0, "cfb_retinaface_candidates: empty image");
   return cfb::rf_candidates(loc, conf, landms, batch, h, w, conf_threshold, rows, counts, (cudaStream_t)stream);
+  API_END(1)
+}
+
+int64_t cfb_yolov5face_predictions(int32_t h, int32_t w) {
+  return h < 32 || w < 32 || h % 32 || w % 32 ? -1 : cfb::yo_predictions(h, w);
+}
+
+cfb_yolov5face* cfb_yolov5face_create(void) {
+  API_BEGIN
+  cfb_yolov5face* n = new cfb_yolov5face();
+  cfb::yo_build(n);
+  return n;
+  API_END(nullptr)
+}
+void cfb_yolov5face_destroy(cfb_yolov5face* n) {
+  if (!n) return;
+  if (n->slab) {
+    int cur = -1;
+    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
+    if (sw) cudaSetDevice(n->device);
+    cudaFree(n->slab);
+    if (sw) cudaSetDevice(cur);
+  }
+  delete n;
+}
+int cfb_yolov5face_set_param(cfb_yolov5face* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_yolov5face_set_param: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  n->raw[name] = {dev_ptr, numel};
+  n->prepared = false;
+  return 0;
+  API_END(1)
+}
+int cfb_yolov5face_prepare(cfb_yolov5face* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_yolov5face_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::yo_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_yolov5face_workspace_bytes(cfb_yolov5face* n, int32_t batch, int32_t h, int32_t w) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_yolov5face_workspace_bytes: NULL net"); return -1; }
+  std::lock_guard<std::mutex> lk(n->mu);
+  float* const raw[3] = {nullptr, nullptr, nullptr};
+  if (cfb::yo_forward(n, (const float*)0x1000, nullptr, 0, 0, 0, 0, nullptr, raw, batch, h, w, nullptr, 0, nullptr, true) != 0) return -1;
+  return (int64_t)n->arena.high() + 4096;
+  API_END(-1)
+}
+int cfb_yolov5face_forward(cfb_yolov5face* n, const float* x_nchw, float* pred, float* raw0, float* raw1, float* raw2, int32_t batch,
+                           int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (x_nchw && pred && workspace)), "cfb_yolov5face_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  float* const raw[3] = {raw0, raw1, raw2};
+  return cfb::yo_forward(n, x_nchw, nullptr, 0, 0, 0, 0, pred, raw, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream,
+                         false);
+  API_END(1)
+}
+int cfb_yolov5face_forward_u8(cfb_yolov5face* n, const uint8_t* img_bgr_hwc, int32_t img_h, int32_t img_w, int32_t top, int32_t left,
+                              float* pred, float* raw0, float* raw1, float* raw2, int32_t batch, int32_t h, int32_t w,
+                              void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (img_bgr_hwc && pred && workspace)), "cfb_yolov5face_forward_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  float* const raw[3] = {raw0, raw1, raw2};
+  return cfb::yo_forward(n, nullptr, img_bgr_hwc, img_h, img_w, top, left, pred, raw, batch, h, w, workspace, workspace_bytes,
+                         (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_yolov5face_candidates(const float* pred, int32_t batch, int32_t h, int32_t w, float conf_threshold, float* rows,
+                              int32_t* counts, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(batch == 0 || (pred && rows && counts), "cfb_yolov5face_candidates: NULL argument");
+  const int64_t P = cfb_yolov5face_predictions(h, w);
+  CFB_REQUIRE(P > 0 && batch >= 0 && P * batch < ((int64_t)1 << 31) / 16, "cfb_yolov5face_candidates: bad size");
+  return cfb::yolo_candidates(pred, batch, (int)P, conf_threshold, rows, counts, (cudaStream_t)stream);
   API_END(1)
 }
 

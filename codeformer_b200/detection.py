@@ -293,10 +293,18 @@ class RetinaFace(nn.Module):
 
 
 def init_detection_model(model_name='retinaface_resnet50', half=False, device='cuda', model_path=None):
-    """``facelib.detection.init_detection_model`` (facelib/detection/__init__.py:13-44) without the download: pass the
-    checkpoint path (``detection_Resnet50_Final.pth``) or load the state dict yourself.  ``module.`` prefixes are stripped."""
+    """``facelib.detection.init_detection_model`` (facelib/detection/__init__.py:13-71) without the download: pass the
+    checkpoint path (``detection_Resnet50_Final.pth`` / ``yolov5l-face.pth``) or load the state dict yourself.
+    RetinaFace: ``module.`` prefixes are stripped.  YOLOv5l: a ``YoloDetector`` whose ``.detector`` loads strictly, as is."""
+    if model_name == 'YOLOv5l':
+        from .yolov5face import YoloDetector
+        model = YoloDetector(config_name='facelib/detection/yolov5face/models/yolov5l.yaml', device=device)
+        if model_path is not None:
+            model.detector.load_state_dict(torch.load(model_path, map_location='cpu'), strict=True)
+        model.detector = model.detector.eval().to(device)
+        return model
     if model_name != 'retinaface_resnet50':
-        raise NotImplementedError(f'{model_name} is not built (codeformer_b200 builds retinaface_resnet50)')
+        raise NotImplementedError(f'{model_name} is not built (codeformer_b200 builds retinaface_resnet50 and YOLOv5l)')
     model = RetinaFace(network_name='resnet50', half=half)
     if model_path is not None:
         load_net = torch.load(model_path, map_location='cpu')

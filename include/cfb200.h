@@ -235,7 +235,8 @@ int       cfb_parse_argmax(const float* logits_nchw, uint8_t* classes, uint8_t* 
  * in: NHWC buffer of in_pitch channels per pixel, channels [0, cin) are read; any h x w.  upsample != 0: nearest x2 first.
  * pad_mode 0 zero / 1 reflect / 2 replicate (of the low-resolution tensor when upsampling).  subsample != 0: stride 2 (the
  * even output positions of the stride-1 result; h, w even).  out: NHWC buffer of out_pitch channels, the cout real channels
- * go to [out_c0, out_c0 + cout).  out = lrelu?(conv + bias + residual) * post_scale + residual2 (post only with residual2). */
+ * go to [out_c0, out_c0 + cout).  out = act(conv + bias + residual) * post_scale + residual2 (post only with residual2);
+ * out_act 0 none / 1 LeakyReLU(0.2) / 3 ReLU / 4 SiLU. */
 int64_t cfb_conv2d_gen_workspace_bytes(int32_t cin, int32_t cout);
 int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_oihw, const float* bias, float* out,
                         int32_t out_pitch, int32_t out_c0, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout,
@@ -250,6 +251,13 @@ int64_t cfb_conv2d_pertap_workspace_bytes(int32_t n, int32_t h, int32_t w, int32
 int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h, int32_t w,
                            int32_t cin, int32_t cout, int32_t ksize, int32_t stride, int32_t out_act, const float* residual,
                            void* workspace, int64_t workspace_bytes, void* stream);
+
+/* The same per-tap engine with the YOLOv5 epilogue (test entry point): 1x1 (stride 1 or 2) or 3x3 stride-2 pad-1 conv,
+ * out_act 0 none / 4 SiLU, written into channels [out_c0, out_c0 + cout) of an NHWC buffer with out_pitch channels per pixel
+ * (multiples of 4); the other channels are left as they are.  Workspace: cfb_conv2d_pertap_workspace_bytes. */
+int cfb_conv2d_pertap_slice_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h,
+                                 int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride, int32_t out_act,
+                                 int32_t out_pitch, int32_t out_c0, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- RetinaFace-ResNet50 face detector (facelib/detection/retinaface; detection.cu + the conv engine) ----
  * Parameters by the reference's state-dict names (BatchNorm folded at prepare).  forward: x fp32 NCHW [batch,3,h,w] (the
@@ -270,6 +278,30 @@ int       cfb_retinaface_forward_u8(cfb_retinaface* net, const uint8_t* img_bgr_
                                     int32_t batch, int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
 int       cfb_retinaface_candidates(const float* loc, const float* conf, const float* landms, int32_t batch, int32_t h, int32_t w,
                                     float conf_threshold, float* rows, int32_t* counts, void* stream);
+
+/* ---- YOLOv5l-face detector (facelib/detection/yolov5face, models/yolov5l.yaml; yolo.cu + the conv engine) ----
+ * Parameters by the reference's state-dict names (BatchNorm folded at prepare; the Detect anchor_grid buffer gives the anchor
+ * sizes in pixels).  h and w are multiples of 32; P = cfb_yolov5face_predictions(h, w) = 3 (hw/64 + hw/256 + hw/1024).
+ * forward: x fp32 NCHW [batch,3,h,w] (RGB / 255) -> pred [batch,P,16] (Detect's decoded output, rows ordered by level, anchor,
+ * y, x) and, where not NULL, the raw head outputs raw_l [batch,3,h/s_l,w/s_l,16] for s_l = 8, 16, 32.
+ * forward_u8: uint8 HWC BGR images [batch,img_h,img_w,3] placed at (top, left) of the h x w letterbox canvas, whose other
+ * pixels are 114; the BGR -> RGB swap and the / 255 are fused (the result equals forward on that canvas bit for bit).
+ * candidates: per image, the pred rows whose objectness (field 4) is > conf_threshold, in prediction order, into rows
+ * [batch,P,16]; counts [batch] (device int32). */
+typedef struct cfb_yolov5face cfb_yolov5face;
+int64_t         cfb_yolov5face_predictions(int32_t h, int32_t w);
+cfb_yolov5face* cfb_yolov5face_create(void);
+void            cfb_yolov5face_destroy(cfb_yolov5face* net);
+int             cfb_yolov5face_set_param(cfb_yolov5face* net, const char* name, const float* dev_ptr, int64_t numel);
+int             cfb_yolov5face_prepare(cfb_yolov5face* net, void* stream);
+int64_t         cfb_yolov5face_workspace_bytes(cfb_yolov5face* net, int32_t batch, int32_t h, int32_t w);
+int             cfb_yolov5face_forward(cfb_yolov5face* net, const float* x_nchw, float* pred, float* raw0, float* raw1, float* raw2,
+                                       int32_t batch, int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int             cfb_yolov5face_forward_u8(cfb_yolov5face* net, const uint8_t* img_bgr_hwc, int32_t img_h, int32_t img_w, int32_t top,
+                                          int32_t left, float* pred, float* raw0, float* raw1, float* raw2, int32_t batch, int32_t h,
+                                          int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int             cfb_yolov5face_candidates(const float* pred, int32_t batch, int32_t h, int32_t w, float conf_threshold, float* rows,
+                                          int32_t* counts, void* stream);
 
 /* Asynchronous failures.  Kernels never trap and never leave a sticky CUDA error behind (the reference's callers catch
  * RuntimeError and fall back to the input face, inference_codeformer.py:209-211; web-demos/hugging_face/app.py:176): a
