@@ -29,6 +29,7 @@ from torch import nn
 
 from . import _lib
 from . import spec as S
+from .native import upload_params
 from .registry import ARCH_REGISTRY
 
 
@@ -349,15 +350,7 @@ class VQAutoEncoder(nn.Module):
                 _lib.check(1, 'cfb_net_create')
             object.__setattr__(self, '_cfb_net', ctypes.c_void_p(h))
             _lib.check(lib.cfb_net_set_engine(self._cfb_net, getattr(self, '_cfb_engine', 0)), 'cfb_net_set_engine')
-        keep = []
-        for k, v in params:
-            if v.device != device:
-                raise RuntimeError(f'parameter {k} is on {v.device} but the input is on {device}; call net.to(device)')
-            t = v.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            keep.append(t)
-            _lib.check(lib.cfb_net_set_param(self._cfb_net, k.encode(), _lib.ptr(t), t.numel()), 'cfb_net_set_param')
+        keep = upload_params(lib, 'net', self._cfb_net, params, device)
         _lib.check(lib.cfb_net_prepare(self._cfb_net, _stream_ptr(device)), 'cfb_net_prepare')
         object.__setattr__(self, '_cfb_sig', sig)
         self._cfb_graphs.clear()                       # captured launch sequences bake in the old weight copies

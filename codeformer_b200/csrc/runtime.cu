@@ -139,6 +139,106 @@ class Arena {
   std::map<size_t, size_t> free_, used_;
 };
 
+// ---- what every network handle shares ----------------------------------------------------------------
+// The parameters the caller registered (device pointers it keeps alive), the slab with the prepared weights on the device
+// that was current at prepare time, and the workspace arena.  `label` names the network in error messages, `api` is the
+// infix of its C functions (cfb_<api>_prepare, ...).
+struct NetCore {
+  std::mutex mu;
+  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
+  float* slab = nullptr;
+  size_t slab_bytes = 0;
+  int device = -1;                    // CUDA device the slab / prepared weights live on
+  int sm_count = 148;
+  bool prepared = false;
+  Arena arena;
+  const char* label;
+  const char* api;
+
+  NetCore(const char* label_, const char* api_) : label(label_), api(api_) {}
+  ~NetCore() { release_slab(); }
+
+  int set_param(const char* name, const float* dev_ptr, int64_t numel) {
+    std::lock_guard<std::mutex> lk(mu);
+    raw[name] = {dev_ptr, numel};
+    prepared = false;
+    return 0;
+  }
+
+  const float* param(const std::string& name, int64_t numel) const {
+    auto it = raw.find(name);
+    if (it == raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
+    if (it->second.second != numel) {
+      set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " +
+                std::to_string(numel));
+      return nullptr;
+    }
+    return it->second.first;
+  }
+
+  // a slab of at least `bytes` on the current device: the net follows the device that is current at prepare time
+  // (net.to(other_gpu) -> a new prepare), so a slab on another device is freed there first
+  int reserve_slab(size_t bytes) {
+    int dev = 0;
+    CFB_CUDA(cudaGetDevice(&dev));
+    if (slab && (device != dev || slab_bytes < bytes)) {
+      if (device != dev && device >= 0) { cudaSetDevice(device); cudaFree(slab); cudaSetDevice(dev); }
+      else cudaFree(slab);
+      slab = nullptr; slab_bytes = 0;
+    }
+    if (!slab) { CFB_CUDA(cudaMalloc((void**)&slab, bytes)); slab_bytes = bytes; }
+    device = dev;
+    return 0;
+  }
+
+  void release_slab() {
+    if (!slab) return;
+    int cur = -1;
+    const bool sw = cudaGetDevice(&cur) == cudaSuccess && device >= 0 && cur != device;
+    if (sw) cudaSetDevice(device);
+    cudaFree(slab);
+    if (sw) cudaSetDevice(cur);
+    slab = nullptr; slab_bytes = 0;
+  }
+
+  // the networks that have only the wgmma path: device check, SM count, the device's status word
+  int begin_prepare(cudaStream_t st) {
+    int dev = 0, major = 0, sms = 148;
+    CFB_CUDA(cudaGetDevice(&dev));
+    CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+    CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    CFB_REQUIRE(major == 9, std::string(label) + ": the wgmma engine needs an sm_90 device (there is no other path)");
+    CFB_CHECK(async_status_init(st));
+    sm_count = sms > 0 ? sms : 148;
+    return 0;
+  }
+
+  // a dry run (workspace sizing) needs neither prepared weights nor a device
+  int begin_forward(bool dry) {
+    CFB_REQUIRE(dry || prepared, "cfb_" + std::string(api) + "_prepare has not been called");
+    if (dry) return 0;
+    int dev = -1;
+    CFB_CUDA(cudaGetDevice(&dev));
+    CFB_REQUIRE(dev == device, std::string(label) + " was prepared on another CUDA device");
+    return async_status_check(("cfb_" + std::string(api) + "_forward").c_str());
+  }
+
+  std::string ws_error() const { return "workspace too small (cfb_" + std::string(api) + "_workspace_bytes)"; }
+
+  int alloc(float** p, size_t elems) {
+    *p = (float*)arena.alloc(elems * sizeof(float));
+    CFB_REQUIRE(*p != nullptr, ws_error());
+    return 0;
+  }
+
+  // host-only dry run of a forward: the arena's high-water mark is the workspace it needs
+  template <class F> int64_t dry_run(F&& forward) {
+    std::lock_guard<std::mutex> lk(mu);
+    if (forward() != 0) return -1;
+    return (int64_t)arena.high() + 4096;
+  }
+};
+
 struct Tensor {
   float* p = nullptr;
   int N = 0, H = 0, W = 0, C = 0;
@@ -181,10 +281,9 @@ using namespace cfb;
 
 constexpr int GN_COUNTERS = 1 << 16;
 
-struct cfb_net {
+struct cfb_net : cfb::NetCore {
+  cfb_net() : NetCore("CodeFormer", "net") {}
   cfb_config cfg;
-  std::mutex mu;
-  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
   std::vector<Block> enc, gen;
   std::map<int, FuseW> fuse;          // keyed by feature size
   std::vector<LayerW> layers;
@@ -193,13 +292,8 @@ struct cfb_net {
   NormW idx_norm;
   const float* position_emb = nullptr;
   const float* codebook = nullptr;    // points into slab copy
-  float* slab = nullptr;
-  size_t slab_bytes = 0;
-  bool prepared = false;
   int64_t last_launches = 0;
-  int sm_count = 148;
   bool tc_ok = false;                 // device is sm_90 => wgmma engine usable
-  Arena arena;
   cudaStream_t st = nullptr;
   // small owned copies of norm params etc. live in the slab too
   std::vector<std::pair<const float**, std::pair<std::string, int64_t>>> vec_params;  // (dst, (name, numel))
@@ -207,7 +301,6 @@ struct cfb_net {
   float* mha_consts = nullptr;        // device: [0] = head_dim^-1/2, [1] = 1
   unsigned* gn_counters = nullptr;    // ticket-counter ring of the split GroupNorm finalize (in the slab, zero between uses)
   int gn_ctr_pos = 0;
-  int device = -1;                    // CUDA device the slab / prepared weights live on
   std::map<int, int64_t> ws_memo;     // batch -> cfb_workspace_bytes (16 host-side dry runs per miss)
   int engine = 0;                     // 0 auto (wgmma where the shape allows), 1 fp32 CUDA cores, 2 wgmma only
   std::map<std::string, std::pair<float*, int64_t>> captures;   // stage name -> (device dst, capacity in floats)
@@ -342,17 +435,6 @@ static int build_plan(cfb_net* n) {
 }
 
 // ---- weight preparation --------------------------------------------------------------------------------
-static const float* find_param(cfb_net* n, const std::string& name, int64_t numel) {
-  auto it = n->raw.find(name);
-  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
-  if (it->second.second != numel) {
-    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " +
-              std::to_string(numel));
-    return nullptr;
-  }
-  return it->second.first;
-}
-
 static int resolve_conv_sources(cfb_net* n, ConvW& c, float* qkv_scratch_w, float* qkv_scratch_b, cudaStream_t st) {
   const int64_t wn = (int64_t)c.cout * c.cin * c.k * c.k;
   const size_t hash = c.name.find('#');
@@ -362,8 +444,8 @@ static int resolve_conv_sources(cfb_net* n, ConvW& c, float* qkv_scratch_w, floa
     const int C = c.cin;
     const char* nm[3] = {".q", ".k", ".v"};
     for (int i = 0; i < 3; ++i) {
-      const float* w = find_param(n, p + nm[i] + ".weight", (int64_t)C * C);
-      const float* b = find_param(n, p + nm[i] + ".bias", C);
+      const float* w = n->param(p + nm[i] + ".weight", (int64_t)C * C);
+      const float* b = n->param(p + nm[i] + ".bias", C);
       if (!w || !b) return 1;
       CFB_CUDA(cudaMemcpyAsync(qkv_scratch_w + (int64_t)i * C * C, w, (size_t)C * C * 4, cudaMemcpyDeviceToDevice, st));
       CFB_CUDA(cudaMemcpyAsync(qkv_scratch_b + (int64_t)i * C, b, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
@@ -376,16 +458,16 @@ static int resolve_conv_sources(cfb_net* n, ConvW& c, float* qkv_scratch_w, floa
     const std::string base = c.name.substr(0, hash);
     const std::string part = c.name.substr(hash + 1);
     const int E = c.cin;
-    const float* w = find_param(n, base + "_weight", (int64_t)3 * E * E);
-    const float* b = find_param(n, base + "_bias", (int64_t)3 * E);
+    const float* w = n->param(base + "_weight", (int64_t)3 * E * E);
+    const float* b = n->param(base + "_bias", (int64_t)3 * E);
     if (!w || !b) return 1;
     const int row0 = part == "qk" ? 0 : 2 * E;
     c.src_w = w + (int64_t)row0 * E; c.src_b = b + row0;
     return 0;
   }
-  c.src_w = find_param(n, c.name + ".weight", wn);
+  c.src_w = n->param(c.name + ".weight", wn);
   if (!c.src_w) return 1;
-  if (c.has_bias) { c.src_b = find_param(n, c.name + ".bias", c.cout); if (!c.src_b) return 1; }
+  if (c.has_bias) { c.src_b = n->param(c.name + ".bias", c.cout); if (!c.src_b) return 1; }
   return 0;
 }
 
@@ -412,21 +494,7 @@ static int prepare(cfb_net* n, cudaStream_t st) {
   CFB_CUDA(cudaGetDevice(&dev));
   CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
-    if (n->device != dev && n->device >= 0) {
-      cudaSetDevice(n->device);
-      cudaFree(n->slab);
-      cudaSetDevice(dev);
-    } else {
-      cudaFree(n->slab);
-    }
-    n->slab = nullptr; n->slab_bytes = 0;
-  }
-  if (!n->slab) {
-    CFB_CUDA(cudaMalloc((void**)&n->slab, total));
-    n->slab_bytes = total;
-  }
-  n->device = dev;
+  CFB_CHECK(n->reserve_slab(total));
   n->sm_count = sms > 0 ? sms : 148;
   n->tc_ok = (major == 9);
   n->ws_memo.clear();
@@ -465,7 +533,7 @@ static int prepare(cfb_net* n, cudaStream_t st) {
     else CFB_CUDA(cudaMemsetAsync(c->bias, 0, (size_t)c->cout * 4, st));
   }
   for (auto& v : n->vec_params) {
-    const float* src = find_param(n, v.second.first, v.second.second);
+    const float* src = n->param(v.second.first, v.second.second);
     if (!src) return 1;
     float* dst = (float*)take((size_t)v.second.second * 4);
     CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)v.second.second * 4, cudaMemcpyDeviceToDevice, st));
@@ -473,7 +541,7 @@ static int prepare(cfb_net* n, cudaStream_t st) {
   }
   {
     const int64_t ne = (int64_t)n->cfg.codebook_size * n->cfg.emb_dim;
-    const float* src = find_param(n, "quantize.embedding.weight", ne);
+    const float* src = n->param("quantize.embedding.weight", ne);
     if (!src) return 1;
     float* dst = (float*)take((size_t)ne * 4);
     CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)ne * 4, cudaMemcpyDeviceToDevice, st));
@@ -481,7 +549,7 @@ static int prepare(cfb_net* n, cudaStream_t st) {
   }
   if (n->cfg.kind == 1) {
     const int64_t ne = (int64_t)n->cfg.latent_size * n->cfg.dim_embd;
-    const float* src = find_param(n, "position_emb", ne);
+    const float* src = n->param("position_emb", ne);
     if (!src) return 1;
     float* dst = (float*)take((size_t)ne * 4);
     CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)ne * 4, cudaMemcpyDeviceToDevice, st));
@@ -1104,48 +1172,55 @@ static int vqae_forward_impl(cfb_net* n, const float* x, float* out, int64_t* id
 // block's buffer, and the third block of an RRDB also applies `*0.2 + x_rrdb` in the same epilogue.
 // =========================================================================================================
 namespace cfb {
+// One conv of the plan of a network on the wgmma engines (RRDBNet, ParseNet, RetinaFace, YOLOv5-face).  The split weights
+// are zero-padded to 64-aligned channel counts; the per-tap engine and the generalised halo engine both read those.
 struct GenConv {
   std::string name;
   int cin = 0, cout = 0;            // real sizes
   int cin_p = 0, cout_p = 0;        // 64-aligned sizes of the split weights
+  int k = 3, stride = 1;
+  bool gen = true;                  // generalised halo engine (3x3 stride 1); otherwise the per-tap engine
+  std::string bn;                   // detectors: prefix of the BatchNorm folded into the weights ("": none)
   float out_scale = 1.f;            // constant folded into 2^-k and the bias
   bool up = false;                  // nearest x2 + conv (four parity convs)
   __half* w_hi = nullptr; __half* w_lo = nullptr; float* bias = nullptr; float* wscale = nullptr;
 };
-}  // namespace cfb
 
-struct cfb_rrdb {
-  int in_ch = 3, out_ch = 3, scale = 4, feat = 64, blocks = 23, grow = 32;
-  std::mutex mu;
-  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
-  std::vector<cfb::GenConv> convs;      // [blocks*15] dense convs, then conv_body, conv_up1, conv_up2, conv_hr
-  float* first_w = nullptr; float* first_b = nullptr;   // conv_first  [tap][cin][64]
-  float* last_w = nullptr; float* last_b = nullptr;     // conv_last   [tap][64][4]
-  float* slab = nullptr; size_t slab_bytes = 0;
-  int device = -1, sm_count = 148;
-  bool prepared = false;
-};
-
-namespace cfb {
-
-static const float* rrdb_param(cfb_rrdb* n, const std::string& name, int64_t numel) {
-  auto it = n->raw.find(name);
-  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
-  if (it->second.second != numel) {
-    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
-    return nullptr;
-  }
-  return it->second.first;
+static GenConv plan_conv(const std::string& name, int cin, int cout, int k = 3, int stride = 1) {
+  GenConv c;
+  c.name = name; c.cin = cin; c.cout = cout; c.k = k; c.stride = stride; c.gen = k == 3 && stride == 1;
+  c.cin_p = (cin + 63) / 64 * 64; c.cout_p = (cout + 63) / 64 * 64;
+  return c;
 }
 
-// zero-padded OIHW copy [cout_p][cin_p][3][3] of a [cout][cin][3][3] weight, then the fp16 hi/lo split of the engine
-static int gen_conv_prepare(GenConv& c, const float* w, const float* b, float* pad_scratch, cudaStream_t st) {
-  const size_t padn = (size_t)c.cout_p * c.cin_p * 9;
-  CFB_CUDA(cudaMemsetAsync(pad_scratch, 0, padn * 4, st));
-  CFB_CUDA(cudaMemcpy2DAsync(pad_scratch, (size_t)c.cin_p * 9 * 4, w, (size_t)c.cin * 9 * 4, (size_t)c.cin * 9 * 4, c.cout,
+// slab space of the planned convs: their split weights, the largest zero-padded fp32 weight (the size of the pad and the
+// BatchNorm-fold scratch) and the widest output (the folded-bias scratch)
+struct SlabPlan {
+  size_t convs = 0, padmax = 0;
+  int cout_max = 0;
+  void add(const GenConv& c) {
+    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : c.k * c.k);
+    convs += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
+    padmax = std::max(padmax, (size_t)c.cout_p * c.cin_p * c.k * c.k * 4);
+    cout_max = std::max(cout_max, c.cout_p);
+  }
+  size_t bytes() const { return convs + 2 * align256(padmax) + align256((size_t)cout_max * 4); }
+};
+
+// The split weights of one conv, carved from `p`: zero-pad the [cout][cin][k][k] fp32 weight to [cout_p][cin_p][k][k], split
+// it into the engine's fp16 hi/lo planes (the four parity 2x2 sets for `up`), copy the bias (b == null: zero) and fold
+// out_scale into 2^-k and the bias.
+static int prepare_conv(GenConv& c, const float* w, const float* b, float* pad, char*& p, cudaStream_t st) {
+  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
+  const int taps = c.k * c.k;
+  const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : taps);
+  c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
+  c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
+  CFB_CUDA(cudaMemsetAsync(pad, 0, (size_t)c.cout_p * c.cin_p * taps * 4, st));
+  CFB_CUDA(cudaMemcpy2DAsync(pad, (size_t)c.cin_p * taps * 4, w, (size_t)c.cin * taps * 4, (size_t)c.cin * taps * 4, c.cout,
                              cudaMemcpyDeviceToDevice, st));
-  if (c.up) CFB_CHECK(tc_split_weights_up4(pad_scratch, c.w_hi, c.w_lo, c.cout_p, c.cin_p, c.wscale, st));
-  else CFB_CHECK(tc_split_weights(pad_scratch, c.w_hi, c.w_lo, c.cout_p, c.cin_p, 3, c.wscale, st));
+  if (c.up) CFB_CHECK(tc_split_weights_up4(pad, c.w_hi, c.w_lo, c.cout_p, c.cin_p, c.wscale, st));
+  else CFB_CHECK(tc_split_weights(pad, c.w_hi, c.w_lo, c.cout_p, c.cin_p, c.k, c.wscale, st));
   CFB_CUDA(cudaMemsetAsync(c.bias, 0, (size_t)c.cout_p * 4, st));
   if (b) CFB_CUDA(cudaMemcpyAsync(c.bias, b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
   if (c.out_scale != 1.f) {
@@ -1155,69 +1230,81 @@ static int gen_conv_prepare(GenConv& c, const float* w, const float* b, float* p
   return 0;
 }
 
+// The slab of one prepare call, carved in order; it starts with the scratch of the weight preparation.
+struct WeightPrep {
+  NetCore& net;
+  cudaStream_t st;
+  char* p;
+  float *pad, *fold_w, *fold_b;
+  WeightPrep(NetCore& n, const SlabPlan& plan, cudaStream_t s) : net(n), st(s), p((char*)n.slab) {
+    pad = (float*)take(plan.padmax);
+    fold_w = (float*)take(plan.padmax);
+    fold_b = (float*)take((size_t)plan.cout_max * 4);
+  }
+  char* take(size_t bytes) { char* r = p; p += align256(bytes); return r; }
+  // eval-mode BatchNorm `bn` (weight, bias, running_mean, running_var) folded into the conv weight `w_name` -> fold_w, fold_b
+  int fold(const std::string& w_name, const std::string& bn, int cout, int per_out) {
+    const float* w = net.param(w_name, (int64_t)cout * per_out);
+    const float* g = net.param(bn + "weight", cout);
+    const float* be = net.param(bn + "bias", cout);
+    const float* mu = net.param(bn + "running_mean", cout);
+    const float* var = net.param(bn + "running_var", cout);
+    if (!w || !g || !be || !mu || !var) return 1;
+    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
+  }
+  int conv(GenConv& c, const float* w, const float* b) { return prepare_conv(c, w, b, pad, p, st); }
+};
+}  // namespace cfb
+
+struct cfb_rrdb : cfb::NetCore {
+  cfb_rrdb() : NetCore("RRDBNet", "rrdb") {}
+  int in_ch = 3, out_ch = 3, scale = 4, feat = 64, blocks = 23, grow = 32;
+  std::vector<cfb::GenConv> convs;      // [blocks*15] dense convs, then conv_body, conv_up1, conv_up2, conv_hr
+  float* first_w = nullptr; float* first_b = nullptr;   // conv_first  [tap][cin][64]
+  float* last_w = nullptr; float* last_b = nullptr;     // conv_last   [tap][64][4]
+};
+
+namespace cfb {
+
 static int rrdb_prepare(cfb_rrdb* n, cudaStream_t st) {
-  int dev = 0, major = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CFB_REQUIRE(major == 9, "RRDBNet: the wgmma engine needs an sm_90 device (there is no other path)");
-  CFB_CHECK(async_status_init(st));
+  CFB_CHECK(n->begin_prepare(st));
   n->convs.clear();
   const int us = n->scale == 2 ? 2 : (n->scale == 1 ? 4 : 1);
   const int cin_first = n->in_ch * us * us;
   for (int b = 0; b < n->blocks; ++b)
     for (int r = 1; r <= 3; ++r)
       for (int k = 1; k <= 5; ++k) {
-        GenConv c;
-        c.name = "body." + std::to_string(b) + ".rdb" + std::to_string(r) + ".conv" + std::to_string(k);
-        c.cin = n->feat + (k - 1) * n->grow; c.cout = k == 5 ? n->feat : n->grow;
-        c.out_scale = k == 5 ? 0.2f : 1.f;
-        n->convs.push_back(c);
+        const std::string nm = "body." + std::to_string(b) + ".rdb" + std::to_string(r) + ".conv" + std::to_string(k);
+        n->convs.push_back(plan_conv(nm, n->feat + (k - 1) * n->grow, k == 5 ? n->feat : n->grow));
+        n->convs.back().out_scale = k == 5 ? 0.2f : 1.f;
       }
-  for (const char* nm : {"conv_body", "conv_up1", "conv_up2", "conv_hr"}) {
-    GenConv c; c.name = nm; c.cin = n->feat; c.cout = n->feat; c.up = (c.name == "conv_up1" || c.name == "conv_up2");
-    n->convs.push_back(c);
+  for (const std::string nm : {"conv_body", "conv_up1", "conv_up2", "conv_hr"}) {
+    n->convs.push_back(plan_conv(nm, n->feat, n->feat));
+    n->convs.back().up = nm == "conv_up1" || nm == "conv_up2";
   }
-  size_t total = 0, padmax = 0;
+  SlabPlan plan;
+  for (const GenConv& c : n->convs) plan.add(c);
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256((size_t)9 * cin_first * 64 * 4) + 256 + align256((size_t)9 * 64 * 4 * 4) + 256));
+  WeightPrep wp(*n, plan, st);
   for (GenConv& c : n->convs) {
-    c.cin_p = (c.cin + 63) / 64 * 64; c.cout_p = (c.cout + 63) / 64 * 64;
-    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : 9);
-    total += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
-    padmax = std::max(padmax, (size_t)c.cout_p * c.cin_p * 9 * 4);
-  }
-  total += align256(padmax) + align256((size_t)9 * cin_first * 64 * 4) + 256 + align256((size_t)9 * 64 * 4 * 4) + 256;
-  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
-    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
-    else cudaFree(n->slab);
-    n->slab = nullptr; n->slab_bytes = 0;
-  }
-  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
-  n->device = dev; n->sm_count = sms;
-  char* p = (char*)n->slab;
-  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  float* pad_scratch = (float*)take(padmax);
-  for (GenConv& c : n->convs) {
-    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : 9);
-    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
-    c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
-    const float* w = rrdb_param(n, c.name + ".weight", (int64_t)c.cout * c.cin * 9);
-    const float* b = rrdb_param(n, c.name + ".bias", c.cout);
+    const float* w = n->param(c.name + ".weight", (int64_t)c.cout * c.cin * 9);
+    const float* b = n->param(c.name + ".bias", c.cout);
     if (!w || !b) return 1;
-    CFB_CHECK(gen_conv_prepare(c, w, b, pad_scratch, st));
+    CFB_CHECK(wp.conv(c, w, b));
   }
   {
-    const float* w = rrdb_param(n, "conv_first.weight", (int64_t)n->feat * cin_first * 9);
-    const float* b = rrdb_param(n, "conv_first.bias", n->feat);
+    const float* w = n->param("conv_first.weight", (int64_t)n->feat * cin_first * 9);
+    const float* b = n->param("conv_first.bias", n->feat);
     if (!w || !b) return 1;
-    n->first_w = (float*)take((size_t)9 * cin_first * 64 * 4); n->first_b = (float*)take(256);
+    n->first_w = (float*)wp.take((size_t)9 * cin_first * 64 * 4); n->first_b = (float*)wp.take(256);
     CFB_CHECK(relayout_oihw_to_tck(w, n->first_w, n->feat, cin_first, 3, st));
     CFB_CUDA(cudaMemcpyAsync(n->first_b, b, (size_t)n->feat * 4, cudaMemcpyDeviceToDevice, st));
   }
   {
-    const float* w = rrdb_param(n, "conv_last.weight", (int64_t)n->out_ch * n->feat * 9);
-    const float* b = rrdb_param(n, "conv_last.bias", n->out_ch);
+    const float* w = n->param("conv_last.weight", (int64_t)n->out_ch * n->feat * 9);
+    const float* b = n->param("conv_last.bias", n->out_ch);
     if (!w || !b) return 1;
-    n->last_w = (float*)take((size_t)9 * 64 * 4 * 4); n->last_b = (float*)take(256);
+    n->last_w = (float*)wp.take((size_t)9 * 64 * 4 * 4); n->last_b = (float*)wp.take(256);
     CFB_CHECK(relayout_thin_out(w, n->last_w, n->out_ch, st));
     CFB_CUDA(cudaMemcpyAsync(n->last_b, b, (size_t)n->out_ch * 4, cudaMemcpyDeviceToDevice, st));
   }
@@ -1246,6 +1333,30 @@ static int gen_conv(const GenLaunch& g, int sm_count, cudaStream_t st) {
   return conv_tc(a, nullptr, sm_count, st);
 }
 
+// A conv on the per-tap engine, weights not set: 1x1 or 3x3, stride 1 or 2 (only the ceil(H/2) x ceil(W/2) outputs; 3x3 pads
+// by 1), written at channel out_c0 of a destination with out_pitch channels per pixel (out_pitch == cout: a dense output).
+static ConvArgs pertap_args(const float* in, int N, int h, int w, int cin, int cout, int k, int stride, float* out, int out_pitch,
+                            int out_c0, int act, const float* res) {
+  ConvArgs a;
+  a.in = in; a.N = N; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = k;
+  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
+  a.mode = stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = (stride == 2 && k == 3) ? 1 : 0;
+  a.residual = res; a.out_act = act; a.out = out;
+  a.out_pitch = out_pitch == cout ? 0 : out_pitch; a.out_c0 = out_c0;
+  return a;
+}
+
+// A planned conv of a network forward on the per-tap engine: its operand planes live in the arena until the launch is enqueued.
+static int pertap_conv(NetCore& n, ConvArgs a, const GenConv& c, bool dry, cudaStream_t st) {
+  a.wgt_hi = c.w_hi; a.wgt_lo = c.w_lo; a.wscale_inv = c.wscale + 1; a.bias = c.bias;
+  CFB_REQUIRE(tc_supported(a), std::string(n.label) + ": conv not supported by the wgmma engine: " + c.name);
+  void* scratch = n.arena.alloc(tc_scratch_bytes(a));
+  CFB_REQUIRE(scratch != nullptr, n.ws_error());
+  if (!dry) CFB_CHECK(conv_tc(a, scratch, n.sm_count, st));
+  n.arena.release(scratch);
+  return 0;
+}
+
 static size_t rrdb_ws_bytes(const cfb_rrdb* n, int N, int H, int W) {
   const int us = n->scale == 2 ? 2 : (n->scale == 1 ? 4 : 1);
   const size_t px = (size_t)N * (H / us) * (W / us);
@@ -1254,11 +1365,7 @@ static size_t rrdb_ws_bytes(const cfb_rrdb* n, int N, int H, int W) {
 }
 
 static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  CFB_REQUIRE(n->prepared, "cfb_rrdb_prepare has not been called");
-  int dev = -1;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_REQUIRE(dev == n->device, "RRDBNet was prepared on another CUDA device");
-  CFB_CHECK(async_status_check("cfb_rrdb_forward"));
+  CFB_CHECK(n->begin_forward(false));
   const int us = n->scale == 2 ? 2 : (n->scale == 1 ? 4 : 1);
   CFB_REQUIRE(H % us == 0 && W % us == 0, "RRDBNet: H and W must be multiples of the pixel-unshuffle factor (arch_util.py:202)");
   if (N == 0 || H == 0 || W == 0) return 0;
@@ -1320,29 +1427,14 @@ static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, i
 namespace cfb {
 struct PnBlock { int kind; int cin, cout; GenConv sc, c1, c2; };     // kind: 0 none, 1 down, 2 up
 }
-struct cfb_parsenet {
+struct cfb_parsenet : cfb::NetCore {
+  cfb_parsenet() : NetCore("ParseNet", "parsenet") {}
   int in_size = 512, out_size = 512, min_feat = 32, base_ch = 64, parsing_ch = 19, res_depth = 10, ch_min = 32, ch_max = 256;
-  std::mutex mu;
-  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
   std::vector<cfb::PnBlock> blocks;       // encoder[1:], body, decoder in order
   int n_enc = 0, n_body = 0, n_dec = 0, head_ch = 64;
   float *first_w = nullptr, *first_b = nullptr, *mask_w = nullptr, *mask_b = nullptr, *img_w = nullptr, *img_b = nullptr;
-  float* slab = nullptr; size_t slab_bytes = 0;
-  int device = -1, sm_count = 148;
-  bool prepared = false;
-  cfb::Arena arena;
 };
 namespace cfb {
-
-static const float* pn_param(cfb_parsenet* n, const std::string& name, int64_t numel) {
-  auto it = n->raw.find(name);
-  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
-  if (it->second.second != numel) {
-    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
-    return nullptr;
-  }
-  return it->second.first;
-}
 
 static int pn_build(cfb_parsenet* n) {       // ParseNet.__init__  parsenet.py:151-186
   auto clip = [&](int x) { return std::max(n->ch_min, std::min(x, n->ch_max)); };
@@ -1353,10 +1445,9 @@ static int pn_build(cfb_parsenet* n) {       // ParseNet.__init__  parsenet.py:1
   int head = n->base_ch;
   auto add = [&](const std::string& p, int kind, int cin, int cout) {
     PnBlock b; b.kind = kind; b.cin = cin; b.cout = cout;
-    b.sc.name = p + ".shortcut_func"; b.c1.name = p + ".conv1"; b.c2.name = p + ".conv2";
-    b.sc.cin = cin; b.sc.cout = cout; b.sc.up = kind == 2;
-    b.c1.cin = cin; b.c1.cout = cout; b.c1.up = kind == 2;
-    b.c2.cin = cout; b.c2.cout = cout;
+    b.sc = plan_conv(p + ".shortcut_func", cin, cout); b.sc.up = kind == 2;
+    b.c1 = plan_conv(p + ".conv1", cin, cout); b.c1.up = kind == 2;
+    b.c2 = plan_conv(p + ".conv2", cout, cout);
     n->blocks.push_back(b);
   };
   for (int i = 0; i < down; ++i) { add("encoder." + std::to_string(i + 1), 1, clip(head), clip(head * 2)); head *= 2; }
@@ -1376,53 +1467,21 @@ static int pn_build(cfb_parsenet* n) {       // ParseNet.__init__  parsenet.py:1
 }
 
 static int pn_prepare(cfb_parsenet* n, cudaStream_t st) {
-  int dev = 0, major = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CFB_REQUIRE(major == 9, "ParseNet: the wgmma engine needs an sm_90 device (there is no other path)");
-  CFB_CHECK(async_status_init(st));
+  CFB_CHECK(n->begin_prepare(st));
   CFB_CHECK(pn_build(n));
-  size_t total = 0, padmax = 0;
-  auto acct = [&](GenConv& c) {
-    c.cin_p = c.cin; c.cout_p = c.cout;
-    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : 9);
-    total += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
-    padmax = std::max(padmax, (size_t)c.cout_p * c.cin_p * 9 * 4);
-  };
-  for (PnBlock& b : n->blocks) { if (b.kind) acct(b.sc); acct(b.c1); acct(b.c2); }
-  total += 2 * align256(padmax) + align256(1024) + align256((size_t)27 * 64 * 4) + 256 + 2 * (align256((size_t)9 * 64 * 20 * 4) + 256);
-  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
-    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
-    else cudaFree(n->slab);
-    n->slab = nullptr; n->slab_bytes = 0;
-  }
-  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
-  n->device = dev; n->sm_count = sms;
-  char* p = (char*)n->slab;
-  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  float* pad_scratch = (float*)take(padmax);
-  float* fold_w = (float*)take(padmax);
-  float* fold_b = (float*)take(1024);
+  SlabPlan plan;
+  for (const PnBlock& b : n->blocks) { if (b.kind) plan.add(b.sc); plan.add(b.c1); plan.add(b.c2); }
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256((size_t)27 * 64 * 4) + 256 + 2 * (align256((size_t)9 * 64 * 20 * 4) + 256)));
+  WeightPrep wp(*n, plan, st);
   auto prep = [&](GenConv& c, bool bn) -> int {
-    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : 9);
-    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
-    c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
-    const float* w = pn_param(n, c.name + ".conv2d.weight", (int64_t)c.cout * c.cin * 9);
-    if (!w) return 1;
-    if (!bn) {
-      const float* b = pn_param(n, c.name + ".conv2d.bias", c.cout);
-      if (!b) return 1;
-      return gen_conv_prepare(c, w, b, pad_scratch, st);
+    if (bn) {
+      CFB_CHECK(wp.fold(c.name + ".conv2d.weight", c.name + ".norm.norm.", c.cout, c.cin * 9));
+      return wp.conv(c, wp.fold_w, wp.fold_b);
     }
-    const float* g = pn_param(n, c.name + ".norm.norm.weight", c.cout);
-    const float* be = pn_param(n, c.name + ".norm.norm.bias", c.cout);
-    const float* mu = pn_param(n, c.name + ".norm.norm.running_mean", c.cout);
-    const float* var = pn_param(n, c.name + ".norm.norm.running_var", c.cout);
-    if (!g || !be || !mu || !var) return 1;
-    CFB_REQUIRE(c.cout <= 256, "ParseNet: more than 256 channels");
-    CFB_CHECK(fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, c.cout, c.cin * 9, st));      // nn.BatchNorm2d default eps
-    return gen_conv_prepare(c, fold_w, fold_b, pad_scratch, st);
+    const float* w = n->param(c.name + ".conv2d.weight", (int64_t)c.cout * c.cin * 9);
+    const float* b = n->param(c.name + ".conv2d.bias", c.cout);
+    if (!w || !b) return 1;
+    return wp.conv(c, w, b);
   };
   for (PnBlock& b : n->blocks) {
     if (b.kind) CFB_CHECK(prep(b.sc, false));
@@ -1430,21 +1489,21 @@ static int pn_prepare(cfb_parsenet* n, cudaStream_t st) {
     CFB_CHECK(prep(b.c2, true));
   }
   {
-    const float* w = pn_param(n, "encoder.0.conv2d.weight", (int64_t)64 * 3 * 9);
-    const float* b = pn_param(n, "encoder.0.conv2d.bias", 64);
+    const float* w = n->param("encoder.0.conv2d.weight", (int64_t)64 * 3 * 9);
+    const float* b = n->param("encoder.0.conv2d.bias", 64);
     if (!w || !b) return 1;
-    n->first_w = (float*)take((size_t)27 * 64 * 4); n->first_b = (float*)take(256);
+    n->first_w = (float*)wp.take((size_t)27 * 64 * 4); n->first_b = (float*)wp.take(256);
     CFB_CHECK(relayout_oihw_to_tck(w, n->first_w, 64, 3, 3, st));
     CFB_CUDA(cudaMemcpyAsync(n->first_b, b, 64 * 4, cudaMemcpyDeviceToDevice, st));
   }
   for (int which = 0; which < 2; ++which) {
     const std::string nm = which ? "out_img_conv" : "out_mask_conv";
     const int co = which ? 3 : n->parsing_ch;
-    const float* w = pn_param(n, nm + ".conv2d.weight", (int64_t)co * 64 * 9);
-    const float* b = pn_param(n, nm + ".conv2d.bias", co);
+    const float* w = n->param(nm + ".conv2d.weight", (int64_t)co * 64 * 9);
+    const float* b = n->param(nm + ".conv2d.bias", co);
     if (!w || !b) return 1;
-    float* wd = (float*)take((size_t)9 * 64 * 20 * 4);
-    float* bd = (float*)take(256);
+    float* wd = (float*)wp.take((size_t)9 * 64 * 20 * 4);
+    float* bd = (float*)wp.take(256);
     CFB_CHECK(relayout_thin_out(w, wd, co, st));
     CFB_CUDA(cudaMemcpyAsync(bd, b, (size_t)co * 4, cudaMemcpyDeviceToDevice, st));
     if (which) { n->img_w = wd; n->img_b = bd; } else { n->mask_w = wd; n->mask_b = bd; }
@@ -1456,26 +1515,15 @@ static int pn_prepare(cfb_parsenet* n, cudaStream_t st) {
 
 static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* out_img, int N, int H, int W, void* ws, int64_t ws_bytes,
                       cudaStream_t st, bool dry) {
-  CFB_REQUIRE(dry || n->prepared, "cfb_parsenet_prepare has not been called");
-  if (!dry) {
-    int dev = -1;
-    CFB_CUDA(cudaGetDevice(&dev));
-    CFB_REQUIRE(dev == n->device, "ParseNet was prepared on another CUDA device");
-    CFB_CHECK(async_status_check("cfb_parsenet_forward"));
-  }
+  CFB_CHECK(n->begin_forward(dry));
   const int div = 1 << n->n_enc;
   CFB_REQUIRE(H % div == 0 && W % div == 0 && H >= 2 * div && W >= 2 * div, "ParseNet: H and W must be multiples of 2^down_steps");
   if (N == 0) return 0;
   Arena& ar = n->arena;
   ar.reset(ws, (size_t)ws_bytes, dry);
-  auto alloc = [&](float** p, size_t elems) -> int {
-    *p = (float*)ar.alloc(elems * sizeof(float));
-    CFB_REQUIRE(*p != nullptr, "workspace too small (cfb_parsenet_workspace_bytes)");
-    return 0;
-  };
   float* t = nullptr;
   int h = H, w = W, c = 64;
-  CFB_CHECK(alloc(&t, (size_t)N * h * w * 64));
+  CFB_CHECK(n->alloc(&t, (size_t)N * h * w * 64));
   if (!dry) CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, t, N, h, w, 3, 1, 1, 64, 0, st));
   float* feat = nullptr;           // encoder output, added back after the body (parsenet.py:190)
   for (size_t i = 0; i < n->blocks.size(); ++i) {
@@ -1488,18 +1536,18 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
     if (b.kind == 1) { ho = h / 2; wo = w / 2; } else if (b.kind == 2) { ho = 2 * h; wo = 2 * w; }
     const int h1 = b.kind == 2 ? ho : h, w1 = b.kind == 2 ? wo : w;          // resolution of conv1's output
     if (b.kind) {
-      CFB_CHECK(alloc(&s, (size_t)N * ho * wo * b.cout));
+      CFB_CHECK(n->alloc(&s, (size_t)N * ho * wo * b.cout));
       GenLaunch g{&b.sc, t, b.cin, h, w, N, s, b.cout, 0, OUT_NONE};
       g.pad_mode = b.kind == 2 ? 2 : 1; g.sub = b.kind == 1;
       if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
     }
-    CFB_CHECK(alloc(&c1, (size_t)N * h1 * w1 * b.cout));
+    CFB_CHECK(n->alloc(&c1, (size_t)N * h1 * w1 * b.cout));
     {
       GenLaunch g{&b.c1, t, b.cin, h, w, N, c1, b.cout, 0, OUT_LRELU};
       g.pad_mode = b.kind == 2 ? 2 : 1;
       if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
     }
-    CFB_CHECK(alloc(&o, (size_t)N * ho * wo * b.cout));
+    CFB_CHECK(n->alloc(&o, (size_t)N * ho * wo * b.cout));
     {
       GenLaunch g{&b.c2, c1, b.cout, h1, w1, N, o, b.cout, 0, OUT_NONE};
       g.pad_mode = 1; g.sub = b.kind == 1;
@@ -1538,27 +1586,19 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
 //                                        positions: element-strided TMA boxes, ceil(H/2) outputs)
 //   FPN top-down add (after the ReLU)   SIMT, torch's nearest index
 // =========================================================================================================
-namespace cfb {
-struct RfConv { GenConv c; std::string bn; int k = 3, stride = 1; bool gen = false; };
-}
-struct cfb_retinaface {
-  std::mutex mu;
-  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
-  std::vector<cfb::RfConv> convs;        // body blocks (conv1, conv2, conv3[, downsample]), fpn, ssh, heads: see rf_build
+struct cfb_retinaface : cfb::NetCore {
+  cfb_retinaface() : NetCore("RetinaFace", "retinaface") {}
+  std::vector<cfb::GenConv> convs;       // body blocks (conv1, conv2, conv3[, downsample]), fpn, ssh, heads: see rf_build
   int blocks[4] = {3, 4, 6, 3};
   float *stem_w = nullptr, *stem_b = nullptr;
-  float* slab = nullptr; size_t slab_bytes = 0;
-  int device = -1, sm_count = 148;
-  bool prepared = false;
-  cfb::Arena arena;
 };
 namespace cfb {
 
 static void rf_build(cfb_retinaface* n) {
   n->convs.clear();
-  auto add = [&](const std::string& w, const std::string& bn, int cin, int cout, int k, int stride, bool gen) {
-    RfConv r; r.c.name = w; r.bn = bn; r.c.cin = cin; r.c.cout = cout; r.k = k; r.stride = stride; r.gen = gen;
-    n->convs.push_back(r);
+  auto add = [&](const std::string& w, const std::string& bn, int cin, int cout, int k, int stride) {
+    n->convs.push_back(plan_conv(w, cin, cout, k, stride));
+    n->convs.back().bn = bn;
   };
   const int widths[4] = {64, 128, 256, 512};
   int cin = 64;
@@ -1567,110 +1607,61 @@ static void rf_build(cfb_retinaface* n) {
     for (int b = 0; b < n->blocks[l]; ++b) {
       const std::string p = "body.layer" + std::to_string(l + 1) + "." + std::to_string(b) + ".";
       const int s = (b == 0 && l > 0) ? 2 : 1;
-      add(p + "conv1.weight", p + "bn1.", cin, wd, 1, 1, false);
-      add(p + "conv2.weight", p + "bn2.", wd, wd, 3, s, s == 1);
-      add(p + "conv3.weight", p + "bn3.", wd, 4 * wd, 1, 1, false);
-      if (b == 0) add(p + "downsample.0.weight", p + "downsample.1.", cin, 4 * wd, 1, s, false);
+      add(p + "conv1.weight", p + "bn1.", cin, wd, 1, 1);
+      add(p + "conv2.weight", p + "bn2.", wd, wd, 3, s);
+      add(p + "conv3.weight", p + "bn3.", wd, 4 * wd, 1, 1);
+      if (b == 0) add(p + "downsample.0.weight", p + "downsample.1.", cin, 4 * wd, 1, s);
       cin = 4 * wd;
     }
   }
   const int ins[3] = {512, 1024, 2048};
   for (int k = 0; k < 3; ++k) {
     const std::string p = "fpn.output" + std::to_string(k + 1) + ".";
-    add(p + "0.weight", p + "1.", ins[k], 256, 1, 1, false);
+    add(p + "0.weight", p + "1.", ins[k], 256, 1, 1);
   }
-  add("fpn.merge1.0.weight", "fpn.merge1.1.", 256, 256, 3, 1, true);
-  add("fpn.merge2.0.weight", "fpn.merge2.1.", 256, 256, 3, 1, true);
+  add("fpn.merge1.0.weight", "fpn.merge1.1.", 256, 256, 3, 1);
+  add("fpn.merge2.0.weight", "fpn.merge2.1.", 256, 256, 3, 1);
   for (int k = 0; k < 3; ++k) {
     const std::string p = "ssh" + std::to_string(k + 1) + ".";
-    add(p + "conv3X3.0.weight", p + "conv3X3.1.", 256, 128, 3, 1, true);
-    add(p + "conv5X5_1.0.weight", p + "conv5X5_1.1.", 256, 64, 3, 1, true);
-    add(p + "conv5X5_2.0.weight", p + "conv5X5_2.1.", 64, 64, 3, 1, true);
-    add(p + "conv7X7_2.0.weight", p + "conv7X7_2.1.", 64, 64, 3, 1, true);
-    add(p + "conv7x7_3.0.weight", p + "conv7x7_3.1.", 64, 64, 3, 1, true);
+    add(p + "conv3X3.0.weight", p + "conv3X3.1.", 256, 128, 3, 1);
+    add(p + "conv5X5_1.0.weight", p + "conv5X5_1.1.", 256, 64, 3, 1);
+    add(p + "conv5X5_2.0.weight", p + "conv5X5_2.1.", 64, 64, 3, 1);
+    add(p + "conv7X7_2.0.weight", p + "conv7X7_2.1.", 64, 64, 3, 1);
+    add(p + "conv7x7_3.0.weight", p + "conv7x7_3.1.", 64, 64, 3, 1);
   }
-  for (int k = 0; k < 3; ++k) add("heads." + std::to_string(k), "", 256, 64, 1, 1, false);   // bbox 8 | class 4 | landmark 20 | 0
-}
-
-static const float* rf_param(cfb_retinaface* n, const std::string& name, int64_t numel) {
-  auto it = n->raw.find(name);
-  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
-  if (it->second.second != numel) {
-    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
-    return nullptr;
-  }
-  return it->second.first;
+  for (int k = 0; k < 3; ++k) add("heads." + std::to_string(k), "", 256, 64, 1, 1);   // bbox 8 | class 4 | landmark 20 | 0
 }
 
 static int rf_prepare(cfb_retinaface* n, cudaStream_t st) {
-  int dev = 0, major = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CFB_REQUIRE(major == 9, "RetinaFace: the wgmma engine needs an sm_90 device (there is no other path)");
-  CFB_CHECK(async_status_init(st));
+  CFB_CHECK(n->begin_prepare(st));
   rf_build(n);
-  size_t total = 0, padmax = 0;
-  for (RfConv& r : n->convs) {
-    r.c.cin_p = r.c.cin; r.c.cout_p = r.c.cout;
-    const size_t wn = (size_t)r.c.cout * r.c.cin * r.k * r.k;
-    total += 2 * align256(wn * 2) + align256((size_t)r.c.cout * 4) + 256;
-    padmax = std::max(padmax, wn * 4);
-  }
-  total += 2 * align256(padmax) + align256(2048 * 4) + align256((size_t)64 * 147 * 4) + align256(256);
-  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
-    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
-    else cudaFree(n->slab);
-    n->slab = nullptr; n->slab_bytes = 0;
-  }
-  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
-  n->device = dev; n->sm_count = sms;
-  char* p = (char*)n->slab;
-  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  float* pad_scratch = (float*)take(padmax);
-  float* fold_w = (float*)take(padmax);
-  float* fold_b = (float*)take(2048 * 4);
-  auto fold = [&](const std::string& w_name, const std::string& bn, int cout, int per_out) -> int {
-    const float* w = rf_param(n, w_name, (int64_t)cout * per_out);
-    const float* g = rf_param(n, bn + "weight", cout);
-    const float* be = rf_param(n, bn + "bias", cout);
-    const float* mu = rf_param(n, bn + "running_mean", cout);
-    const float* var = rf_param(n, bn + "running_var", cout);
-    if (!w || !g || !be || !mu || !var) return 1;
-    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
-  };
-  for (RfConv& r : n->convs) {
-    GenConv& c = r.c;
-    const size_t wn = (size_t)c.cout * c.cin * r.k * r.k;
-    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
-    c.bias = (float*)take((size_t)c.cout * 4); c.wscale = (float*)take(8);
-    if (r.bn.empty()) {        // heads: [bbox 8 | class 4 | landmark 20 | zero 32] x 256, with their biases
-      CFB_CUDA(cudaMemsetAsync(fold_w, 0, wn * 4, st));
-      CFB_CUDA(cudaMemsetAsync(fold_b, 0, 64 * 4, st));
+  SlabPlan plan;
+  for (const GenConv& c : n->convs) plan.add(c);
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256((size_t)64 * 147 * 4) + align256(256)));
+  WeightPrep wp(*n, plan, st);
+  for (GenConv& c : n->convs) {
+    if (c.bn.empty()) {        // heads: [bbox 8 | class 4 | landmark 20 | zero 32] x 256, with their biases
+      CFB_CUDA(cudaMemsetAsync(wp.fold_w, 0, (size_t)c.cout * c.cin * 4, st));
+      CFB_CUDA(cudaMemsetAsync(wp.fold_b, 0, 64 * 4, st));
       const std::string lv = c.name.substr(6);
       const struct { const char* head; int rows, row0; } parts[3] = {{"BboxHead.", 8, 0}, {"ClassHead.", 4, 8}, {"LandmarkHead.", 20, 12}};
       for (const auto& h : parts) {
         const std::string base = std::string(h.head) + lv + ".conv1x1.";
-        const float* w = rf_param(n, base + "weight", (int64_t)h.rows * 256);
-        const float* b = rf_param(n, base + "bias", h.rows);
+        const float* w = n->param(base + "weight", (int64_t)h.rows * 256);
+        const float* b = n->param(base + "bias", h.rows);
         if (!w || !b) return 1;
-        CFB_CUDA(cudaMemcpyAsync(fold_w + (size_t)h.row0 * 256, w, (size_t)h.rows * 256 * 4, cudaMemcpyDeviceToDevice, st));
-        CFB_CUDA(cudaMemcpyAsync(fold_b + h.row0, b, (size_t)h.rows * 4, cudaMemcpyDeviceToDevice, st));
+        CFB_CUDA(cudaMemcpyAsync(wp.fold_w + (size_t)h.row0 * 256, w, (size_t)h.rows * 256 * 4, cudaMemcpyDeviceToDevice, st));
+        CFB_CUDA(cudaMemcpyAsync(wp.fold_b + h.row0, b, (size_t)h.rows * 4, cudaMemcpyDeviceToDevice, st));
       }
     } else {
-      CFB_CHECK(fold(c.name, r.bn, c.cout, c.cin * r.k * r.k));
+      CFB_CHECK(wp.fold(c.name, c.bn, c.cout, c.cin * c.k * c.k));
     }
-    if (r.gen) {
-      CFB_CHECK(gen_conv_prepare(c, fold_w, fold_b, pad_scratch, st));
-    } else {
-      CFB_CHECK(tc_split_weights(fold_w, c.w_hi, c.w_lo, c.cout, c.cin, r.k, c.wscale, st));
-      CFB_CUDA(cudaMemcpyAsync(c.bias, fold_b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
-    }
+    CFB_CHECK(wp.conv(c, wp.fold_w, wp.fold_b));
   }
-  n->stem_w = (float*)take((size_t)64 * 147 * 4); n->stem_b = (float*)take(256);
-  CFB_CHECK(fold("body.conv1.weight", "body.bn1.", 64, 147));
-  CFB_CUDA(cudaMemcpyAsync(n->stem_w, fold_w, (size_t)64 * 147 * 4, cudaMemcpyDeviceToDevice, st));
-  CFB_CUDA(cudaMemcpyAsync(n->stem_b, fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  n->stem_w = (float*)wp.take((size_t)64 * 147 * 4); n->stem_b = (float*)wp.take(256);
+  CFB_CHECK(wp.fold("body.conv1.weight", "body.bn1.", 64, 147));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, wp.fold_w, (size_t)64 * 147 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, wp.fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
   CFB_CUDA(cudaStreamSynchronize(st));
   n->prepared = true;
   return 0;
@@ -1685,51 +1676,29 @@ static int64_t rf_priors(int H, int W) {
 
 static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* img, float* loc, float* conf, float* landms, int N,
                       int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
-  CFB_REQUIRE(dry || n->prepared, "cfb_retinaface_prepare has not been called");
-  if (!dry) {
-    int dev = -1;
-    CFB_CUDA(cudaGetDevice(&dev));
-    CFB_REQUIRE(dev == n->device, "RetinaFace was prepared on another CUDA device");
-    CFB_CHECK(async_status_check("cfb_retinaface_forward"));
-  }
+  CFB_CHECK(n->begin_forward(dry));
   CFB_REQUIRE(H >= 1 && W >= 1 && N >= 0, "RetinaFace: empty image");
   CFB_REQUIRE(rf_priors(H, W) * N < ((int64_t)1 << 31) / 16, "RetinaFace: image too large");
   if (N == 0) return 0;
   if (n->convs.empty()) rf_build(n);
   Arena& ar = n->arena;
   ar.reset(ws, (size_t)ws_bytes, dry);
-  auto alloc = [&](float** p, size_t elems) -> int {
-    *p = (float*)ar.alloc(elems * sizeof(float));
-    CFB_REQUIRE(*p != nullptr, "workspace too small (cfb_retinaface_workspace_bytes)");
-    return 0;
-  };
   // one conv of the plan: 3x3 stride 1 on the generalised engine, everything else on the per-tap engine
-  auto conv = [&](const RfConv& r, const float* in, int h, int w, float* out, int act, const float* res, int out_pitch = 0,
+  auto conv = [&](const GenConv& c, const float* in, int h, int w, float* out, int act, const float* res, int out_pitch = 0,
                   int out_c0 = 0) -> int {
-    if (r.gen) {
-      GenLaunch g{&r.c, in, r.c.cin, h, w, N, out, out_pitch ? out_pitch : r.c.cout, out_c0, act};
-      g.res = res; g.res_pitch = r.c.cout;
+    if (c.gen) {
+      GenLaunch g{&c, in, c.cin_p, h, w, N, out, out_pitch ? out_pitch : c.cout, out_c0, act};
+      g.res = res; g.res_pitch = c.cout;
       return dry ? 0 : gen_conv(g, n->sm_count, st);
     }
-    ConvArgs a;
-    a.in = in; a.N = N; a.H = h; a.W = w; a.Cin = r.c.cin; a.Cout = r.c.cout; a.ksize = r.k;
-    a.Ho = r.stride == 2 ? (h + 1) / 2 : h; a.Wo = r.stride == 2 ? (w + 1) / 2 : w;
-    a.mode = r.stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = (r.stride == 2 && r.k == 3) ? 1 : 0;
-    a.wgt_hi = r.c.w_hi; a.wgt_lo = r.c.w_lo; a.wscale_inv = r.c.wscale + 1; a.bias = r.c.bias;
-    a.residual = res; a.out_act = act; a.out = out;
-    CFB_REQUIRE(tc_supported(a), "RetinaFace: conv not supported by the wgmma engine: " + r.c.name);
-    void* scratch = ar.alloc(tc_scratch_bytes(a));
-    CFB_REQUIRE(scratch != nullptr, "workspace too small (cfb_retinaface_workspace_bytes)");
-    if (!dry) CFB_CHECK(conv_tc(a, scratch, n->sm_count, st));
-    ar.release(scratch);
-    return 0;
+    return pertap_conv(*n, pertap_args(in, N, h, w, c.cin_p, c.cout_p, c.k, c.stride, out, out_pitch, out_c0, act, res), c, dry, st);
   };
   const int H2 = (H - 1) / 2 + 1, W2 = (W - 1) / 2 + 1;
   int h = (H2 - 1) / 2 + 1, w = (W2 - 1) / 2 + 1;
   float *s0 = nullptr, *cur = nullptr;
-  CFB_CHECK(alloc(&s0, (size_t)N * H2 * W2 * 64));
+  CFB_CHECK(n->alloc(&s0, (size_t)N * H2 * W2 * 64));
   if (!dry) CFB_CHECK(rf_stem(x, img, n->stem_w, n->stem_b, s0, N, H, W, st));
-  CFB_CHECK(alloc(&cur, (size_t)N * h * w * 64));
+  CFB_CHECK(n->alloc(&cur, (size_t)N * h * w * 64));
   if (!dry) CFB_CHECK(rf_maxpool(s0, cur, N, H2, W2, st));
   ar.release(s0);
   size_t ci = 0;
@@ -1737,22 +1706,22 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
   int ch[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
   for (int l = 0; l < 4; ++l) {
     for (int b = 0; b < n->blocks[l]; ++b) {
-      const RfConv& c1 = n->convs[ci++];
-      const RfConv& c2 = n->convs[ci++];
-      const RfConv& c3 = n->convs[ci++];
-      const RfConv* ds = b == 0 ? &n->convs[ci++] : nullptr;
+      const GenConv& c1 = n->convs[ci++];
+      const GenConv& c2 = n->convs[ci++];
+      const GenConv& c3 = n->convs[ci++];
+      const GenConv* ds = b == 0 ? &n->convs[ci++] : nullptr;
       const int ho = c2.stride == 2 ? (h + 1) / 2 : h, wo = c2.stride == 2 ? (w + 1) / 2 : w;
       float *t1 = nullptr, *t2 = nullptr, *res = cur, *y = nullptr;
-      CFB_CHECK(alloc(&t1, (size_t)N * h * w * c1.c.cout));
+      CFB_CHECK(n->alloc(&t1, (size_t)N * h * w * c1.cout));
       CFB_CHECK(conv(c1, cur, h, w, t1, OUT_RELU, nullptr));
-      CFB_CHECK(alloc(&t2, (size_t)N * ho * wo * c2.c.cout));
+      CFB_CHECK(n->alloc(&t2, (size_t)N * ho * wo * c2.cout));
       CFB_CHECK(conv(c2, t1, h, w, t2, OUT_RELU, nullptr));
       ar.release(t1);
       if (ds) {
-        CFB_CHECK(alloc(&res, (size_t)N * ho * wo * ds->c.cout));
+        CFB_CHECK(n->alloc(&res, (size_t)N * ho * wo * ds->cout));
         CFB_CHECK(conv(*ds, cur, h, w, res, OUT_NONE, nullptr));
       }
-      CFB_CHECK(alloc(&y, (size_t)N * ho * wo * c3.c.cout));
+      CFB_CHECK(n->alloc(&y, (size_t)N * ho * wo * c3.cout));
       CFB_CHECK(conv(c3, t2, ho, wo, y, OUT_RELU, res));          // relu(bn3(conv3(.)) + identity)
       ar.release(t2);
       if (res != cur) ar.release(res);
@@ -1764,20 +1733,20 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
   // FPN (retinaface_net.py:76-96): output_k = relu(bn(conv1x1(C_k))); output_2 += nearest(output_3); merge2; output_1 += ...
   float* O[3];
   for (int k = 0; k < 3; ++k) {
-    CFB_CHECK(alloc(&O[k], (size_t)N * ch[k] * cw[k] * 256));
+    CFB_CHECK(n->alloc(&O[k], (size_t)N * ch[k] * cw[k] * 256));
     CFB_CHECK(conv(n->convs[ci + k], C[k], ch[k], cw[k], O[k], OUT_RELU, nullptr));
     ar.release(C[k]);
   }
-  const RfConv& merge1 = n->convs[ci + 3];
-  const RfConv& merge2 = n->convs[ci + 4];
+  const GenConv& merge1 = n->convs[ci + 3];
+  const GenConv& merge2 = n->convs[ci + 4];
   ci += 5;
   float *m2 = nullptr, *m1 = nullptr;
   if (!dry) CFB_CHECK(rf_add_nearest(O[1], O[2], N, ch[1], cw[1], ch[2], cw[2], 256, st));
-  CFB_CHECK(alloc(&m2, (size_t)N * ch[1] * cw[1] * 256));
+  CFB_CHECK(n->alloc(&m2, (size_t)N * ch[1] * cw[1] * 256));
   CFB_CHECK(conv(merge2, O[1], ch[1], cw[1], m2, OUT_RELU, nullptr));
   ar.release(O[1]);
   if (!dry) CFB_CHECK(rf_add_nearest(O[0], m2, N, ch[0], cw[0], ch[1], cw[1], 256, st));
-  CFB_CHECK(alloc(&m1, (size_t)N * ch[0] * cw[0] * 256));
+  CFB_CHECK(n->alloc(&m1, (size_t)N * ch[0] * cw[0] * 256));
   CFB_CHECK(conv(merge1, O[0], ch[0], cw[0], m1, OUT_RELU, nullptr));
   ar.release(O[0]);
   float* fpn[3] = {m1, m2, O[2]};
@@ -1785,20 +1754,20 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
   // epilogues; then the three 1x1 heads of the level in one conv
   float* hd[3];
   for (int k = 0; k < 3; ++k) {
-    const RfConv* s = &n->convs[ci + 5 * k];
+    const GenConv* s = &n->convs[ci + 5 * k];
     const int hk = ch[k], wk = cw[k];
     float *f = nullptr, *t5 = nullptr, *t7 = nullptr;
-    CFB_CHECK(alloc(&f, (size_t)N * hk * wk * 256));
+    CFB_CHECK(n->alloc(&f, (size_t)N * hk * wk * 256));
     CFB_CHECK(conv(s[0], fpn[k], hk, wk, f, OUT_RELU, nullptr, 256, 0));
-    CFB_CHECK(alloc(&t5, (size_t)N * hk * wk * 64));
+    CFB_CHECK(n->alloc(&t5, (size_t)N * hk * wk * 64));
     CFB_CHECK(conv(s[1], fpn[k], hk, wk, t5, OUT_RELU, nullptr));
     CFB_CHECK(conv(s[2], t5, hk, wk, f, OUT_RELU, nullptr, 256, 128));
-    CFB_CHECK(alloc(&t7, (size_t)N * hk * wk * 64));
+    CFB_CHECK(n->alloc(&t7, (size_t)N * hk * wk * 64));
     CFB_CHECK(conv(s[3], t5, hk, wk, t7, OUT_RELU, nullptr));
     CFB_CHECK(conv(s[4], t7, hk, wk, f, OUT_RELU, nullptr, 256, 192));
     ar.release(t5); ar.release(t7);
     ar.release(fpn[k]);
-    CFB_CHECK(alloc(&hd[k], (size_t)N * hk * wk * 64));
+    CFB_CHECK(n->alloc(&hd[k], (size_t)N * hk * wk * 64));
     CFB_CHECK(conv(n->convs[ci + 15 + k], f, hk, wk, hd[k], OUT_NONE, nullptr));
     ar.release(f);
   }
@@ -1822,18 +1791,10 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
 // convs 9 / 13 / 17 / 20 write into the concat buffers of layers 21 / 18 / 18 / 21.  The copy kernel fills the rest: the
 // nearest x2 upsamples (layers 10, 14) and the backbone features of layers 11 and 15.
 // =========================================================================================================
-namespace cfb {
-struct YoConv { GenConv c; int k = 1, stride = 1; bool gen = false, bn = true; };
-}
-struct cfb_yolov5face {
-  std::mutex mu;
-  std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
-  std::unordered_map<std::string, cfb::YoConv> convs;     // by module prefix, e.g. "model.1.m.0.cv2"
+struct cfb_yolov5face : cfb::NetCore {
+  cfb_yolov5face() : NetCore("YOLOv5-face", "yolov5face") {}
+  std::unordered_map<std::string, cfb::GenConv> convs;     // by module prefix, e.g. "model.1.m.0.cv2"
   float *stem_w = nullptr, *stem_b = nullptr, *anchor_grid = nullptr;
-  float* slab = nullptr; size_t slab_bytes = 0;
-  int device = -1, sm_count = 148;
-  bool prepared = false;
-  cfb::Arena arena;
 };
 namespace cfb {
 
@@ -1847,9 +1808,9 @@ static const YoC3 kYoC3[8] = {{1, 64, 128, 3, true},     {3, 256, 256, 9, true},
 static void yo_build(cfb_yolov5face* n) {
   n->convs.clear();
   auto add = [&](const std::string& name, int cin, int cout, int k, int stride, bool bn = true) {
-    YoConv r; r.c.name = name; r.c.cin = cin; r.c.cout = cout; r.k = k; r.stride = stride; r.gen = k == 3 && stride == 1; r.bn = bn;
-    r.c.cin_p = (cin + 63) / 64 * 64; r.c.cout_p = (cout + 63) / 64 * 64;
-    n->convs[name] = r;
+    GenConv c = plan_conv(name, cin, cout, k, stride);
+    if (bn) c.bn = name + ".bn.";
+    n->convs[name] = c;
   };
   add("model.0.stem_2a", 64, 32, 1, 1);
   add("model.0.stem_2b", 32, 64, 3, 2);
@@ -1878,87 +1839,33 @@ static void yo_build(cfb_yolov5face* n) {
   for (int l = 0; l < 3; ++l) add("model.23.m." + std::to_string(l), ch[l], 48, 1, 1, false);
 }
 
-static const float* yo_param(cfb_yolov5face* n, const std::string& name, int64_t numel) {
-  auto it = n->raw.find(name);
-  if (it == n->raw.end()) { set_error("missing parameter '" + name + "'"); return nullptr; }
-  if (it->second.second != numel) {
-    set_error("parameter '" + name + "' has " + std::to_string(it->second.second) + " elements, expected " + std::to_string(numel));
-    return nullptr;
-  }
-  return it->second.first;
-}
-
 static int yo_prepare(cfb_yolov5face* n, cudaStream_t st) {
-  int dev = 0, major = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CFB_REQUIRE(major == 9, "YOLOv5-face: the wgmma engine needs an sm_90 device (there is no other path)");
-  CFB_CHECK(async_status_init(st));
+  CFB_CHECK(n->begin_prepare(st));
   yo_build(n);
-  size_t total = 0, padmax = 0;
+  SlabPlan plan;
+  for (const auto& kv : n->convs) plan.add(kv.second);
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256((size_t)64 * 27 * 4) + align256(256) + align256(18 * 4)));
+  WeightPrep wp(*n, plan, st);
   for (auto& kv : n->convs) {
-    const GenConv& c = kv.second.c;
-    const size_t wn = (size_t)c.cout_p * c.cin_p * kv.second.k * kv.second.k;
-    total += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
-    padmax = std::max(padmax, wn * 4);
-  }
-  total += 2 * align256(padmax) + align256(1024 * 4) + align256((size_t)64 * 27 * 4) + align256(256) + align256(18 * 4);
-  if (n->slab && (n->device != dev || n->slab_bytes < total)) {
-    if (n->device != dev && n->device >= 0) { cudaSetDevice(n->device); cudaFree(n->slab); cudaSetDevice(dev); }
-    else cudaFree(n->slab);
-    n->slab = nullptr; n->slab_bytes = 0;
-  }
-  if (!n->slab) { CFB_CUDA(cudaMalloc((void**)&n->slab, total)); n->slab_bytes = total; }
-  n->device = dev; n->sm_count = sms;
-  char* p = (char*)n->slab;
-  auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  float* pad_scratch = (float*)take(padmax);
-  float* fold_w = (float*)take(padmax);
-  float* fold_b = (float*)take(1024 * 4);
-  auto fold = [&](const std::string& m, int cout, int per_out) -> int {   // Conv m: m.conv.weight + m.bn.*
-    const float* w = yo_param(n, m + ".conv.weight", (int64_t)cout * per_out);
-    const float* g = yo_param(n, m + ".bn.weight", cout);
-    const float* be = yo_param(n, m + ".bn.bias", cout);
-    const float* mu = yo_param(n, m + ".bn.running_mean", cout);
-    const float* var = yo_param(n, m + ".bn.running_var", cout);
-    if (!w || !g || !be || !mu || !var) return 1;
-    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
-  };
-  for (auto& kv : n->convs) {
-    YoConv& r = kv.second;
-    GenConv& c = r.c;
-    const int taps = r.k * r.k;
-    const size_t wn = (size_t)c.cout_p * c.cin_p * taps;
-    c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
-    c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
-    if (r.bn) {
-      CFB_CHECK(fold(c.name, c.cout, c.cin * taps));
+    GenConv& c = kv.second;
+    if (!c.bn.empty()) {
+      CFB_CHECK(wp.fold(c.name + ".conv.weight", c.bn, c.cout, c.cin * c.k * c.k));
     } else {                 // Detect: plain conv with bias
-      const float* w = yo_param(n, c.name + ".weight", (int64_t)c.cout * c.cin);
-      const float* b = yo_param(n, c.name + ".bias", c.cout);
+      const float* w = n->param(c.name + ".weight", (int64_t)c.cout * c.cin);
+      const float* b = n->param(c.name + ".bias", c.cout);
       if (!w || !b) return 1;
-      CFB_CUDA(cudaMemcpyAsync(fold_w, w, (size_t)c.cout * c.cin * 4, cudaMemcpyDeviceToDevice, st));
-      CFB_CUDA(cudaMemcpyAsync(fold_b, b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
+      CFB_CUDA(cudaMemcpyAsync(wp.fold_w, w, (size_t)c.cout * c.cin * 4, cudaMemcpyDeviceToDevice, st));
+      CFB_CUDA(cudaMemcpyAsync(wp.fold_b, b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
     }
-    if (r.gen) {
-      CFB_CHECK(gen_conv_prepare(c, fold_w, fold_b, pad_scratch, st));
-    } else {                 // zero-padded [cout_p][cin_p][k][k] (stem_2a / stem_2b / Detect), then the fp16 hi/lo split
-      CFB_CUDA(cudaMemsetAsync(pad_scratch, 0, wn * 4, st));
-      CFB_CUDA(cudaMemcpy2DAsync(pad_scratch, (size_t)c.cin_p * taps * 4, fold_w, (size_t)c.cin * taps * 4, (size_t)c.cin * taps * 4,
-                                 c.cout, cudaMemcpyDeviceToDevice, st));
-      CFB_CHECK(tc_split_weights(pad_scratch, c.w_hi, c.w_lo, c.cout_p, c.cin_p, r.k, c.wscale, st));
-      CFB_CUDA(cudaMemsetAsync(c.bias, 0, (size_t)c.cout_p * 4, st));
-      CFB_CUDA(cudaMemcpyAsync(c.bias, fold_b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
-    }
+    CFB_CHECK(wp.conv(c, wp.fold_w, wp.fold_b));      // stem_2a / stem_2b / Detect: zero-padded to 64 channels
   }
-  n->stem_w = (float*)take((size_t)64 * 27 * 4); n->stem_b = (float*)take(256);
-  CFB_CHECK(fold("model.0.stem_1", 64, 27));
-  CFB_CUDA(cudaMemcpyAsync(n->stem_w, fold_w, (size_t)64 * 27 * 4, cudaMemcpyDeviceToDevice, st));
-  CFB_CUDA(cudaMemcpyAsync(n->stem_b, fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
-  const float* ag = yo_param(n, "model.23.anchor_grid", 18);
+  n->stem_w = (float*)wp.take((size_t)64 * 27 * 4); n->stem_b = (float*)wp.take(256);
+  CFB_CHECK(wp.fold("model.0.stem_1.conv.weight", "model.0.stem_1.bn.", 64, 27));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, wp.fold_w, (size_t)64 * 27 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, wp.fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  const float* ag = n->param("model.23.anchor_grid", 18);
   if (!ag) return 1;
-  n->anchor_grid = (float*)take(18 * 4);
+  n->anchor_grid = (float*)wp.take(18 * 4);
   CFB_CUDA(cudaMemcpyAsync(n->anchor_grid, ag, 18 * 4, cudaMemcpyDeviceToDevice, st));
   CFB_CUDA(cudaStreamSynchronize(st));
   n->prepared = true;
@@ -1972,13 +1879,7 @@ static int64_t yo_predictions(int H, int W) {
 
 static int yo_forward(cfb_yolov5face* n, const float* x, const unsigned char* img, int ih, int iw, int top, int left, float* pred,
                       float* const raw[3], int N, int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
-  CFB_REQUIRE(dry || n->prepared, "cfb_yolov5face_prepare has not been called");
-  if (!dry) {
-    int dev = -1;
-    CFB_CUDA(cudaGetDevice(&dev));
-    CFB_REQUIRE(dev == n->device, "YOLOv5-face was prepared on another CUDA device");
-    CFB_CHECK(async_status_check("cfb_yolov5face_forward"));
-  }
+  CFB_CHECK(n->begin_forward(dry));
   CFB_REQUIRE(H >= 32 && W >= 32 && H % 32 == 0 && W % 32 == 0 && N >= 0, "YOLOv5-face: H and W must be positive multiples of 32");
   CFB_REQUIRE(!img || (ih >= 1 && iw >= 1 && top >= 0 && left >= 0 && top + ih <= H && left + iw <= W),
               "YOLOv5-face: the image must lie inside the letterbox canvas");
@@ -1987,32 +1888,17 @@ static int yo_forward(cfb_yolov5face* n, const float* x, const unsigned char* im
   if (n->convs.empty()) yo_build(n);
   Arena& ar = n->arena;
   ar.reset(ws, (size_t)ws_bytes, dry);
-  auto alloc = [&](float** p, int h, int w, int c) -> int {
-    *p = (float*)ar.alloc((size_t)N * h * w * c * sizeof(float));
-    CFB_REQUIRE(*p != nullptr, "workspace too small (cfb_yolov5face_workspace_bytes)");
-    return 0;
-  };
+  auto alloc = [&](float** p, int h, int w, int c) { return n->alloc(p, (size_t)N * h * w * c); };
   // one conv: 3x3 stride 1 on the generalised engine (res2: the Bottleneck shortcut), everything else on the per-tap engine
   auto conv = [&](const std::string& name, const float* in, int h, int w, float* out, int out_pitch, int out_c0, int act,
                   const float* res2 = nullptr, int res2_pitch = 0) -> int {
-    const YoConv& r = n->convs.at(name);
-    if (r.gen) {
-      GenLaunch g{&r.c, in, r.c.cin_p, h, w, N, out, out_pitch, out_c0, act};
+    const GenConv& c = n->convs.at(name);
+    if (c.gen) {
+      GenLaunch g{&c, in, c.cin_p, h, w, N, out, out_pitch, out_c0, act};
       g.res2 = res2; g.res2_pitch = res2_pitch;
       return dry ? 0 : gen_conv(g, n->sm_count, st);
     }
-    ConvArgs a;
-    a.in = in; a.N = N; a.H = h; a.W = w; a.Cin = r.c.cin_p; a.Cout = r.c.cout_p; a.ksize = r.k;
-    a.Ho = r.stride == 2 ? (h + 1) / 2 : h; a.Wo = r.stride == 2 ? (w + 1) / 2 : w;
-    a.mode = r.stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = r.stride == 2 ? 1 : 0;
-    a.wgt_hi = r.c.w_hi; a.wgt_lo = r.c.w_lo; a.wscale_inv = r.c.wscale + 1; a.bias = r.c.bias;
-    a.out_act = act; a.out = out; a.out_pitch = out_pitch == r.c.cout_p ? 0 : out_pitch; a.out_c0 = out_c0;
-    CFB_REQUIRE(tc_supported(a), "YOLOv5-face: conv not supported by the wgmma engine: " + name);
-    void* scratch = ar.alloc(tc_scratch_bytes(a));
-    CFB_REQUIRE(scratch != nullptr, "workspace too small (cfb_yolov5face_workspace_bytes)");
-    if (!dry) CFB_CHECK(conv_tc(a, scratch, n->sm_count, st));
-    ar.release(scratch);
-    return 0;
+    return pertap_conv(*n, pertap_args(in, N, h, w, c.cin_p, c.cout_p, c.k, c.stride, out, out_pitch, out_c0, act, nullptr), c, dry, st);
   };
   // C3 (common.py): cv3(cat(m(cv1(x)), cv2(x))) with the cat as one [2c_] buffer; out: a dense [c2] buffer
   auto c3 = [&](int i, const float* in, int h, int w, float** out) -> int {
@@ -2172,17 +2058,7 @@ cfb_net* cfb_net_create(const cfb_config* cfg) {
   API_END(nullptr)
 }
 
-void cfb_net_destroy(cfb_net* n) {
-  if (!n) return;
-  if (n->slab) {
-    int cur = -1;
-    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
-    if (sw) cudaSetDevice(n->device);
-    cudaFree(n->slab);
-    if (sw) cudaSetDevice(cur);
-  }
-  delete n;
-}
+void cfb_net_destroy(cfb_net* n) { delete n; }     // ~NetCore frees the slab on its device
 
 cfb_rrdb* cfb_rrdb_create(int32_t num_in_ch, int32_t num_out_ch, int32_t scale, int32_t num_feat, int32_t num_block, int32_t num_grow_ch) {
   API_BEGIN
@@ -2196,24 +2072,11 @@ cfb_rrdb* cfb_rrdb_create(int32_t num_in_ch, int32_t num_out_ch, int32_t scale, 
   return n;
   API_END(nullptr)
 }
-void cfb_rrdb_destroy(cfb_rrdb* n) {
-  if (!n) return;
-  if (n->slab) {
-    int cur = -1;
-    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
-    if (sw) cudaSetDevice(n->device);
-    cudaFree(n->slab);
-    if (sw) cudaSetDevice(cur);
-  }
-  delete n;
-}
+void cfb_rrdb_destroy(cfb_rrdb* n) { delete n; }
 int cfb_rrdb_set_param(cfb_rrdb* n, const char* name, const float* dev_ptr, int64_t numel) {
   API_BEGIN
   CFB_REQUIRE(n && name && dev_ptr, "cfb_rrdb_set_param: NULL argument");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->raw[name] = {dev_ptr, numel};
-  n->prepared = false;
-  return 0;
+  return n->set_param(name, dev_ptr, numel);
   API_END(1)
 }
 int cfb_rrdb_prepare(cfb_rrdb* n, void* stream) {
@@ -2246,24 +2109,11 @@ cfb_parsenet* cfb_parsenet_create(int32_t in_size, int32_t out_size, int32_t min
   return n;
   API_END(nullptr)
 }
-void cfb_parsenet_destroy(cfb_parsenet* n) {
-  if (!n) return;
-  if (n->slab) {
-    int cur = -1;
-    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
-    if (sw) cudaSetDevice(n->device);
-    cudaFree(n->slab);
-    if (sw) cudaSetDevice(cur);
-  }
-  delete n;
-}
+void cfb_parsenet_destroy(cfb_parsenet* n) { delete n; }
 int cfb_parsenet_set_param(cfb_parsenet* n, const char* name, const float* dev_ptr, int64_t numel) {
   API_BEGIN
   CFB_REQUIRE(n && name && dev_ptr, "cfb_parsenet_set_param: NULL argument");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->raw[name] = {dev_ptr, numel};
-  n->prepared = false;
-  return 0;
+  return n->set_param(name, dev_ptr, numel);
   API_END(1)
 }
 int cfb_parsenet_prepare(cfb_parsenet* n, void* stream) {
@@ -2276,9 +2126,9 @@ int cfb_parsenet_prepare(cfb_parsenet* n, void* stream) {
 int64_t cfb_parsenet_workspace_bytes(cfb_parsenet* n, int32_t batch, int32_t h, int32_t w) {
   API_BEGIN
   if (!n) { cfb::set_error("cfb_parsenet_workspace_bytes: NULL net"); return -1; }
-  std::lock_guard<std::mutex> lk(n->mu);
-  if (cfb::pn_forward(n, (const float*)0x1000, (float*)0x1000, (float*)0x1000, batch, h, w, nullptr, 0, nullptr, true) != 0) return -1;
-  return (int64_t)n->arena.high() + 4096;
+  return n->dry_run([&] {
+    return cfb::pn_forward(n, (const float*)0x1000, (float*)0x1000, (float*)0x1000, batch, h, w, nullptr, 0, nullptr, true);
+  });
   API_END(-1)
 }
 int cfb_parsenet_forward(cfb_parsenet* n, const float* x, float* out_mask, float* out_img, int32_t batch, int32_t h, int32_t w,
@@ -2315,21 +2165,37 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
   int dev = 0, sms = 148;
   CFB_CUDA(cudaGetDevice(&dev));
   CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cfb::GenConv c;
-  c.cin = cin; c.cout = cout; c.cin_p = (cin + 63) / 64 * 64; c.cout_p = (cout + 63) / 64 * 64; c.up = upsample != 0;
+  cfb::GenConv c = cfb::plan_conv("", cin, cout);
+  c.up = upsample != 0;
   char* p = (char*)(((uintptr_t)workspace + 255) / 256 * 256);
   float* pad = (float*)p; p += align256((size_t)c.cout_p * c.cin_p * 9 * 4);
-  const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : 9);
-  c.w_hi = (__half*)p; p += align256(wn * 2);
-  c.w_lo = (__half*)p; p += align256(wn * 2);
-  c.bias = (float*)p; p += align256((size_t)c.cout_p * 4);
-  c.wscale = (float*)p;
-  CFB_CHECK(cfb::gen_conv_prepare(c, weight_oihw, bias, pad, st));
+  CFB_CHECK(cfb::prepare_conv(c, weight_oihw, bias, pad, p, st));
   cfb::GenLaunch g{&c, in, in_pitch, h, w, n, out, out_pitch, out_c0, out_act};
   g.res = residual; g.res_pitch = res_pitch; g.res2 = residual2; g.res2_pitch = res2_pitch; g.post = post_scale;
   g.pad_mode = pad_mode; g.sub = subsample != 0;
   return cfb::gen_conv(g, sms, st);
   API_END(1)
+}
+
+// body of the two per-tap test entry points (after their own argument checks): split the weight into the workspace, run
+static int pertap_nhwc(const char* fn, cfb::ConvArgs a, const float* weight_oihw, const float* bias, int32_t stride, void* workspace,
+                       int64_t workspace_bytes, cudaStream_t st) {
+  CFB_CHECK(cfb::async_status_init(st));
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CFB_REQUIRE(cfb::tc_supported(a), std::string(fn) + ": shape not supported by the wgmma engine");
+  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_pertap_workspace_bytes(a.N, a.H, a.W, a.Cin, a.Cout, a.ksize, stride),
+              std::string(fn) + ": workspace too small");
+  const size_t wn = (size_t)a.Cout * a.Cin * a.ksize * a.ksize;
+  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+  __half* whi = (__half*)p; p += align256(wn * 2);
+  __half* wlo = (__half*)p; p += align256(wn * 2);
+  float* wsc = (float*)p; p += 256;
+  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
+  CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, a.Cout, a.Cin, a.ksize, wsc, st));
+  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.bias = bias;
+  return cfb::conv_tc(a, p, sms, st);
 }
 
 int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h, int32_t w,
@@ -2339,27 +2205,8 @@ int cfb_conv2d_pertap_nhwc(const float* in, const float* weight_oihw, const floa
   CFB_REQUIRE(in && weight_oihw && out && workspace, "cfb_conv2d_pertap_nhwc: NULL argument");
   CFB_REQUIRE(stride == 1 || stride == 2, "cfb_conv2d_pertap_nhwc: stride must be 1 or 2");
   CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_RELU, "cfb_conv2d_pertap_nhwc: activation must be none or ReLU");
-  cudaStream_t st = (cudaStream_t)stream;
-  CFB_CHECK(cfb::async_status_init(st));
-  int dev = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cfb::ConvArgs a;
-  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
-  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
-  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
-  CFB_REQUIRE(cfb::tc_supported(a), "cfb_conv2d_pertap_nhwc: shape not supported by the wgmma engine");
-  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_pertap_workspace_bytes(n, h, w, cin, cout, ksize, stride),
-              "cfb_conv2d_pertap_nhwc: workspace too small");
-  const size_t wn = (size_t)cout * cin * ksize * ksize;
-  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
-  __half* whi = (__half*)p; p += align256(wn * 2);
-  __half* wlo = (__half*)p; p += align256(wn * 2);
-  float* wsc = (float*)p; p += 256;
-  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
-  CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, ksize, wsc, st));
-  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.bias = bias; a.residual = residual; a.out_act = out_act; a.out = out;
-  return cfb::conv_tc(a, p, sms, st);
+  return pertap_nhwc("cfb_conv2d_pertap_nhwc", cfb::pertap_args(in, n, h, w, cin, cout, ksize, stride, out, 0, 0, out_act, residual),
+                     weight_oihw, bias, stride, workspace, workspace_bytes, (cudaStream_t)stream);
   API_END(1)
 }
 
@@ -2371,37 +2218,15 @@ int cfb_conv2d_pertap_slice_nhwc(const float* in, const float* weight_oihw, cons
   CFB_REQUIRE(stride == 1 || stride == 2, "cfb_conv2d_pertap_slice_nhwc: stride must be 1 or 2");
   CFB_REQUIRE(ksize == 1 || stride == 2, "cfb_conv2d_pertap_slice_nhwc: 3x3 convs run stride 2 on the per-tap engine");
   CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_SILU, "cfb_conv2d_pertap_slice_nhwc: activation must be none or SiLU");
-  cudaStream_t st = (cudaStream_t)stream;
-  CFB_CHECK(cfb::async_status_init(st));
-  int dev = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  cfb::ConvArgs a;
-  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
-  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
-  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
-  CFB_REQUIRE(cfb::tc_supported(a), "cfb_conv2d_pertap_slice_nhwc: shape not supported by the wgmma engine");
-  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_pertap_workspace_bytes(n, h, w, cin, cout, ksize, stride),
-              "cfb_conv2d_pertap_slice_nhwc: workspace too small");
-  const size_t wn = (size_t)cout * cin * ksize * ksize;
-  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
-  __half* whi = (__half*)p; p += align256(wn * 2);
-  __half* wlo = (__half*)p; p += align256(wn * 2);
-  float* wsc = (float*)p; p += 256;
-  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
-  CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, ksize, wsc, st));
-  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.bias = bias; a.out_act = out_act; a.out = out;
-  a.out_pitch = out_pitch == cout ? 0 : out_pitch; a.out_c0 = out_c0;
-  return cfb::conv_tc(a, p, sms, st);
+  return pertap_nhwc("cfb_conv2d_pertap_slice_nhwc",
+                     cfb::pertap_args(in, n, h, w, cin, cout, ksize, stride, out, out_pitch, out_c0, out_act, nullptr), weight_oihw,
+                     bias, stride, workspace, workspace_bytes, (cudaStream_t)stream);
   API_END(1)
 }
 
 int64_t cfb_conv2d_pertap_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride) {
   if (n < 0 || h < 1 || w < 1 || cin < 1 || cout < 1 || !(ksize == 1 || ksize == 3) || !(stride == 1 || stride == 2)) return -1;
-  cfb::ConvArgs a;
-  a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize;
-  a.Ho = stride == 2 ? (h + 1) / 2 : h; a.Wo = stride == 2 ? (w + 1) / 2 : w;
-  a.mode = stride == 2 ? cfb::CONV_DOWN : cfb::CONV_SAME; a.down_pad = (stride == 2 && ksize == 3) ? 1 : 0;
+  const cfb::ConvArgs a = cfb::pertap_args(nullptr, n, h, w, cin, cout, ksize, stride, nullptr, 0, 0, cfb::OUT_NONE, nullptr);
   const size_t wn = (size_t)cout * cin * ksize * ksize;
   return (int64_t)(2 * align256(wn * 2) + 256 + cfb::tc_scratch_bytes(a) + 4096);
 }
@@ -2415,24 +2240,11 @@ cfb_retinaface* cfb_retinaface_create(void) {
   return n;
   API_END(nullptr)
 }
-void cfb_retinaface_destroy(cfb_retinaface* n) {
-  if (!n) return;
-  if (n->slab) {
-    int cur = -1;
-    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
-    if (sw) cudaSetDevice(n->device);
-    cudaFree(n->slab);
-    if (sw) cudaSetDevice(cur);
-  }
-  delete n;
-}
+void cfb_retinaface_destroy(cfb_retinaface* n) { delete n; }
 int cfb_retinaface_set_param(cfb_retinaface* n, const char* name, const float* dev_ptr, int64_t numel) {
   API_BEGIN
   CFB_REQUIRE(n && name && dev_ptr, "cfb_retinaface_set_param: NULL argument");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->raw[name] = {dev_ptr, numel};
-  n->prepared = false;
-  return 0;
+  return n->set_param(name, dev_ptr, numel);
   API_END(1)
 }
 int cfb_retinaface_prepare(cfb_retinaface* n, void* stream) {
@@ -2445,9 +2257,9 @@ int cfb_retinaface_prepare(cfb_retinaface* n, void* stream) {
 int64_t cfb_retinaface_workspace_bytes(cfb_retinaface* n, int32_t batch, int32_t h, int32_t w) {
   API_BEGIN
   if (!n) { cfb::set_error("cfb_retinaface_workspace_bytes: NULL net"); return -1; }
-  std::lock_guard<std::mutex> lk(n->mu);
-  if (cfb::rf_forward(n, (const float*)0x1000, nullptr, nullptr, nullptr, nullptr, batch, h, w, nullptr, 0, nullptr, true) != 0) return -1;
-  return (int64_t)n->arena.high() + 4096;
+  return n->dry_run([&] {
+    return cfb::rf_forward(n, (const float*)0x1000, nullptr, nullptr, nullptr, nullptr, batch, h, w, nullptr, 0, nullptr, true);
+  });
   API_END(-1)
 }
 int cfb_retinaface_forward(cfb_retinaface* n, const float* x_nchw, float* loc, float* conf, float* landms, int32_t batch, int32_t h,
@@ -2487,24 +2299,11 @@ cfb_yolov5face* cfb_yolov5face_create(void) {
   return n;
   API_END(nullptr)
 }
-void cfb_yolov5face_destroy(cfb_yolov5face* n) {
-  if (!n) return;
-  if (n->slab) {
-    int cur = -1;
-    const bool sw = cudaGetDevice(&cur) == cudaSuccess && n->device >= 0 && cur != n->device;
-    if (sw) cudaSetDevice(n->device);
-    cudaFree(n->slab);
-    if (sw) cudaSetDevice(cur);
-  }
-  delete n;
-}
+void cfb_yolov5face_destroy(cfb_yolov5face* n) { delete n; }
 int cfb_yolov5face_set_param(cfb_yolov5face* n, const char* name, const float* dev_ptr, int64_t numel) {
   API_BEGIN
   CFB_REQUIRE(n && name && dev_ptr, "cfb_yolov5face_set_param: NULL argument");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->raw[name] = {dev_ptr, numel};
-  n->prepared = false;
-  return 0;
+  return n->set_param(name, dev_ptr, numel);
   API_END(1)
 }
 int cfb_yolov5face_prepare(cfb_yolov5face* n, void* stream) {
@@ -2517,10 +2316,10 @@ int cfb_yolov5face_prepare(cfb_yolov5face* n, void* stream) {
 int64_t cfb_yolov5face_workspace_bytes(cfb_yolov5face* n, int32_t batch, int32_t h, int32_t w) {
   API_BEGIN
   if (!n) { cfb::set_error("cfb_yolov5face_workspace_bytes: NULL net"); return -1; }
-  std::lock_guard<std::mutex> lk(n->mu);
   float* const raw[3] = {nullptr, nullptr, nullptr};
-  if (cfb::yo_forward(n, (const float*)0x1000, nullptr, 0, 0, 0, 0, nullptr, raw, batch, h, w, nullptr, 0, nullptr, true) != 0) return -1;
-  return (int64_t)n->arena.high() + 4096;
+  return n->dry_run([&] {
+    return cfb::yo_forward(n, (const float*)0x1000, nullptr, 0, 0, 0, 0, nullptr, raw, batch, h, w, nullptr, 0, nullptr, true);
+  });
   API_END(-1)
 }
 int cfb_yolov5face_forward(cfb_yolov5face* n, const float* x_nchw, float* pred, float* raw0, float* raw1, float* raw2, int32_t batch,
@@ -2590,10 +2389,7 @@ int cfb_debug_set_stamps(int64_t* stamps) {
 int cfb_net_set_param(cfb_net* n, const char* name, const float* dev_ptr, int64_t numel) {
   API_BEGIN
   CFB_REQUIRE(n && name && dev_ptr, "cfb_net_set_param: NULL argument");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->raw[name] = {dev_ptr, numel};
-  n->prepared = false;
-  return 0;
+  return n->set_param(name, dev_ptr, numel);
   API_END(1)
 }
 

@@ -9,7 +9,6 @@ BatchNorm buffers, so ``detection_Resnet50_Final.pth`` loads strictly), same ``f
 as in the reference.  No CPU fallback; inference only.  The package imports neither torchvision nor cv2.
 """
 import ctypes
-import threading
 from collections import OrderedDict
 
 import numpy as np
@@ -17,6 +16,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .native import NativeNet
 
 RESNET50_BLOCKS = (3, 4, 6, 3)
 
@@ -134,80 +134,53 @@ def finish_detections(cand, conf_threshold, nms_threshold):
     return np.concatenate((bounding_boxes, landmarks), axis=1)
 
 
-class RetinaFace(nn.Module):
+def bn_net_init(name, entry, g):
+    """Default state of the detectors' entries: conv weights N(0, 1/fan_in), BatchNorm (1, 0) with running stats (0, 1),
+    conv biases 0."""
+    shape, dtype = entry
+    leaf = name.rsplit('.', 1)[-1]
+    if dtype == torch.int64:
+        return torch.tensor(0, dtype=torch.long)
+    if leaf in ('running_mean', 'running_var'):
+        return torch.zeros(shape) if leaf == 'running_mean' else torch.ones(shape)
+    if len(shape) == 4:
+        fan_in = shape[1] * shape[2] * shape[3]
+        return nn.Parameter(torch.randn(shape, generator=g) / fan_in ** 0.5)
+    return nn.Parameter(torch.ones(shape) if leaf == 'weight' else torch.zeros(shape))
+
+
+def cuda_u8_image(image, device, owner, kinds='a numpy array or a CUDA tensor'):
+    """One uint8 HWC BGR image of ``detect_faces`` (a numpy array, copied to ``device``, or a CUDA tensor) as a CUDA tensor."""
+    if isinstance(image, np.ndarray):
+        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+            raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {image.dtype} {image.shape}')
+        if device.type != 'cuda':
+            raise RuntimeError(f'{owner}: the module is not on a CUDA device; there is no CPU fallback')
+        return torch.from_numpy(np.ascontiguousarray(image)).to(device)
+    if torch.is_tensor(image):
+        if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
+            raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {image.dtype} {tuple(image.shape)}')
+        if not image.is_cuda:
+            raise RuntimeError(f'{owner}: a torch image must be a CUDA tensor; there is no CPU fallback')
+        return image
+    raise NotImplementedError(f'detect_faces takes {kinds}, got {type(image).__name__}')
+
+
+class RetinaFace(NativeNet):
     """Parameter holder with the reference's ``state_dict``, ``forward`` and ``detect_faces`` on the wgmma conv engine."""
 
     def __init__(self, network_name='resnet50', half=False, phase='test'):
-        super().__init__()
         if network_name != 'resnet50':
             raise NotImplementedError(f'codeformer_b200 builds RetinaFace with network_name="resnet50" (got {network_name!r}; '
                                       'mobile0.25 needs depthwise convs)')
         if half:
             raise NotImplementedError('codeformer_b200.RetinaFace runs in float32 (half=True is not built)')
+        super().__init__('retinaface', (), retinaface_spec(), bn_net_init)
         self.phase = phase
         self.half_inference = False
         self.model_name = f'retinaface_{network_name}'
         self.resize = 1.
-        g = torch.Generator().manual_seed(0)
-        for name, (shape, dtype) in retinaface_spec().items():
-            mod, parts = self, name.split('.')
-            for p in parts[:-1]:
-                if not hasattr(mod, p):
-                    mod.add_module(p, nn.Module())
-                mod = getattr(mod, p)
-            if dtype == torch.int64:
-                mod.register_buffer(parts[-1], torch.tensor(0, dtype=torch.long))
-            elif parts[-1] in ('running_mean', 'running_var'):
-                mod.register_buffer(parts[-1], torch.zeros(shape) if parts[-1] == 'running_mean' else torch.ones(shape))
-            elif len(shape) == 4:
-                fan_in = shape[1] * shape[2] * shape[3]
-                mod.register_parameter(parts[-1], nn.Parameter(torch.randn(shape, generator=g) / fan_in ** 0.5))
-            else:
-                is_gamma = parts[-1] == 'weight'
-                mod.register_parameter(parts[-1], nn.Parameter(torch.ones(shape) if is_gamma else torch.zeros(shape)))
-        object.__setattr__(self, '_lock', threading.Lock())
-        object.__setattr__(self, '_net', None)
-        object.__setattr__(self, '_sig', None)
-        object.__setattr__(self, '_keep', None)
-        object.__setattr__(self, '_ws', None)
         self.eval()
-
-    def train(self, mode=True):
-        if mode:
-            raise RuntimeError('codeformer_b200.RetinaFace is inference-only (BatchNorm runs on its running statistics); call .eval()')
-        return super().train(False)
-
-    def _prepare(self, device):
-        lib = _lib.load()
-        params = [(k, v) for k, v in self.state_dict(keep_vars=True).items() if v.dtype != torch.int64]
-        sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._net is not None and sig == self._sig:
-            return
-        if self._net is None:
-            h = lib.cfb_retinaface_create()
-            if not h:
-                _lib.check(1, 'cfb_retinaface_create')
-            object.__setattr__(self, '_net', ctypes.c_void_p(h))
-        keep = []
-        for k, v in params:
-            if v.device != device:
-                raise RuntimeError(f'parameter {k} is on {v.device} but the input is on {device}; call net.to(device)')
-            t = v.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            keep.append(t)
-            _lib.check(lib.cfb_retinaface_set_param(self._net, k.encode(), _lib.ptr(t), t.numel()), 'cfb_retinaface_set_param')
-        _lib.check(lib.cfb_retinaface_prepare(self._net, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)),
-                   'cfb_retinaface_prepare')
-        object.__setattr__(self, '_sig', sig)
-        object.__setattr__(self, '_keep', keep)
-
-    def __del__(self):
-        try:
-            if getattr(self, '_net', None) is not None:
-                _lib.load().cfb_retinaface_destroy(self._net)
-        except Exception:
-            pass
 
     def _run(self, x, u8):
         lib = _lib.load()
@@ -219,15 +192,10 @@ class RetinaFace(nn.Module):
             loc = torch.empty((B, P, 4), dtype=torch.float32, device=dev)
             conf = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
             landms = torch.empty((B, P, 10), dtype=torch.float32, device=dev)
-            need = lib.cfb_retinaface_workspace_bytes(self._net, B, H, W)
-            if need < 0:
-                _lib.check(1, 'cfb_retinaface_workspace_bytes')
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                object.__setattr__(self, '_ws', None)
-                object.__setattr__(self, '_ws', torch.empty(int(need), dtype=torch.uint8, device=dev))
+            ws = self._workspace(B, H, W, dev)
             fn = lib.cfb_retinaface_forward_u8 if u8 else lib.cfb_retinaface_forward
-            _lib.check(fn(self._net, _lib.ptr(x), _lib.ptr(loc), _lib.ptr(conf), _lib.ptr(landms), B, H, W, _lib.ptr(self._ws),
-                          self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'cfb_retinaface_forward')
+            _lib.check(fn(self._net, _lib.ptr(x), _lib.ptr(loc), _lib.ptr(conf), _lib.ptr(landms), B, H, W, _lib.ptr(ws),
+                          ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'cfb_retinaface_forward')
         return loc, conf, landms
 
     def forward(self, inputs):
@@ -270,21 +238,7 @@ class RetinaFace(nn.Module):
         (box, score, 5 landmarks), highest score first after NMS."""
         if not use_origin_size:
             raise NotImplementedError('codeformer_b200.RetinaFace.detect_faces runs at the original size (use_origin_size=True)')
-        if isinstance(image, np.ndarray):
-            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-                raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {image.dtype} {image.shape}')
-            dev = next(self.parameters()).device
-            if dev.type != 'cuda':
-                raise RuntimeError('RetinaFace.detect_faces: the module is not on a CUDA device; there is no CPU fallback')
-            img = torch.from_numpy(np.ascontiguousarray(image)).to(dev)
-        elif torch.is_tensor(image):
-            if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
-                raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {image.dtype} {tuple(image.shape)}')
-            if not image.is_cuda:
-                raise RuntimeError('RetinaFace.detect_faces: a torch image must be a CUDA tensor; there is no CPU fallback')
-            img = image
-        else:
-            raise NotImplementedError(f'detect_faces takes a numpy array or a CUDA tensor, got {type(image).__name__}')
+        img = cuda_u8_image(image, next(self.parameters()).device, 'RetinaFace.detect_faces')
         self.resize = 1
         h, w = int(img.shape[0]), int(img.shape[1])
         loc, conf, landms = self.forward_u8(img.unsqueeze(0))

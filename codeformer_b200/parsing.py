@@ -9,13 +9,13 @@ the conv weights when the native copy is prepared.  ``face_parse_mask`` is the c
 (argmax over the 19 classes + MASK_COLORMAP) on the device.  No CPU fallback; inference only (BatchNorm uses running stats).
 """
 import ctypes
-import threading
 
 import numpy as np
 import torch
 import torch.nn as nn
 
 from . import _lib
+from .native import NativeNet
 
 
 def parsenet_plan(in_size=512, out_size=512, min_feat_size=32, base_ch=64, res_depth=10, ch_range=(32, 256)):
@@ -87,73 +87,31 @@ def random_parsenet_state_dict(spec, seed=1):
     return sd
 
 
-class ParseNet(nn.Module):
+def _parsenet_init(name, entry, g):
+    """The reference's default initialisation: BatchNorm (1, 0) with running stats (0, 1), filters U(+-1/sqrt(fan_in)),
+    conv biases 0."""
+    shape, dtype = entry
+    leaf = name.rsplit('.', 1)[-1]
+    if dtype == torch.int64:
+        return torch.tensor(0, dtype=torch.long)
+    if leaf in ('running_mean', 'running_var'):
+        return torch.zeros(shape) if leaf == 'running_mean' else torch.ones(shape)
+    if len(shape) == 4:
+        fan_in = shape[1] * shape[2] * shape[3]
+        return nn.Parameter((torch.rand(shape, generator=g) * 2 - 1) / fan_in ** 0.5)
+    return nn.Parameter(torch.ones(shape) if name.endswith('norm.weight') else torch.zeros(shape))
+
+
+class ParseNet(NativeNet):
     """Parameter holder with the reference's ``state_dict`` + ``forward`` on the wgmma conv engine."""
 
     def __init__(self, in_size=128, out_size=128, min_feat_size=32, base_ch=64, parsing_ch=19, res_depth=10,
                  relu_type='LeakyReLU', norm_type='bn', ch_range=[32, 256]):
-        super().__init__()
         if relu_type.lower() != 'leakyrelu' or norm_type.lower() != 'bn':
             raise NotImplementedError("codeformer_b200 builds ParseNet with relu_type='LeakyReLU', norm_type='bn' (the shipped model)")
+        super().__init__('parsenet', (in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, int(ch_range[0]), int(ch_range[1])),
+                         parsenet_spec(in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, tuple(ch_range)), _parsenet_init)
         self.res_depth, self.parsing_ch = res_depth, parsing_ch
-        self._cfg = (in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, int(ch_range[0]), int(ch_range[1]))
-        g = torch.Generator().manual_seed(0)
-        for name, (shape, dtype) in parsenet_spec(in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, tuple(ch_range)).items():
-            mod, parts = self, name.split('.')
-            for p in parts[:-1]:
-                if not hasattr(mod, p):
-                    mod.add_module(p, nn.Module())
-                mod = getattr(mod, p)
-            if dtype == torch.int64:
-                mod.register_buffer(parts[-1], torch.tensor(0, dtype=torch.long))
-            elif parts[-1] in ('running_mean', 'running_var'):
-                mod.register_buffer(parts[-1], torch.zeros(shape) if parts[-1] == 'running_mean' else torch.ones(shape))
-            elif len(shape) == 4:
-                fan_in = shape[1] * shape[2] * shape[3]
-                mod.register_parameter(parts[-1], nn.Parameter((torch.rand(shape, generator=g) * 2 - 1) / fan_in ** 0.5))
-            else:
-                mod.register_parameter(parts[-1], nn.Parameter(torch.ones(shape) if name.endswith('norm.weight') else torch.zeros(shape)))
-        object.__setattr__(self, '_lock', threading.Lock())
-        object.__setattr__(self, '_net', None)
-        object.__setattr__(self, '_sig', None)
-        object.__setattr__(self, '_keep', None)
-        object.__setattr__(self, '_ws', None)
-
-    def train(self, mode=True):
-        if mode:
-            raise RuntimeError('codeformer_b200.ParseNet is inference-only (BatchNorm runs on its running statistics); call .eval()')
-        return super().train(False)
-
-    def _prepare(self, device):
-        lib = _lib.load()
-        params = [(k, v) for k, v in self.state_dict(keep_vars=True).items() if v.dtype != torch.int64]
-        sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._net is not None and sig == self._sig:
-            return
-        if self._net is None:
-            h = lib.cfb_parsenet_create(*self._cfg)
-            if not h:
-                _lib.check(1, 'cfb_parsenet_create')
-            object.__setattr__(self, '_net', ctypes.c_void_p(h))
-        keep = []
-        for k, v in params:
-            if v.device != device:
-                raise RuntimeError(f'parameter {k} is on {v.device} but the input is on {device}; call net.to(device)')
-            t = v.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            keep.append(t)
-            _lib.check(lib.cfb_parsenet_set_param(self._net, k.encode(), _lib.ptr(t), t.numel()), 'cfb_parsenet_set_param')
-        _lib.check(lib.cfb_parsenet_prepare(self._net, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)), 'cfb_parsenet_prepare')
-        object.__setattr__(self, '_sig', sig)
-        object.__setattr__(self, '_keep', keep)
-
-    def __del__(self):
-        try:
-            if getattr(self, '_net', None) is not None:
-                _lib.load().cfb_parsenet_destroy(self._net)
-        except Exception:
-            pass
 
     def forward(self, x, return_img=True):
         """x [B,3,H,W] fp32 CUDA -> (out_mask [B,parsing_ch,H,W], out_img [B,3,H,W])  (parsenet.py:188-194)."""
@@ -169,14 +127,9 @@ class ParseNet(nn.Module):
             self._prepare(dev)
             mask = torch.empty((B, self.parsing_ch, H, W), dtype=torch.float32, device=dev)
             img = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev) if return_img else None
-            need = lib.cfb_parsenet_workspace_bytes(self._net, B, H, W)
-            if need < 0:
-                _lib.check(1, 'cfb_parsenet_workspace_bytes')
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                object.__setattr__(self, '_ws', None)
-                object.__setattr__(self, '_ws', torch.empty(int(need), dtype=torch.uint8, device=dev))
-            _lib.check(lib.cfb_parsenet_forward(self._net, _lib.ptr(x), _lib.ptr(mask), _lib.ptr(img), B, H, W, _lib.ptr(self._ws),
-                                                self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+            ws = self._workspace(B, H, W, dev)
+            _lib.check(lib.cfb_parsenet_forward(self._net, _lib.ptr(x), _lib.ptr(mask), _lib.ptr(img), B, H, W, _lib.ptr(ws),
+                                                ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                        'cfb_parsenet_forward')
         return mask, img
 

@@ -11,7 +11,6 @@ colour handling, reflect pre/mod padding, the tile loop -- written against torch
 """
 import ctypes
 import math
-import threading
 
 import numpy as np
 import torch
@@ -20,76 +19,31 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import spec as S
+from .native import NativeNet
 from .registry import ARCH_REGISTRY
 
 
+def _rrdbnet_init(name, shape, g):
+    """Kaiming-normal * 0.1 weights and zero biases, like default_init_weights (arch_util.py:18-36)."""
+    if name.endswith('.weight'):
+        fan_in = shape[1] * shape[2] * shape[3]
+        return nn.Parameter(torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_in) * 0.1)
+    return nn.Parameter(torch.zeros(shape))
+
+
 @ARCH_REGISTRY.register()
-class RRDBNet(nn.Module):
+class RRDBNet(NativeNet):
     """Parameters of the reference's RRDBNet (identical ``state_dict``) with ``forward`` on the wgmma conv engine."""
 
+    train = nn.Module.train          # no BatchNorm: training mode changes nothing here
+
     def __init__(self, num_in_ch, num_out_ch, scale=4, num_feat=64, num_block=23, num_grow_ch=32):
-        super().__init__()
         if num_feat != 64 or num_grow_ch != 32:
             raise NotImplementedError('codeformer_b200 builds RRDBNet for num_feat=64, num_grow_ch=32 (the RealESRGAN models)')
+        super().__init__('rrdb', (num_in_ch, num_out_ch, scale, num_feat, num_block, num_grow_ch),
+                         S.rrdbnet_spec(num_in_ch, num_out_ch, scale, num_feat, num_block, num_grow_ch), _rrdbnet_init)
         self.scale, self.num_in_ch, self.num_out_ch = scale, num_in_ch, num_out_ch
         self.num_feat, self.num_block, self.num_grow_ch = num_feat, num_block, num_grow_ch
-        g = torch.Generator().manual_seed(0)
-        params = {}
-        for name, shape in S.rrdbnet_spec(num_in_ch, num_out_ch, scale, num_feat, num_block, num_grow_ch).items():
-            if name.endswith('.weight'):                       # kaiming-normal * 0.1 like default_init_weights (arch_util.py:18-36)
-                fan_in = shape[1] * shape[2] * shape[3]
-                t = torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_in) * 0.1
-            else:
-                t = torch.zeros(shape)
-            params[name] = t
-        # nested modules so that state_dict() yields the reference's dotted names
-        self._register_tree(params)
-        object.__setattr__(self, '_lock', threading.Lock())
-        object.__setattr__(self, '_net', None)
-        object.__setattr__(self, '_sig', None)
-        object.__setattr__(self, '_keep', None)
-        object.__setattr__(self, '_ws', None)
-
-    def _register_tree(self, params):
-        for name, t in params.items():
-            mod = self
-            parts = name.split('.')
-            for p in parts[:-1]:
-                if not hasattr(mod, p):
-                    mod.add_module(p, nn.Module())
-                mod = getattr(mod, p)
-            mod.register_parameter(parts[-1], nn.Parameter(t))
-
-    def _prepare(self, device):
-        lib = _lib.load()
-        params = list(self.state_dict(keep_vars=True).items())
-        sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._net is not None and sig == self._sig:
-            return
-        if self._net is None:
-            h = lib.cfb_rrdb_create(self.num_in_ch, self.num_out_ch, self.scale, self.num_feat, self.num_block, self.num_grow_ch)
-            if not h:
-                _lib.check(1, 'cfb_rrdb_create')
-            object.__setattr__(self, '_net', ctypes.c_void_p(h))
-        keep = []
-        for k, v in params:
-            if v.device != device:
-                raise RuntimeError(f'parameter {k} is on {v.device} but the input is on {device}; call net.to(device)')
-            t = v.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            keep.append(t)
-            _lib.check(lib.cfb_rrdb_set_param(self._net, k.encode(), _lib.ptr(t), t.numel()), 'cfb_rrdb_set_param')
-        _lib.check(lib.cfb_rrdb_prepare(self._net, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)), 'cfb_rrdb_prepare')
-        object.__setattr__(self, '_sig', sig)
-        object.__setattr__(self, '_keep', keep)
-
-    def __del__(self):
-        try:
-            if getattr(self, '_net', None) is not None:
-                _lib.load().cfb_rrdb_destroy(self._net)
-        except Exception:
-            pass
 
     def forward(self, x):
         """x [B, num_in_ch, H, W] fp32 CUDA -> [B, num_out_ch, H*scale, W*scale] (rrdbnet_arch.py:103-119)."""
@@ -110,11 +64,8 @@ class RRDBNet(nn.Module):
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
             out = torch.empty((B, self.num_out_ch, H // us * 4, W // us * 4), dtype=torch.float32, device=dev)
-            need = lib.cfb_rrdb_workspace_bytes(self._net, B, H, W)
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                object.__setattr__(self, '_ws', None)
-                object.__setattr__(self, '_ws', torch.empty(int(need), dtype=torch.uint8, device=dev))
-            _lib.check(lib.cfb_rrdb_forward(self._net, _lib.ptr(x), _lib.ptr(out), B, H, W, _lib.ptr(self._ws), self._ws.numel(),
+            ws = self._workspace(B, H, W, dev)
+            _lib.check(lib.cfb_rrdb_forward(self._net, _lib.ptr(x), _lib.ptr(out), B, H, W, _lib.ptr(ws), ws.numel(),
                                             ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'cfb_rrdb_forward')
         return out
 

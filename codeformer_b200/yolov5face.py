@@ -11,15 +11,14 @@ as in the reference.  No CPU fallback; inference only.  The package imports neit
 import ctypes
 import math
 import os
-import threading
 from collections import OrderedDict
 
 import numpy as np
 import torch
-import torch.nn as nn
 
 from . import _lib
-from .detection import nms
+from .detection import bn_net_init, cuda_u8_image, nms
+from .native import NativeNet
 
 # (layer, c1, c2, bottlenecks) of the C3 blocks of yolov5l.yaml; the backbone ones (1, 3, 5) have shortcuts
 YOLOV5L_C3 = ((1, 64, 128, 3), (3, 256, 256, 9), (5, 512, 512, 9), (8, 1024, 1024, 3), (12, 1024, 512, 3), (16, 512, 256, 3),
@@ -199,77 +198,23 @@ def letterbox_geometry(h0, w0, target_size=None):
     return first, second, (nh + top + bottom, nw + left + right), (top, left)
 
 
-class YOLOv5lFace(nn.Module):
+def _yolov5l_init(name, entry, g):
+    """The detectors' defaults (``bn_net_init``), plus Detect's anchor buffers."""
+    leaf = name.rsplit('.', 1)[-1]
+    if leaf in ('anchors', 'anchor_grid'):
+        return _anchor_buffers()[0 if leaf == 'anchors' else 1].clone()
+    return bn_net_init(name, entry, g)
+
+
+class YOLOv5lFace(NativeNet):
     """Parameter holder with the reference ``Model('yolov5l.yaml')``'s ``state_dict``, ``stride`` and ``forward`` on the wgmma
     conv engine."""
 
     def __init__(self):
-        super().__init__()
-        g = torch.Generator().manual_seed(0)
-        anchors, anchor_grid = _anchor_buffers()
-        for name, (shape, dtype) in yolov5l_spec().items():
-            mod, parts = self, name.split('.')
-            for p in parts[:-1]:
-                if not hasattr(mod, p):
-                    mod.add_module(p, nn.Module())
-                mod = getattr(mod, p)
-            if dtype == torch.int64:
-                mod.register_buffer(parts[-1], torch.tensor(0, dtype=torch.long))
-            elif parts[-1] in ('anchors', 'anchor_grid'):
-                mod.register_buffer(parts[-1], anchors.clone() if parts[-1] == 'anchors' else anchor_grid.clone())
-            elif parts[-1] in ('running_mean', 'running_var'):
-                mod.register_buffer(parts[-1], torch.zeros(shape) if parts[-1] == 'running_mean' else torch.ones(shape))
-            elif len(shape) == 4:
-                fan_in = shape[1] * shape[2] * shape[3]
-                mod.register_parameter(parts[-1], nn.Parameter(torch.randn(shape, generator=g) / fan_in ** 0.5))
-            else:
-                is_gamma = parts[-1] == 'weight'
-                mod.register_parameter(parts[-1], nn.Parameter(torch.ones(shape) if is_gamma else torch.zeros(shape)))
+        super().__init__('yolov5face', (), yolov5l_spec(), _yolov5l_init)
         self.stride = torch.tensor([8., 16., 32.])
         self.yaml_file = 'yolov5l.yaml'
-        object.__setattr__(self, '_lock', threading.Lock())
-        object.__setattr__(self, '_net', None)
-        object.__setattr__(self, '_sig', None)
-        object.__setattr__(self, '_keep', None)
-        object.__setattr__(self, '_ws', None)
         self.eval()
-
-    def train(self, mode=True):
-        if mode:
-            raise RuntimeError('codeformer_b200.YOLOv5lFace is inference-only (BatchNorm runs on its running statistics); call .eval()')
-        return super().train(False)
-
-    def _prepare(self, device):
-        lib = _lib.load()
-        params = [(k, v) for k, v in self.state_dict(keep_vars=True).items() if v.dtype != torch.int64]
-        sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._net is not None and sig == self._sig:
-            return
-        if self._net is None:
-            h = lib.cfb_yolov5face_create()
-            if not h:
-                _lib.check(1, 'cfb_yolov5face_create')
-            object.__setattr__(self, '_net', ctypes.c_void_p(h))
-        keep = []
-        for k, v in params:
-            if v.device != device:
-                raise RuntimeError(f'parameter {k} is on {v.device} but the input is on {device}; call .to(device)')
-            t = v.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            keep.append(t)
-            _lib.check(lib.cfb_yolov5face_set_param(self._net, k.encode(), _lib.ptr(t), t.numel()), 'cfb_yolov5face_set_param')
-        _lib.check(lib.cfb_yolov5face_prepare(self._net, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)),
-                   'cfb_yolov5face_prepare')
-        object.__setattr__(self, '_sig', sig)
-        object.__setattr__(self, '_keep', keep)
-
-    def __del__(self):
-        try:
-            if getattr(self, '_net', None) is not None:
-                _lib.load().cfb_yolov5face_destroy(self._net)
-        except Exception:
-            pass
 
     def _run(self, x, H, W, u8=None, raw=True):
         """x: fp32 NCHW [B,3,H,W], or uint8 BGR [B,h,w,3] with u8 = (top, left) inside the H x W canvas."""
@@ -284,19 +229,14 @@ class YOLOv5lFace(nn.Module):
             pred = torch.empty((B, P, 16), dtype=torch.float32, device=dev)
             raws = [torch.empty((B, 3, H // s, W // s, 16), dtype=torch.float32, device=dev) for s in STRIDES] if raw else []
             rp = [_lib.ptr(r) for r in raws] if raw else [None] * 3
-            need = lib.cfb_yolov5face_workspace_bytes(self._net, B, H, W)
-            if need < 0:
-                _lib.check(1, 'cfb_yolov5face_workspace_bytes')
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                object.__setattr__(self, '_ws', None)
-                object.__setattr__(self, '_ws', torch.empty(int(need), dtype=torch.uint8, device=dev))
+            ws = self._workspace(B, H, W, dev)
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             if u8 is None:
-                _lib.check(lib.cfb_yolov5face_forward(self._net, _lib.ptr(x), _lib.ptr(pred), *rp, B, H, W, _lib.ptr(self._ws),
-                                                      self._ws.numel(), st), 'cfb_yolov5face_forward')
+                _lib.check(lib.cfb_yolov5face_forward(self._net, _lib.ptr(x), _lib.ptr(pred), *rp, B, H, W, _lib.ptr(ws),
+                                                      ws.numel(), st), 'cfb_yolov5face_forward')
             else:
                 _lib.check(lib.cfb_yolov5face_forward_u8(self._net, _lib.ptr(x), x.shape[1], x.shape[2], u8[0], u8[1], _lib.ptr(pred),
-                                                         *rp, B, H, W, _lib.ptr(self._ws), self._ws.numel(), st),
+                                                         *rp, B, H, W, _lib.ptr(ws), ws.numel(), st),
                            'cfb_yolov5face_forward_u8')
         return pred, raws
 
@@ -365,20 +305,7 @@ class YoloDetector:
         dev = next(self.detector.parameters()).device
         if dev.type != 'cuda':
             raise RuntimeError('YoloDetector.detect_faces: the detector is not on a CUDA device; there is no CPU fallback')
-        batch = []
-        for im in images:
-            if isinstance(im, np.ndarray):
-                if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
-                    raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {im.dtype} {im.shape}')
-                batch.append(torch.from_numpy(np.ascontiguousarray(im)).to(dev))
-            elif torch.is_tensor(im):
-                if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
-                    raise NotImplementedError(f'detect_faces takes uint8 HWC BGR images with 3 channels, got {im.dtype} {tuple(im.shape)}')
-                if not im.is_cuda:
-                    raise RuntimeError('YoloDetector.detect_faces: a torch image must be a CUDA tensor; there is no CPU fallback')
-                batch.append(im.to(dev))
-            else:
-                raise NotImplementedError(f'detect_faces takes numpy arrays or CUDA tensors, got {type(im).__name__}')
+        batch = [cuda_u8_image(im, dev, 'YoloDetector.detect_faces', 'numpy arrays or CUDA tensors').to(dev) for im in images]
         shapes = [tuple(int(s) for s in im.shape) for im in batch]
         if len(set(shapes)) != 1:
             raise ValueError(f'detect_faces: the images of one call must have the same size, got {shapes}')
