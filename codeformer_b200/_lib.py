@@ -64,6 +64,9 @@ SIGNATURES = {
                                    _P, _P, _P, c_int32, POINTER(c_float)]),
     'cfb_debug_conv_tc': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                  _P, _P, c_int32, _P, _P, _P, c_float, _P, _P, _P, c_int64, _P, POINTER(c_int32)]),
+    'cfb_debug_gn_partials_workspace_bytes': (c_int64, [c_int32, c_int32]),
+    'cfb_debug_gn_coef_from_partials': (c_int, [_P, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, c_int64, _P]),
+    'cfb_debug_gn_cat_partials': (c_int, [_P, _P, _P, c_int64, c_int32, _P]),
     'cfb_rrdb_create': (c_void_p, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32]),
     'cfb_rrdb_destroy': (None, [_P]),
     'cfb_rrdb_set_param': (c_int, [_P, c_char_p, _P, c_int64]),

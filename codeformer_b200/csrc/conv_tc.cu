@@ -578,7 +578,7 @@ struct TcParams {
   float* out;
   __half* pl_hi;            // optional: `out` again as fp16 hi / lo planes (operand of a following raw-input conv)
   __half* pl_lo;
-  float* gn_part;           // optional GroupNorm(32) partial sums of `out`: [m_tile*4 + warp][32][2]
+  float* gn_part;           // optional GroupNorm(32) partials of `out`: [m_tile*4 + warp][32][mean, M2]
   int gn_cpg;               // channels per group = Cout/32
 #if CFB_TC_STAMPS
   long long* dbg;           // diagnostics (cfb_debug_set_stamps): CTA 0 writes clock64() at its role hand-offs; null in production
@@ -647,7 +647,7 @@ struct TcCfg {
 // The MMA warpgroup therefore only accumulates `chunk` k-blocks (64 K-elements each) per partial sum, issuing the small
 // cross terms (lo*hi, hi*lo) of every k-step before hi*hi, and the epilogue warps fold every finished partial sum into fp32
 // registers with round-to-nearest adds.
-// CPG > 0: the epilogue also emits GroupNorm(32) partial sums of the stored tile (CPG = Cout/32 channels per group).
+// CPG > 0: the epilogue also emits GroupNorm(32) partials (mean, M2) of the stored tile (CPG = Cout/32 channels per group).
 // CM (channel-major, BN = 64 only): the MMA warpgroup computes the tile transposed, D^T[64 channels x 128 pixels] =
 // W[64 x K] * X[128 x K]^T, as one m64n128k16 per product and k-step (weights = A operand, halo patch = B operand), and stores
 // each partial sum into the slot as [pixel][channel]: the epilogue is that of the pixel-major 128 x 64 tile.
@@ -1164,7 +1164,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // statistics are off, and the host has moved p.out to the slice's first channel)
     const int64_t SW = (int64_t)(p.up4 ? 2 : 1) * (HALO ? p.Cout : p.out_pitch), SH = SW * p.Wo;
     // every tile lies inside the image unless the image size is not a multiple of the tile (per-tap engine only): then the
-    // outside rows / columns of the last tiles are neither stored nor counted in the GroupNorm partials
+    // outside rows / columns of the last tiles are not stored (such convs emit no GroupNorm partials)
     const int ts = p.up4 ? 2 : 1;
     const bool whole_tiles = HALO || (p.tiles_y * BH * ts == p.Ho && p.tiles_x * BW * ts == p.Wo);
     int slot = 0;
@@ -1328,7 +1328,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         // global offsets of the (row, chunk) items of this lane, then their residual loads in flight at once: all 8 rows, or two
         // batches of 4 in the register-capped (96-register) BN = 64 transform variants
         constexpr int RB = (XF && !WIDE) ? 4 : 8;
-        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
+        // GroupNorm partials: sums of deviations from the first value of the group this lane sees (k0, k1), so that a large
+        // group mean does not cancel against the sum of squares (statistics need whole tiles: every value is inside)
+        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f, k0 = 0.f, k1 = 0.f;
 #pragma unroll
         for (int ib = 0; ib < 8; ib += RB) {
         int64_t offs[RB];
@@ -1391,25 +1393,29 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             *reinterpret_cast<uint2*>(p.pl_lo + off) = pl;
           }
           if constexpr (CPG == 2) {
-            s0 += v.x + v.y; q0 += fmaf(v.x, v.x, v.y * v.y);
-            s1 += v.z + v.w; q1 += fmaf(v.z, v.z, v.w * v.w);
+            if (it == 0) { k0 = v.x; k1 = v.z; }
+            const float a = v.x - k0, b = v.y - k0, c = v.z - k1, d = v.w - k1;
+            s0 += a + b; q0 += fmaf(a, a, b * b);
+            s1 += c + d; q1 += fmaf(c, c, d * d);
           } else if constexpr (CPG >= 4) {
-            s0 += (v.x + v.y) + (v.z + v.w);
-            q0 += fmaf(v.x, v.x, v.y * v.y) + fmaf(v.z, v.z, v.w * v.w);
+            if (it == 0) k0 = v.x;
+            const float a = v.x - k0, b = v.y - k0, c = v.z - k0, d = v.w - k0;
+            s0 += (a + b) + (c + d);
+            q0 += fmaf(a, a, b * b) + fmaf(c, c, d * d);
           }
         }
         }
         if constexpr (CPG > 0) {
-          // GroupNorm partial sums of the values just stored: reduce over the 4 row-lanes (xor 8, 16) and, for groups
-          // wider than one chunk, over the chunk-lanes of the group; fixed order => deterministic
-          s0 += __shfl_xor_sync(0xffffffffu, s0, 8); q0 += __shfl_xor_sync(0xffffffffu, q0, 8);
-          s0 += __shfl_xor_sync(0xffffffffu, s0, 16); q0 += __shfl_xor_sync(0xffffffffu, q0, 16);
-          if constexpr (CPG == 2) {
-            s1 += __shfl_xor_sync(0xffffffffu, s1, 8); q1 += __shfl_xor_sync(0xffffffffu, q1, 8);
-            s1 += __shfl_xor_sync(0xffffffffu, s1, 16); q1 += __shfl_xor_sync(0xffffffffu, q1, 16);
-          }
-          if constexpr (CPG >= 8) { s0 += __shfl_xor_sync(0xffffffffu, s0, 1); q0 += __shfl_xor_sync(0xffffffffu, q0, 1); }
-          if constexpr (CPG >= 16) { s0 += __shfl_xor_sync(0xffffffffu, s0, 2); q0 += __shfl_xor_sync(0xffffffffu, q0, 2); }
+          // GroupNorm partials of the values just stored, as (mean, M2 = sum of squared deviations from the mean) of each
+          // slot: this lane's 8 rows x (CPG >= 4 ? 4 : 2) values first, then equal-count merges over the 4 row-lanes (xor 8,
+          // 16) and, for groups wider than one chunk, over the chunk-lanes of the group; fixed order => deterministic
+          constexpr float NL = CPG == 2 ? 16.f : 32.f;
+          gn_lane_moments(s0, q0, k0, NL);
+          if constexpr (CPG == 2) gn_lane_moments(s1, q1, k1, NL);
+          gn_merge_xor(s0, q0, 8, NL); gn_merge_xor(s0, q0, 16, 2.f * NL);
+          if constexpr (CPG == 2) { gn_merge_xor(s1, q1, 8, NL); gn_merge_xor(s1, q1, 16, 2.f * NL); }
+          if constexpr (CPG >= 8) gn_merge_xor(s0, q0, 1, 4.f * NL);
+          if constexpr (CPG >= 16) gn_merge_xor(s0, q0, 2, 8.f * NL);
           constexpr int CL = (CPG >= 4) ? CPG / 4 : 1;         // chunk-lanes per group
           if (rsub == 0 && (cch & (CL - 1)) == 0) {
             float* gp = p.gn_part + ((int64_t)mt * 4 + lg) * 64;
@@ -1660,9 +1666,10 @@ static int tc_tile_kind(const ConvArgs& a, const TcGeom& g) {
 
 int tc_tile_n(const ConvArgs& a) { return tc_tile_kind(a, tc_geometry(a)); }
 
-// GroupNorm partial sums can be emitted for Cout in {64, 128, 256, 512} (2 .. 16 channels per group inside a 64-wide n-tile)
+// GroupNorm partials can be emitted for Cout in {64, 128, 256, 512} on whole tiles (2 .. 16 channels per group inside a 64-wide n-tile)
 bool tc_can_emit_stats(const ConvArgs& a) {
-  if (!tc_supported(a)) return false;
+  // every slot must hold 32 pixels of the image: (mean, M2) slots cannot skip the outside rows of a ragged tile
+  if (!tc_tiles_exact(a)) return false;
   if (a.Cout % 128 == 0) return a.Cout == 128 || a.Cout == 256 || a.Cout == 512;
   return a.Cout == 64;
 }

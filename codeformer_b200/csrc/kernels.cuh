@@ -98,6 +98,25 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     }                                                                                               \
     ::cfb::count_launch();                                                                          \
   } while (0)
+
+// ---- GroupNorm partial slots ----------------------------------------------------------------------
+// A slot holds (mean, M2) of its values, M2 = sum of squared deviations from the slot mean, never (sum, sum of squares): with
+// a group mean r times its standard deviation, fp32 sums of squares lose the variance to cancellation like (1 + r^2) * 2^-24,
+// the moments only like r * 2^-24 (through the rounding of the mean).  Producers sum the deviations from one value k of the
+// lane (s = sum (x - k), q = sum (x - k)^2 over n values) and turn them into moments ...
+__device__ __forceinline__ void gn_lane_moments(float& s, float& q, float k, float n) {
+  const float d = s * (1.f / n);          // n is a power of two: exact
+  q = fmaxf(fmaf(-s, d, q), 0.f);
+  s = k + d;
+}
+// ... then merge equal counts (n values each) with lane ^ o (Chan et al.): mean = (ma + mb) / 2, M2 = M2a + M2b +
+// (ma - mb)^2 * 2n / 4.  Symmetric in the two lanes, so both hold the same bits afterwards.
+__device__ __forceinline__ void gn_merge_xor(float& mean, float& m2, int o, float n) {
+  const float om = __shfl_xor_sync(0xffffffffu, mean, o), oq = __shfl_xor_sync(0xffffffffu, m2, o);
+  const float d = mean - om;
+  m2 = (m2 + oq) + (d * d) * (0.5f * n);
+  mean = 0.5f * (mean + om);
+}
 #endif
 
 enum InAct { IN_NONE = 0, IN_SILU = 1 };
@@ -129,7 +148,7 @@ struct ConvArgs {
   const float* sft_scale = nullptr;
   float sft_w = 0.f;
   float* out = nullptr;             // [N,Ho,Wo,Cout]
-  // tensor-core engine only: GroupNorm(32) partial sums of `out`, [N*tiles_per_image*4][32 groups][2] floats
+  // tensor-core engine only: GroupNorm(32) partials of `out`, [N*tiles_per_image*4][32 groups][mean, M2] floats
   float* gn_part = nullptr;
   // tensor-core engine only: also emit `out` as fp16 hi/lo operand planes for a following conv that consumes it raw
   void* out_planes = nullptr;       // [hi plane | lo plane], each align1024(N*Ho*Wo*Cout*2) bytes
@@ -162,7 +181,7 @@ struct ConvArgs {
 
 int conv_f32(const ConvArgs& a, cudaStream_t st);                       // CUDA-core fp32 implicit GEMM
 // first conv: x NCHW [N,3,H,W] -> NHWC [N,H,W,Cout], 3x3 p1; weight [27][Cout] (tap-major, then cin)
-// gn_part (optional): GroupNorm(32) partial sums of `out`, [N * H*W/32 slots][32 groups][sum, sum of squares] (the layout
+// gn_part (optional): GroupNorm(32) partials of `out`, [N * H*W/32 slots][32 groups][mean, M2] (the layout
 // gn_coef_from_partials reads; slots per image = H*W/32)
 int conv_first(const float* x_nchw, const float* wgt, const float* bias, float* out, int N, int H, int W, int Cout,
                cudaStream_t st, float* gn_part = nullptr);
@@ -216,13 +235,13 @@ int relayout_oihw_to_tck(const float* oihw, float* out, int Cout, int Cin, int k
 size_t gn_workspace_bytes(int N, int HW, int C);
 int gn_coef(const float* x, const float* gamma, const float* beta, float* scale, float* shift, int N, int HW, int C,
             int groups, float eps, void* ws, cudaStream_t st);
-// finalize from the tensor-core epilogue's partial sums (slots per image = tiles_per_image*4)
+// finalize from the (mean, M2) slots of the tensor-core epilogue or conv_first (slots per image = H*W/32)
 // scratch: gn_final_scratch_bytes(N, slots) bytes; counters: N zero-initialised unsigned (left zero again by the kernel)
 size_t gn_final_scratch_bytes(int N, int slots);
 int gn_coef_from_partials(const float* part, int slots, const float* gamma, const float* beta, float* scale, float* shift,
                           int N, int HW, int C, int groups, float eps, void* scratch, unsigned* counters, cudaStream_t st);
-// partial sums of cat([a,b]) (2C channels, 32 groups) from the partial sums of a and b (C channels each)
-int gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, cudaStream_t st);
+// partials of cat([a,b]) (2C channels, 32 groups) from the partials of a and b (C channels each)
+int gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, int C, cudaStream_t st);
 int affine_act(const float* x, const float* scale, const float* shift, float* y, int N, int HW, int C, int act,
                cudaStream_t st);
 

@@ -814,7 +814,7 @@ struct Fwd {
       cat.gn_slots = dec.gn_slots;
       CFB_CHECK(alloc_raw((void**)&cat_part, (size_t)dec.N * cat.gn_slots * 64 * sizeof(float)));
       cat.gn_part = cat_part;
-      if (!dry) CFB_CHECK(gn_cat_partials(enc_feat.gn_part, dec.gn_part, cat.gn_part, (int64_t)dec.N * cat.gn_slots, st));
+      if (!dry) CFB_CHECK(gn_cat_partials(enc_feat.gn_part, dec.gn_part, cat.gn_part, (int64_t)dec.N * cat.gn_slots, dec.C, st));
     }
     Tensor e;
     CFB_CHECK(resblock(f.enc, cat, e, true));      // scale.0 / shift.0 both read `e` raw: one set of planes, no prep
@@ -2888,6 +2888,30 @@ int cfb_group_norm_coef(const float* x, const float* gamma, const float* beta, f
   CFB_REQUIRE(x && gamma && beta && scale && shift && workspace, "cfb_group_norm_coef: NULL argument");
   CFB_REQUIRE(workspace_bytes >= (int64_t)cfb::gn_workspace_bytes(n, hw, c), "cfb_group_norm_coef: workspace too small");
   return cfb::gn_coef(x, gamma, beta, scale, shift, n, hw, c, groups, eps, workspace, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_debug_gn_partials_workspace_bytes(int32_t n, int32_t slots) {
+  return (int64_t)(align256(cfb::gn_final_scratch_bytes(n, slots)) + align256((size_t)n * sizeof(unsigned)));
+}
+int cfb_debug_gn_coef_from_partials(const float* part, int32_t slots, const float* gamma, const float* beta, float* scale,
+                                    float* shift, int32_t n, int32_t hw, int32_t c, float eps, void* workspace,
+                                    int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(part && gamma && beta && scale && shift && workspace && n >= 0 && slots > 0,
+              "cfb_debug_gn_coef_from_partials: bad argument");
+  CFB_REQUIRE(workspace_bytes >= cfb_debug_gn_partials_workspace_bytes(n, slots), "cfb_debug_gn_coef_from_partials: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  // finalize scratch, then the ticket counters, which the kernel needs zero on entry
+  unsigned* ctr = (unsigned*)((char*)workspace + align256(cfb::gn_final_scratch_bytes(n, slots)));
+  CFB_CUDA(cudaMemsetAsync(ctr, 0, (size_t)n * sizeof(unsigned), st));
+  return cfb::gn_coef_from_partials(part, slots, gamma, beta, scale, shift, n, hw, c, 32, eps, workspace, ctr, st);
+  API_END(1)
+}
+int cfb_debug_gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, int32_t c,
+                              void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(a_part && b_part && out_part && total_slots >= 0 && c > 0 && c % 32 == 0, "cfb_debug_gn_cat_partials: bad argument");
+  return cfb::gn_cat_partials(a_part, b_part, out_part, total_slots, c, (cudaStream_t)stream);
   API_END(1)
 }
 int cfb_affine_act(const float* x, const float* scale, const float* shift, float* y, int32_t n, int32_t hw, int32_t c,

@@ -310,22 +310,26 @@ __global__ void __launch_bounds__(256) conv_first_kernel(const float* __restrict
     for (int j = 0; j < CPT; j += 4) *reinterpret_cast<float4*>(o + j) = make_float4(acc[p][j], acc[p][j + 1], acc[p][j + 2], acc[p][j + 3]);
   }
   if (gn_part != nullptr) {
-    // GroupNorm(32) partial sums of the values just stored, in the layout of the tensor-core epilogue's partials ([slot][32
-    // groups][sum, sum of squares], one slot per warp = 32 consecutive pixels; H*W % 256 == 0 keeps a CTA inside one image):
-    // the first ResBlock's norm1 then needs no pass over this tensor.  A thread owns 4 pixels x CPT channels = CPT/2 groups of
-    // two channels (COUT = 64); the 8 lanes with the same channel slice are reduced in a fixed order.
+    // GroupNorm(32) partials of the values just stored, in the layout of the tensor-core epilogue's partials ([slot][32
+    // groups][mean, M2], one slot per warp = 32 consecutive pixels; H*W % 256 == 0 keeps a CTA inside one image): the first
+    // ResBlock's norm1 then needs no pass over this tensor.  A thread owns 4 pixels x CPT channels = CPT/2 groups of two
+    // channels (COUT = 64): their 8 values around the first one, then equal-count merges over the 8 lanes with the same
+    // channel slice in a fixed order.
     static_assert(COUT == 64, "GroupNorm partials: two channels per group");
     float gs[CPT / 2], gq[CPT / 2];
 #pragma unroll
     for (int g = 0; g < CPT / 2; ++g) {
+      const float k = acc[0][2 * g];
       float a = 0.f, b = 0.f;
 #pragma unroll
       for (int p = 0; p < 4; ++p) {
-        a += acc[p][2 * g] + acc[p][2 * g + 1];
-        b += fmaf(acc[p][2 * g], acc[p][2 * g], acc[p][2 * g + 1] * acc[p][2 * g + 1]);
+        const float u = acc[p][2 * g] - k, v = acc[p][2 * g + 1] - k;
+        a += u + v;
+        b += fmaf(u, u, v * v);
       }
+      gn_lane_moments(a, b, k, 8.f);
 #pragma unroll
-      for (int o = 4; o < 32; o <<= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+      for (int o = 4, n = 8; o < 32; o <<= 1, n <<= 1) gn_merge_xor(a, b, o, (float)n);
       gs[g] = a; gq[g] = b;
     }
     if ((threadIdx.x & 31) < 4) {
@@ -534,10 +538,12 @@ size_t gn_workspace_bytes(int N, int HW, int C) {
   return (size_t)N * chunks * 32 * 2 * sizeof(double);
 }
 
+// The sums are fp64 from the first value on: a thread adds up to 1024 pixels, and fp32 sums of squares of a group whose mean
+// is r times its standard deviation would lose the variance like (1 + r^2) * 2^-24 (the kernel stays bound by its loads).
 __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict__ x, double* __restrict__ part, int HW,
                                                          int C, int CP, int groups) {
-  __shared__ float ssum[256 * 4];
-  __shared__ float ssq[256 * 4];
+  __shared__ double ssum[256 * 4];
+  __shared__ double ssq[256 * 4];
   __shared__ double csum[1024];
   __shared__ double csq[1024];
   const int t = threadIdx.x;
@@ -546,18 +552,19 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict
   const int c4 = t % C4, pl = t / C4;
   const int chunk = blockIdx.x, n = blockIdx.y, chunks = gridDim.x;
   const float* base = x + ((int64_t)n * HW + (int64_t)chunk * CP) * C + c4 * 4;
-  float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
+  double s[4] = {0.0, 0.0, 0.0, 0.0}, q[4] = {0.0, 0.0, 0.0, 0.0};
   for (int p = pl; p < CP; p += PL) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(base + (int64_t)p * C));
-    s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
-    q[0] = fmaf(v.x, v.x, q[0]); q[1] = fmaf(v.y, v.y, q[1]); q[2] = fmaf(v.z, v.z, q[2]); q[3] = fmaf(v.w, v.w, q[3]);
+    const double a = v.x, b = v.y, c = v.z, d = v.w;
+    s[0] += a; s[1] += b; s[2] += c; s[3] += d;
+    q[0] = fma(a, a, q[0]); q[1] = fma(b, b, q[1]); q[2] = fma(c, c, q[2]); q[3] = fma(d, d, q[3]);
   }
 #pragma unroll
   for (int j = 0; j < 4; ++j) { ssum[pl * C + c4 * 4 + j] = s[j]; ssq[pl * C + c4 * 4 + j] = q[j]; }
   __syncthreads();
   for (int c = t; c < C; c += 256) {
     double a = 0.0, b = 0.0;
-    for (int l = 0; l < PL; ++l) { a += (double)ssum[l * C + c]; b += (double)ssq[l * C + c]; }
+    for (int l = 0; l < PL; ++l) { a += ssum[l * C + c]; b += ssq[l * C + c]; }
     csum[c] = a; csq[c] = b;
   }
   __syncthreads();
@@ -636,18 +643,25 @@ __global__ void __launch_bounds__(256) gn_final_f32_kernel(const float* __restri
   const int g = t & 31, stripe = t >> 5;
   const int per = (slots + G - 1) / G;
   const int lo = blk * per, hi = min(slots, lo + per);
-  double a = 0.0, b = 0.0;
+  const int cpg = C / 32;
+  // slot k holds (mean_k, M2_k) of m values.  With the image's slot 0 mean K as a shift, d_k = mean_k - K:
+  //   a = sum d_k,  b = sum (M2_k + m d_k^2) = sum over all values of (x - K)^2
+  // so that mean = K + a / slots and var = b / (slots m) - (a / slots)^2 cancel only at the spread of the slot means
   const float2* base = reinterpret_cast<const float2*>(part) + (int64_t)n * slots * 32 + g;
+  const double K = (double)__ldg(base).x, m = (double)HW * cpg / slots;
+  double a = 0.0, b = 0.0;
   int k = lo + stripe;
   for (; k + 24 < hi; k += 32) {     // 4 independent loads in flight
     const float2 v0 = __ldg(base + (int64_t)k * 32), v1 = __ldg(base + (int64_t)(k + 8) * 32);
     const float2 v2 = __ldg(base + (int64_t)(k + 16) * 32), v3 = __ldg(base + (int64_t)(k + 24) * 32);
-    a += ((double)v0.x + (double)v1.x) + ((double)v2.x + (double)v3.x);
-    b += ((double)v0.y + (double)v1.y) + ((double)v2.y + (double)v3.y);
+    const double d0 = (double)v0.x - K, d1 = (double)v1.x - K, d2 = (double)v2.x - K, d3 = (double)v3.x - K;
+    a += (d0 + d1) + (d2 + d3);
+    b += (fma(m * d0, d0, (double)v0.y) + fma(m * d1, d1, (double)v1.y)) + (fma(m * d2, d2, (double)v2.y) + fma(m * d3, d3, (double)v3.y));
   }
   for (; k < hi; k += 8) {
     const float2 v = __ldg(base + (int64_t)k * 32);
-    a += (double)v.x; b += (double)v.y;
+    const double d = (double)v.x - K;
+    a += d; b += fma(m * d, d, (double)v.y);
   }
   ps[stripe][g] = a; pq[stripe][g] = b;
   __syncthreads();
@@ -673,13 +687,11 @@ __global__ void __launch_bounds__(256) gn_final_f32_kernel(const float* __restri
     }
     if (t == 0) counters[n] = 0u;
   }
-  const int cpg = C / 32;
   if (t < 32) {
-    const double cnt = (double)HW * cpg;
-    const double mean = sa / cnt;
-    double var = sb / cnt - mean * mean;
+    const double dm = sa / slots;
+    double var = sb / ((double)HW * cpg) - dm * dm;
     if (var < 0.0) var = 0.0;
-    gmean[t] = mean;
+    gmean[t] = K + dm;                   // t < 32: K is group t's
     grstd[t] = 1.0 / sqrt(var + (double)eps);
   }
   __syncthreads();
@@ -697,6 +709,7 @@ size_t gn_final_scratch_bytes(int N, int slots) {
 int gn_coef_from_partials(const float* part, int slots, const float* gamma, const float* beta, float* scale, float* shift,
                           int N, int HW, int C, int groups, float eps, void* scratch, unsigned* counters, cudaStream_t st) {
   CFB_REQUIRE(groups == 32 && C % 32 == 0, "gn_coef_from_partials: 32 groups only");
+  CFB_REQUIRE(slots > 0 && (int64_t)slots * 32 == HW, "gn_coef_from_partials: a slot holds 32 pixels of the image");
   if (N == 0) return 0;
   const int G = gn_final_split(slots);
   CFB_REQUIRE(G == 1 || (scratch && counters), "gn_coef_from_partials: scratch / counters missing");
@@ -707,8 +720,9 @@ int gn_coef_from_partials(const float* part, int slots, const float* gamma, cons
 }
 
 __global__ void gn_cat_partials_kernel(const float2* __restrict__ a, const float2* __restrict__ b, float2* __restrict__ out,
-                                       int64_t total) {
-  // group g of the concatenated tensor = two adjacent groups of one source: channels/group doubles, 32 groups stay
+                                       int64_t total, float half_cnt) {
+  // group g of the concatenated tensor = two adjacent groups of one source: channels/group doubles, 32 groups stay.  The two
+  // (mean, M2) of cnt values each merge as  mean = (mu + mv) / 2,  M2 = M2u + M2v + (mu - mv)^2 * cnt / 2
   pdl_launch_dependents();
   pdl_wait();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -716,15 +730,18 @@ __global__ void gn_cat_partials_kernel(const float2* __restrict__ a, const float
     const int64_t slot = i >> 5;
     const float2* src = (g < 16) ? a + slot * 32 + 2 * g : b + slot * 32 + 2 * (g - 16);
     const float2 u = __ldg(src), v = __ldg(src + 1);
-    out[i] = make_float2(u.x + v.x, u.y + v.y);
+    const float d = u.x - v.x;
+    out[i] = make_float2(0.5f * (u.x + v.x), (u.y + v.y) + (d * d) * half_cnt);
   }
 }
-int gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, cudaStream_t st) {
+int gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, int C, cudaStream_t st) {
+  CFB_REQUIRE(C % 32 == 0, "gn_cat_partials: 32 groups of C channels");
   const int64_t total = total_slots * 32;
   if (total == 0) return 0;
   const int64_t blocks = (total + 255) / 256;
+  // a slot of a source group holds 32 pixels x C/32 channels = C values
   CFB_LAUNCH_PDL(gn_cat_partials_kernel, dim3((unsigned)(blocks > 2048 ? 2048 : blocks)), dim3(256), 0, st, (const float2*)a_part,
-                 (const float2*)b_part, (float2*)out_part, total);
+                 (const float2*)b_part, (float2*)out_part, total, 0.5f * (float)C);
   return 0;
 }
 

@@ -187,7 +187,8 @@ int cfb_debug_time_conv(const float* in, const float* weight_oihw, float* out, i
  * (Upsample); xform 1 = fused operand transform (in_scale/in_shift optional: null = plain hi/lo split of the raw values), with
  * in2 != null channels [cin1, cin) read from in2 (torch.cat of Fuse_sft_block); residual, SFT (out = sft_dec + sft_w *
  * (sft_dec * sft_scale + conv)), out_planes (fp16 hi | lo planes of out, each align1024(n*Ho*Wo*cout*2) bytes) and gn_part
- * (GroupNorm(32) partial sums, 4 * 2 * 32 floats per 128-pixel tile) optional.  *tile_n receives the tile of the launched
+ * (GroupNorm(32) partials, per 32-pixel slot and group the (mean, M2) of its values: 4 * 32 * 2 floats per 128-pixel tile)
+ * optional.  *tile_n receives the tile of the launched
  * kernel: 128 (128 pixels x 128 channels), 64 (128 pixels x 64 channels, pixel-major) or -64 (128 pixels x 64 channels,
  * channel-major: computed transposed with the weights as the wgmma A operand).
  * workspace >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, 3, mode). */
@@ -196,6 +197,17 @@ int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const flo
                       const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
                       const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
                       void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n);
+/* diagnostics / tests: the GroupNorm(32) finalize of the forward on partials in the layout cfb_debug_conv_tc writes (slots of
+ * 32 pixels, [n][slots][32 groups][2] floats): scale[n,c] = rstd*gamma, shift[n,c] = beta - mean*rstd*gamma over hw pixels
+ * of c channels.  The workspace (>= cfb_debug_gn_partials_workspace_bytes) holds the split-finalize scratch and the ticket
+ * counters; the call zeroes the counters.  cfb_debug_gn_cat_partials merges the partials of two sources of c channels each
+ * into those of torch.cat([a, b], 1) (2c channels, the same slots), as Fuse_sft_block's GroupNorm takes them. */
+int64_t cfb_debug_gn_partials_workspace_bytes(int32_t n, int32_t slots);
+int cfb_debug_gn_coef_from_partials(const float* part, int32_t slots, const float* gamma, const float* beta, float* scale,
+                                    float* shift, int32_t n, int32_t hw, int32_t c, float eps, void* workspace,
+                                    int64_t workspace_bytes, void* stream);
+int cfb_debug_gn_cat_partials(const float* a_part, const float* b_part, float* out_part, int64_t total_slots, int32_t c,
+                              void* stream);
 /* ---- RRDBNet (SURVEY.md section 8 row f4): the upsampler behind RealESRGANer.enhance ----
  * /root/reference/basicsr/archs/rrdbnet_arch.py:67-120 (constructor :86, forward :103-119); the caller's tiling loop
  * (basicsr/utils/realesrgan_utils.py:100-175) stays in Python (codeformer_b200/upsampler.py).

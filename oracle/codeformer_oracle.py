@@ -214,7 +214,7 @@ def get_codebook_feat(sd: SD, indices: Tensor, shape) -> Tensor:
     indices = indices.view(-1, 1)
     onehot = torch.zeros(indices.shape[0], E.shape[0]).to(indices)
     onehot.scatter_(1, indices, 1)
-    z_q = torch.matmul(onehot.float(), E)
+    z_q = torch.matmul(onehot.to(E.dtype), E)
     if shape is not None:
         z_q = z_q.view(shape).permute(0, 3, 1, 2).contiguous()
     return z_q

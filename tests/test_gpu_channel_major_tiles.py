@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_wide_tiles import ROOT, _bits, _case_id, _run, plane_bytes, reference
+from tests.test_gpu_wide_tiles import ROOT, _bits, _case_id, _run, assert_gn_partials, plane_bytes, reference
 from tests.util import maxabs
 
 pytestmark = pytest.mark.gpu
@@ -76,7 +76,7 @@ def kernel_results():
 
 
 @pytest.mark.parametrize('i', range(len(CASES)), ids=[_case_id(c) for c in CASES])
-def test_channel_major_tiles_equal_pixel_major_tiles_and_torch(kernel_results, i):
+def test_channel_major_tiles_equal_pixel_major_tiles_torch_and_gn_moments(kernel_results, i):
     N, Cin, Cout, H, mode, operand, cin1, resid, sft, planes, gn = CASES[i]
     cm, pm = kernel_results[None], kernel_results['64']
     assert int(cm[f'tile{i}']) == -64 and int(pm[f'tile{i}']) == 64, 'the two sides must run channel- and pixel-major tiles'
@@ -95,8 +95,4 @@ def test_channel_major_tiles_equal_pixel_major_tiles_and_torch(kernel_results, i
     if gn:
         gc = cm[f'gn{i}']
         assert np.array_equal(_bits(gc), _bits(pm[f'gn{i}'])), 'GroupNorm partials differ'
-        part = gc.reshape(N, -1, 32, 2).astype(np.float64).sum(1)           # [N, group, (sum, sum of squares)]
-        grp = oc.reshape(N, -1, 32, Cout // 32).astype(np.float64)
-        s, q = grp.sum((1, 3)), (grp * grp).sum((1, 3))
-        assert np.abs(part[..., 0] - s).max() < 1e-4 * np.abs(grp).sum((1, 3)).max()
-        assert np.abs(part[..., 1] - q).max() < 1e-4 * q.max()
+        assert_gn_partials(gc, oc, N, Cout)
