@@ -71,6 +71,7 @@ SIGNATURES = {
     'cfb_rrdb_destroy': (None, [_P]),
     'cfb_rrdb_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
     'cfb_rrdb_prepare': (c_int, [_P, _P]),
+    'cfb_rrdb_set_precision': (c_int, [_P, c_int32]),
     'cfb_rrdb_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32]),
     'cfb_rrdb_forward': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_parsenet_create': (c_void_p, [c_int32] * 8),
@@ -83,6 +84,9 @@ SIGNATURES = {
     'cfb_conv2d_gen_workspace_bytes': (c_int64, [c_int32, c_int32]),
     'cfb_conv2d_gen_nhwc': (c_int, [_P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                     c_int32, c_int32, c_int32, _P, c_int32, _P, c_int32, c_float, _P, c_int64, _P]),
+    'cfb_conv2d_gen_nhwc_prec': (c_int, [_P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                         c_int32, c_int32, c_int32, c_int32, _P, c_int32, _P, c_int32, c_float, _P, c_int64, _P,
+                                         c_int32]),
     'cfb_conv2d_pertap_workspace_bytes': (c_int64, [c_int32] * 7),
     'cfb_conv2d_pertap_nhwc': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P,
                                        _P, c_int64, _P]),

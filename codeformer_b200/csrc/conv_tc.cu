@@ -458,7 +458,8 @@ __device__ __forceinline__ void sts128f(uint32_t addr, float a, float b, float c
 // 8 raw values -> y = act(x * sc + sh) -> fp16 hi / lo words.  MODE 2: affine + SiLU, 1: affine, 0: plain split.
 // SiLU = y / (1 + 2^(-y log2 e)) with ex2.approx / rcp.approx (~2^-21 relative: below the hi/lo operand error of 2^-22..2^-21).
 // lo = rn(y - hi) is formed as -(hi - y) with one subtract per element and a sign flip of the packed pair.
-template <int MODE>
+// LO = false (single-pass fp16 variant): hi only, lv is left unwritten.
+template <int MODE, bool LO = true>
 __device__ __forceinline__ void xf_chunk(const uint4& a, const uint4& b, const float (&sc)[8], const float (&sh)[8], uint4& hv,
                                          uint4& lv, float& amax) {
   const uint32_t raw[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
@@ -475,15 +476,17 @@ __device__ __forceinline__ void xf_chunk(const uint4& a, const uint4& b, const f
     }
     amax = fmaxf(amax, fmaxf(fabsf(y[0]), fabsf(y[1])));
     hw[q] = pack_f16x2(y[0], y[1]);
-    const float d0 = f16_minus_f32(hw[q] & 0xffffu, y[0]);      // hi - y = -lo
-    const float d1 = f16_minus_f32(hw[q] >> 16, y[1]);
-    lw[q] = pack_f16x2(d0, d1) ^ 0x80008000u;
+    if constexpr (LO) {
+      const float d0 = f16_minus_f32(hw[q] & 0xffffu, y[0]);    // hi - y = -lo
+      const float d1 = f16_minus_f32(hw[q] >> 16, y[1]);
+      lw[q] = pack_f16x2(d0, d1) ^ 0x80008000u;
+    }
   }
   hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-  lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+  if constexpr (LO) lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
 }
-// One patch: RPP rows per pass (8 lanes per row), two passes in flight per iteration.
-template <int MODE, int RPP, int NPASS, int PW, int ROWS>
+// One patch: RPP rows per pass (8 lanes per row), two passes in flight per iteration.  LO = false: the hi plane only.
+template <int MODE, int RPP, int NPASS, int PW, int ROWS, bool LO = true>
 __device__ __forceinline__ void xf_patch(uint32_t src_base, uint32_t hi_base, uint32_t lo_base, int c0, int j, int rsub,
                                          const float (&sc)[8], const float (&sh)[8], bool border, int y0, int x0, int Hin,
                                          int Win, float& amax) {
@@ -508,17 +511,17 @@ __device__ __forceinline__ void xf_patch(uint32_t src_base, uint32_t hi_base, ui
       if (act[u]) {
         const int r = rsub + (it + u) * RPP;
         uint4 hv, lv;
-        xf_chunk<MODE>(a[u], b[u], sc, sh, hv, lv, amax);
+        xf_chunk<MODE, LO>(a[u], b[u], sc, sh, hv, lv, amax);
         if (border) {
           const int py = r / PW, px = r - py * PW;
           if (!((unsigned)(y0 + py) < (unsigned)Hin && (unsigned)(x0 + px) < (unsigned)Win)) {
             hv = make_uint4(0u, 0u, 0u, 0u);
-            lv = make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (LO) lv = make_uint4(0u, 0u, 0u, 0u);
           }
         }
         const uint32_t hrow = hi_base + (uint32_t)r * 128u, lrow = lo_base + (uint32_t)r * 128u;
         sts128(hrow + ((((uint32_t)j) ^ ((hrow >> 7) & 7u)) << 4), hv);
-        sts128(lrow + ((((uint32_t)j) ^ ((lrow >> 7) & 7u)) << 4), lv);
+        if constexpr (LO) sts128(lrow + ((((uint32_t)j) ^ ((lrow >> 7) & 7u)) << 4), lv);
       }
     }
     __syncwarp();
@@ -651,12 +654,17 @@ struct TcCfg {
 // CM (channel-major, BN = 64 only): the MMA warpgroup computes the tile transposed, D^T[64 channels x 128 pixels] =
 // W[64 x K] * X[128 x K]^T, as one m64n128k16 per product and k-step (weights = A operand, halo patch = B operand), and stores
 // each partial sum into the slot as [pixel][channel]: the epilogue is that of the pixel-major 128 x 64 tile.
-template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false>
+// P1 (single-pass fp16, GEN without SiLU only): one product A_hi B_hi per k-step instead of three.  Only the hi weight plane
+// fp16(w * 2^k) is loaded, the transform warps write only the hi plane fp16(y); accumulation, chunked partial sums and their
+// round-to-nearest folds are those of the split scheme, and wscale_inv undoes 2^k exactly.
+template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false,
+          bool P1 = false>
 __global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
   static_assert(!XF || HALO, "the fused operand transform exists for the halo engine only");
   static_assert(!GEN || (XF && CPG == 0), "the generalised addressing exists for the fused-transform engine only");
+  static_assert(!P1 || (GEN && BN == 64 && !SILU), "the single-pass fp16 variant is built for the generalised engine only");
   static_assert(!K1 || (XF && !GEN && CPG == 0), "K1 = fused transform of a 1x1 conv (patch = tile): its own instantiation");
   using Cfg = TcCfg<BN>;
   constexpr bool WIDE = Cfg::WIDE;
@@ -762,9 +770,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 const uint32_t sb = smem_u32(ring_base + stage * RING_BYTES);
                 const uint32_t fb = smem_u32(full + stage);
                 const bool drop = p.fault && blockIdx.x == 0 && tile == first_tile && kb == 0 && tap == 0;   // injected fault
-                mbar_expect_tx(fb, (uint32_t)Cfg::H_B_SLOT);
+                mbar_expect_tx(fb, (uint32_t)(P1 ? Cfg::B_BYTES : Cfg::H_B_SLOT));
                 if (!drop) tma_load_3d(sb, &tmB_hi, fb, kb * 64, nt * BN, btap);
-                tma_load_3d(sb + Cfg::B_BYTES, &tmB_lo, fb, kb * 64, nt * BN, btap);
+                if constexpr (!P1) tma_load_3d(sb + Cfg::B_BYTES, &tmB_lo, fb, kb * 64, nt * BN, btap);
               }
               __syncwarp();
               if (++stage == NRING) { stage = 0; phase ^= 1; }
@@ -972,9 +980,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 #pragma unroll
             for (int mh = 0; mh < 2; ++mh) {
               const uint64_t da_hi = wg_desc(a_hi0 + mh * a_half + 32 * k, a_sbo), da_lo = wg_desc(a_lo0 + mh * a_half + 32 * k, a_sbo);
-              wg_mma_64x64(acc[mh], da_lo, db_hi, (first && k == 0) ? 0u : 1u);
-              wg_mma_64x64(acc[mh], da_hi, db_lo, 1u);
-              wg_mma_64x64(acc[mh], da_hi, db_hi, 1u);
+              if constexpr (P1) {
+                wg_mma_64x64(acc[mh], da_hi, db_hi, (first && k == 0) ? 0u : 1u);
+              } else {
+                wg_mma_64x64(acc[mh], da_lo, db_hi, (first && k == 0) ? 0u : 1u);
+                wg_mma_64x64(acc[mh], da_hi, db_lo, 1u);
+                wg_mma_64x64(acc[mh], da_hi, db_hi, 1u);
+              }
             }
           }
           wg_commit();
@@ -1106,9 +1118,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             else if (mode == 1) xf_patch<1, RPP, NPASS1, 8, 128>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
             else xf_patch<0, RPP, NPASS1, 8, 128>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
           } else {
-            if (mode == 2) xf_patch<2, RPP, NPASS, XF_PW, XF_ROWS>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
-            else if (mode == 1) xf_patch<1, RPP, NPASS, XF_PW, XF_ROWS>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
-            else xf_patch<0, RPP, NPASS, XF_PW, XF_ROWS>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
+            if (mode == 2) xf_patch<2, RPP, NPASS, XF_PW, XF_ROWS, !P1>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
+            else if (mode == 1) xf_patch<1, RPP, NPASS, XF_PW, XF_ROWS, !P1>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
+            else xf_patch<0, RPP, NPASS, XF_PW, XF_ROWS, !P1>(src_base, base0, lo_base, c0, j, rsub, sc, sh, border, y0, x0, Hin, Win, amax);
           }
           if constexpr (GEN) {
             if (p.pad_mode && border) {
@@ -1132,9 +1144,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 const uint32_t hs = base0 + (uint32_t)rs * 128u, hd = base0 + (uint32_t)r * 128u;
                 const uint32_t ls = lo_base + (uint32_t)rs * 128u, ld = lo_base + (uint32_t)r * 128u;
                 const uint4 hv = lds128(hs + ((((uint32_t)j) ^ ((hs >> 7) & 7u)) << 4));
-                const uint4 lv = lds128(ls + ((((uint32_t)j) ^ ((ls >> 7) & 7u)) << 4));
-                sts128(hd + ((((uint32_t)j) ^ ((hd >> 7) & 7u)) << 4), hv);
-                sts128(ld + ((((uint32_t)j) ^ ((ld >> 7) & 7u)) << 4), lv);
+                if constexpr (P1) {
+                  sts128(hd + ((((uint32_t)j) ^ ((hd >> 7) & 7u)) << 4), hv);
+                } else {
+                  const uint4 lv = lds128(ls + ((((uint32_t)j) ^ ((ls >> 7) & 7u)) << 4));
+                  sts128(hd + ((((uint32_t)j) ^ ((hd >> 7) & 7u)) << 4), hv);
+                  sts128(ld + ((((uint32_t)j) ^ ((ld >> 7) & 7u)) << 4), lv);
+                }
               }
             }
           }
@@ -1588,7 +1604,8 @@ size_t tc_scratch_bytes(const ConvArgs& a) {
 
 struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
 
-template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false>
+template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false,
+          bool P1 = false>
 static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int SMEM = XF ? Cfg::X_SMEM_BYTES : (HALO ? Cfg::H_SMEM_BYTES : Cfg::SMEM_BYTES);
@@ -1601,20 +1618,24 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
   CFB_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count ? total : sm_count;
-  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st, m.a_hi,
-                 m.a_lo, m.b_hi, m.b_lo, p);
+  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st,
+                 m.a_hi, m.a_lo, m.b_hi, m.b_lo, p);
   return 0;
 }
 template <int CPG>
-static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, int tile = TC_TILE_N) {
+static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, int tile = TC_TILE_N,
+                     bool single_pass = false) {
   // the SiLU epilogue (YOLOv5) is built into two variants only, so the others keep their register budgets
   CFB_REQUIRE(p.out_act != OUT_SILU || (CPG == 0 && (gen || (!p.xform && p.PW == 0))),
               "conv_tc: the SiLU epilogue is built for the per-tap and generalised engines without statistics");
+  // the single-pass fp16 variant is built for the generalised engine without the SiLU epilogue (RRDBNet) only
+  CFB_REQUIRE(!single_pass || (CPG == 0 && gen && p.out_act != OUT_SILU),
+              "conv_tc: single-pass fp16 is built for the generalised engine without the SiLU epilogue");
   if (tile == TC_TILE_CM) {    // channel-major 128 x 64 tiles: conv_tc() only asks for them where tc_tile_kind() says so
     if constexpr (CPG <= 2) {
       CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: channel-major tiles need the 3x3 / Upsample halo engine");
@@ -1636,6 +1657,7 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   if constexpr (CPG == 0) {
     if (gen) {
       CFB_REQUIRE(p.xform && p.PW == 10 && p.PH == 18, "conv_tc: generalised variant needs the halo + transform engine");
+      if (single_pass) return launch_tc2<64, 0, true, true, true, false, false, false, true>(m, p, sm_count, st);
       if (p.out_act == OUT_SILU) return launch_tc2<64, 0, true, true, true, false, false, true>(m, p, sm_count, st);
       return launch_tc2<64, 0, true, true, true>(m, p, sm_count, st);
     }
@@ -1806,13 +1828,13 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   p.pl_lo = a.out_planes ? (__half*)((char*)a.out_planes + (((size_t)a.N * a.Ho * a.Wo * a.Cout * 2 + 1023) / 1024 * 1024)) : nullptr;
   const int cpg = a.gn_part ? a.Cout / 32 : 0;
   CFB_REQUIRE(!a.gn_part || tc_can_emit_stats(a), "conv_tc: GroupNorm partials are not available for this Cout");
-  if (a.gen) return launch_tc<0>(mp, p, sm_count, st, true);
+  if (a.gen) return launch_tc<0>(mp, p, sm_count, st, true, TC_TILE_N, a.single_pass);
   switch (cpg) {
-    case 0: return launch_tc<0>(mp, p, sm_count, st, false, tile);
-    case 2: return launch_tc<2>(mp, p, sm_count, st, false, tile);
-    case 4: return launch_tc<4>(mp, p, sm_count, st, false, tile);
-    case 8: return launch_tc<8>(mp, p, sm_count, st, false, tile);
-    case 16: return launch_tc<16>(mp, p, sm_count, st, false, tile);
+    case 0: return launch_tc<0>(mp, p, sm_count, st, false, tile, a.single_pass);
+    case 2: return launch_tc<2>(mp, p, sm_count, st, false, tile, a.single_pass);
+    case 4: return launch_tc<4>(mp, p, sm_count, st, false, tile, a.single_pass);
+    case 8: return launch_tc<8>(mp, p, sm_count, st, false, tile, a.single_pass);
+    case 16: return launch_tc<16>(mp, p, sm_count, st, false, tile, a.single_pass);
   }
   CFB_REQUIRE(false, "conv_tc: no kernel variant for this configuration");
   return 1;

@@ -80,7 +80,7 @@ int async_status_check(const char* where) {
   if (!bits) return 0;
   std::string msg = std::string(where) + ": a kernel of an earlier launch on this device reported";
   if (bits & CFB_STATUS_TIMEOUT) msg += " [barrier time-out: the tensor-core pipeline was aborted, results of that launch are invalid]";
-  if (bits & CFB_STATUS_OVERFLOW) msg += " [fp16 operand overflow: an activation exceeded 65504 on the split-fp16 tensor-core path]";
+  if (bits & CFB_STATUS_OVERFLOW) msg += " [fp16 operand overflow: an activation exceeded 65504 on the fp16 tensor-core operand path]";
   if (bits & CFB_STATUS_TIMEOUT) {
     if (cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();   // the aborted launch has drained; the context is healthy
     tc_clear_abort();
@@ -1262,6 +1262,7 @@ struct cfb_rrdb : cfb::NetCore {
   std::vector<cfb::GenConv> convs;      // [blocks*15] dense convs, then conv_body, conv_up1, conv_up2, conv_hr
   float* first_w = nullptr; float* first_b = nullptr;   // conv_first  [tap][cin][64]
   float* last_w = nullptr; float* last_b = nullptr;     // conv_last   [tap][64][4]
+  int precision = 0;                                    // GEN convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
 };
 
 namespace cfb {
@@ -1318,6 +1319,7 @@ struct GenLaunch {          // one generalised conv: src window -> destination s
   float* out; int out_pitch, out_c0; int act;
   const float* res = nullptr; int res_pitch = 0; const float* res2 = nullptr; int res2_pitch = 0; float post = 1.f;
   int pad_mode = 0; bool sub = false;
+  bool single_pass = false;   // fp16 operands, one product per k-step (ConvArgs::single_pass)
 };
 static int gen_conv(const GenLaunch& g, int sm_count, cudaStream_t st) {
   ConvArgs a;
@@ -1330,6 +1332,7 @@ static int gen_conv(const GenLaunch& g, int sm_count, cudaStream_t st) {
   a.in_pitch = g.in_pitch; a.pad_mode = g.pad_mode; a.subsample = g.sub;
   a.out_pitch = g.out_pitch; a.out_c0 = g.out_c0; a.cout_valid = g.c->cout;
   a.res_pitch = g.res_pitch; a.residual2 = g.res2; a.res2_pitch = g.res2_pitch; a.post_scale = g.post;
+  a.single_pass = g.single_pass;
   return conv_tc(a, nullptr, sm_count, st);
 }
 
@@ -1383,6 +1386,8 @@ static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, i
   CFB_CUDA(cudaMemsetAsync(D[0], 0, px * 192 * 3 * sizeof(float), st));
   CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, F, N, h, w, n->in_ch, us, 0, 64, 0, st));
   CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, D[0], N, h, w, n->in_ch, us, 0, 192, 0, st));
+  // every GEN conv runs in the handle's precision; conv_first / conv_last are the fp32 SIMT thin convs in both
+  auto conv = [&](GenLaunch& g) { g.single_pass = n->precision == 1; return gen_conv(g, n->sm_count, st); };
   int X = 0, Y = 1;            // x of the current RRDB lives in D[X]; D[2] is the middle buffer
   const int Z = 2;
   for (int b = 0; b < n->blocks; ++b) {
@@ -1397,17 +1402,17 @@ static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, i
           g.out = D[dst[r]]; g.out_c0 = 0; g.res = S; g.res_pitch = 192;               // x5 * 0.2 + x   (rrdbnet_arch.py:40)
           if (r == 2) { g.res2 = D[X]; g.res2_pitch = 192; g.post = 0.2f; }            // out * 0.2 + x  (rrdbnet_arch.py:63)
         }
-        CFB_CHECK(gen_conv(g, n->sm_count, st));
+        CFB_CHECK(conv(g));
       }
     }
     std::swap(X, Y);
   }
   const size_t nb = (size_t)n->blocks * 15;
   { GenLaunch g{&n->convs[nb + 0], D[X], 192, h, w, N, Bd, 64, 0, OUT_NONE}; g.res = F; g.res_pitch = 64;   // feat + conv_body(body(feat))
-    CFB_CHECK(gen_conv(g, n->sm_count, st)); }
-  { GenLaunch g{&n->convs[nb + 1], Bd, 64, h, w, N, U1, 64, 0, OUT_LRELU}; CFB_CHECK(gen_conv(g, n->sm_count, st)); }
-  { GenLaunch g{&n->convs[nb + 2], U1, 64, 2 * h, 2 * w, N, U2, 64, 0, OUT_LRELU}; CFB_CHECK(gen_conv(g, n->sm_count, st)); }
-  { GenLaunch g{&n->convs[nb + 3], U2, 64, 4 * h, 4 * w, N, HR, 64, 0, OUT_LRELU}; CFB_CHECK(gen_conv(g, n->sm_count, st)); }
+    CFB_CHECK(conv(g)); }
+  { GenLaunch g{&n->convs[nb + 1], Bd, 64, h, w, N, U1, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
+  { GenLaunch g{&n->convs[nb + 2], U1, 64, 2 * h, 2 * w, N, U2, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
+  { GenLaunch g{&n->convs[nb + 3], U2, 64, 4 * h, 4 * w, N, HR, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
   CFB_CHECK(conv_thin_out(HR, n->last_w, n->last_b, out, N, 4 * h, 4 * w, n->out_ch, 0, st));
   return 0;
 }
@@ -2086,6 +2091,15 @@ int cfb_rrdb_prepare(cfb_rrdb* n, void* stream) {
   return cfb::rrdb_prepare(n, (cudaStream_t)stream);
   API_END(1)
 }
+int cfb_rrdb_set_precision(cfb_rrdb* n, int32_t precision) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_rrdb_set_precision: NULL net");
+  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_rrdb_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
+  std::lock_guard<std::mutex> lk(n->mu);
+  n->precision = precision;
+  return 0;
+  API_END(1)
+}
 int64_t cfb_rrdb_workspace_bytes(cfb_rrdb* n, int32_t batch, int32_t h, int32_t w) {
   if (!n || batch < 0 || h < 0 || w < 0) return -1;
   return (int64_t)cfb::rrdb_ws_bytes(n, batch, h, w);
@@ -2156,8 +2170,19 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
                         int32_t upsample, int32_t pad_mode, int32_t subsample, int32_t out_act, const float* residual,
                         int32_t res_pitch, const float* residual2, int32_t res2_pitch, float post_scale, void* workspace,
                         int64_t workspace_bytes, void* stream) {
+  return cfb_conv2d_gen_nhwc_prec(in, in_pitch, weight_oihw, bias, out, out_pitch, out_c0, n, h, w, cin, cout, upsample, pad_mode,
+                                  subsample, out_act, residual, res_pitch, residual2, res2_pitch, post_scale, workspace,
+                                  workspace_bytes, stream, 0);
+}
+
+int cfb_conv2d_gen_nhwc_prec(const float* in, int32_t in_pitch, const float* weight_oihw, const float* bias, float* out,
+                             int32_t out_pitch, int32_t out_c0, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout,
+                             int32_t upsample, int32_t pad_mode, int32_t subsample, int32_t out_act, const float* residual,
+                             int32_t res_pitch, const float* residual2, int32_t res2_pitch, float post_scale, void* workspace,
+                             int64_t workspace_bytes, void* stream, int32_t precision) {
   API_BEGIN
   CFB_REQUIRE(in && weight_oihw && out && workspace, "cfb_conv2d_gen_nhwc: NULL argument");
+  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_conv2d_gen_nhwc_prec: precision must be 0 (fp32, split) or 1 (fp16)");
   CFB_REQUIRE(workspace_bytes >= cfb_conv2d_gen_workspace_bytes(cin, cout), "cfb_conv2d_gen_nhwc: workspace too small");
   CFB_REQUIRE(cin >= 1 && cout >= 1 && cout % 4 == 0, "cfb_conv2d_gen_nhwc: cout must be a multiple of 4");
   cudaStream_t st = (cudaStream_t)stream;
@@ -2172,7 +2197,7 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
   CFB_CHECK(cfb::prepare_conv(c, weight_oihw, bias, pad, p, st));
   cfb::GenLaunch g{&c, in, in_pitch, h, w, n, out, out_pitch, out_c0, out_act};
   g.res = residual; g.res_pitch = res_pitch; g.res2 = residual2; g.res2_pitch = res2_pitch; g.post = post_scale;
-  g.pad_mode = pad_mode; g.sub = subsample != 0;
+  g.pad_mode = pad_mode; g.sub = subsample != 0; g.single_pass = precision == 1;
   return cfb::gen_conv(g, sms, st);
   API_END(1)
 }

@@ -44,6 +44,24 @@ class RRDBNet(NativeNet):
                          S.rrdbnet_spec(num_in_ch, num_out_ch, scale, num_feat, num_block, num_grow_ch), _rrdbnet_init)
         self.scale, self.num_in_ch, self.num_out_ch = scale, num_in_ch, num_out_ch
         self.num_feat, self.num_block, self.num_grow_ch = num_feat, num_block, num_grow_ch
+        object.__setattr__(self, '_precision', 'fp32')
+
+    PRECISIONS = {'fp32': 0, 'fp16': 1}
+
+    @property
+    def precision(self):
+        """``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core product
+        per k-step, fp32 accumulation and fp32 activations -- what the reference computes with ``half=True``.  conv_first and
+        conv_last stay fp32 in both."""
+        return self._precision
+
+    def set_precision(self, precision):
+        """Select the conv precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and re-preparation;
+        switching never re-prepares the weights.  Returns the module."""
+        if precision not in self.PRECISIONS:
+            raise ValueError(f"RRDBNet.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
+        object.__setattr__(self, '_precision', precision)
+        return self
 
     def forward(self, x):
         """x [B, num_in_ch, H, W] fp32 CUDA -> [B, num_out_ch, H*scale, W*scale] (rrdbnet_arch.py:103-119)."""
@@ -63,6 +81,7 @@ class RRDBNet(NativeNet):
         dev = x.device
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
+            _lib.check(lib.cfb_rrdb_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_rrdb_set_precision')
             out = torch.empty((B, self.num_out_ch, H // us * 4, W // us * 4), dtype=torch.float32, device=dev)
             ws = self._workspace(B, H, W, dev)
             _lib.check(lib.cfb_rrdb_forward(self._net, _lib.ptr(x), _lib.ptr(out), B, H, W, _lib.ptr(ws), ws.numel(),
@@ -74,12 +93,15 @@ class RealESRGANer:
     """The reference's helper around the upsampling network (realesrgan_utils.py:14-250): ``enhance(img)`` takes an HWC
     uint8 / uint16 BGR (or gray, or BGRA) image and returns ``(upsampled image, mode)``.  ``model`` is any module mapping
     [1,3,h,w] -> [1,3,h*scale,w*scale] on ``device`` (``codeformer_b200.RRDBNet`` in production; the tests also pass CPU
-    stand-ins to compare the tiling against the reference's)."""
+    stand-ins to compare the tiling against the reference's).  ``precision`` (not in the reference): ``None`` leaves the model
+    as it is, a string is passed to ``model.set_precision`` -- the reference's ``half=use_half`` maps to
+    ``precision='fp16' if use_half else None``."""
 
-    def __init__(self, scale, model_path=None, model=None, tile=0, tile_pad=10, pre_pad=10, half=False, device=None, gpu_id=None):
+    def __init__(self, scale, model_path=None, model=None, tile=0, tile_pad=10, pre_pad=10, half=False, device=None, gpu_id=None,
+                 precision=None):
         self.scale, self.tile_size, self.tile_pad, self.pre_pad = scale, tile, tile_pad, pre_pad
         self.mod_scale = None
-        self.half = False          # accepted for signature parity; the H100 path keeps fp32 semantics at tensor-core speed
+        self.half = False          # accepted for signature parity and ignored; fp16 operands are opted into with `precision`
         if device is None:
             device = torch.device('cuda', gpu_id if gpu_id is not None else torch.cuda.current_device())
         self.device = torch.device(device)
@@ -87,6 +109,8 @@ class RealESRGANer:
             loadnet = torch.load(model_path, map_location=torch.device('cpu'))
             model.load_state_dict(loadnet['params_ema' if 'params_ema' in loadnet else 'params'], strict=True)
         model.eval()
+        if precision is not None:
+            model.set_precision(precision)
         self.model = model.to(self.device)
 
     def pre_process(self, img):

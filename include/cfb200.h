@@ -219,6 +219,11 @@ cfb_rrdb* cfb_rrdb_create(int32_t num_in_ch, int32_t num_out_ch, int32_t scale, 
 void      cfb_rrdb_destroy(cfb_rrdb* net);
 int       cfb_rrdb_set_param(cfb_rrdb* net, const char* name, const float* dev_ptr, int64_t numel);
 int       cfb_rrdb_prepare(cfb_rrdb* net, void* stream);
+/* Precision of the 3x3 / Upsample convs (every conv except conv_first and conv_last, which stay fp32): 0 = fp32 (default;
+ * split fp16 x3 operands, fp32 parity), 1 = fp16 (the reference's half=True: fp16 operands, one tensor-core product per
+ * k-step, fp32 accumulation and fp32 activations).  Other values are an error.  Takes effect at the next forward; no
+ * re-prepare. */
+int       cfb_rrdb_set_precision(cfb_rrdb* net, int32_t precision);
 int64_t   cfb_rrdb_workspace_bytes(cfb_rrdb* net, int32_t batch, int32_t h, int32_t w);
 int       cfb_rrdb_forward(cfb_rrdb* net, const float* x, float* out, int32_t batch, int32_t h, int32_t w,
                            void* workspace, int64_t workspace_bytes, void* stream);
@@ -255,6 +260,13 @@ int cfb_conv2d_gen_nhwc(const float* in, int32_t in_pitch, const float* weight_o
                         int32_t upsample, int32_t pad_mode, int32_t subsample, int32_t out_act, const float* residual,
                         int32_t res_pitch, const float* residual2, int32_t res2_pitch, float post_scale, void* workspace,
                         int64_t workspace_bytes, void* stream);
+/* The same with the operand precision of cfb_rrdb_set_precision: 0 fp32 (split; == cfb_conv2d_gen_nhwc), 1 fp16 (out_act 4,
+ * SiLU, is not built for it). */
+int cfb_conv2d_gen_nhwc_prec(const float* in, int32_t in_pitch, const float* weight_oihw, const float* bias, float* out,
+                             int32_t out_pitch, int32_t out_c0, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout,
+                             int32_t upsample, int32_t pad_mode, int32_t subsample, int32_t out_act, const float* residual,
+                             int32_t res_pitch, const float* residual2, int32_t res2_pitch, float post_scale, void* workspace,
+                             int64_t workspace_bytes, void* stream, int32_t precision);
 
 /* One 1x1 or 3x3 conv of the per-tap engine on any h x w (test entry point for the detector's conv forms).  stride 2 computes
  * only the output positions, ceil(h/2) x ceil(w/2): 3x3 with padding 1, 1x1 without.  in / out / residual NHWC, cin and cout
