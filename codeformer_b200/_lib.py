@@ -34,6 +34,7 @@ SIGNATURES = {
     'cfb_workspace_bytes': (c_int64, [_P, c_int32]),
     'cfb_last_launch_count': (c_int64, [_P]),
     'cfb_net_set_engine': (c_int, [_P, c_int32]),
+    'cfb_net_set_precision': (c_int, [_P, c_int32]),
     'cfb_net_capture': (c_int, [_P, c_char_p, _P, c_int64]),
     'cfb_codeformer_forward': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_float, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_host_io_bytes': (c_int64, [_P, c_int32]),
@@ -64,6 +65,9 @@ SIGNATURES = {
                                    _P, _P, _P, c_int32, POINTER(c_float)]),
     'cfb_debug_conv_tc': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                  _P, _P, c_int32, _P, _P, _P, c_float, _P, _P, _P, c_int64, _P, POINTER(c_int32)]),
+    'cfb_debug_conv_tc_prec': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                      _P, _P, c_int32, _P, _P, _P, c_float, _P, _P, _P, c_int64, _P, POINTER(c_int32), c_int32,
+                                      c_int32, c_int32]),
     'cfb_debug_gn_partials_workspace_bytes': (c_int64, [c_int32, c_int32]),
     'cfb_debug_gn_coef_from_partials': (c_int, [_P, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, c_int64, _P]),
     'cfb_debug_gn_cat_partials': (c_int, [_P, _P, _P, c_int64, c_int32, _P]),

@@ -322,6 +322,7 @@ class VQAutoEncoder(nn.Module):
         object.__setattr__(self, '_cfb_keep', None)
         object.__setattr__(self, '_cfb_ws', {})
         object.__setattr__(self, '_cfb_graphs', {})
+        object.__setattr__(self, '_cfb_precision', 'fp32')
 
     def _cfb_config(self) -> '_lib.CfbConfig':
         c = _lib.CfbConfig()
@@ -337,12 +338,15 @@ class VQAutoEncoder(nn.Module):
         return c
 
     def _cfb_prepare(self, device):
-        """(Re)build the native weight copies when parameters were loaded, moved or modified."""
+        """(Re)build the native weight copies when parameters were loaded, moved or modified; hand the precision on."""
         lib = _lib.load()
         params = list(self.state_dict(keep_vars=True).items())
         sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._cfb_net is not None and sig == self._cfb_sig:
-            return
+        if self._cfb_net is None or sig != self._cfb_sig:
+            self._cfb_prepare_weights(lib, params, sig, device)
+        _lib.check(lib.cfb_net_set_precision(self._cfb_net, self.PRECISIONS[self._cfb_precision]), 'cfb_net_set_precision')
+
+    def _cfb_prepare_weights(self, lib, params, sig, device):
         if self._cfb_net is None:
             cfg = self._cfb_config()
             h = lib.cfb_net_create(ctypes.byref(cfg))
@@ -396,6 +400,25 @@ class VQAutoEncoder(nn.Module):
         self._cfb_graphs.clear()
         if self._cfb_net is not None:
             _lib.check(_lib.load().cfb_net_set_engine(self._cfb_net, code), 'cfb_net_set_engine')
+
+    PRECISIONS = {'fp32': 0, 'fp16': 1}
+
+    @property
+    def precision(self):
+        """Precision of the decoder convs -- the generator's and the Fuse_sft_blocks' (not the AttnBlocks', not the last
+        conv).  ``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core
+        product per k-step, fp32 accumulation and fp32 activations.  The encoder, the Transformer and the quantizer are the
+        same in both, so ``logits``, ``lq_feat`` and the code indices are bit-identical; only the decoded image changes."""
+        return self._cfb_precision
+
+    def set_precision(self, precision):
+        """Select the decoder precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and
+        re-preparation; switching never re-prepares the weights.  'fp16' needs the tensor-core engine ('auto' or 'tc'):
+        with ``set_engine('f32')`` the forward raises.  Returns the module."""
+        if precision not in self.PRECISIONS:
+            raise ValueError(f"{type(self).__name__}.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
+        object.__setattr__(self, '_cfb_precision', precision)
+        return self
 
     def capture(self, stage: str, dst: Optional[torch.Tensor]):
         """Parity hook (cfb_net_capture): copy the NHWC activation after ``stage`` into ``dst`` on the next forwards."""
@@ -572,7 +595,7 @@ class CodeFormer(VQAutoEncoder):
 
     # The reference's callers feed ONE face per call (inference_codeformer.py:197-206); at that size the forward is ~440
     # small launches and launch latency dominates.  Small batches are therefore replayed from a CUDA graph captured once
-    # per (batch, w, adain, code_only): static input/output buffers, same kernels, same results.
+    # per (batch, w, adain, code_only, precision): static input/output buffers, same kernels, same results.
     cuda_graph_max_batch = 4
     cuda_graph_cache_size = 6
 
@@ -580,8 +603,8 @@ class CodeFormer(VQAutoEncoder):
         lib = _lib.load()
         dev = x.device
         B = x.shape[0]
-        key = (dev.index, B, w, adain, code_only)
-        ent = self._cfb_graphs.pop(key, None)                # re-inserted below: dict order = least recently used first
+        key = (dev.index, B, w, adain, code_only, self._cfb_precision)      # the launch sequence depends on the precision
+        ent = self._cfb_graphs.pop(key, None)              # re-inserted below: dict order = least recently used first
         if ent is None:
             while len(self._cfb_graphs) >= self.cuda_graph_cache_size:      # callers sweep w (Gradio slider): evict the LRU
                 self._cfb_graphs.pop(next(iter(self._cfb_graphs)))          # entry only; each pins one workspace
@@ -642,7 +665,7 @@ class CodeFormer(VQAutoEncoder):
             graph_ok = B <= self.cuda_graph_max_batch and os.environ.get('CFB_CUDA_GRAPH', '1') != '0' \
                 and not getattr(self, '_cfb_hooks', None) and not torch.cuda.is_current_stream_capturing()
             if graph_ok:
-                key = ('u8', dev.index, B, w, adain)
+                key = ('u8', dev.index, B, w, adain, self._cfb_precision)
                 ent = self._cfb_graphs.pop(key, None)
                 if ent is None:
                     while len(self._cfb_graphs) >= self.cuda_graph_cache_size:

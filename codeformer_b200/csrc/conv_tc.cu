@@ -654,9 +654,11 @@ struct TcCfg {
 // CM (channel-major, BN = 64 only): the MMA warpgroup computes the tile transposed, D^T[64 channels x 128 pixels] =
 // W[64 x K] * X[128 x K]^T, as one m64n128k16 per product and k-step (weights = A operand, halo patch = B operand), and stores
 // each partial sum into the slot as [pixel][channel]: the epilogue is that of the pixel-major 128 x 64 tile.
-// P1 (single-pass fp16, GEN without SiLU only): one product A_hi B_hi per k-step instead of three.  Only the hi weight plane
-// fp16(w * 2^k) is loaded, the transform warps write only the hi plane fp16(y); accumulation, chunked partial sums and their
-// round-to-nearest folds are those of the split scheme, and wscale_inv undoes 2^k exactly.
+// P1 (single-pass fp16): one product A_hi B_hi per k-step instead of three.  Only the hi weight plane fp16(w * 2^k) is
+// loaded, the transform warps write only the hi plane fp16(y), and a raw-planes input has only its hi plane fp16(x) loaded;
+// accumulation, chunked partial sums and their round-to-nearest folds are those of the split scheme, and wscale_inv undoes
+// 2^k exactly.  Built for GEN without SiLU (RRDBNet), the 128-wide and channel-major halo tiles and the per-tap engine
+// (CodeFormer's generator and Fuse_sft_block convs); K1 and the SiLU epilogue stay split.
 template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false,
           bool P1 = false>
 __global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
@@ -664,12 +666,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
   static_assert(!XF || HALO, "the fused operand transform exists for the halo engine only");
   static_assert(!GEN || (XF && CPG == 0), "the generalised addressing exists for the fused-transform engine only");
-  static_assert(!P1 || (GEN && BN == 64 && !SILU), "the single-pass fp16 variant is built for the generalised engine only");
   static_assert(!K1 || (XF && !GEN && CPG == 0), "K1 = fused transform of a 1x1 conv (patch = tile): its own instantiation");
   using Cfg = TcCfg<BN>;
   constexpr bool WIDE = Cfg::WIDE;
   static_assert(!WIDE || (HALO && !GEN && !K1 && CPG != 2), "128-wide tiles exist for the 3x3 / Upsample halo engine");
   static_assert(!CM || (BN == 64 && HALO && !GEN && !K1), "channel-major tiles exist for the 64-channel 3x3 / Upsample halo convs");
+  static_assert(!P1 || (!SILU && !K1 && (GEN || WIDE || CM || !HALO)),
+                "the single-pass fp16 variant is built for the generalised, 128-wide, channel-major and per-tap engines");
   constexpr int MMA_WARPS = Cfg::MMA_WARPS, EPI_WARPS = Cfg::EPI_WARPS;
   constexpr int A_SLOTS = XF ? Cfg::X_A_SLOTS : Cfg::H_A_SLOTS;
   constexpr int STAGES = Cfg::STAGES;
@@ -755,9 +758,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               if (elect_one()) {
                 const uint32_t sa = smem_u32(smem + aslot * Cfg::H_A_SLOT);
                 const uint32_t ab = smem_u32(afull + aslot);
-                mbar_expect_tx(ab, (uint32_t)(2 * p.PW * p.PH * 128));
+                mbar_expect_tx(ab, (uint32_t)((P1 ? 1 : 2) * p.PW * p.PH * 128));
                 tma_load_4d(sa, &tmA_hi, ab, kb * 64, x0 - p.pad, y0 - p.pad, n);
-                tma_load_4d(sa + Cfg::H_A_PLANE, &tmA_lo, ab, kb * 64, x0 - p.pad, y0 - p.pad, n);
+                if constexpr (!P1) tma_load_4d(sa + Cfg::H_A_PLANE, &tmA_lo, ab, kb * 64, x0 - p.pad, y0 - p.pad, n);
               }
               __syncwarp();
               if (++aslot == A_SLOTS) { aslot = 0; aphase ^= 1; }
@@ -797,11 +800,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 const int b3 = p.b_batched ? nimg : btap;
                 const uint32_t fb = smem_u32(full + stage);
                 const bool drop = p.fault && blockIdx.x == 0 && tile == first_tile && kb == 0 && tap == 0;   // injected fault
-                mbar_expect_tx(fb, (uint32_t)Cfg::STAGE_BYTES);
+                mbar_expect_tx(fb, (uint32_t)(P1 ? TC_A_BYTES + Cfg::B_BYTES : Cfg::STAGE_BYTES));
                 tma_load_4d(sa, &tmA_hi, fb, ac, x0 + s - p.pad, y0 + r - p.pad, a_img);
-                tma_load_4d(sa + TC_A_BYTES, &tmA_lo, fb, ac, x0 + s - p.pad, y0 + r - p.pad, a_img);
+                if constexpr (!P1) tma_load_4d(sa + TC_A_BYTES, &tmA_lo, fb, ac, x0 + s - p.pad, y0 + r - p.pad, a_img);
                 if (!drop) tma_load_3d(sa + 2 * TC_A_BYTES, &tmB_hi, fb, bc, brow, b3);
-                tma_load_3d(sa + 2 * TC_A_BYTES + Cfg::B_BYTES, &tmB_lo, fb, bc, brow, b3);
+                if constexpr (!P1) tma_load_3d(sa + 2 * TC_A_BYTES + Cfg::B_BYTES, &tmB_lo, fb, bc, brow, b3);
               }
               __syncwarp();
               if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -815,7 +818,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // Per k-block (64 K-elements) and 64-row half of the tile: 4 k-steps x {A_lo B_hi, A_hi B_lo, A_hi B_hi}.  BN = 64: one
     // warpgroup issues both halves (m64n64k16); BN = 128: warpgroup `wg` issues half `wg` (m64n128k16); CM: one warpgroup
     // issues the whole transposed tile (m64n128k16, weights as A: W_hi X_lo, W_lo X_hi, W_hi X_hi -- the same products in
-    // the same order).
+    // the same order).  P1: A_hi B_hi (CM: W_hi X_hi) only.
     // A descriptors: per-tap engine = 128 rows of 128 B in 8-row groups 1024 B apart (rows 64..127 start 8 KB in).  Halo
     // engine: rows of the tile are pixels (h, w) of a 16x8 patch; patch row h is one 8-row core-matrix group that starts
     // (h + r) * PW + s rows into the halo buffer => group stride PW*128 B and a start address that is only 128-byte
@@ -871,7 +874,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               for (int k = 0; k < 4; ++k) {
                 const uint64_t db_hi = wg_desc(bsm + 32 * k, 1024u), db_lo = wg_desc(bsm + Cfg::B_BYTES + 32 * k, 1024u);
                 const uint64_t da_hi = wg_desc(a_hi0 + 32 * k, a_sbo), da_lo = wg_desc(a_lo0 + 32 * k, a_sbo);
-                if constexpr (CM) {
+                if constexpr (P1 && CM) {
+                  wg_mma_64x128(acc[0], db_hi, da_hi, (it == c0 && k == 0) ? 0u : 1u);
+                } else if constexpr (P1) {
+                  wg_mma_64x128(acc[0], da_hi, db_hi, (it == c0 && k == 0) ? 0u : 1u);
+                } else if constexpr (CM) {
                   wg_mma_64x128(acc[0], db_hi, da_lo, (it == c0 && k == 0) ? 0u : 1u);
                   wg_mma_64x128(acc[0], db_lo, da_hi, 1u);
                   wg_mma_64x128(acc[0], db_hi, da_hi, 1u);
@@ -1627,15 +1634,49 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
                  m.a_hi, m.a_lo, m.b_hi, m.b_lo, p);
   return 0;
 }
+// Single-pass fp16 (ConvArgs::single_pass) exists only for the convs that run in fp16 mode: the generalised convs of RRDBNet,
+// and the generator / Fuse_sft_block convs of CodeFormer -- 128-wide halo tiles (fused transform with GroupNorm partials, or
+// raw planes), channel-major halo tiles (fused transform with partials, or raw planes) and the per-tap 1x1 conv on raw planes.
+// Anything else is an error: a conv never runs split when single pass was asked for.
+template <int CPG>
+static int launch_tc_p1(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen, int tile) {
+  constexpr bool T = true, F = false;
+  const bool halo3 = p.PW == 10 && p.PH == 18;
+  if (p.out_act != OUT_SILU) {
+    if (gen) {
+      if constexpr (CPG == 0) {
+        if (p.xform && halo3) return launch_tc2<64, 0, T, T, T, F, F, F, T>(m, p, sm_count, st);
+      }
+    } else if (tile == 128 && halo3) {
+      if constexpr (CPG == 4 || CPG == 8 || CPG == 16) {
+        if (p.xform) return launch_tc2<128, CPG, T, T, F, F, F, F, T>(m, p, sm_count, st);
+      }
+      if constexpr (CPG != 2) {
+        if (!p.xform) return launch_tc2<128, CPG, T, F, F, F, F, F, T>(m, p, sm_count, st);
+      }
+    } else if (tile == TC_TILE_CM && halo3) {
+      if constexpr (CPG == 2) {
+        if (p.xform) return launch_tc2<64, 2, T, T, F, F, T, F, T>(m, p, sm_count, st);
+      }
+      if constexpr (CPG <= 2) {
+        if (!p.xform) return launch_tc2<64, CPG, T, F, F, F, T, F, T>(m, p, sm_count, st);
+      }
+    } else if (tile == TC_TILE_N && !p.xform && p.PW == 0 && p.taps == 1) {
+      if constexpr (CPG == 0) return launch_tc2<64, 0, F, F, F, F, F, F, T>(m, p, sm_count, st);
+    }
+  }
+  CFB_REQUIRE(false, "conv_tc: single-pass fp16 is built for the generalised engine, the 128-wide and channel-major halo tiles "
+                     "and the per-tap 1x1 conv, without the SiLU epilogue");
+  return 1;
+}
+
 template <int CPG>
 static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st, bool gen = false, int tile = TC_TILE_N,
                      bool single_pass = false) {
   // the SiLU epilogue (YOLOv5) is built into two variants only, so the others keep their register budgets
   CFB_REQUIRE(p.out_act != OUT_SILU || (CPG == 0 && (gen || (!p.xform && p.PW == 0))),
               "conv_tc: the SiLU epilogue is built for the per-tap and generalised engines without statistics");
-  // the single-pass fp16 variant is built for the generalised engine without the SiLU epilogue (RRDBNet) only
-  CFB_REQUIRE(!single_pass || (CPG == 0 && gen && p.out_act != OUT_SILU),
-              "conv_tc: single-pass fp16 is built for the generalised engine without the SiLU epilogue");
+  if (single_pass) return launch_tc_p1<CPG>(m, p, sm_count, st, gen, tile);
   if (tile == TC_TILE_CM) {    // channel-major 128 x 64 tiles: conv_tc() only asks for them where tc_tile_kind() says so
     if constexpr (CPG <= 2) {
       CFB_REQUIRE(p.PW == 10 && p.PH == 18, "conv_tc: channel-major tiles need the 3x3 / Upsample halo engine");
@@ -1657,7 +1698,6 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   if constexpr (CPG == 0) {
     if (gen) {
       CFB_REQUIRE(p.xform && p.PW == 10 && p.PH == 18, "conv_tc: generalised variant needs the halo + transform engine");
-      if (single_pass) return launch_tc2<64, 0, true, true, true, false, false, false, true>(m, p, sm_count, st);
       if (p.out_act == OUT_SILU) return launch_tc2<64, 0, true, true, true, false, false, true>(m, p, sm_count, st);
       return launch_tc2<64, 0, true, true, true>(m, p, sm_count, st);
     }

@@ -177,8 +177,9 @@ struct ConvArgs {
   const float* residual2 = nullptr;   // out = act(conv + bias + residual) * post_scale + residual2
   int res2_pitch = 0;
   float post_scale = 1.f;
-  // gen only, opt-in: fp16 operands, one A_hi*B_hi wgmma product per k-step instead of the split scheme's three (fp32
-  // accumulation and output as before); the lo weight plane stays prepared but is not read
+  // opt-in: fp16 operands, one A_hi*B_hi wgmma product per k-step instead of the split scheme's three (fp32 accumulation and
+  // output as before); the lo weight plane stays prepared but is not read, nor is the lo plane of a raw-planes input.  Built
+  // for gen, the 128-wide and channel-major halo tiles and the per-tap 1x1 conv (conv_tc raises elsewhere)
   bool single_pass = false;
 };
 

@@ -303,6 +303,7 @@ struct cfb_net : cfb::NetCore {
   int gn_ctr_pos = 0;
   std::map<int, int64_t> ws_memo;     // batch -> cfb_workspace_bytes (16 host-side dry runs per miss)
   int engine = 0;                     // 0 auto (wgmma where the shape allows), 1 fp32 CUDA cores, 2 wgmma only
+  int precision = 0;                  // generator + fusion convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
   std::map<std::string, std::pair<float*, int64_t>> captures;   // stage name -> (device dst, capacity in floats)
 };
 
@@ -578,6 +579,7 @@ struct Fwd {
   // caller-side image plumbing fused into the first / last conv (cfb_codeformer_forward_u8): uint8 HWC BGR faces
   const unsigned char* in_u8 = nullptr;
   unsigned char* out_u8 = nullptr;
+  bool single_pass = false;   // the convs issued now run single-pass fp16 (ConvArgs::single_pass): set by generator()
 
   int alloc(Tensor& t, int N, int H, int W, int C) {
     t.N = N; t.H = H; t.W = W; t.C = C; t.owned = true; t.gn_part = nullptr; t.gn_slots = 0; t.planes = nullptr;
@@ -633,6 +635,8 @@ struct Fwd {
     a.in_scale = o.in_scale; a.in_shift = o.in_shift; a.in_act = o.in_act; a.residual = o.residual;
     a.out_act = o.out_act; a.sft_dec = o.sft_dec; a.sft_scale = o.sft_scale; a.sft_w = o.sft_w;
     bool use_tc = engine == 2 || (engine == 0 && n->tc_ok && tc_tiles_exact(a));
+    CFB_REQUIRE(dry || !single_pass || use_tc, "conv: precision fp16 runs on the wgmma engine only: " + w.name);
+    a.single_pass = single_pass;
     const bool no_f32 = o.planes_only && o.want_planes && use_tc && !o.out_ptr;
     if (o.out_ptr) {
       out.p = o.out_ptr; out.N = in.N; out.H = Ho; out.W = Wo; out.C = w.cout; out.owned = false;
@@ -901,9 +905,13 @@ struct Fwd {
 
   // Generator.forward with the SFT fusion of codeformer_arch.py:272-277; writes NCHW into out_nchw
   int generator(Tensor x, float* out_nchw, std::map<int, Tensor>* taps, const std::vector<int>& fuse_blocks, float w) {
+    // fp16 precision: the convs of every generator block and of the fusion run single pass, except the AttnBlocks' q,k,v and
+    // proj_out (about 2 of 586 GF per face); conv_last is the fp32 SIMT conv in both precisions
+    const bool p1 = n->precision == 1;
     float *ps = nullptr, *ph = nullptr;
     for (size_t i = 0; i < n->gen.size(); ++i) {
       const Block& b = n->gen[i];
+      single_pass = p1 && b.kind != B_ATTN;
       bool pl = next_takes_planes(n->gen, i);
       if (taps && w > 0.f)
         for (int fb : fuse_blocks)
@@ -942,6 +950,7 @@ struct Fwd {
             auto fw = n->fuse.find(x.W);
             CFB_REQUIRE(fw != n->fuse.end(), "fusion: no Fuse_sft_block for this size");
             Tensor fz;
+            single_pass = p1;
             CFB_CHECK(fuse(fw->second, it->second, x, w, fz));
             release(x);
             release(it->second);
@@ -1078,6 +1087,8 @@ static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float
   CFB_REQUIRE(n->cfg.kind == 1, "net was created as VQAutoEncoder");
   CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
   if (!dry) CFB_CHECK(check_device(n));
+  CFB_REQUIRE(dry || n->precision == 0 || (n->engine != 1 && n->tc_ok),
+              "precision fp16 (single pass) runs on the wgmma engine only: use engine 'auto' or 'tc' on an sm_90 device");
   CFB_REQUIRE(B >= 0, "negative batch");
   if (B == 0) return 0;
   n->arena.reset(ws, (size_t)ws_bytes, dry);
@@ -1120,6 +1131,8 @@ static int vqae_forward_impl(cfb_net* n, const float* x, float* out, int64_t* id
   CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
   if (B == 0) return 0;
   if (!dry) CFB_CHECK(check_device(n));
+  CFB_REQUIRE(dry || n->precision == 0 || (n->engine != 1 && n->tc_ok),
+              "precision fp16 (single pass) runs on the wgmma engine only: use engine 'auto' or 'tc' on an sm_90 device");
   n->arena.reset(ws, (size_t)ws_bytes, dry);
   Fwd f{n, st, n->arena, dry, n->engine};
   const cfb_config& c = n->cfg;
@@ -2471,6 +2484,16 @@ int cfb_net_set_engine(cfb_net* n, int32_t engine) {
   API_END(1)
 }
 
+int cfb_net_set_precision(cfb_net* n, int32_t precision) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_net_set_precision: NULL net");
+  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_net_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
+  std::lock_guard<std::mutex> lk(n->mu);
+  n->precision = precision;
+  return 0;
+  API_END(1)
+}
+
 int cfb_net_capture(cfb_net* n, const char* stage, float* dst, int64_t capacity) {
   API_BEGIN
   CFB_REQUIRE(n && stage, "cfb_net_capture: NULL argument");
@@ -2820,21 +2843,36 @@ int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const flo
                       const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
                       const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
                       void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n) {
+  return cfb_debug_conv_tc_prec(in, in2, cin1, weight_oihw, bias, out, n, h, w, cin, cout, mode, xform, in_scale, in_shift, in_act,
+                                residual, sft_dec, sft_scale, sft_w, out_planes, gn_part, workspace, workspace_bytes, stream,
+                                tile_n, 3, cfb::OUT_NONE, 0);
+}
+
+int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                           float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                           const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                           const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
+                           void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
+                           int32_t out_act, int32_t precision) {
   API_BEGIN
   CFB_REQUIRE(in && weight_oihw && out && workspace && tile_n, "cfb_debug_conv_tc: NULL argument");
   CFB_REQUIRE(mode == cfb::CONV_SAME || mode == cfb::CONV_UP, "cfb_debug_conv_tc: mode must be 0 or 2");
-  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, 3, mode), "cfb_debug_conv_tc: workspace too small");
+  CFB_REQUIRE(ksize == 3 || (ksize == 1 && mode == cfb::CONV_SAME && !xform), "cfb_debug_conv_tc_prec: ksize 3, or 1 (raw, mode 0)");
+  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_debug_conv_tc_prec: precision must be 0 (fp32, split) or 1 (fp16)");
+  CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_LRELU, "cfb_debug_conv_tc_prec: out_act must be 0 or 1 (LeakyReLU)");
+  CFB_REQUIRE(workspace_bytes >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, ksize, mode), "cfb_debug_conv_tc: workspace too small");
   CFB_CHECK(cfb::async_status_init(nullptr));
   cudaStream_t st = (cudaStream_t)stream;
   cfb::ConvArgs a;
-  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = 3; a.mode = mode;
+  a.in = in; a.N = n; a.H = h; a.W = w; a.Cin = cin; a.Cout = cout; a.ksize = ksize; a.mode = mode;
   a.Ho = mode == cfb::CONV_UP ? h * 2 : h;
   a.Wo = mode == cfb::CONV_UP ? w * 2 : w;
   a.bias = bias; a.in_scale = in_scale; a.in_shift = in_shift; a.in_act = in_act; a.residual = residual; a.out = out;
   a.sft_dec = sft_dec; a.sft_scale = sft_scale; a.sft_w = sft_w; a.out_planes = out_planes; a.gn_part = gn_part;
   a.in2 = in2; a.Cin1 = in2 ? cin1 : 0;
+  a.out_act = out_act; a.single_pass = precision == 1;
   CFB_REQUIRE(cfb::tc_supported(a), "cfb_debug_conv_tc: shape not on the wgmma engine");
-  const size_t wn = (size_t)cout * cin * 9;
+  const size_t wn = (size_t)cout * cin * ksize * ksize;
   const size_t wsplit = mode == cfb::CONV_UP ? (size_t)16 * cout * cin : wn;
   char* p = (char*)workspace + align256(wn * 4);
   __half* whi = (__half*)p; p += align256(wsplit * 2);
@@ -2850,7 +2888,7 @@ int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const flo
   CFB_CUDA(cudaGetDevice(&dev));
   CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   if (mode == cfb::CONV_UP) CFB_CHECK(cfb::tc_split_weights_up4(weight_oihw, whi, wlo, cout, cin, wsc, st));
-  else CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, 3, wsc, st));
+  else CFB_CHECK(cfb::tc_split_weights(weight_oihw, whi, wlo, cout, cin, ksize, wsc, st));
   *tile_n = cfb::tc_tile_n(a);
   CFB_CHECK(cfb::conv_tc(a, p, sms, st));
   return 0;

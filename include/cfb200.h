@@ -72,6 +72,12 @@ int64_t  cfb_workspace_bytes(cfb_net* net, int32_t batch);     /* scratch needed
 /* engine of the dense convolutions / linears: 0 = auto (wgmma tensor cores wherever the shape allows, default),
  * 1 = fp32 CUDA-core implicit GEMM everywhere, 2 = wgmma only (unsupported shapes are an error) */
 int      cfb_net_set_engine(cfb_net* net, int32_t engine);
+/* Precision of the generator and Fuse_sft_block convs (the decoder: everything after the code lookup / quantizer except the
+ * AttnBlocks' q,k,v / proj_out and conv_last): 0 = fp32 (default; split fp16 x3 operands, fp32 parity), 1 = fp16 (fp16
+ * operands, one tensor-core product per k-step, fp32 accumulation and fp32 activations).  The encoder, the Transformer, the
+ * quantizer and so logits, lq_feat and the code indices are the same in both.  fp16 needs engine 0 or 2 on an sm_90 device
+ * (the forward raises otherwise).  Other values are an error.  Takes effect at the next forward; no re-prepare. */
+int      cfb_net_set_precision(cfb_net* net, int32_t precision);
 /* parity hook: after stage `name` ("enc.<i>", "gen.<i>", "fuse.<size>", "ft.<l>", "quant") of the next forwards, copy
  * that NHWC fp32 activation to dst (device, `capacity` floats).  dst = NULL removes the hook. */
 int      cfb_net_capture(cfb_net* net, const char* stage, float* dst, int64_t capacity);
@@ -197,6 +203,17 @@ int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const flo
                       const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
                       const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
                       void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n);
+/* The same with the kernel size, the activation epilogue and the operand precision of cfb_net_set_precision: ksize 3, or 1
+ * (mode 0, xform 0: the per-tap engine on raw planes, *tile_n = 64); out_act 0 none | 1 LeakyReLU(0.2) (Fuse_sft_block's
+ * scale.0 / shift.0); precision 0 fp32 (split; == cfb_debug_conv_tc with out_act 0), 1 fp16 (single pass; built for the
+ * 128-wide and channel-major 3x3 / Upsample tiles and the 1x1 conv -- other forms are an error).
+ * workspace >= cfb_conv2d_workspace_bytes(n, h, w, cin, cout, ksize, mode). */
+int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                           float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                           const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                           const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
+                           void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
+                           int32_t out_act, int32_t precision);
 /* diagnostics / tests: the GroupNorm(32) finalize of the forward on partials in the layout cfb_debug_conv_tc writes (slots of
  * 32 pixels, [n][slots][32 groups][2] floats): scale[n,c] = rstd*gamma, shift[n,c] = beta - mean*rstd*gamma over hw pixels
  * of c channels.  The workspace (>= cfb_debug_gn_partials_workspace_bytes) holds the split-finalize scratch and the ticket
