@@ -187,10 +187,7 @@ class VectorQuantizer(nn.Module):
 
     # Fused path (include/cfb200.h: cfb_vq_nearest_fast): the split codebook + |e|^2 are prepared once per embedding version and
     # the workspace is kept per shape.  The library runs the whole forward as ONE kernel (conv_tc.cu: vq_fused_kernel), so a call
-    # is one launch on the caller's tensors; replaying it from a CUDA graph would only add the staging copies of z / z_q
-    # (measured: no gain), hence ``vq_graphs`` is off by default.  CFB_VQ_FUSED=0 (the 4-launch sequence) still profits from it.
-    vq_graphs = False
-
+    # is one launch on the caller's tensors.
     def _forward_fused(self, lib, z, E, return_min_encodings):
         dev = z.device
         B, D, H, W = z.shape
@@ -202,57 +199,25 @@ class VectorQuantizer(nn.Module):
             prep = torch.empty(int(lib.cfb_vq_prepared_bytes(K, D)), dtype=torch.uint8, device=dev)
             _lib.check(lib.cfb_vq_prepare(_lib.ptr(E), K, D, _lib.ptr(prep), prep.numel(), _stream_ptr(dev)), 'cfb_vq_prepare')
             cache.clear()
-            cache.update(sig=sig, prep=prep, E=E, graphs={})
+            cache.update(sig=sig, prep=prep, E=E)
         prep, E = cache['prep'], cache['E']
         T = B * H * W
-
-        def launch(zs, zq, idx, stats, onehot, ws):
-            _lib.check(lib.cfb_vq_nearest_fast(_lib.ptr(zs), _lib.ptr(E), _lib.ptr(prep), B, H, W, D, K, float(self.beta),
-                                               _lib.ptr(zq), _lib.ptr(idx), _lib.ptr(stats), _lib.ptr(onehot), _lib.ptr(ws),
-                                               ws.numel(), _stream_ptr(dev)), 'cfb_vq_nearest_fast')
-
-        def buffers(keep_ws=False):
-            ws = cache.setdefault('ws', {}).get((B, H, W)) if keep_ws else None
-            if ws is None:
-                ws = torch.empty(int(lib.cfb_vq_fast_workspace_bytes(B, H * W, D, K)), dtype=torch.uint8, device=dev)
-                if keep_ws:
-                    if len(cache['ws']) >= 4:
-                        cache['ws'].pop(next(iter(cache['ws'])))
-                    cache['ws'][(B, H, W)] = ws
-            return (torch.empty_like(z), torch.empty((T, 1), dtype=torch.int64, device=dev),
-                    torch.empty(4, dtype=torch.float32, device=dev),
-                    torch.empty((T, K), dtype=torch.float32, device=dev) if return_min_encodings else None, ws)
-        use_graph = T > 0 and (self.vq_graphs or os.environ.get('CFB_VQ_FUSED', '1') == '0') \
-            and os.environ.get('CFB_CUDA_GRAPH', '1') != '0' and not torch.cuda.is_current_stream_capturing()
-        if use_graph:
-            key = (B, H, W, bool(return_min_encodings))
-            ent = cache['graphs'].get(key)
-            if ent is None:
-                if len(cache['graphs']) >= 4:
-                    cache['graphs'].pop(next(iter(cache['graphs'])))
-                zs = torch.empty_like(z)
-                bufs = buffers()
-                zs.copy_(z)
-                launch(zs, *bufs)                                   # eager warm-up (function attributes) before the capture
-                torch.cuda.current_stream(dev).synchronize()
-                g = torch.cuda.CUDAGraph()
-                try:
-                    with torch.cuda.graph(g):
-                        launch(zs, *bufs)
-                    ent = (g, zs, bufs)
-                except Exception:
-                    ent = False
-                cache['graphs'][key] = ent
-            if ent:
-                g, zs, (zq, idx, stats, onehot, _) = ent
-                zs.copy_(z)
-                g.replay()
-                st = stats.clone()
-                return zq.clone(), st[0], {'perplexity': st[1], 'min_encodings': None if onehot is None else onehot.clone(),
-                                            'min_encoding_indices': idx.clone(), 'mean_distance': st[2]}
         # the kept workspace is only scratch of one launch; calls of one module are ordered by the caller's stream
-        zq, idx, stats, onehot, ws = buffers(keep_ws=not torch.cuda.is_current_stream_capturing())
-        launch(z, zq, idx, stats, onehot, ws)
+        keep_ws = not torch.cuda.is_current_stream_capturing()
+        ws = cache.setdefault('ws', {}).get((B, H, W)) if keep_ws else None
+        if ws is None:
+            ws = torch.empty(int(lib.cfb_vq_fast_workspace_bytes(B, H * W, D, K)), dtype=torch.uint8, device=dev)
+            if keep_ws:
+                if len(cache['ws']) >= 4:
+                    cache['ws'].pop(next(iter(cache['ws'])))
+                cache['ws'][(B, H, W)] = ws
+        zq = torch.empty_like(z)
+        idx = torch.empty((T, 1), dtype=torch.int64, device=dev)
+        stats = torch.empty(4, dtype=torch.float32, device=dev)
+        onehot = torch.empty((T, K), dtype=torch.float32, device=dev) if return_min_encodings else None
+        _lib.check(lib.cfb_vq_nearest_fast(_lib.ptr(z), _lib.ptr(E), _lib.ptr(prep), B, H, W, D, K, float(self.beta),
+                                           _lib.ptr(zq), _lib.ptr(idx), _lib.ptr(stats), _lib.ptr(onehot), _lib.ptr(ws),
+                                           ws.numel(), _stream_ptr(dev)), 'cfb_vq_nearest_fast')
         return zq, stats[0], {'perplexity': stats[1], 'min_encodings': onehot, 'min_encoding_indices': idx, 'mean_distance': stats[2]}
 
     def get_codebook_feat(self, indices, shape):

@@ -564,7 +564,6 @@ struct TcParams {
   const float* residual2; // out = (conv + bias + residual) * post_scale + residual2
   int res2_pitch;
   float post_scale;
-  const float* vq_e2; const float* vq_z2; float2* vq_cand; double* vq_dpart;   // VectorQuantizer argmin epilogue (see ConvArgs)
   int fault;              // test hook (cfb_debug_inject_fault): CTA 0 drops the weight load of its first stage -> barrier time-out
   int xform;              // XF kernel variant requested (in_scale may be null: raw split)
   int a_split;            // XF: k-blocks [0, a_split) are read from fp32 source 0 (tmA_hi), the rest from source 1 (tmA_lo)
@@ -1254,26 +1253,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       // instruction.  Each warp instead transposes 32x32-float blocks through a private 4 KB XOR-swizzled smem patch (BN = 128:
       // reads the tile slot directly): afterwards lane l holds the 16-byte chunk (l & 7) of row (l >> 3) + 4*it, i.e. 8 lanes
       // cover one full 128-byte line and every global access (residual / SFT loads, the store) is a fully used line.
-      if constexpr (!HALO && !GEN) if (p.vq_cand) {
-        // VectorQuantizer.forward (vqgan_arch.py:40-46): this thread owns token row `pix` and HC codes; d = (|z|^2 + |e|^2) - 2 z.e
-        // in the reference's operation order, first minimum of the slice (ascending index, strict <); no staging, no store of
-        // the [tokens, codes] matrix.  The candidates of a token (2 per n-tile) are reduced by vq_select_cand.
-        const float z2 = __ldg(p.vq_z2 + pix);
-        float best = INFINITY, dsum = 0.f;
-        int bi = col0;
-#pragma unroll
-        for (int j = 0; j < HC; ++j) {
-          const float d = (z2 + __ldg(p.vq_e2 + col0 + j)) - 2.f * (acc[j] * wsi);
-          dsum += d;
-          if (d < best) { best = d; bi = col0 + j; }
-        }
-        p.vq_cand[pix * (2 * p.n_tiles) + nt * 2 + half] = make_float2(best, __int_as_float(bi));
-        double ds = (double)dsum;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) ds += __shfl_xor_sync(0xffffffffu, ds, o);
-        if (lane == 0) p.vq_dpart[((int64_t)mt * p.n_tiles + nt) * 8 + (warp - 2)] = ds;
-        continue;
-      }
       const uint32_t stg = smem_u32(stage_buf) + (uint32_t)(warp - 2) * 4096u;     // 32 rows x 8 chunks of 16 B
       const uint32_t stg_w = stg + (uint32_t)lane * 128u;                          // this lane's row (write side)
       const int cch = lane & 7, rsub = lane >> 3;
@@ -1840,7 +1819,7 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     // per-tap engine writing a channel slice: the tile offsets use the destination pitch, which only the plain store follows
     CFB_REQUIRE(!geo.halo && p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.out_c0 + a.Cout <= p.out_pitch,
                 "conv_tc: a destination slice needs the per-tap engine, 4-aligned and inside the pitch");
-    CFB_REQUIRE(!a.residual && !a.sft_dec && !a.out_planes && !a.gn_part && !a.vq_cand && !a.residual2 && a.cout_valid == 0,
+    CFB_REQUIRE(!a.residual && !a.sft_dec && !a.out_planes && !a.gn_part && !a.residual2 && a.cout_valid == 0,
                 "conv_tc: a destination slice of the per-tap engine takes bias and activation only");
   }
   if (p.taps * p.kblocks <= 12) p.chunk = p.taps * p.kblocks;   // short K (Cin = 64): one partial sum, no 8+1 split
@@ -1849,8 +1828,6 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
 #if CFB_TC_STAMPS
   p.dbg = g_stamps.load();
 #endif
-  p.vq_e2 = a.vq_e2; p.vq_z2 = a.vq_z2; p.vq_cand = a.vq_cand; p.vq_dpart = a.vq_dpart;
-  CFB_REQUIRE(!a.vq_cand || (a.vq_e2 && a.vq_z2 && a.vq_dpart && a.ksize == 1 && !a.gen && !a.xform), "conv_tc: VQ argmin epilogue needs e2, z2 and the 1x1 engine");
   p.a_split = a.in2 ? a.Cin1 / 64 : a.Cin / 64;
   if (a.xform) {
     CFB_REQUIRE(a.skip_prep && tc_can_xform(a), "conv_tc: fused operand transform not available for this conv");
@@ -1932,7 +1909,6 @@ int bmm_tc(const BmmArgs& g, int sm_count, cudaStream_t st) {
 #if CFB_TC_STAMPS
   p.dbg = g_stamps.load();
 #endif
-  p.vq_e2 = nullptr; p.vq_z2 = nullptr; p.vq_cand = nullptr; p.vq_dpart = nullptr;
   p.Hin = 16; p.Win = 16; p.pad_mode = 0; p.sub = 0; p.out_pitch = out_pitch; p.out_c0 = 0; p.cout_valid = out_pitch; p.res_pitch = out_pitch;
   p.residual2 = nullptr; p.res2_pitch = out_pitch; p.post_scale = 1.f;
   p.bias = nullptr; p.residual = nullptr; p.out_act = OUT_NONE; p.sft_dec = nullptr; p.sft_scale = nullptr; p.sft_w = 0.f;
@@ -2144,7 +2120,7 @@ vq_fused_kernel(const __grid_constant__ CUtensorMap tmB_hi, const __grid_constan
   } else if (warp < 4) {
     // the MMA warpgroup: thread t holds rows 16*warp + lane/4 (+8) of each 64-row half and codes 8j + 2*(lane%4) (+1) of the
     // chunk; the same k-step order as conv_tc_kernel (per k-step and half: A_lo B_hi, A_hi B_lo, A_hi B_hi), so the dot products
-    // equal those of the 4-launch path bit for bit
+    // equal the stored ones of cfb_vq_nearest bit for bit
     const float wsi = __ldg(p.wscale_inv);
     float z2[4], best[4], dsum = 0.f;
     int bi[4];

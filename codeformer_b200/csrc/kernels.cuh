@@ -155,12 +155,6 @@ struct ConvArgs {
   bool skip_prep = false;           // operand planes in `scratch` are already valid (kernel-only timing)
   bool xform = false;      // tensor engine: read the fp32 activation `in` directly and apply in_scale/in_shift/in_act + the fp16 hi/lo
                            // split inside the conv kernel (tc_can_xform); in_scale == null: plain split of the raw values
-  // VectorQuantizer distance GEMM with the argmin in the epilogue (vqgan_arch.py:40-46): instead of storing z.E^T, every
-  // epilogue thread forms d = (|z|^2 + |e|^2) - 2 z.e for its token row and column slice and writes its first minimum
-  const float* vq_e2 = nullptr;     // [Cout] |e_j|^2
-  const float* vq_z2 = nullptr;     // [tokens] |z_t|^2
-  float2* vq_cand = nullptr;        // [tokens][2 * Cout / BN] (distance, index bits)
-  double* vq_dpart = nullptr;       // [m_tiles * n_tiles * 8] partial sums of all distances (mean_distance)
   bool halo1x1 = false;    // 1x1 conv with a GroupNorm-affine input (AttnBlock q,k,v): run it on the halo engine (patch = tile, one
                            // tap) so that the fused operand transform applies -- no separate operand-preparation pass
   const float* in2 = nullptr;   // xform only: channels [Cin1, Cin) come from this second NHWC tensor (torch.cat of Fuse_sft_block)
@@ -272,13 +266,7 @@ size_t vq_workspace_bytes(int T, int D, int K);
 int vq_nearest(const float* z, const float* codebook, int T, int D, int K, float beta, int64_t* idx, float* zq,
                float* stats, float* onehot, void* ws, cudaStream_t st);
 
-// fused path (config 3): z NCHW -> operand planes + |z|^2 (vq_prep_nchw), distance GEMM with argmin epilogue (conv_tc),
-// candidate reduction + gather + straight-through z_q in NCHW + loss partials (vq_select_cand), statistics (vq_final2)
-int vq_prep_nchw(const float* z_nchw, void* planes, float* z2, unsigned* hist, int N, int D, int HW, int K, cudaStream_t st);
-int vq_select_cand(const float* z_nchw, const float* codebook, const float2* cand, int ncand, int N, int D, int HW, int K,
-                   int64_t* idx, float* zq_nchw, double* se_part, unsigned* hist, cudaStream_t st);
-int vq_final2(const double* se_part, int n_se, const double* d_part, int n_d, const unsigned* hist, int T, int D, int K, float beta,
-              float* stats, cudaStream_t st);
+// one-kernel path (cfb_vq_nearest_fast): |e_k|^2 of the prepared codebook, and the one-hot rows of its indices
 int vq_e2(const float* codebook, float* e2, int K, int D, cudaStream_t st);
 int onehot_from_idx(const int64_t* idx, float* onehot, int T, int K, cudaStream_t st);
 

@@ -2654,7 +2654,8 @@ int cfb_vq_nearest(const float* z, const float* codebook, int32_t batch, int32_t
   float* zqt = (float*)p; p += tb;
   CFB_CHECK(cfb::nchw_to_nhwc(z, zt, batch, dim, h * w, st));
   cfb::ConvArgs a;
-  if (vq_tc_args(a, batch, h, w, dim, codes)) {
+  // conv_tc's operand prep takes dim = 64 * 2^k (<= 2048); other widths (e.g. 320) run on the SIMT kernel
+  if (vq_tc_args(a, batch, h, w, dim, codes) && dim >= 64 && dim <= 2048 && 256 % (dim / 8) == 0) {
     __half* whi = (__half*)p; p += align256((size_t)codes * dim * 2);
     __half* wlo = (__half*)p; p += align256((size_t)codes * dim * 2);
     float* wsc = (float*)p; p += 256;
@@ -2676,11 +2677,10 @@ int cfb_vq_nearest(const float* z, const float* codebook, int32_t batch, int32_t
   API_END(1)
 }
 
-// ---- VectorQuantizer.forward, fused path (BASELINE config 3): 4 launches on NCHW tensors ------------------------------------
+// ---- VectorQuantizer.forward, fused path (BASELINE config 3): ONE kernel (conv_tc.cu: vq_fused_kernel) on NCHW tensors ------
 int32_t cfb_vq_fast_supported(int32_t batch, int32_t h, int32_t w, int32_t dim, int32_t codes) {
   cfb::ConvArgs a;
-  if (!vq_tc_args(a, batch, h, w, dim, codes)) return 0;
-  return (codes % 128 == 0 && dim % 64 == 0 && dim <= 352 && (h * w) % 128 == 0 && batch >= 0) ? 1 : 0;
+  return vq_tc_args(a, batch, h, w, dim, codes) && cfb::vq_fused_supported(batch, dim, h * w, codes) ? 1 : 0;
 }
 int64_t cfb_vq_prepared_bytes(int32_t codes, int32_t dim) {
   // split codebook (hi, lo), weight scale, |e|^2, and the self-cleaning code histogram + ticket of the one-kernel path
@@ -2702,11 +2702,10 @@ int cfb_vq_prepare(const float* codebook, int32_t codes, int32_t dim, void* prep
   API_END(1)
 }
 int64_t cfb_vq_fast_workspace_bytes(int32_t batch, int32_t hw, int32_t dim, int32_t codes) {
-  const int64_t T = (int64_t)batch * hw;
-  const int64_t planes = 2 * ((T * dim * 2 + 1023) / 1024 * 1024);
-  const int64_t ncand = 2 * (codes / cfb::TC_TILE_N);
-  return planes + align256(T * 4) + align256(T * ncand * 8) + align256((T / 128 + 1) * (codes / cfb::TC_TILE_N) * 8 * 8) + align256((T / 32 + 1) * 8) +
-         align256((size_t)codes * 4) + 8192;
+  // vq_fused's partial sums (squared error, sum of distances: 2 doubles per CTA of 128 tokens) behind the 1024-byte alignment
+  // cfb_vq_nearest_fast applies to the workspace pointer
+  const int64_t ctas = (int64_t)batch * ((hw + 127) / 128);
+  return ctas * 16 + 1024;
 }
 int cfb_vq_nearest_fast(const float* z, const float* codebook, const void* prepared, int32_t batch, int32_t h, int32_t w, int32_t dim,
                         int32_t codes, float beta, float* z_q, int64_t* idx, float* stats, float* min_encodings, void* workspace,
@@ -2725,36 +2724,11 @@ int cfb_vq_nearest_fast(const float* z, const float* codebook, const void* prepa
   const __half* wlo = (const __half*)q; q += align256((size_t)codes * dim * 2);
   const float* wsc = (const float*)q; q += 256;
   const float* e2 = (const float*)q;
-  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
-  if (cfb::vq_fused_supported(batch, dim, HW, codes) && !(getenv("CFB_VQ_FUSED") && atoi(getenv("CFB_VQ_FUSED")) == 0)) {
-    // ONE kernel (conv_tc.cu: vq_fused_kernel): histogram / ticket live in the prepared buffer (zero between calls);
-    // CFB_VQ_FUSED=0 selects the 4-launch path below
-    unsigned* fh = (unsigned*)((char*)e2 + align256((size_t)codes * 4));
-    unsigned* ticket = (unsigned*)((char*)fh + align256((size_t)codes * 4));
-    CFB_CHECK(cfb::vq_fused(z, codebook, whi, wlo, wsc + 1, e2, fh, ticket, (double*)p, batch, dim, HW, codes, beta, z_q, idx, stats, st));
-    if (min_encodings) CFB_CHECK(cfb::onehot_from_idx(idx, min_encodings, (int)T, codes, st));
-    return 0;
-  }
-  void* planes = p; p += 2 * (((size_t)T * dim * 2 + 1023) / 1024 * 1024);
-  float* z2 = (float*)p; p += align256((size_t)T * 4);
-  const int ncand = 2 * (codes / cfb::TC_TILE_N);      // two candidates (column halves) per n-tile of the distance GEMM
-  float2* cand = (float2*)p; p += align256((size_t)T * ncand * 8);
-  const int n_d = (int)(T / 128) * (codes / cfb::TC_TILE_N) * 8;
-  double* dpart = (double*)p; p += align256((size_t)(T / 128 + 1) * (codes / cfb::TC_TILE_N) * 8 * 8);
-  const int n_se = (int)(T / 32);
-  double* separt = (double*)p; p += align256((size_t)(T / 32 + 1) * 8);
-  unsigned* hist = (unsigned*)p;
-  int dev = 0, sms = 148;
-  CFB_CUDA(cudaGetDevice(&dev));
-  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CFB_CHECK(cfb::vq_prep_nchw(z, planes, z2, hist, batch, dim, HW, codes, st));
-  cfb::ConvArgs a;
-  a.N = batch; a.H = h; a.W = w; a.Cin = dim; a.Ho = h; a.Wo = w; a.Cout = codes; a.ksize = 1; a.mode = cfb::CONV_SAME;
-  a.wgt_hi = whi; a.wgt_lo = wlo; a.wscale_inv = wsc + 1; a.skip_prep = true;
-  a.vq_e2 = e2; a.vq_z2 = z2; a.vq_cand = cand; a.vq_dpart = dpart;
-  CFB_CHECK(cfb::conv_tc(a, planes, sms, st));
-  CFB_CHECK(cfb::vq_select_cand(z, codebook, cand, ncand, batch, dim, HW, codes, idx, z_q, separt, hist, st));
-  CFB_CHECK(cfb::vq_final2(separt, n_se, dpart, n_d, hist, (int)T, dim, codes, beta, stats, st));
+  // the code histogram and the last-CTA ticket live in the prepared buffer (zero between calls)
+  unsigned* hist = (unsigned*)((char*)e2 + align256((size_t)codes * 4));
+  unsigned* ticket = (unsigned*)((char*)hist + align256((size_t)codes * 4));
+  double* part = (double*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+  CFB_CHECK(cfb::vq_fused(z, codebook, whi, wlo, wsc + 1, e2, hist, ticket, part, batch, dim, HW, codes, beta, z_q, idx, stats, st));
   if (min_encodings) CFB_CHECK(cfb::onehot_from_idx(idx, min_encodings, (int)T, codes, st));
   return 0;
   API_END(1)

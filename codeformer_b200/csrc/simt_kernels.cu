@@ -1722,134 +1722,7 @@ int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* ma
 }  // namespace cfb
 
 namespace cfb {
-// ---- VectorQuantizer fused path (BASELINE config 3): 4 launches, z and z_q stay NCHW (the caller's layout) ----------------
-// K1: z [N, D, HW] NCHW -> fp16 hi/lo operand planes [N*HW, D] (token-major) + |z_t|^2; also clears the code histogram.
-// One CTA = 32 consecutive tokens of one image; reads are 128-byte lines along HW, the planes are written 512 B per token.
-__global__ void __launch_bounds__(256) vq_prep_nchw_kernel(const float* __restrict__ z, __half* __restrict__ hi, __half* __restrict__ lo,
-                                                           float* __restrict__ z2, unsigned* __restrict__ hist, int D, int HW, int K) {
-  extern __shared__ float tile[];                 // [D][33]
-  const int n = blockIdx.y, t0 = blockIdx.x * 32, w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (blockIdx.y == 0) for (int k = blockIdx.x * 256 + threadIdx.x; k < K; k += gridDim.x * 256) hist[k] = 0u;
-  const float* zb = z + (int64_t)n * D * HW + t0;
-  for (int c = w; c < D; c += 8) tile[c * 33 + l] = __ldg(zb + (int64_t)c * HW + l);
-  __syncthreads();
-  for (int tl = w * 4; tl < w * 4 + 4; ++tl) {
-    const int64_t tok = (int64_t)n * HW + t0 + tl;
-    float ss = 0.f;
-    for (int c8 = l; c8 < D / 8; c8 += 32) {
-      __align__(16) __half hh[8];
-      __align__(16) __half ll[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float v = tile[(c8 * 8 + j) * 33 + tl];
-        ss = fmaf(v, v, ss);
-        hh[j] = __float2half_rn(v);
-        ll[j] = __float2half_rn(v - __half2float(hh[j]));
-      }
-      *reinterpret_cast<uint4*>(hi + tok * D + c8 * 8) = *reinterpret_cast<const uint4*>(hh);
-      *reinterpret_cast<uint4*>(lo + tok * D + c8 * 8) = *reinterpret_cast<const uint4*>(ll);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    if (l == 0) z2[tok] = ss;
-  }
-}
-int vq_prep_nchw(const float* z_nchw, void* planes, float* z2, unsigned* hist, int N, int D, int HW, int K, cudaStream_t st) {
-  CFB_REQUIRE(D % 8 == 0 && D <= 352 && HW % 32 == 0, "vq_prep_nchw: D must be a multiple of 8 (<= 352), HW of 32");
-  if (N == 0) return 0;
-  const size_t plane = ((size_t)N * HW * D * 2 + 1023) / 1024 * 1024;
-  vq_prep_nchw_kernel<<<dim3(HW / 32, N), 256, (size_t)D * 33 * 4, st>>>(z_nchw, (__half*)planes, (__half*)((char*)planes + plane), z2,
-                                                                      hist, D, HW, K);
-  CFB_LAUNCH_CHECK();
-  return 0;
-}
-
-// K3: reduce the per-slice candidates of every token (lowest distance, lowest index on ties = torch.argmin's first minimum),
-// write the index, count it, and emit the straight-through z_q = z + (e - z) in NCHW plus the squared-error partial sums.
-__global__ void __launch_bounds__(256) vq_select_cand_kernel(const float* __restrict__ z, const float* __restrict__ E,
-                                                             const float2* __restrict__ cand, int ncand, int D, int HW, int K,
-                                                             int64_t* __restrict__ idx, float* __restrict__ zq,
-                                                             double* __restrict__ se_part, unsigned* __restrict__ hist) {
-  __shared__ int sidx[32];
-  __shared__ double red[8];
-  const int n = blockIdx.y, t0 = blockIdx.x * 32, w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  for (int tl = w * 4; tl < w * 4 + 4; ++tl) {
-    const int64_t tok = (int64_t)n * HW + t0 + tl;
-    float best = INFINITY;
-    int bi = 0x7fffffff;
-    for (int c = l; c < ncand; c += 32) {
-      const float2 v = __ldg(cand + tok * ncand + c);
-      const int vi = __float_as_int(v.y);
-      if (v.x < best || (v.x == best && vi < bi)) { best = v.x; bi = vi; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-    }
-    bi = min(max(bi, 0), K - 1);               // NaN distances: a valid index, never out of bounds
-    if (l == 0) { sidx[tl] = bi; idx[tok] = (int64_t)bi; atomicAdd(hist + bi, 1u); }
-  }
-  __syncthreads();
-  const int my = sidx[l];
-  const float* zb = z + (int64_t)n * D * HW + t0 + l;
-  float* qb = zq + (int64_t)n * D * HW + t0 + l;
-  double se = 0.0;
-  for (int c = w; c < D; c += 8) {
-    const float zz = __ldg(zb + (int64_t)c * HW);
-    const float diff = __ldg(E + (int64_t)my * D + c) - zz;
-    se += (double)(diff * diff);
-    qb[(int64_t)c * HW] = zz + diff;           // z + (z_q - z), vqgan_arch.py:57
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
-  if (l == 0) red[w] = se;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double a = 0.0;
-    for (int i = 0; i < 8; ++i) a += red[i];
-    se_part[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = a;
-  }
-}
-int vq_select_cand(const float* z_nchw, const float* codebook, const float2* cand, int ncand, int N, int D, int HW, int K,
-                   int64_t* idx, float* zq_nchw, double* se_part, unsigned* hist, cudaStream_t st) {
-  CFB_REQUIRE(HW % 32 == 0, "vq_select_cand: HW must be a multiple of 32");
-  if (N == 0) return 0;
-  vq_select_cand_kernel<<<dim3(HW / 32, N), 256, 0, st>>>(z_nchw, codebook, cand, ncand, D, HW, K, idx, zq_nchw, se_part, hist);
-  CFB_LAUNCH_CHECK();
-  return 0;
-}
-
-__global__ void vq_final2_kernel(const double* __restrict__ se_part, int n_se, const double* __restrict__ d_part, int n_d,
-                                 const unsigned* __restrict__ hist, int T, int D, int K, float beta, float* __restrict__ stats) {
-  __shared__ double sred[3][256];
-  const int t = threadIdx.x;
-  double ent = 0.0, se = 0.0, ds = 0.0;
-  for (int k = t; k < K; k += 256) {
-    const float em = (float)hist[k] / (float)T;
-    ent += (double)(em * logf(em + 1e-10f));
-  }
-  for (int i = t; i < n_se; i += 256) se += se_part[i];
-  for (int i = t; i < n_d; i += 256) ds += d_part[i];
-  sred[0][t] = ent; sred[1][t] = se; sred[2][t] = ds;
-  __syncthreads();
-  if (t == 0) {
-    double e = 0.0, s = 0.0, d = 0.0;
-    for (int i = 0; i < 256; ++i) { e += sred[0][i]; s += sred[1][i]; d += sred[2][i]; }      // fixed order: deterministic
-    const float mse = (float)(s / ((double)T * D));
-    stats[0] = mse + beta * mse;               // vqgan_arch.py:55
-    stats[1] = expf(-(float)e);                // perplexity, :60-61
-    stats[2] = (float)(d / ((double)T * K));   // mean_distance, :42
-    stats[3] = 0.f;
-  }
-}
-int vq_final2(const double* se_part, int n_se, const double* d_part, int n_d, const unsigned* hist, int T, int D, int K, float beta,
-              float* stats, cudaStream_t st) {
-  vq_final2_kernel<<<1, 256, 0, st>>>(se_part, n_se, d_part, n_d, hist, T, D, K, beta, stats);
-  CFB_LAUNCH_CHECK();
-  return 0;
-}
+// ---- VectorQuantizer one-kernel path (cfb_vq_nearest_fast): |e|^2 of the prepared codebook, one-hot rows of the indices ----
 __global__ void vq_e2_only_kernel(const float* __restrict__ E, float* __restrict__ e2, int K, int D) {
   const int code = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int l = threadIdx.x & 31;

@@ -134,12 +134,12 @@ int cfb_vq_nearest(const float* z, const float* codebook, int32_t batch, int32_t
 
 /* VectorQuantizer.forward, fused path (vqgan_arch.py:33-70; BASELINE configs[2]): the codebook is split for the tensor cores and
  * its |e|^2 computed ONCE (cfb_vq_prepare, redo when the embedding changes).  A call is then ONE kernel on the caller's NCHW
- * tensors when h*w % 128 == 0, dim <= 256, codes <= 1024 (vq_fused_kernel: z tile -> shared-memory operand planes, codebook
- * through TMA, distances on wgmma with the argmin taken from the register accumulators, gather + straight-through z_q + loss,
- * statistics by the last CTA; the prepared buffer also holds the kernel's self-cleaning histogram, so calls sharing one
- * prepared buffer must not overlap), otherwise 4 launches (operand planes + |z|^2, distance GEMM with the argmin in its
- * epilogue, candidate reduction + gather, statistics).  The [tokens, codes] matrix is never stored.  Same outputs as cfb_vq_nearest.
- * cfb_vq_fast_supported: 16x16-style latents (h*w % 128 == 0), dim % 64 == 0, codes % 128 == 0, sm_90. */
+ * tensors (vq_fused_kernel: z tile -> shared-memory operand planes, codebook through TMA, distances on wgmma with the argmin
+ * taken from the register accumulators, gather + straight-through z_q + loss, statistics by the last CTA; the prepared buffer
+ * also holds the kernel's self-cleaning histogram, so calls sharing one prepared buffer must not overlap).  The [tokens, codes]
+ * matrix is never stored.  Same outputs as cfb_vq_nearest.
+ * cfb_vq_fast_supported: sm_90, 16x16-style latents (h*w % 128 == 0, exact tensor-core tiles), dim % 64 == 0 and
+ * 64 <= dim <= 256, codes % 64 == 0 and codes <= 1024; other shapes go to cfb_vq_nearest. */
 int32_t cfb_vq_fast_supported(int32_t batch, int32_t h, int32_t w, int32_t dim, int32_t codes);
 int64_t cfb_vq_prepared_bytes(int32_t codes, int32_t dim);
 int     cfb_vq_prepare(const float* codebook, int32_t codes, int32_t dim, void* prepared, int64_t prepared_bytes, void* stream);

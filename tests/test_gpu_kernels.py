@@ -215,39 +215,49 @@ def test_vq_edge_cases():
     assert zq.shape == (0, 256, 16, 16) and st['min_encoding_indices'].shape == (0, 1)
 
 
-@pytest.mark.parametrize('one_kernel', [True, False])
-def test_vq_fused_path_equals_the_unfused_one(one_kernel, monkeypatch):
-    """The fused paths -- ONE kernel (z tile in shared memory, argmin from the wgmma accumulators, statistics by the last CTA)
-    and the 4-launch variant (argmin in the GEMM epilogue) -- with the prepared codebook and CUDA-graph replay, against the
-    unfused path (stored dot products) on the config-3 inputs: same indices, z_q and statistics; a changed embedding is picked up."""
+# (dim, codes, seed, one kernel): the config-3 shape and inputs (seed 0 = vq_micro_inputs('B')); codes % 128 == 64 inside the
+# one kernel's limits; emb_dim 320 and 2048 codes outside them, where the module runs cfb_vq_nearest (the SIMT kernel at
+# emb_dim 320, whose width the tensor-core operand prep does not take; stored dot products at 2048 codes).  The other seeds keep every token's two nearest codes >= 8e-4 apart in float64 (for E and -E), far above the
+# rounding of the fp32 distances, so the float64 argmin is a fair check.
+VQ_PATH_CASES = [(256, 1024, 0, 1), (256, 960, 3, 1), (320, 1024, 5, 0), (256, 2048, 3, 0)]
+
+
+@pytest.mark.parametrize('dim,codes,seed,one_kernel', VQ_PATH_CASES)
+def test_vq_fused_path_equals_the_unfused_one(dim, codes, seed, one_kernel):
+    """VectorQuantizer.forward -- the ONE-kernel fused path (z tile in shared memory, argmin from the wgmma accumulators,
+    statistics by the last CTA) with the prepared codebook where the shape allows it -- called twice, against the unfused path
+    (stored dot products) and a float64 argmin: same indices, z_q and statistics; a changed embedding is picked up."""
     import codeformer_b200 as cb
-    monkeypatch.setenv('CFB_VQ_FUSED', '1' if one_kernel else '0')
     lib = _lib.load()
-    E, z = vq_micro_inputs('B')
-    vq = cb.VectorQuantizer(1024, 256, 0.25)
+    g = torch.Generator().manual_seed(seed)
+    E = torch.randn(codes, dim, generator=g)
+    z = torch.randn(32, dim, 16, 16, generator=g)
+    zf = z.permute(0, 2, 3, 1).reshape(-1, dim).double()
+    vq = cb.VectorQuantizer(codes, dim, 0.25)
     vq.embedding.weight.data.copy_(E)
     vq = vq.cuda()
     zd = z.cuda()
-    assert lib.cfb_vq_fast_supported(32, 16, 16, 256, 1024) == 1
-    zq, loss, st = vq(zd)                                           # fused (graph captured on this call)
-    zq2, loss2, st2 = vq(zd)                                        # graph replay
+    assert lib.cfb_vq_fast_supported(32, 16, 16, dim, codes) == one_kernel
+    zq, loss, st = vq(zd)
+    zq2, loss2, st2 = vq(zd)                                        # prepared codebook and workspace reused
     assert torch.equal(zq, zq2) and torch.equal(st['min_encoding_indices'], st2['min_encoding_indices']) and float(loss) == float(loss2)
     Ed = vq.embedding.weight.detach().contiguous()
     zq_o = torch.empty_like(zd)
     idx_o = torch.empty((8192, 1), dtype=torch.int64, device='cuda')
     stats_o = torch.empty(4, device='cuda')
-    wsb = lib.cfb_vq_workspace_bytes(32, 256, 256, 1024)
+    wsb = lib.cfb_vq_workspace_bytes(32, 256, dim, codes)
     ws = torch.empty(int(wsb), dtype=torch.uint8, device='cuda')
-    _lib.check(lib.cfb_vq_nearest(_lib.ptr(zd), _lib.ptr(Ed), 32, 16, 16, 256, 1024, 0.25, _lib.ptr(zq_o), _lib.ptr(idx_o),
+    _lib.check(lib.cfb_vq_nearest(_lib.ptr(zd), _lib.ptr(Ed), 32, 16, 16, dim, codes, 0.25, _lib.ptr(zq_o), _lib.ptr(idx_o),
                                   _lib.ptr(stats_o), None, _lib.ptr(ws), wsb, G.stream()), 'cfb_vq_nearest')
     torch.cuda.synchronize()
     assert torch.equal(st['min_encoding_indices'], idx_o) and torch.equal(zq, zq_o)
     assert abs(float(loss) - float(stats_o[0])) < 1e-6 * float(stats_o[0])
     assert abs(float(st['mean_distance']) - float(stats_o[2])) < 1e-5 * float(stats_o[2])
+    d = (zf ** 2).sum(1, keepdim=True) + (E.double() ** 2).sum(1) - 2 * zf @ E.double().t()
+    assert torch.equal(st['min_encoding_indices'].cpu()[:, 0], d.argmin(1))
     with torch.no_grad():
         vq.embedding.weight.mul_(-1.0)                              # in-place update bumps the version: re-prepared
     idx_neg = vq(zd)[2]['min_encoding_indices']
     assert not torch.equal(idx_neg, st['min_encoding_indices'])
-    d = ((z.permute(0, 2, 3, 1).reshape(-1, 256).double() ** 2).sum(1, keepdim=True) + (E.double() ** 2).sum(1)
-         + 2 * z.permute(0, 2, 3, 1).reshape(-1, 256).double() @ E.double().t())
+    d = (zf ** 2).sum(1, keepdim=True) + (E.double() ** 2).sum(1) + 2 * zf @ E.double().t()
     assert torch.equal(idx_neg.cpu()[:, 0], d.argmin(1))
