@@ -125,6 +125,12 @@ SIGNATURES = {
     'cfb_resize_linear_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
     'cfb_paste_faces_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
     'cfb_paste_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, c_double, _P, _P, _P, c_int64, _P]),
+    'cfb_resize_area_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'cfb_resize_linear_scale_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, c_double, c_double, _P]),
+    'cfb_warp_affine_multi_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, _P, c_int32, _P, c_int32, c_int32, c_int32, c_int32,
+                                         c_int32, c_int32, _P]),
+    'cfb_paste_faces_multi_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
+    'cfb_paste_faces_multi': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, _P, c_double, _P, _P, c_int64, _P]),
 }
 
 _lib = None

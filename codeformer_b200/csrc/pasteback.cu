@@ -16,13 +16,19 @@
 // 0; at the canvas border both follow cv2 (no erosion, reflect-101).
 //
 // The steps that do not depend on the blend order run for all faces at once (blockIdx.z = face).  The areas of the first
-// erosion are read back once per image (they fix the kernel sizes); then one composite launch per face, in face order.
+// erosion are read back once per call (they fix the kernel sizes); then one composite launch per face, in face order.
+// cfb_paste_faces_multi runs the same launch sequence over the faces of several equal-size canvases in one call.
+//
+//   INTER_AREA    (shrinking, cfb_resize_area_u8) integer factors: window sums, a 2 x 2 halving (s + 2) >> 2, otherwise
+//                 cvRound(s * (1.f / area)); other factors: computeResizeAreaTab weights in double stored as float, a float
+//                 row sum per source row and a float sum of the rows, both in cv2's tap order, then cvRound and clamp.
 // Arithmetic that cv2 does unfused is written with _rn intrinsics so nvcc cannot contract it into FMAs.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -185,6 +191,82 @@ __global__ void k_resize_u8(const uint8_t* __restrict__ src, int h, int w, uint8
     const int v = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
     o[c] = (uint8_t)min(max(v, 0), 255);
   }
+}
+
+// INTER_AREA, integer factors (resizeAreaFast): window sums; 2 x 2 rounds as (s + 2) >> 2, others cvRound(s * (1.f / area))
+__global__ void k_resize_area_fast_u8(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst, int oh, int ow,
+                                      int sx, int sy, float inv_area, int n) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh || f >= n) return;
+  src += (size_t)f * h * w * 3;
+  int s[3] = {0, 0, 0};
+  for (int i = 0; i < sy; ++i) {
+    const uint8_t* p = src + ((size_t)(y * sy + i) * w + (size_t)x * sx) * 3;
+    for (int j = 0; j < sx * 3; j += 3) { s[0] += p[j]; s[1] += p[j + 1]; s[2] += p[j + 2]; }
+  }
+  uint8_t* o = dst + (((size_t)f * oh + y) * ow + x) * 3;
+  for (int c = 0; c < 3; ++c)
+    o[c] = (uint8_t)(sx == 2 && sy == 2 ? (s[c] + 2) >> 2 : min(max(__float2int_rn(__fmul_rn((float)s[c], inv_area)), 0), 255));
+}
+
+// INTER_AREA, general path (resizeArea): per source row the float row sum of the x taps, then the float sum of
+// beta * row over the y taps, both in table order; taps padded to kx / ky with weight 0 (adding +0 is exact)
+__global__ void k_resize_area_u8(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst, int oh, int ow,
+                                 const int* __restrict__ xi, const float* __restrict__ xa, int kx,
+                                 const int* __restrict__ yi, const float* __restrict__ ya, int ky, int n) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh || f >= n) return;
+  src += (size_t)f * h * w * 3;
+  float sum[3] = {0.f, 0.f, 0.f};
+  for (int t = 0; t < ky; ++t) {
+    const uint8_t* row = src + (size_t)yi[y * ky + t] * w * 3;
+    const float beta = ya[y * ky + t];
+    float buf[3] = {0.f, 0.f, 0.f};
+    for (int u = 0; u < kx; ++u) {
+      const uint8_t* p = row + (size_t)xi[x * kx + u] * 3;
+      const float a = xa[x * kx + u];
+      for (int c = 0; c < 3; ++c) buf[c] = __fadd_rn(buf[c], __fmul_rn((float)p[c], a));
+    }
+    for (int c = 0; c < 3; ++c) sum[c] = __fadd_rn(sum[c], __fmul_rn(beta, buf[c]));
+  }
+  uint8_t* o = dst + (((size_t)f * oh + y) * ow + x) * 3;
+  for (int c = 0; c < 3; ++c) o[c] = (uint8_t)min(max(__float2int_rn(sum[c]), 0), 255);
+}
+
+// computeResizeAreaTab in double (cv2's arithmetic), as [dsize, K] source indices and weights padded with weight 0
+int area_taps(int ssize, int dsize, double scale, std::vector<int>& idx, std::vector<float>& wt) {
+  std::vector<std::vector<std::pair<int, float>>> taps(dsize);
+  for (int dx = 0; dx < dsize; ++dx) {
+    const double fsx1 = dx * scale, fsx2 = fsx1 + scale;
+    const double cell = std::min(scale, ssize - fsx1);
+    int sx1 = (int)std::ceil(fsx1), sx2 = (int)std::floor(fsx2);
+    sx2 = std::min(sx2, ssize - 1);
+    sx1 = std::min(sx1, sx2);
+    if (sx1 - fsx1 > 1e-3) taps[dx].push_back({sx1 - 1, (float)((sx1 - fsx1) / cell)});
+    for (int sx = sx1; sx < sx2; ++sx) taps[dx].push_back({sx, (float)(1.0 / cell)});
+    if (fsx2 - sx2 > 1e-3) taps[dx].push_back({sx2, (float)(std::min(std::min(fsx2 - sx2, 1.), cell) / cell)});
+  }
+  size_t K = 1;
+  for (const auto& t : taps) K = std::max(K, t.size());
+  idx.assign((size_t)dsize * K, 0);
+  wt.assign((size_t)dsize * K, 0.f);
+  for (int d = 0; d < dsize; ++d)
+    for (size_t t = 0; t < taps[d].size(); ++t) { idx[d * K + t] = taps[d][t].first; wt[d * K + t] = taps[d][t].second; }
+  return (int)K;
+}
+
+// crops of several equal-size images: crop f samples image img_of[f] (the k_warp_crop arithmetic)
+__global__ void k_warp_crop_multi(const uint8_t* __restrict__ src, int h, int w, const double* __restrict__ maps,
+                                  const int* __restrict__ img_of, int n, uint8_t* __restrict__ out, int oh, int ow, int mode,
+                                  int c0, int c1, int c2) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= ow || y >= oh || f >= n) return;
+  int ix, iy, fx, fy, v[3];
+  const int cval[3] = {c0, c1, c2};
+  warp_coord(maps + 6 * f, x, y, ix, iy, fx, fy);
+  sample_u8(src + (size_t)img_of[f] * h * w * 3, h, w, ix, iy, fx, fy, mode, cval, v);
+  uint8_t* o = out + (((size_t)f * oh + y) * ow + x) * 3;
+  o[0] = (uint8_t)v[0]; o[1] = (uint8_t)v[1]; o[2] = (uint8_t)v[2];
 }
 
 __global__ void k_resize_f64(const double* __restrict__ src, int h, int w, double* __restrict__ dst, int oh, int ow,
@@ -410,11 +492,11 @@ struct Layout {
   size_t canvas, roi, parse0, parse1, parse_rs, faces, area, pgauss, gauss, total;
 };
 
-Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gauss_floats) {
+Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gauss_floats, int n_img = 1) {
   Layout L{};
   size_t o = 0;
   auto take = [&](size_t b) { const size_t r = o; o += align256(b); return r; };
-  L.canvas = take((size_t)H * W * 3 * (use_parse ? 8 : 4));
+  L.canvas = take((size_t)n_img * H * W * 3 * (use_parse ? 8 : 4));
   L.roi = take(P.roi_floats * 4);
   const size_t pm = (size_t)n * kParse * kParse * 8;
   L.parse0 = take(use_parse ? pm : 0);
@@ -435,14 +517,16 @@ int max_gauss_floats(const Plan& P) {
   return s;
 }
 
+// n_img canvases [n_img,H,W,3]; face i goes into canvas img_of[i] (img_of == nullptr: all into canvas 0).  Every step
+// before the composite is per face, so a face's result does not depend on the other canvases of the batch.
 template <typename T>
-int paste_impl(uint8_t* canvas_u8, int H, int W, const uint8_t* faces, int n, int S, const uint8_t* parse_u8,
-               const double* inv, double upscale, float* dbg, int32_t* w_edge_out, char* ws, int64_t ws_bytes,
-               cudaStream_t st) {
+int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int W, const uint8_t* faces, int n, int S,
+               const uint8_t* parse_u8, const double* inv, double upscale, float* dbg, int32_t* w_edge_out, char* ws,
+               int64_t ws_bytes, cudaStream_t st) {
   const bool use_parse = parse_u8 != nullptr;
   Plan P;
   CFB_CHECK(make_plan(H, W, n, S, inv, P));
-  const Layout L = layout(H, W, n, S, use_parse, P, max_gauss_floats(P));
+  const Layout L = layout(H, W, n, S, use_parse, P, max_gauss_floats(P), n_img);
   CFB_REQUIRE((int64_t)L.total <= ws_bytes, "cfb_paste_faces: workspace too small");
   T* canvas = (T*)(ws + L.canvas);
   float* roi = (float*)(ws + L.roi);
@@ -450,7 +534,7 @@ int paste_impl(uint8_t* canvas_u8, int H, int W, const uint8_t* faces, int n, in
   double* darea = (double*)(ws + L.area);
   float* dgauss = (float*)(ws + L.gauss);
   double* dpk = (double*)(ws + L.pgauss);
-  const size_t npx = (size_t)H * W * 3;
+  const size_t npx = (size_t)n_img * H * W * 3;
   k_canvas_in<T><<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(canvas_u8, canvas, npx);
   CFB_LAUNCH_CHECK();
   const dim3 b(32, 8);
@@ -522,8 +606,9 @@ int paste_impl(uint8_t* canvas_u8, int H, int W, const uint8_t* faces, int n, in
     for (int i = 0; i < n; ++i) {
       const PbFace& F = P.faces[i];
       if (F.rw == 0 || F.rh == 0) continue;
+      T* cv = canvas + (img_of ? (size_t)img_of[i] * H * W * 3 : 0);
       k_composite<T><<<grid2(F.rw, F.rh, 1, b), b, 0, st>>>(dfaces, i, faces + (size_t)i * S * S * 3, S,
-                                                             parse_src ? parse_src + (size_t)i * S * S : nullptr, roi, canvas, W);
+                                                             parse_src ? parse_src + (size_t)i * S * S : nullptr, roi, cv, W);
       CFB_LAUNCH_CHECK();
     }
   }
@@ -581,6 +666,123 @@ int cfb_resize_linear_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, ui
   API_END(1)
 }
 
+int cfb_resize_area_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_resize_area_u8: bad size");
+  CFB_REQUIRE(out_h <= h && out_w <= w, "cfb_resize_area_u8: shrinking only (use cfb_resize_linear_u8 to enlarge)");
+  CFB_REQUIRE(n == 0 || (src && dst), "cfb_resize_area_u8: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h == out_h && w == out_w) {                  // cv2.resize to the same size is a copy
+    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  const double scale_x = 1. / ((double)out_w / w), scale_y = 1. / ((double)out_h / h);
+  const int isx = (int)std::nearbyint(scale_x), isy = (int)std::nearbyint(scale_y);
+  const dim3 b(32, 8);
+  if (std::abs(scale_x - isx) < 2.220446049250313e-16 && std::abs(scale_y - isy) < 2.220446049250313e-16) {
+    cfb::k_resize_area_fast_u8<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(src, h, w, dst, out_h, out_w, isx, isy,
+                                                                             1.f / (float)(isx * isy), n);
+    CFB_LAUNCH_CHECK();
+    return 0;
+  }
+  std::vector<int> xi, yi;
+  std::vector<float> xa, ya;
+  const int kx = cfb::area_taps(w, out_w, scale_x, xi, xa), ky = cfb::area_taps(h, out_h, scale_y, yi, ya);
+  const size_t nx = xi.size(), ny = yi.size();
+  std::vector<char> host((nx + ny) * 8);
+  memcpy(host.data(), xi.data(), nx * 4);
+  memcpy(host.data() + nx * 4, xa.data(), nx * 4);
+  memcpy(host.data() + nx * 8, yi.data(), ny * 4);
+  memcpy(host.data() + nx * 8 + ny * 4, ya.data(), ny * 4);
+  char* dtab = nullptr;
+  CFB_CUDA(cudaMallocAsync((void**)&dtab, host.size(), st));
+  CFB_CUDA(cudaMemcpyAsync(dtab, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  cfb::k_resize_area_u8<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(
+      src, h, w, dst, out_h, out_w, (const int*)dtab, (const float*)(dtab + nx * 4), kx, (const int*)(dtab + nx * 8),
+      (const float*)(dtab + nx * 8 + ny * 4), ky, n);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(dtab, st));
+  return 0;
+  API_END(1)
+}
+
+int cfb_resize_linear_scale_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
+                               double fx, double fy, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_resize_linear_scale_u8: bad size");
+  CFB_REQUIRE(fx >= 1. && fy >= 1., "cfb_resize_linear_scale_u8: enlarging factors (>= 1) only");
+  CFB_REQUIRE(n == 0 || (src && dst), "cfb_resize_linear_scale_u8: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h == out_h && w == out_w && fx == 1. && fy == 1.) {
+    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  const dim3 b(32, 8);
+  cfb::k_resize_u8<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(src, h, w, dst, out_h, out_w, 1. / fx, 1. / fy, n);
+  CFB_LAUNCH_CHECK();
+  return 0;
+  API_END(1)
+}
+
+int cfb_warp_affine_multi_u8(const uint8_t* imgs, int32_t n_img, int32_t h, int32_t w, const double* affines,
+                             const int32_t* img_index, int32_t n, uint8_t* out, int32_t out_h, int32_t out_w,
+                             int32_t border_mode, int32_t v0, int32_t v1, int32_t v2, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && n_img > 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_warp_affine_multi_u8: bad size");
+  CFB_REQUIRE(n == 0 || (imgs && affines && img_index && out), "cfb_warp_affine_multi_u8: NULL argument");
+  CFB_REQUIRE(border_mode == 0 || border_mode == 2 || border_mode == 4, "cfb_warp_affine_multi_u8: border mode must be 0 (constant), 2 (reflect) or 4 (reflect-101)");
+  if (n == 0) return 0;
+  for (int i = 0; i < n; ++i)
+    CFB_REQUIRE(img_index[i] >= 0 && img_index[i] < n_img, "cfb_warp_affine_multi_u8: image index out of range");
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<char> host((size_t)n * (6 * 8 + 4));
+  double* maps = (double*)host.data();
+  for (int i = 0; i < n; ++i) cfb::invert_affine(affines + 6 * i, maps + 6 * i);
+  memcpy(host.data() + (size_t)n * 48, img_index, (size_t)n * 4);
+  char* d = nullptr;
+  CFB_CUDA(cudaMallocAsync((void**)&d, host.size(), st));
+  CFB_CUDA(cudaMemcpyAsync(d, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  const dim3 b(32, 8);
+  cfb::k_warp_crop_multi<<<cfb::grid2(out_w, out_h, n, b), b, 0, st>>>(imgs, h, w, (const double*)d, (const int*)(d + (size_t)n * 48),
+                                                                        n, out, out_h, out_w, border_mode, v0, v1, v2);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(d, st));
+  return 0;
+  API_END(1)
+}
+
+int64_t cfb_paste_faces_multi_workspace_bytes(int32_t n_img, int32_t h_up, int32_t w_up, int32_t n, int32_t face_size,
+                                              int32_t use_parse, const double* inverse_affines) {
+  if (n_img <= 0 || h_up <= 0 || w_up <= 0 || n < 0 || face_size <= 0 || (n > 0 && !inverse_affines)) {
+    cfb::set_error("cfb_paste_faces_multi_workspace_bytes: bad argument");
+    return -1;
+  }
+  cfb::Plan P;
+  cfb::make_plan(h_up, w_up, n, face_size, inverse_affines, P);
+  return (int64_t)cfb::layout(h_up, w_up, n, face_size, use_parse != 0, P, cfb::max_gauss_floats(P), n_img).total;
+}
+
+int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_t w_up, const uint8_t* faces, int32_t n,
+                          int32_t face_size, const uint8_t* parse_masks, const double* inverse_affines, const int32_t* img_index,
+                          double upscale, int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n_img > 0 && h_up > 0 && w_up > 0 && n >= 0 && face_size > 0 && upscale > 0, "cfb_paste_faces_multi: bad size");
+  CFB_REQUIRE(canvases && workspace && (n == 0 || (faces && inverse_affines && img_index)), "cfb_paste_faces_multi: NULL argument");
+  for (int i = 0; i < n; ++i)
+    CFB_REQUIRE(img_index[i] >= 0 && img_index[i] < n_img, "cfb_paste_faces_multi: image index out of range");
+  const int64_t need = cfb_paste_faces_multi_workspace_bytes(n_img, h_up, w_up, n, face_size, parse_masks != nullptr, inverse_affines);
+  CFB_REQUIRE(need > 0 && workspace_bytes >= need, "cfb_paste_faces_multi: workspace too small (cfb_paste_faces_multi_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (parse_masks)
+    return cfb::paste_impl<double>(canvases, n_img, img_index, h_up, w_up, faces, n, face_size, parse_masks, inverse_affines,
+                                   upscale, nullptr, w_edge_out, (char*)workspace, workspace_bytes, st);
+  return cfb::paste_impl<float>(canvases, n_img, img_index, h_up, w_up, faces, n, face_size, nullptr, inverse_affines, upscale,
+                                nullptr, w_edge_out, (char*)workspace, workspace_bytes, st);
+  API_END(1)
+}
+
 int64_t cfb_paste_faces_workspace_bytes(int32_t h_up, int32_t w_up, int32_t n, int32_t face_size, int32_t use_parse,
                                         const double* inverse_affines) {
   if (h_up <= 0 || w_up <= 0 || n < 0 || face_size <= 0 || (n > 0 && !inverse_affines)) {
@@ -603,10 +805,10 @@ int cfb_paste_faces(uint8_t* canvas, int32_t h_up, int32_t w_up, const uint8_t* 
   CFB_REQUIRE(need > 0 && workspace_bytes >= need, "cfb_paste_faces: workspace too small (cfb_paste_faces_workspace_bytes)");
   cudaStream_t st = (cudaStream_t)stream;
   if (parse_masks)
-    return cfb::paste_impl<double>(canvas, h_up, w_up, faces, n, face_size, parse_masks, inverse_affines, upscale,
+    return cfb::paste_impl<double>(canvas, 1, nullptr, h_up, w_up, faces, n, face_size, parse_masks, inverse_affines, upscale,
                                    debug_canvas, w_edge_out, (char*)workspace, workspace_bytes, st);
-  return cfb::paste_impl<float>(canvas, h_up, w_up, faces, n, face_size, nullptr, inverse_affines, upscale, debug_canvas,
-                                w_edge_out, (char*)workspace, workspace_bytes, st);
+  return cfb::paste_impl<float>(canvas, 1, nullptr, h_up, w_up, faces, n, face_size, nullptr, inverse_affines, upscale,
+                                debug_canvas, w_edge_out, (char*)workspace, workspace_bytes, st);
   API_END(1)
 }
 

@@ -86,6 +86,124 @@ def resize_linear(img, size):
     return out if batched else out[0]
 
 
+def resize_area(img, size):
+    """``cv2.resize(img, size, interpolation=INTER_AREA)`` (size = (w, h), shrinking only) on CUDA uint8 [h,w,3] or
+    [N,h,w,3] (``cfb_resize_area_u8``)."""
+    batched = img.dim() == 4
+    img = _check_image(img, 'resize_area', 4 if batched else 3)
+    x = img if batched else img[None]
+    n, h, w = x.shape[:3]
+    if size[0] > w or size[1] > h:
+        raise NotImplementedError(f'resize_area shrinks only ({w}x{h} -> {size[0]}x{size[1]}); use resize_linear to enlarge')
+    out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint8, device=img.device)
+    with torch.cuda.device(img.device):
+        _lib.check(_lib.load().cfb_resize_area_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _stream(img.device)),
+                   'cfb_resize_area_u8')
+    return out if batched else out[0]
+
+
+def resize_linear_factor(img, f):
+    """``cv2.resize(img, (0, 0), fx=f, fy=f, interpolation=INTER_LINEAR)`` for f >= 1 on CUDA uint8 [h,w,3] or [N,h,w,3]:
+    the output is (round(h f), round(w f)) and the taps follow f itself (``cfb_resize_linear_scale_u8``)."""
+    batched = img.dim() == 4
+    img = _check_image(img, 'resize_linear_factor', 4 if batched else 3)
+    x = img if batched else img[None]
+    n, h, w = x.shape[:3]
+    oh, ow = int(np.rint(h * f)), int(np.rint(w * f))
+    out = torch.empty((n, oh, ow, 3), dtype=torch.uint8, device=img.device)
+    with torch.cuda.device(img.device):
+        _lib.check(_lib.load().cfb_resize_linear_scale_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), oh, ow, float(f), float(f),
+                                                          _stream(img.device)), 'cfb_resize_linear_scale_u8')
+    return out if batched else out[0]
+
+
+def _index(img_index, n, n_img):
+    idx = np.ascontiguousarray(np.asarray(img_index, np.int32).reshape(-1))
+    if idx.shape[0] != n:
+        raise RuntimeError(f'expected {n} image indices, got {idx.shape[0]}')
+    if n and (idx.min() < 0 or idx.max() >= n_img):
+        raise RuntimeError(f'image index out of range [0, {n_img})')
+    return idx
+
+
+def warp_faces_multi(imgs, affines, img_index, face_size=512, border_mode='constant', border_value=(135, 133, 132)):
+    """``warp_faces`` across images in one launch: imgs CUDA uint8 [B,h,w,3], crop i = ``cv2.warpAffine(imgs[img_index[i]],
+    affines[i], ...)`` -> CUDA uint8 [N,face_size,face_size,3]."""
+    imgs = _check_image(imgs, 'warp_faces_multi', 4)
+    if border_mode not in BORDER_MODES:
+        raise ValueError(f"border_mode must be one of {sorted(BORDER_MODES)}, got {border_mode!r}")
+    m = _matrices(affines) if len(affines) else np.zeros((0, 6), np.float64)
+    n = m.shape[0]
+    B, h, w = imgs.shape[:3]
+    idx = _index(img_index, n, B)
+    out = torch.empty((n, face_size, face_size, 3), dtype=torch.uint8, device=imgs.device)
+    bv = [int(v) for v in border_value]
+    with torch.cuda.device(imgs.device):
+        _lib.check(_lib.load().cfb_warp_affine_multi_u8(_lib.ptr(imgs), B, h, w, m.ctypes.data_as(ctypes.c_void_p),
+                                                        idx.ctypes.data_as(ctypes.c_void_p), n, _lib.ptr(out), face_size,
+                                                        face_size, BORDER_MODES[border_mode], bv[0], bv[1], bv[2],
+                                                        _stream(imgs.device)), 'cfb_warp_affine_multi_u8')
+    return out
+
+
+def _paste_multi(canvases, restored, inverse_affines, img_index, upscale, masks):
+    """The paste over several canvases [B,h_up,w_up,3] (the backgrounds, already at the output size) with matrices already
+    adjusted; face i goes into canvas img_index[i].  Returns (CUDA uint8 [B,h_up,w_up,3], w_edge per face)."""
+    canvases = _check_image(canvases, 'paste_faces_multi', 4).clone()
+    restored = _check_image(restored, 'paste_faces_multi: restored faces', 4)
+    n, S = restored.shape[0], restored.shape[1]
+    if restored.shape[2] != S:
+        raise RuntimeError(f'paste_faces_multi: restored faces must be square, got {tuple(restored.shape)}')
+    B, h_up, w_up = canvases.shape[:3]
+    m = _matrices(inverse_affines, n) if n else np.zeros((0, 6), np.float64)
+    idx = _index(img_index, n, B)
+    if masks is not None:
+        if not (torch.is_tensor(masks) and masks.is_cuda and masks.dtype == torch.uint8 and tuple(masks.shape) == (n, PARSE_SIZE, PARSE_SIZE)):
+            raise RuntimeError(f'paste_faces_multi: parse masks must be CUDA uint8 [{n},512,512]')
+        masks = masks.contiguous()
+    lib = _lib.load()
+    dev = canvases.device
+    mp = m.ctypes.data_as(ctypes.c_void_p)
+    need = lib.cfb_paste_faces_multi_workspace_bytes(B, h_up, w_up, n, S, int(masks is not None), mp)
+    if need < 0:
+        _lib.check(1, 'cfb_paste_faces_multi_workspace_bytes')
+    ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+    w_edge = np.zeros(max(n, 1), np.int32)
+    with torch.cuda.device(dev):
+        _lib.check(lib.cfb_paste_faces_multi(_lib.ptr(canvases), B, h_up, w_up, _lib.ptr(restored), n, S, _lib.ptr(masks), mp,
+                                             idx.ctypes.data_as(ctypes.c_void_p), float(upscale),
+                                             w_edge.ctypes.data_as(ctypes.c_void_p), _lib.ptr(ws), ws.numel(), _stream(dev)),
+                   'cfb_paste_faces_multi')
+    return canvases, w_edge[:n]
+
+
+def paste_faces_multi(imgs, restored, inverse_affines, img_index, upscale, face_parse=None, upsample_imgs=None,
+                      face_size=512, masks=None):
+    """``paste_faces`` across images: imgs CUDA uint8 [B,h,w,3] (equal-size input images), restored [N,S,S,3], face i
+    belonging to image img_index[i]; ``upsample_imgs`` (optional, CUDA uint8 [B,h_up,w_up,3]) replaces the resized
+    backgrounds.  Each output image equals ``paste_faces`` of that image and its own faces.  -> CUDA uint8
+    [B,h_up,w_up,3]."""
+    imgs = _check_image(imgs, 'paste_faces_multi', 4)
+    if restored.dim() != 4:
+        raise RuntimeError('paste_faces_multi: restored faces must be [N,S,S,3]')
+    S = restored.shape[1]
+    if S not in (face_size, face_size * upscale):
+        raise RuntimeError(f'paste_faces_multi: restored faces are {S} wide; expected {face_size} or {face_size} * upscale')
+    B, h, w = imgs.shape[:3]
+    h_up, w_up = int(h * upscale), int(w * upscale)
+    if upsample_imgs is None:
+        canvases = resize_linear(imgs, (w_up, h_up))
+    else:
+        canvases = _check_image(upsample_imgs, 'paste_faces_multi: upsample_imgs', 4)
+        if tuple(canvases.shape[:3]) != (B, h_up, w_up):
+            raise NotImplementedError(f'paste_faces_multi: upsample_imgs must be [{B},{h_up},{w_up},3], got {tuple(canvases.shape)}')
+    inv = adjust_inverse_affines([np.array(m, np.float64).reshape(2, 3) for m in inverse_affines], upscale,
+                                 S != face_size)
+    if face_parse is not None and masks is None and restored.shape[0] > 0:
+        masks = parse_masks(_check_image(restored, 'paste_faces_multi: restored faces', 4), face_parse)
+    return _paste_multi(canvases, restored, inv, img_index, upscale, masks)[0]
+
+
 def adjust_inverse_affines(inverse_affines, upscale, upsampled):
     """The reference's in-place adjustment before the warp (face_restoration_helper.py:388-399): with a face upsampler
     ``/= upscale`` and ``[:, 2] *= upscale``; otherwise ``[:, 2] += 0.5 * upscale`` when upscale > 1."""

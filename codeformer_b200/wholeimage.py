@@ -1,0 +1,242 @@
+"""Whole-image restoration over batches of images or video frames.
+
+``restore_images`` gives, for every image, exactly what the per-image loop of inference_codeformer.py:178-229 gives with
+``FaceRestoreHelper(upscale, face_size=512, crop_ratio=(1, 1), det_model, save_ext='png', use_parse=parser is not None)``
+and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of images whose short side is below 512),
+``get_face_landmarks_5(only_center_face, resize=640, eye_dist_threshold=5)``, ``align_warp_face``, CodeFormer with
+``adain=True``, ``add_restored_face``, the optional background upsampler, ``get_inverse_affine`` and
+``paste_faces_to_input_image``.  It runs them across images instead of one image at a time:
+
+  * images of equal size are stacked and go through the resizes and the detector as one batch (the detector's resize to
+    a short side of 640 is ``cfb_resize_area_u8`` when it shrinks, cv2's INTER_AREA);
+  * the crops of all images of a chunk are warped in one launch (``cfb_warp_affine_multi_u8``) and restored by
+    ``CodeFormer.forward_u8`` in batches of at most ``max_batch`` faces; the parse masks are batched the same way;
+  * the paste-back runs once per chunk of images (``cfb_paste_faces_multi``), one read-back of the erosion areas.
+
+What stays on the host, as in the reference: the NMS and the landmark filter, ``get_center_face``,
+``cv2.estimateAffinePartial2D(LMEDS)`` (cv2 is imported lazily, as ``align_warp_face`` does), and the background / face
+upsamplers' ``enhance`` per image.  Every result is per image: batching and chunking do not change any byte.
+"""
+import numpy as np
+import torch
+
+from . import _lib
+from .detection import RetinaFace, cuda_u8_image
+from .detection import finish_detections as retinaface_finish
+from .pasteback import (_paste_multi, adjust_inverse_affines, parse_masks, resize_area, resize_linear, resize_linear_factor,
+                        warp_faces_multi)
+from .yolov5face import YoloDetector, _resize_u8, letterbox_geometry
+from .yolov5face import finish_detections as yolo_finish
+
+FACE_SIZE = 512
+# FaceRestoreHelper's 5-point template for face_size 512, crop_ratio (1, 1)
+FACE_TEMPLATE = np.array([[192.98138, 239.94708], [318.90277, 240.1936], [256.63416, 314.01935],
+                          [201.26117, 371.41043], [313.08905, 371.15118]]) * (FACE_SIZE / 512.0)
+
+
+def is_gray(img, threshold=10):
+    """facelib's ``is_gray`` on a host uint8 BGR image: the mean variance of the channel differences is <= threshold."""
+    c = [np.asarray(img[:, :, i], dtype=np.int16) for i in range(3)]
+    diff = ((c[0] - c[1]).var() + (c[1] - c[2]).var() + (c[2] - c[0]).var()) / 3.0
+    return bool(diff <= threshold)
+
+
+def _device_is_gray(img, threshold=10):
+    """``is_gray`` of a CUDA image from exact integer moments (the variances numpy computes, up to its rounding)."""
+    x = img.to(torch.int64)
+    n = x.shape[0] * x.shape[1]
+    total = 0.0
+    for a, b in ((0, 1), (1, 2), (2, 0)):
+        d = x[:, :, a] - x[:, :, b]
+        s, s2 = int(d.sum()), int((d * d).sum())
+        total += (n * s2 - s * s) / (n * n)
+    return bool(total / 3.0 <= threshold)
+
+
+def get_center_face(det_faces, h=0, w=0):
+    """facelib's ``get_center_face`` (face_restoration_helper.py:40-52) with the image centre."""
+    center = np.array([w / 2, h / 2])
+    dist = [np.linalg.norm(np.array([(f[0] + f[2]) / 2, (f[1] + f[3]) / 2]) - center) for f in det_faces]
+    idx = dist.index(min(dist))
+    return det_faces[idx], idx
+
+
+def _detect(detector, x):
+    """``detect_faces`` of each image of x (CUDA uint8 [B,h,w,3]) with the detector's defaults, one forward for the batch:
+    a list of B host arrays (or None), as ``detect_faces`` returns them."""
+    B, h, w = x.shape[:3]
+    if isinstance(detector, RetinaFace):
+        loc, conf, landms = detector.forward_u8(x)
+        cands = detector.candidates(loc, conf, landms, h, w, 0.8)
+        return [retinaface_finish(c.cpu().numpy(), 0.8, 0.4) for c in cands]
+    if isinstance(detector, YoloDetector):
+        first, second, (H, W), (top, left) = letterbox_geometry(h, w, detector.target_size)
+        if first is not None:
+            x = _resize_u8(x, *first)
+        if second is not None:
+            x = _resize_u8(x, *second)
+        pred, _ = detector.detector.forward_u8(x, (H, W), (top, left), raw=False)
+        cands = detector.detector.candidates(pred, H, W, 0.7)
+        return [yolo_finish([c], (H, W), [(h, w, 3)], 0.7, 0.5, detector.min_face) for c in cands]
+    raise NotImplementedError(f'restore_images: detector {type(detector).__name__} is not built; use '
+                              'init_detection_model("retinaface_resnet50") or init_detection_model("YOLOv5l")')
+
+
+def _landmarks(bboxes, scale, h, w, only_center_face, eye_dist_threshold):
+    """The host part of ``get_face_landmarks_5`` after ``detect_faces``: rescale, eye-distance filter, centre face."""
+    if bboxes is None or bboxes.shape[0] == 0:
+        return []
+    bboxes = bboxes / scale
+    lms, det_faces = [], []
+    for bbox in bboxes:
+        eye_dist = np.linalg.norm([bbox[6] - bbox[8], bbox[7] - bbox[9]])
+        if eye_dist_threshold is not None and eye_dist < eye_dist_threshold:
+            continue
+        lms.append(np.array([[bbox[i], bbox[i + 1]] for i in range(5, 15, 2)]))
+        det_faces.append(bbox[0:5])
+    if not det_faces:
+        return []
+    if only_center_face:
+        _, idx = get_center_face(det_faces, h, w)
+        lms = [lms[idx]]
+    return lms
+
+
+def _chunks(images, max_batch):
+    """Indices of the images grouped by size (first appearance order), each group cut into runs of <= max_batch."""
+    groups = {}
+    for i, im in enumerate(images):
+        groups.setdefault(tuple(im.shape), []).append(i)
+    out = []
+    for idx in groups.values():
+        out += [idx[k:k + max_batch] for k in range(0, len(idx), max_batch)]
+    return out
+
+
+def _as_input(img, dev):
+    """-> (CUDA uint8 [h,w,3], host array or None, came from the host)."""
+    if isinstance(img, np.ndarray):
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+            raise NotImplementedError(f'restore_images takes uint8 HWC BGR images with 3 channels (gray, alpha and 16-bit '
+                                      f'images stay caller-side), got {img.dtype} {img.shape}')
+        return cuda_u8_image(img, dev, 'restore_images'), img, True
+    if torch.is_tensor(img):
+        if not img.is_cuda:
+            raise RuntimeError('restore_images: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
+        return cuda_u8_image(img, dev, 'restore_images').contiguous(), None, False
+    raise NotImplementedError(f'restore_images takes numpy arrays or CUDA tensors, got {type(img).__name__}')
+
+
+def _restore(net, crops, w, max_batch, errors):
+    """CodeFormer over the crops in batches of <= max_batch; a failed batch gives its input faces back (the reference's
+    per-face fallback, inference_codeformer.py:208-210)."""
+    out = torch.empty_like(crops)
+    dev = crops.device
+    for lo in range(0, crops.shape[0], max_batch):
+        hi = min(crops.shape[0], lo + max_batch)
+        try:
+            res = net.forward_u8(crops[lo:hi], w=w, adain=True)
+            torch.cuda.current_stream(dev).synchronize()
+            _lib.check(_lib.load().cfb_check_async_status(), 'restore_images')
+            out[lo:hi] = res
+        except RuntimeError as err:
+            errors.append((lo, str(err)))
+            out[lo:hi] = crops[lo:hi]
+    return out
+
+
+def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_center_face=False, detection_resize=640,
+                   eye_dist_threshold=5, bg_upsampler=None, face_upsampler=None, max_batch=32, return_faces=False):
+    """Restore whole images in batches.  ``images``: a list of uint8 HWC BGR numpy arrays or CUDA tensors.  ``net``: a
+    ``CodeFormer``; ``detector``: ``init_detection_model('retinaface_resnet50' | 'YOLOv5l')``; ``parser``: a ParseNet
+    (``init_parsing_model()``) or None for use_parse=False.  ``bg_upsampler`` / ``face_upsampler``: objects with
+    ``enhance(img, outscale=upscale)`` (``RealESRGANer``), called per image / per face on the host.
+
+    Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
+    also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted.  Each image equals the
+    reference loop body on that image alone, whatever ``max_batch`` is.  ``self.last_restore_errors`` of the reference's
+    fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back."""
+    import cv2    # estimateAffinePartial2D(LMEDS) / invertAffineTransform stay on the host, as in the reference
+    images = list(images)
+    dev = next(net.parameters()).device
+    if dev.type != 'cuda':
+        raise RuntimeError('restore_images: the network is not on a CUDA device; there is no CPU fallback')
+    max_batch = max(1, int(max_batch))
+    inputs = [_as_input(im, dev) for im in images]
+    results, crops_out, faces_out = [None] * len(images), [None] * len(images), [None] * len(images)
+    errors = []
+    for idx in _chunks([t for t, _, _ in inputs], max_batch):
+        x = torch.stack([inputs[i][0] for i in idx])
+        h0, w0 = x.shape[1:3]
+        # read_image: gray test, then an INTER_LINEAR enlargement (fx = fy) when the short side is below 512
+        gray = [is_gray(inputs[i][1]) if inputs[i][2] else _device_is_gray(inputs[i][0]) for i in idx]
+        if min(h0, w0) < 512:
+            x = resize_linear_factor(x, 512.0 / min(h0, w0))
+        h, wd = x.shape[1:3]
+        # get_face_landmarks_5(resize=640): INTER_AREA when shrinking, INTER_LINEAR otherwise
+        scale = detection_resize / min(h, wd)
+        dh, dw = int(h * scale), int(wd * scale)
+        xd = resize_area(x, (dw, dh)) if scale < 1 else resize_linear(x, (dw, dh))
+        with torch.no_grad():
+            dets = _detect(detector, xd)
+        lms = [_landmarks(d, scale, h, wd, only_center_face, eye_dist_threshold) for d in dets]
+        affines, owner = [], []
+        for k, lm in enumerate(lms):
+            for landmark in lm:
+                affines.append(cv2.estimateAffinePartial2D(landmark, FACE_TEMPLATE, method=cv2.LMEDS)[0])
+                owner.append(k)
+            if lm and gray[k]:
+                raise NotImplementedError('restore_images: the gray branch of add_restored_face gives float faces; the '
+                                          'paste-back of gray images stays caller-side')
+        crops = warp_faces_multi(x, affines, owner, FACE_SIZE)
+        with torch.no_grad():
+            restored = _restore(net, crops, w, max_batch, errors)
+        S = FACE_SIZE
+        if face_upsampler is not None and len(affines):
+            host = restored.cpu().numpy()
+            up = [face_upsampler.enhance(f, outscale=upscale)[0] for f in host]
+            restored = torch.from_numpy(np.ascontiguousarray(np.stack(up))).to(dev)
+            S = FACE_SIZE * upscale
+            if restored.shape[1] != S or restored.shape[2] != S:
+                raise RuntimeError(f'restore_images: the face upsampler returned {tuple(restored.shape[1:3])}, expected {S}x{S}')
+        h_up, w_up = int(h * upscale), int(wd * upscale)
+        if bg_upsampler is not None:
+            bgs = []
+            for i in idx:
+                src = inputs[i][1] if inputs[i][2] else inputs[i][0].cpu().numpy()
+                bg = np.asarray(bg_upsampler.enhance(src, outscale=upscale)[0])
+                if bg.shape[:2] != (h_up, w_up):
+                    raise NotImplementedError(f'restore_images: the background upsampler returned {bg.shape[:2]}, the output '
+                                              f'is {h_up}x{w_up}; the reference resizes it with INTER_LANCZOS4, which is not built')
+                bgs.append(torch.from_numpy(np.ascontiguousarray(bg)))
+            canvases = torch.stack(bgs).to(dev)
+        else:
+            canvases = resize_linear(x, (w_up, h_up))
+        invs = []
+        for a in affines:
+            inv = cv2.invertAffineTransform(a)
+            inv *= upscale
+            invs.append(inv)
+        adjust_inverse_affines(invs, upscale, face_upsampler is not None)
+        masks = None
+        if parser is not None and restored.shape[0] > 0:
+            with torch.no_grad():
+                masks = torch.cat([parse_masks(restored[lo:lo + max_batch], parser)
+                                   for lo in range(0, restored.shape[0], max_batch)])
+        out, _ = _paste_multi(canvases, restored, invs, owner, upscale, masks)
+        owner = np.asarray(owner, np.int64)
+        for k, i in enumerate(idx):
+            sel = torch.from_numpy(np.nonzero(owner == k)[0]).to(dev)
+            if inputs[i][2]:
+                results[i] = out[k].cpu().numpy()
+                crops_out[i], faces_out[i] = crops[sel].cpu().numpy(), restored[sel].cpu().numpy()
+            else:
+                results[i] = out[k]
+                crops_out[i], faces_out[i] = crops[sel], restored[sel]
+    restore_images.last_errors = errors
+    if return_faces:
+        return results, crops_out, faces_out
+    return results
+
+
+restore_images.last_errors = []

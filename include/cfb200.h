@@ -387,6 +387,28 @@ int cfb_paste_faces(uint8_t* canvas, int32_t h_up, int32_t w_up, const uint8_t* 
                     const uint8_t* parse_masks, const double* inverse_affines, double upscale, float* debug_canvas,
                     int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- whole-image mode over batches of equal-size images ----
+ * cfb_resize_area_u8: cv2.resize(src[i], (out_w, out_h), INTER_AREA) for n images [n,h,w,3], shrinking only (out_h <= h,
+ *   out_w <= w): resizeAreaFast's integer sums for integer factors, computeResizeAreaTab weights with float sums otherwise.
+ * cfb_resize_linear_scale_u8: cv2.resize(src[i], (0, 0), fx=fx, fy=fy, INTER_LINEAR) for enlarging factors (>= 1), the
+ *   output size being the caller's (cv2: round(w * fx), round(h * fy)); the taps follow fx / fy, not the size ratio.
+ * cfb_warp_affine_multi_u8: cfb_warp_affine_u8 over a batch imgs [n_img,h,w,3]; crop i samples image img_index[i] (host).
+ * cfb_paste_faces_multi: cfb_paste_faces over n_img canvases [n_img,h_up,w_up,3]; face i goes into canvas img_index[i]
+ *   (host int32[n]).  Each canvas ends byte for byte as cfb_paste_faces of its own faces would leave it; composites run in
+ *   face order, and the areas of all faces are read back in one synchronisation of `stream`. */
+int cfb_resize_area_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
+                       void* stream);
+int cfb_resize_linear_scale_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
+                               double fx, double fy, void* stream);
+int cfb_warp_affine_multi_u8(const uint8_t* imgs, int32_t n_img, int32_t h, int32_t w, const double* affines,
+                             const int32_t* img_index, int32_t n, uint8_t* out, int32_t out_h, int32_t out_w,
+                             int32_t border_mode, int32_t v0, int32_t v1, int32_t v2, void* stream);
+int64_t cfb_paste_faces_multi_workspace_bytes(int32_t n_img, int32_t h_up, int32_t w_up, int32_t n, int32_t face_size,
+                                              int32_t use_parse, const double* inverse_affines);
+int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_t w_up, const uint8_t* faces, int32_t n,
+                          int32_t face_size, const uint8_t* parse_masks, const double* inverse_affines, const int32_t* img_index,
+                          double upscale, int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
