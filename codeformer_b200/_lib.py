@@ -78,6 +78,8 @@ SIGNATURES = {
     'cfb_rrdb_set_precision': (c_int, [_P, c_int32]),
     'cfb_rrdb_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32]),
     'cfb_rrdb_forward': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_rrdb_forward_u8_tiles': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, _P, c_int32, c_int32, c_int32, _P, _P,
+                                          c_int64, _P]),
     'cfb_parsenet_create': (c_void_p, [c_int32] * 8),
     'cfb_parsenet_destroy': (None, [_P]),
     'cfb_parsenet_set_param': (c_int, [_P, c_char_p, _P, c_int64]),

@@ -200,6 +200,23 @@ int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, f
                  int pad_mode, int out_pitch, int out_c0, cudaStream_t st);
 int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bias, float* out_nchw, int N, int H, int W, int Cout,
                   int pad_mode, cudaStream_t st);
+// RRDBNet's tiles read from / written to uint8 images (cfb_rrdb_forward_u8_tiles): one row of its tile table.  The table of
+// one launch travels by value in the kernel parameters (9 * 4 * 64 bytes, under the 4 KB parameter limit).
+struct RrdbU8Tile {
+  int img;                       // source image / canvas index
+  int in_y, in_x;                // input window origin, in the coordinates of the pre_pad + mod-padded image
+  int crop_y, crop_x, crop_h, crop_w;   // kept rectangle of the tile's output
+  int out_y, out_x;              // its canvas position
+};
+struct RrdbU8Tiles {
+  static constexpr int kMax = 64;
+  RrdbU8Tile t[kMax];
+};
+int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w, int pre_pad, const RrdbU8Tiles& tiles,
+                          const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us, int out_pitch, int out_c0,
+                          cudaStream_t st);
+int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
+                           unsigned char* canvas_bgr_hwc, int out_h, int out_w, int N, int H, int W, cudaStream_t st);
 int relayout_thin_out(const float* oihw, float* out, int Cout, cudaStream_t st);
 int fold_bn(const float* w, const float* gamma, const float* beta, const float* mean, const float* var, float eps, float* wout,
             float* bout, int Cout, int per_out, cudaStream_t st);

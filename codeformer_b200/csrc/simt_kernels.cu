@@ -1523,10 +1523,35 @@ __device__ __forceinline__ int pad_index(int i, int n, int mode, bool& inside) {
   return i;
 }
 
-// x [N, Cimg, H*us, W*us] NCHW -> out [N, H, W, out_pitch] (channels out_c0 .. out_c0+63), 3x3 pad 1.
+// Image sources of conv_thin_in: value of image channel c at row y, column x (before pixel_unshuffle) of batch element n.
+struct NchwSrc {                 // x [N, Cimg, Hi, Wi] fp32
+  const float* x; int Cimg, Hi, Wi;
+  __device__ __forceinline__ float operator()(int n, int c, int y, int x_) const {
+    return __ldg(x + (((int64_t)n * Cimg + c) * Hi + y) * Wi + x_);
+  }
+};
+
+// Index of row / column i of an image of n rows after F.pad(.., (0, p), 'reflect') (p < n): the bottom / right pad only.
+__device__ __forceinline__ int reflect_tail(int i, int n) { return i < n ? i : 2 * (n - 1) - i; }
+
+// The tiles of RealESRGANer.pre_process + tile_process read from uint8 HWC BGR source images (realesrgan_utils.py:71-175):
+// element n is the window at (in_y, in_x) of image `img` after the pre_pad reflect pad (bottom / right) and the reflect pad
+// to the pixel-unshuffle multiple; the value is the reference's float32 img / 255 (an IEEE division), BGR -> RGB.
+struct U8TileSrc {
+  const unsigned char* img; int H, W, Hp, Wp;        // source size, size after the pre_pad (Hp = H + pre_pad)
+  RrdbU8Tiles tab;                                   // by value: the table travels in the launch's parameters
+  __device__ __forceinline__ float operator()(int n, int c, int y, int x_) const {
+    const RrdbU8Tile& t = tab.t[n];
+    const int sy = reflect_tail(reflect_tail(t.in_y + y, Hp), H), sx = reflect_tail(reflect_tail(t.in_x + x_, Wp), W);
+    return __fdiv_rn((float)__ldg(img + (((int64_t)t.img * H + sy) * W + sx) * 3 + (2 - c)), 255.f);
+  }
+};
+
+// x [N, Cimg, H*us, W*us] (read through Src) -> out [N, H, W, out_pitch] (channels out_c0 .. out_c0+63), 3x3 pad 1.
 // us > 1: pixel_unshuffle(x, us) first -- channel c*us*us + dy*us + dx of the conv input is x[c][y*us+dy][x*us+dx].
 // weights: [tap][cin][64] (relayout_oihw_to_tck).
-__global__ void __launch_bounds__(256) conv_thin_in_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
+template <class Src>
+__global__ void __launch_bounds__(256) conv_thin_in_kernel(const Src x, const float* __restrict__ wgt,
                                                            const float* __restrict__ bias, float* __restrict__ out, int N, int H,
                                                            int W, int Cimg, int us, int pad_mode, int out_pitch, int out_c0) {
   extern __shared__ __align__(16) float wsm[];       // [9 * Cin][64]
@@ -1540,7 +1565,6 @@ __global__ void __launch_bounds__(256) conv_thin_in_kernel(const float* __restri
   const int rem = (int)(pix - (int64_t)n * H * W);
   const int oy = rem / W, ox = rem - oy * W;
   float4 acc = bias ? __ldg(reinterpret_cast<const float4*>(bias + cq * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-  const int Hi = H * us, Wi = W * us;
   for (int r = 0; r < 3; ++r) {
     bool iny;
     const int iy = pad_index(oy + r - 1, H, pad_mode, iny);
@@ -1550,7 +1574,7 @@ __global__ void __launch_bounds__(256) conv_thin_in_kernel(const float* __restri
       if (!(iny && inx)) continue;
       for (int ci = 0; ci < Cin; ++ci) {
         const int c = ci / (us * us), d = ci - c * us * us, dy = d / us, dx = d - dy * us;
-        const float v = __ldg(x + (((int64_t)n * Cimg + c) * Hi + (iy * us + dy)) * Wi + (ix * us + dx));
+        const float v = x(n, c, iy * us + dy, ix * us + dx);
         const float4 w4 = *reinterpret_cast<const float4*>(wsm + ((r * 3 + s) * Cin + ci) * 64 + cq * 4);
         acc.x = fmaf(v, w4.x, acc.x); acc.y = fmaf(v, w4.y, acc.y); acc.z = fmaf(v, w4.z, acc.z); acc.w = fmaf(v, w4.w, acc.w);
       }
@@ -1558,8 +1582,9 @@ __global__ void __launch_bounds__(256) conv_thin_in_kernel(const float* __restri
   }
   *reinterpret_cast<float4*>(out + pix * out_pitch + out_c0 + cq * 4) = acc;
 }
-int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int Cimg, int us,
-                 int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
+template <class Src>
+static int launch_thin_in(const Src& x, const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int Cimg, int us,
+                          int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
   const int Cin = Cimg * us * us;
   CFB_REQUIRE(Cin >= 1 && Cin <= 48 && out_pitch % 4 == 0 && out_c0 % 4 == 0, "conv_thin_in: at most 48 input channels");
   const int64_t M = (int64_t)N * H * W;
@@ -1569,18 +1594,63 @@ int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, f
   int dev = 0;
   CFB_CUDA(cudaGetDevice(&dev));
   if (!(attr_done.load() & (1ull << (dev & 63)))) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_thin_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 9 * 48 * 64 * 4));
+    CFB_CUDA(cudaFuncSetAttribute(conv_thin_in_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, 9 * 48 * 64 * 4));
     attr_done.fetch_or(1ull << (dev & 63));
   }
-  conv_thin_in_kernel<<<(unsigned)((M + 15) / 16), 256, smem, st>>>(x_nchw, wgt_tck, bias, out, N, H, W, Cimg, us, pad_mode, out_pitch, out_c0);
+  conv_thin_in_kernel<Src><<<(unsigned)((M + 15) / 16), 256, smem, st>>>(x, wgt_tck, bias, out, N, H, W, Cimg, us, pad_mode, out_pitch, out_c0);
   CFB_LAUNCH_CHECK();
   return 0;
 }
+int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int Cimg, int us,
+                 int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
+  return launch_thin_in(NchwSrc{x_nchw, Cimg, H * us, W * us}, wgt_tck, bias, out, N, H, W, Cimg, us, pad_mode, out_pitch, out_c0, st);
+}
+int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w, int pre_pad, const RrdbU8Tiles& tiles,
+                          const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us, int out_pitch, int out_c0,
+                          cudaStream_t st) {
+  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_in_u8_tiles: too many tiles for one launch");
+  const U8TileSrc x{img_bgr_hwc, img_h, img_w, img_h + pre_pad, img_w + pre_pad, tiles};
+  return launch_thin_in(x, wgt_tck, bias, out, N, H, W, 3, us, 0, out_pitch, out_c0, st);
+}
 
-// in [N, H, W, 64] NHWC -> out [N, Cout, H, W] NCHW (Cout <= CP), 3x3 pad 1; weights [tap][64][CP] (zero-padded columns)
-template <int CP>
+// Destinations of conv_thin_out: `wants` selects the output pixels to compute, `store` writes one pixel's Cout values.
+struct NchwDst {                 // out [N, Cout, H, W] fp32
+  float* out;
+  __device__ __forceinline__ bool wants(int, int, int) const { return true; }
+  template <int CP>
+  __device__ __forceinline__ void store(int n, int oy, int ox, int H, int W, int Cout, const float (&acc)[CP]) const {
+    for (int c = 0; c < Cout; ++c) out[(((int64_t)n * Cout + c) * H + oy) * W + ox] = acc[c];
+  }
+};
+
+// The crop-back of tile_process and post_process with the reference's uint8 conversion (realesrgan_utils.py:147-186,
+// 203-210): pixel (oy, ox) of tile n is kept when it lies in the tile's crop and its canvas position (out + offset into the
+// crop) lies inside the out_h x out_w canvas of image `img` (the mod pad and pre_pad rows / columns fall outside); it is
+// written as uint8 HWC BGR: clamp to [0, 1], float32 * 255, round half to even.
+struct U8CanvasDst {
+  unsigned char* canvas; int out_h, out_w;
+  RrdbU8Tiles tab;
+  __device__ __forceinline__ bool pos(int n, int oy, int ox, int& Y, int& X) const {
+    const RrdbU8Tile& t = tab.t[n];
+    const int cy = oy - t.crop_y, cx = ox - t.crop_x;
+    Y = t.out_y + cy; X = t.out_x + cx;
+    return (unsigned)cy < (unsigned)t.crop_h && (unsigned)cx < (unsigned)t.crop_w && Y < out_h && X < out_w;
+  }
+  __device__ __forceinline__ bool wants(int n, int oy, int ox) const { int Y, X; return pos(n, oy, ox, Y, X); }
+  template <int CP>
+  __device__ __forceinline__ void store(int n, int oy, int ox, int, int, int, const float (&acc)[CP]) const {
+    int Y, X;
+    pos(n, oy, ox, Y, X);
+    unsigned char* px = canvas + (((int64_t)tab.t[n].img * out_h + Y) * out_w + X) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) px[2 - c] = (unsigned char)rintf(__fmul_rn(fminf(fmaxf(acc[c], 0.f), 1.f), 255.f));
+  }
+};
+
+// in [N, H, W, 64] NHWC -> Dst (Cout <= CP channels), 3x3 pad 1; weights [tap][64][CP] (zero-padded columns)
+template <int CP, class Dst>
 __global__ void __launch_bounds__(128) conv_thin_out_kernel(const float* __restrict__ in, const float* __restrict__ wgt,
-                                                            const float* __restrict__ bias, float* __restrict__ out, int N, int H,
+                                                            const float* __restrict__ bias, const Dst out, int N, int H,
                                                             int W, int Cout, int pad_mode) {
   extern __shared__ __align__(16) float wsm[];       // [9 * 64][CP]
   for (int i = threadIdx.x; i < 9 * 64 * CP; i += 128) wsm[i] = wgt[i];
@@ -1590,6 +1660,7 @@ __global__ void __launch_bounds__(128) conv_thin_out_kernel(const float* __restr
   const int n = (int)(pix / ((int64_t)H * W));
   const int rem = (int)(pix - (int64_t)n * H * W);
   const int oy = rem / W, ox = rem - oy * W;
+  if (!out.wants(n, oy, ox)) return;
   float acc[CP];
 #pragma unroll
   for (int c = 0; c < CP; ++c) acc[c] = (bias && c < Cout) ? __ldg(bias + c) : 0.f;
@@ -1615,7 +1686,7 @@ __global__ void __launch_bounds__(128) conv_thin_out_kernel(const float* __restr
       }
     }
   }
-  for (int c = 0; c < Cout; ++c) out[(((int64_t)n * Cout + c) * H + oy) * W + ox] = acc[c];
+  out.store(n, oy, ox, H, W, Cout, acc);
 }
 int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bias, float* out_nchw, int N, int H, int W, int Cout,
                   int pad_mode, cudaStream_t st) {
@@ -1626,13 +1697,24 @@ int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bia
   int dev = 0;
   CFB_CUDA(cudaGetDevice(&dev));
   if (!(attr_done.load() & (1ull << (dev & 63)))) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_thin_out_kernel<20>, cudaFuncAttributeMaxDynamicSharedMemorySize, 9 * 64 * 20 * 4));
+    CFB_CUDA(cudaFuncSetAttribute(conv_thin_out_kernel<20, NchwDst>, cudaFuncAttributeMaxDynamicSharedMemorySize, 9 * 64 * 20 * 4));
     attr_done.fetch_or(1ull << (dev & 63));
   }
+  const NchwDst dst{out_nchw};
   if (Cout <= 4)
-    conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, out_nchw, N, H, W, Cout, pad_mode);
+    conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, Cout, pad_mode);
   else
-    conv_thin_out_kernel<20><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 20 * 4, st>>>(in_nhwc64, wgt_tcp, bias, out_nchw, N, H, W, Cout, pad_mode);
+    conv_thin_out_kernel<20><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 20 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, Cout, pad_mode);
+  CFB_LAUNCH_CHECK();
+  return 0;
+}
+int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
+                           unsigned char* canvas_bgr_hwc, int out_h, int out_w, int N, int H, int W, cudaStream_t st) {
+  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_out_u8_tiles: too many tiles for one launch");
+  const int64_t M = (int64_t)N * H * W;
+  if (M == 0) return 0;
+  const U8CanvasDst dst{canvas_bgr_hwc, out_h, out_w, tiles};
+  conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, 3, 0);
   CFB_LAUNCH_CHECK();
   return 0;
 }

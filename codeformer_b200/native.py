@@ -61,6 +61,15 @@ class NativeNet(nn.Module):
                                'statistics); call .eval()')
         return super().train(False)
 
+    def _handle(self):
+        """The native handle, created on first use (host-only: the workspace queries need no device)."""
+        if self._net is None:
+            h = getattr(_lib.load(), f'cfb_{self._api}_create')(*self._create_args)
+            if not h:
+                _lib.check(1, f'cfb_{self._api}_create')
+            object.__setattr__(self, '_net', ctypes.c_void_p(h))
+        return self._net
+
     def _prepare(self, device):
         """(Re)build the native weight copies when parameters were loaded, moved or modified."""
         lib = _lib.load()
@@ -68,12 +77,7 @@ class NativeNet(nn.Module):
         sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
         if self._net is not None and sig == self._sig:
             return
-        if self._net is None:
-            h = getattr(lib, f'cfb_{self._api}_create')(*self._create_args)
-            if not h:
-                _lib.check(1, f'cfb_{self._api}_create')
-            object.__setattr__(self, '_net', ctypes.c_void_p(h))
-        keep = upload_params(lib, self._api, self._net, params, device)
+        keep = upload_params(lib, self._api, self._handle(), params, device)
         _lib.check(getattr(lib, f'cfb_{self._api}_prepare')(self._net, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)),
                    f'cfb_{self._api}_prepare')
         object.__setattr__(self, '_sig', sig)
@@ -81,7 +85,7 @@ class NativeNet(nn.Module):
 
     def _workspace(self, batch, h, w, device):
         """The module's workspace for a batch x h x w forward on ``device``: grows, never shrinks."""
-        need = getattr(_lib.load(), f'cfb_{self._api}_workspace_bytes')(self._net, batch, h, w)
+        need = getattr(_lib.load(), f'cfb_{self._api}_workspace_bytes')(self._handle(), batch, h, w)
         if need < 0:
             _lib.check(1, f'cfb_{self._api}_workspace_bytes')
         if self._ws is None or self._ws.numel() < need or self._ws.device != device:

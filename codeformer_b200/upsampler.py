@@ -89,6 +89,44 @@ class RRDBNet(NativeNet):
         return out
 
 
+    def forward_u8_tiles(self, images, pre_pad, tiles, tile_h, tile_w, out):
+        """One forward at batch ``len(tiles)`` of equal tile_h x tile_w tiles read from ``images`` (CUDA uint8 [B,H,W,3] BGR)
+        and cropped into ``out`` (CUDA uint8 [B,H*scale,W*scale,3] BGR): ``cfb_rrdb_forward_u8_tiles`` (include/cfb200.h),
+        rows of ``tiles`` = (image, in_y, in_x, crop_y, crop_x, crop_h, crop_w, out_y, out_x).  Used by
+        ``RealESRGANer.enhance_batch``, which makes the table."""
+        B, H, W, _ = images.shape
+        rows = np.ascontiguousarray(np.asarray(tiles, dtype=np.int32).reshape(-1, 9))
+        lib = _lib.load()
+        dev = images.device
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            _lib.check(lib.cfb_rrdb_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_rrdb_set_precision')
+            ws = self._workspace(rows.shape[0], tile_h, tile_w, dev)
+            _lib.check(lib.cfb_rrdb_forward_u8_tiles(self._net, _lib.ptr(images), B, H, W, pre_pad,
+                                                     rows.ctypes.data_as(ctypes.c_void_p), rows.shape[0], tile_h, tile_w,
+                                                     _lib.ptr(out), _lib.ptr(ws), ws.numel(),
+                                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                       'cfb_rrdb_forward_u8_tiles')
+        return out
+
+
+def unshuffle_factor(scale):
+    """pixel_unshuffle factor of RRDBNet's input, which is also pre_process's mod_scale (1: no mod pad)."""
+    return 2 if scale == 2 else (4 if scale == 1 else 1)
+
+
+def reflect_pad_index(n, pre_pad, scale):
+    """Source index of every row (or column) of pre_process's padded image: F.pad(.., (0, pre_pad), 'reflect') of n rows, then
+    the reflect pad to the pixel-unshuffle multiple.  The uint8 input conv of ``cfb_rrdb_forward_u8_tiles`` composes the same
+    two maps per pixel."""
+    def tail(i, m):
+        return np.where(i < m, i, 2 * (m - 1) - i)
+    m = unshuffle_factor(scale)
+    p = n + pre_pad
+    i = np.arange(p + (m - p % m) % m)
+    return tail(tail(i, p), n)
+
+
 class RealESRGANer:
     """The reference's helper around the upsampling network (realesrgan_utils.py:14-250): ``enhance(img)`` takes an HWC
     uint8 / uint16 BGR (or gray, or BGRA) image and returns ``(upsampled image, mode)``.  ``model`` is any module mapping
@@ -144,6 +182,91 @@ class RealESRGANer:
                              'crop': ((y0 - py0) * sc, (y0 - py0) * sc + (y1 - y0) * sc, (x0 - px0) * sc, (x0 - px0) * sc + (x1 - x0) * sc)})
         return plan
 
+    # Default bound of enhance_batch's workspace: tiles of one shape go through one forward as long as its workspace
+    # (cfb_rrdb_workspace_bytes) stays within this budget, and at least one tile always does.  A 480 x 480 tile at x2 takes
+    # about 0.69 GB, so the default runs six of them per forward.  The network's workspace only grows.
+    WORKSPACE_BUDGET = 4 << 30
+
+    def tile_groups(self, batch, height, width, max_tiles=None, tile_bytes=None):
+        """The forwards of ``enhance_batch`` for ``batch`` images of height x width: a list of (tile_h, tile_w, rows), rows =
+        (image, in_y, in_x, crop_y, crop_x, crop_h, crop_w, out_y, out_x) of tiles of one input-window shape, from
+        ``tile_plan`` over the padded image (``tile == 0``: the whole padded image as one tile).  Tiles that lie in the pads only
+        are dropped: post_process discards their output.  Each shape is cut into runs of at most ``max_tiles`` tiles;
+        ``max_tiles=None`` takes as many as ``WORKSPACE_BUDGET`` holds, from ``tile_bytes(n, tile_h, tile_w)`` (the workspace of
+        an n-tile forward).  A pure function of the sizes."""
+        sc = self.scale
+        hp, wp = len(reflect_pad_index(height, self.pre_pad, sc)), len(reflect_pad_index(width, self.pre_pad, sc))
+        if self.tile_size > 0:
+            plan = self.tile_plan(hp, wp)
+        else:
+            plan = [{'in': (0, hp, 0, wp), 'out': (0, hp * sc, 0, wp * sc), 'crop': (0, hp * sc, 0, wp * sc)}]
+        shapes = {}
+        for b in range(batch):
+            for t in plan:
+                py0, py1, px0, px1 = t['in']
+                oy0, _, ox0, _ = t['out']
+                cy0, cy1, cx0, cx1 = t['crop']
+                if oy0 >= height * sc or ox0 >= width * sc:
+                    continue
+                shapes.setdefault((py1 - py0, px1 - px0), []).append((b, py0, px0, cy0, cx0, cy1 - cy0, cx1 - cx0, oy0, ox0))
+        out = []
+        for (th, tw), rows in shapes.items():
+            k = max_tiles
+            if k is None:
+                one = tile_bytes(1, th, tw)
+                k = max(1, (self.WORKSPACE_BUDGET - one) // (tile_bytes(2, th, tw) - one) + 1)
+            k = max(1, int(k))
+            out += [(th, tw, rows[i:i + k]) for i in range(0, len(rows), k)]
+        return out
+
+    def _device_path(self, outscale):
+        """enhance / enhance_batch run on the device: the model is this package's 3-channel RRDBNet, no LANCZOS resize."""
+        m = self.model
+        return (isinstance(m, RRDBNet) and m.num_in_ch == 3 and m.num_out_ch == 3 and
+                (outscale is None or outscale == float(self.scale)))
+
+    @torch.no_grad()
+    def enhance_batch(self, images, outscale=None, max_tiles=None):
+        """``enhance`` of every image of ``images`` (CUDA uint8 [B,H,W,3] BGR) on the device, as CUDA uint8
+        [B,H*scale,W*scale,3] BGR; each image equals ``enhance(img)[0]`` byte for byte.  The tiles of all images are grouped
+        by input-window shape (``tile_groups``) and every group runs as forwards of at most ``max_tiles`` tiles (default:
+        as many as ``WORKSPACE_BUDGET`` holds) that read the uint8 images and write the uint8 result directly.  Keeps no
+        state on ``self``: threads may share one upsampler.
+
+        Raises NotImplementedError for ``outscale`` other than None / ``scale`` (the reference's INTER_LANCZOS4 resize is
+        not built), for images that are not uint8 with 3 channels and for models other than a 3-channel
+        ``codeformer_b200.RRDBNet``; RuntimeError for CPU tensors and for pads not smaller than the dimension they reflect;
+        AssertionError, as RRDBNet.forward, for tiles whose size is not a multiple of the pixel-unshuffle factor."""
+        if outscale is not None and outscale != float(self.scale):
+            raise NotImplementedError(f'RealESRGANer.enhance_batch: outscale {outscale} != scale {self.scale} needs the '
+                                      'reference\'s INTER_LANCZOS4 resize, which is not built')
+        if not self._device_path(None):
+            raise NotImplementedError('RealESRGANer.enhance_batch: built for a codeformer_b200.RRDBNet with 3 input and 3 output '
+                                      f'channels, got {type(self.model).__name__}')
+        if not torch.is_tensor(images):
+            raise NotImplementedError(f'RealESRGANer.enhance_batch takes a CUDA uint8 tensor, got {type(images).__name__}')
+        if not images.is_cuda:
+            raise RuntimeError('RealESRGANer.enhance_batch: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
+        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
+            raise NotImplementedError(f'RealESRGANer.enhance_batch takes uint8 [B,H,W,3] BGR images (16-bit, gray and alpha '
+                                      f'images go through enhance), got {images.dtype} {tuple(images.shape)}')
+        B, H, W, _ = images.shape
+        sc = self.scale
+        out = torch.empty((B, H * sc, W * sc, 3), dtype=torch.uint8, device=images.device)
+        if B == 0 or H == 0 or W == 0:
+            return out
+        images = images.contiguous()
+        us = unshuffle_factor(sc)
+        lib = _lib.load()
+
+        def tile_bytes(n, th, tw):
+            return lib.cfb_rrdb_workspace_bytes(self.model._handle(), n, th, tw)
+        for th, tw, rows in self.tile_groups(B, H, W, max_tiles, tile_bytes):
+            if th % us or tw % us:
+                raise AssertionError('pixel_unshuffle needs H and W divisible by the factor (arch_util.py:202)')
+            self.model.forward_u8_tiles(images, self.pre_pad, rows, th, tw, out)
+        return out
+
     def tile_process(self):
         b, c, height, width = self.img.shape
         self.output = self.img.new_zeros((b, c, height * self.scale, width * self.scale))
@@ -174,7 +297,12 @@ class RealESRGANer:
 
     @torch.no_grad()
     def enhance(self, img, outscale=None, alpha_upsampler='realesrgan'):
+        """The reference's ``enhance``.  uint8 3-channel images with this package's RRDBNet and no LANCZOS resize go through
+        ``enhance_batch`` (the same bytes); every other case through pre_process / tile_process / post_process."""
         import cv2
+        if img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and self._device_path(outscale):
+            x = torch.from_numpy(np.ascontiguousarray(img)).to(self.device)
+            return self.enhance_batch(x[None])[0].cpu().numpy(), 'RGB'
         h_input, w_input = img.shape[0:2]
         img = img.astype(np.float32)
         max_range = 65535 if np.max(img) > 256 else 255              # :193-199

@@ -13,9 +13,12 @@ and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of im
     ``CodeFormer.forward_u8`` in batches of at most ``max_batch`` faces; the parse masks are batched the same way;
   * the paste-back runs once per chunk of images (``cfb_paste_faces_multi``), one read-back of the erosion areas.
 
+  * a ``codeformer_b200.RealESRGANer`` background / face upsampler whose scale is ``upscale`` runs once per chunk on the
+    device (``enhance_batch``): the chunk's images, then its restored faces, each as one batch of tiles.
+
 What stays on the host, as in the reference: the NMS and the landmark filter, ``get_center_face``,
-``cv2.estimateAffinePartial2D(LMEDS)`` (cv2 is imported lazily, as ``align_warp_face`` does), and the background / face
-upsamplers' ``enhance`` per image.  Every result is per image: batching and chunking do not change any byte.
+``cv2.estimateAffinePartial2D(LMEDS)`` (cv2 is imported lazily, as ``align_warp_face`` does), and the ``enhance`` of any
+other upsampler, per image.  Every result is per image: batching and chunking do not change any byte.
 """
 import numpy as np
 import torch
@@ -23,6 +26,7 @@ import torch
 from . import _lib
 from .detection import RetinaFace, cuda_u8_image
 from .detection import finish_detections as retinaface_finish
+from .upsampler import RealESRGANer
 from .pasteback import (_paste_multi, adjust_inverse_affines, parse_masks, resize_area, resize_linear, resize_linear_factor,
                         warp_faces_multi)
 from .yolov5face import YoloDetector, _resize_u8, letterbox_geometry
@@ -145,12 +149,19 @@ def _restore(net, crops, w, max_batch, errors):
     return out
 
 
+def _on_device(upsampler, upscale):
+    """The upsampler runs through ``enhance_batch``: this package's RealESRGANer over its RRDBNet, no LANCZOS resize."""
+    return isinstance(upsampler, RealESRGANer) and upsampler._device_path(upscale)
+
+
 def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_center_face=False, detection_resize=640,
                    eye_dist_threshold=5, bg_upsampler=None, face_upsampler=None, max_batch=32, return_faces=False):
     """Restore whole images in batches.  ``images``: a list of uint8 HWC BGR numpy arrays or CUDA tensors.  ``net``: a
     ``CodeFormer``; ``detector``: ``init_detection_model('retinaface_resnet50' | 'YOLOv5l')``; ``parser``: a ParseNet
     (``init_parsing_model()``) or None for use_parse=False.  ``bg_upsampler`` / ``face_upsampler``: objects with
-    ``enhance(img, outscale=upscale)`` (``RealESRGANer``), called per image / per face on the host.
+    ``enhance(img, outscale=upscale)`` (``RealESRGANer``).  A ``codeformer_b200.RealESRGANer`` over ``RRDBNet`` with
+    ``scale == upscale`` runs on the device, once per chunk of images for the backgrounds and once for the restored faces
+    (``enhance_batch``); any other upsampler is called per image / per face on the host.
 
     Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
     also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted.  Each image equals the
@@ -193,14 +204,22 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
             restored = _restore(net, crops, w, max_batch, errors)
         S = FACE_SIZE
         if face_upsampler is not None and len(affines):
-            host = restored.cpu().numpy()
-            up = [face_upsampler.enhance(f, outscale=upscale)[0] for f in host]
-            restored = torch.from_numpy(np.ascontiguousarray(np.stack(up))).to(dev)
+            if _on_device(face_upsampler, upscale):
+                restored = face_upsampler.enhance_batch(restored, outscale=upscale)
+            else:
+                host = restored.cpu().numpy()
+                up = [face_upsampler.enhance(f, outscale=upscale)[0] for f in host]
+                restored = torch.from_numpy(np.ascontiguousarray(np.stack(up))).to(dev)
             S = FACE_SIZE * upscale
             if restored.shape[1] != S or restored.shape[2] != S:
                 raise RuntimeError(f'restore_images: the face upsampler returned {tuple(restored.shape[1:3])}, expected {S}x{S}')
         h_up, w_up = int(h * upscale), int(wd * upscale)
-        if bg_upsampler is not None:
+        if bg_upsampler is not None and _on_device(bg_upsampler, upscale):
+            canvases = bg_upsampler.enhance_batch(torch.stack([inputs[i][0] for i in idx]), outscale=upscale)
+            if canvases.shape[1:3] != (h_up, w_up):
+                raise NotImplementedError(f'restore_images: the background upsampler returned {tuple(canvases.shape[1:3])}, the '
+                                          f'output is {h_up}x{w_up}; the reference resizes it with INTER_LANCZOS4, which is not built')
+        elif bg_upsampler is not None:
             bgs = []
             for i in idx:
                 src = inputs[i][1] if inputs[i][2] else inputs[i][0].cpu().numpy()

@@ -244,6 +244,19 @@ int       cfb_rrdb_set_precision(cfb_rrdb* net, int32_t precision);
 int64_t   cfb_rrdb_workspace_bytes(cfb_rrdb* net, int32_t batch, int32_t h, int32_t w);
 int       cfb_rrdb_forward(cfb_rrdb* net, const float* x, float* out, int32_t batch, int32_t h, int32_t w,
                            void* workspace, int64_t workspace_bytes, void* stream);
+/* RealESRGANer's pre_process + tile_process + post_process and its uint8 conversion (realesrgan_utils.py:71-210) for tiles of
+ * equal size, from uint8 HWC BGR images to uint8 HWC BGR images, as one forward at batch num_tiles.
+ * images_bgr: [num_images, img_h, img_w, 3] on the device; the padded image is img_h + pre_pad (+ the reflect pad to the
+ * pixel-unshuffle multiple) high, likewise wide; each pad must be smaller than the dimension it reflects.
+ * tiles: host int32 [num_tiles][9] = image, in_y, in_x (window origin in the padded image), crop_y, crop_x, crop_h, crop_w
+ * (kept rectangle of the tile's tile_h*scale x tile_w*scale output), out_y, out_x (its place in the output); tile_h and tile_w
+ * must be multiples of the pixel-unshuffle factor.  out_bgr: [num_images, img_h*scale, img_w*scale, 3]; pixels past it (the
+ * pads) are discarded.  The input value is float32 u8 / 255, the output clamp(v, 0, 1) * 255 rounded half to even.  Built for
+ * 3 channels in and out; honours cfb_rrdb_set_precision; workspace: cfb_rrdb_workspace_bytes(net, num_tiles, tile_h, tile_w).
+ * The table travels in the launch parameters: no host synchronisation. */
+int       cfb_rrdb_forward_u8_tiles(cfb_rrdb* net, const uint8_t* images_bgr, int32_t num_images, int32_t img_h, int32_t img_w,
+                                    int32_t pre_pad, const int32_t* tiles, int32_t num_tiles, int32_t tile_h, int32_t tile_w,
+                                    uint8_t* out_bgr, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- ParseNet (SURVEY.md section 8 row f3): face parsing of the restored face for the paste-back blend ----
  * /root/reference/facelib/parsing/parsenet.py:140-194; built by init_parsing_model('parsenet') as ParseNet(in_size=512,
