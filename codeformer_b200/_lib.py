@@ -133,6 +133,13 @@ SIGNATURES = {
                                          c_int32, c_int32, _P]),
     'cfb_paste_faces_multi_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
     'cfb_paste_faces_multi': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, _P, c_double, _P, _P, c_int64, _P]),
+    'cfb_resize_lanczos4_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'cfb_lanczos4_table': (None, [c_int32, c_int32, _P, _P]),
+    'cfb_gray_adain_faces': (c_int, [_P, _P, c_int32, c_int32, _P, _P, _P]),
+    'cfb_f64_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
+    'cfb_paste_faces_f64_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
+    'cfb_paste_faces_f64': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, _P, c_double, _P, _P, _P, _P,
+                                    c_int64, _P]),
 }
 
 _lib = None

@@ -22,6 +22,11 @@
 //   INTER_AREA    (shrinking, cfb_resize_area_u8) integer factors: window sums, a 2 x 2 halving (s + 2) >> 2, otherwise
 //                 cvRound(s * (1.f / area)); other factors: computeResizeAreaTab weights in double stored as float, a float
 //                 row sum per source row and a float sum of the rows, both in cv2's tap order, then cvRound and clamp.
+//   LANCZOS4      (cfb_resize_lanczos4_u8) cv2's fixed point: eight int16 taps per axis (float weights * 2048, not
+//                 renormalised), clamped source coordinates, an int32 horizontal pass and a vertical pass (v + 2^21) >> 22.
+//   gray images   add_restored_face's adain_npy(bgr2gray(restored), cropped) in float64 (cfb_gray_adain_faces) and the paste
+//                 of float64 faces (cfb_paste_faces_f64): warpAffine on CV_64F blends with the float32 weight table in
+//                 double, and the canvas is float64 from the first face on.
 // Arithmetic that cv2 does unfused is written with _rn intrinsics so nvcc cannot contract it into FMAs.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -140,6 +145,30 @@ __device__ __forceinline__ void sample_u8(const uint8_t* src, int h, int w, int 
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) out[c] = min(max((acc[c] + (1 << 14)) >> 15, 0), 255);
+}
+
+// warpAffine's float32 weight table for 1/32 steps: (1-b)(1-a), (1-b)a, b(1-a), ba rounded to float32
+__device__ __forceinline__ void bilinear_wt(int fx, int fy, float* wt) {
+  const float a = fx * (1.f / 32.f), b = fy * (1.f / 32.f);
+  wt[0] = __fmul_rn(1.f - b, 1.f - a); wt[1] = __fmul_rn(1.f - b, a); wt[2] = __fmul_rn(b, 1.f - a); wt[3] = __fmul_rn(b, a);
+}
+
+// bilinear f64 sample of `nch` interleaved channels of an S x S image, constant border 0 (cv2.warpAffine on CV_64F):
+// products and the left-to-right sum in double
+template <int NCH>
+__device__ __forceinline__ void sample_f64(const double* src, int S, int ix, int iy, int fx, int fy, double* out) {
+  float wt[4];
+  bilinear_wt(fx, fy, wt);
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int yy = iy + (t >> 1), xx = ix + (t & 1);
+    const bool in = yy >= 0 && yy < S && xx >= 0 && xx < S;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const double s = in ? src[((size_t)yy * S + xx) * NCH + c] : 0.;
+      out[c] = t == 0 ? __dmul_rn(s, (double)wt[0]) : __dadd_rn(out[c], __dmul_rn(s, (double)wt[t]));
+    }
+  }
 }
 
 // ---- kernels ----------------------------------------------------------------------------------------------------
@@ -418,48 +447,89 @@ __global__ void k_canvas_out(const T* __restrict__ src, uint8_t* __restrict__ ds
   if (dbg) dbg[i] = (float)v;
 }
 
-// one face into the canvas: inv_restored (u8 warp), the parse warp (f64 bilinear), min(parse, soft), the blend
-template <typename T>
-__global__ void k_composite(const PbFace* __restrict__ faces, int fi, const uint8_t* __restrict__ face, int S,
-                            const double* __restrict__ parse, const float* __restrict__ ws, T* __restrict__ canvas, int W) {
+// one face into the canvas: inv_restored (u8 fixed-point warp, or the f64 warp for FT = double), the parse warp (f64
+// bilinear), min(parse, soft), the blend.  A float64 face makes the canvas float64 with or without the parse mask; without
+// it numpy multiplies (1 - soft) (float32) with the canvas, which is still uint8 for the first face of an image (a float32
+// product) and float64 afterwards (`first`).
+template <typename T, typename FT>
+__global__ void k_composite(const PbFace* __restrict__ faces, int fi, const FT* __restrict__ face, int S,
+                            const double* __restrict__ parse, const float* __restrict__ ws, T* __restrict__ canvas, int W,
+                            bool first) {
   const PbFace& F = faces[fi];
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= F.rw || y >= F.rh) return;
-  int ix, iy, fx, fy, v[3];
+  int ix, iy, fx, fy;
   warp_coord(F.A, F.x0 + x, F.y0 + y, ix, iy, fx, fy);
-  const int zero[3] = {0, 0, 0};
-  sample_u8(face, S, S, ix, iy, fx, fy, 0, zero, v);
   const size_t plane = (size_t)F.rw * F.rh, p = (size_t)y * F.rw + x;
   const float ero = ws[F.off + 2 * plane + p], soft = ws[F.off + 1 * plane + p];
   T* c = canvas + ((size_t)(F.y0 + y) * W + F.x0 + x) * 3;
-  if constexpr (sizeof(T) == 8) {
-    double m = (double)soft;
+  if constexpr (sizeof(FT) == 8) {
+    static_assert(sizeof(T) == 8, "float64 faces blend into a float64 canvas");
+    double v[3];
+    sample_f64<3>(face, S, ix, iy, fx, fy, v);
     if (parse) {
-      const float a = fx * (1.f / 32.f), b = fy * (1.f / 32.f);
-      const float wt[4] = {__fmul_rn(1.f - b, 1.f - a), __fmul_rn(1.f - b, a), __fmul_rn(b, 1.f - a), __fmul_rn(b, a)};
-      double acc = 0.;
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const int yy = iy + (t >> 1), xx = ix + (t & 1);
-        const double s = (yy >= 0 && yy < S && xx >= 0 && xx < S) ? parse[(size_t)yy * S + xx] : 0.;
-        acc = t == 0 ? __dmul_rn(s, (double)wt[0]) : __dadd_rn(acc, __dmul_rn(s, (double)wt[t]));
-      }
+      double m = (double)soft, acc;
+      sample_f64<1>(parse, S, ix, iy, fx, fy, &acc);
       if (acc < m) m = acc;
-    }
-    const double om = __dsub_rn(1., m);
+      const double om = __dsub_rn(1., m);
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
-      const double pasted = (double)__fmul_rn(ero, (float)v[ch]);
-      c[ch] = __dadd_rn(__dmul_rn(m, pasted), __dmul_rn(om, (double)c[ch]));
+      for (int ch = 0; ch < 3; ++ch)
+        c[ch] = __dadd_rn(__dmul_rn(m, __dmul_rn((double)ero, v[ch])), __dmul_rn(om, c[ch]));
+    } else {
+      const float om = __fsub_rn(1.f, soft);
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const double bg = first ? (double)__fmul_rn(om, (float)c[ch]) : __dmul_rn((double)om, c[ch]);
+        c[ch] = __dadd_rn(__dmul_rn((double)soft, __dmul_rn((double)ero, v[ch])), bg);
+      }
     }
   } else {
-    const float om = __fsub_rn(1.f, soft);
+    int v[3];
+    const int zero[3] = {0, 0, 0};
+    sample_u8(face, S, S, ix, iy, fx, fy, 0, zero, v);
+    if constexpr (sizeof(T) == 8) {
+      double m = (double)soft;
+      if (parse) {
+        double acc;
+        sample_f64<1>(parse, S, ix, iy, fx, fy, &acc);
+        if (acc < m) m = acc;
+      }
+      const double om = __dsub_rn(1., m);
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
-      const float pasted = __fmul_rn(ero, (float)v[ch]);
-      c[ch] = __fadd_rn(__fmul_rn(soft, pasted), __fmul_rn(om, (float)c[ch]));
+      for (int ch = 0; ch < 3; ++ch) {
+        const double pasted = (double)__fmul_rn(ero, (float)v[ch]);
+        c[ch] = __dadd_rn(__dmul_rn(m, pasted), __dmul_rn(om, (double)c[ch]));
+      }
+    } else {
+      const float om = __fsub_rn(1.f, soft);
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float pasted = __fmul_rn(ero, (float)v[ch]);
+        c[ch] = __fadd_rn(__fmul_rn(soft, pasted), __fmul_rn(om, (float)c[ch]));
+      }
     }
   }
+}
+
+// per-image maximum of a float64 canvas: block (slice, image) -> partial[image * gridDim.x + slice]
+__global__ void k_canvas_max(const double* __restrict__ canvas, size_t per_img, double* __restrict__ partial) {
+  const double* p = canvas + (size_t)blockIdx.y * per_img;
+  double m = -INFINITY;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < per_img; i += (size_t)gridDim.x * blockDim.x) m = fmax(m, p[i]);
+  __shared__ double red[256];
+  red[threadIdx.x] = m;
+  __syncthreads();
+  for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + o]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) partial[blockIdx.y * gridDim.x + blockIdx.x] = red[0];
+}
+
+// astype(np.uint16): truncate toward zero, keep the low 16 bits
+__global__ void k_canvas_out16(const double* __restrict__ src, uint16_t* __restrict__ dst, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (uint16_t)((long long)src[i] & 65535);
 }
 
 inline dim3 grid2(int w, int h, int z, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y, z); }
@@ -489,14 +559,17 @@ int make_plan(int H, int W, int n, int S, const double* inv, Plan& P) {
 }
 
 struct Layout {
-  size_t canvas, roi, parse0, parse1, parse_rs, faces, area, pgauss, gauss, total;
+  size_t canvas, roi, parse0, parse1, parse_rs, faces, area, pgauss, gauss, cmax, total;
 };
 
-Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gauss_floats, int n_img = 1) {
+constexpr int kMaxSlices = 64;        // k_canvas_max partials per image
+
+// f64_faces: float64 restored faces (a gray image), whose canvas is float64 with or without the parse masks
+Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gauss_floats, int n_img = 1, bool f64_faces = false) {
   Layout L{};
   size_t o = 0;
   auto take = [&](size_t b) { const size_t r = o; o += align256(b); return r; };
-  L.canvas = take((size_t)n_img * H * W * 3 * (use_parse ? 8 : 4));
+  L.canvas = take((size_t)n_img * H * W * 3 * (use_parse || f64_faces ? 8 : 4));
   L.roi = take(P.roi_floats * 4);
   const size_t pm = (size_t)n * kParse * kParse * 8;
   L.parse0 = take(use_parse ? pm : 0);
@@ -506,6 +579,7 @@ Layout layout(int H, int W, int n, int S, bool use_parse, const Plan& P, int gau
   L.area = take((size_t)std::max(n, 1) * 8);
   L.pgauss = take(kParseK * 8);
   L.gauss = take((size_t)gauss_floats * 4);
+  L.cmax = take(f64_faces ? (size_t)n_img * kMaxSlices * 8 : 0);
   L.total = o;
   return L;
 }
@@ -519,14 +593,17 @@ int max_gauss_floats(const Plan& P) {
 
 // n_img canvases [n_img,H,W,3]; face i goes into canvas img_of[i] (img_of == nullptr: all into canvas 0).  Every step
 // before the composite is per face, so a face's result does not depend on the other canvases of the batch.
-template <typename T>
-int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int W, const uint8_t* faces, int n, int S,
+// FT = double (float64 faces): canvas_u16 (optional) receives astype(np.uint16) of every canvas and wide_out[i] (host) tells
+// whether canvas i exceeds 256, where the reference returns the uint16 image.
+template <typename T, typename FT = uint8_t>
+int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int W, const FT* faces, int n, int S,
                const uint8_t* parse_u8, const double* inv, double upscale, float* dbg, int32_t* w_edge_out, char* ws,
-               int64_t ws_bytes, cudaStream_t st) {
+               int64_t ws_bytes, cudaStream_t st, uint16_t* canvas_u16 = nullptr, int32_t* wide_out = nullptr) {
   const bool use_parse = parse_u8 != nullptr;
+  constexpr bool kF64 = sizeof(FT) == 8;
   Plan P;
   CFB_CHECK(make_plan(H, W, n, S, inv, P));
-  const Layout L = layout(H, W, n, S, use_parse, P, max_gauss_floats(P), n_img);
+  const Layout L = layout(H, W, n, S, use_parse, P, max_gauss_floats(P), n_img, kF64);
   CFB_REQUIRE((int64_t)L.total <= ws_bytes, "cfb_paste_faces: workspace too small");
   T* canvas = (T*)(ws + L.canvas);
   float* roi = (float*)(ws + L.roi);
@@ -603,18 +680,202 @@ int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int 
     CFB_LAUNCH_CHECK();
     k_blur_roi<<<g, b, 0, st>>>(dfaces, roi, dgauss, 0, 1, true, H, W);   // plane 1: inv_soft_mask
     CFB_LAUNCH_CHECK();
+    std::vector<char> touched(n_img, 0);      // the canvas of an image is still uint8-valued until its first face
     for (int i = 0; i < n; ++i) {
       const PbFace& F = P.faces[i];
+      const int im = img_of ? img_of[i] : 0;
+      const bool first = !touched[im];
+      touched[im] = 1;
       if (F.rw == 0 || F.rh == 0) continue;
-      T* cv = canvas + (img_of ? (size_t)img_of[i] * H * W * 3 : 0);
-      k_composite<T><<<grid2(F.rw, F.rh, 1, b), b, 0, st>>>(dfaces, i, faces + (size_t)i * S * S * 3, S,
-                                                             parse_src ? parse_src + (size_t)i * S * S : nullptr, roi, cv, W);
+      T* cv = canvas + (size_t)im * H * W * 3;
+      k_composite<T, FT><<<grid2(F.rw, F.rh, 1, b), b, 0, st>>>(dfaces, i, faces + (size_t)i * S * S * 3, S,
+                                                                 parse_src ? parse_src + (size_t)i * S * S : nullptr, roi, cv, W,
+                                                                 first);
       CFB_LAUNCH_CHECK();
+    }
+  }
+  if constexpr (kF64) {
+    if (wide_out) {
+      double* dmax = (double*)(ws + L.cmax);
+      k_canvas_max<<<dim3(kMaxSlices, n_img), 256, 0, st>>>(canvas, (size_t)H * W * 3, dmax);
+      CFB_LAUNCH_CHECK();
+      std::vector<double> mx((size_t)n_img * kMaxSlices);
+      CFB_CUDA(cudaMemcpyAsync(mx.data(), dmax, mx.size() * 8, cudaMemcpyDeviceToHost, st));
+      CFB_CUDA(cudaStreamSynchronize(st));
+      bool any = false;
+      for (int i = 0; i < n_img; ++i) {
+        wide_out[i] = *std::max_element(mx.begin() + (size_t)i * kMaxSlices, mx.begin() + (size_t)(i + 1) * kMaxSlices) > 256.;
+        any = any || wide_out[i];
+      }
+      if (any && canvas_u16) {
+        k_canvas_out16<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(canvas, canvas_u16, npx);
+        CFB_LAUNCH_CHECK();
+      }
     }
   }
   k_canvas_out<T><<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(canvas, canvas_u8, dbg, npx);
   CFB_LAUNCH_CHECK();
   return 0;
+}
+
+
+// ---- INTER_LANCZOS4 ------------------------------------------------------------------------------------------------
+// cv2's interpolateLanczos4: the window from one sin / cos of -(x + 3) pi / 4 rotated by multiples of 45 degrees, each tap
+// divided by its own y * y, normalised by the float sum; x < FLT_EPSILON is the unit tap
+void lanczos4_coeffs(float x, float* cf) {
+  static const double s45 = 0.70710678118654752440084436210485;
+  static const double cs[8][2] = {{1, 0}, {-s45, -s45}, {0, 1}, {s45, -s45}, {-1, 0}, {s45, s45}, {0, -1}, {-s45, s45}};
+  if (x < 1.1920929e-07f) {
+    for (int i = 0; i < 8; ++i) cf[i] = 0.f;
+    cf[3] = 1.f;
+    return;
+  }
+  const double pi = 3.1415926535897932384626433832795;
+  const double xd = (double)x, y0 = -(xd + 3) * pi * 0.25, s0 = std::sin(y0), c0 = std::cos(y0);
+  float sum = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    const double y = (double)(float)(-(xd + 3 - i) * pi * 0.25);
+    cf[i] = (float)((cs[i][0] * s0 + cs[i][1] * c0) / (y * y));
+    sum += cf[i];
+  }
+  sum = 1.f / sum;
+  for (int i = 0; i < 8; ++i) cf[i] *= sum;
+}
+
+// per output coordinate: floor of the source coordinate (taps at idx - 3 .. idx + 4, clamped by the kernel) and the eight
+// weights * 2048 saturated to int16, as cv::resize builds them
+void lanczos4_table(int ssize, int dsize, int32_t* idx, int16_t* coef) {
+  const double scale = 1. / ((double)dsize / ssize);
+  for (int d = 0; d < dsize; ++d) {
+    float f = (float)((d + 0.5) * scale - 0.5);
+    const int s = (int)std::floor(f);
+    f -= s;
+    float cf[8];
+    lanczos4_coeffs(f, cf);
+    idx[d] = s;
+    for (int k = 0; k < 8; ++k)
+      coef[d * 8 + k] = (int16_t)std::max(-32768.f, std::min(32767.f, std::nearbyint(cf[k] * 2048.f)));
+  }
+}
+
+constexpr int kLzTileW = 64;     // output columns of a block
+constexpr int kLzRows = 48;      // source rows a block may hold (the host picks the band height to fit)
+
+// one block: a band of `band` output rows x kLzTileW output columns of image blockIdx.z.  The horizontal pass of every
+// source row the band needs goes to shared memory as int32, the vertical pass reads it back: no intermediate image.
+__global__ void __launch_bounds__(256) k_resize_lanczos4_u8(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst,
+                                                            int oh, int ow, const int* __restrict__ xi, const short* __restrict__ xt,
+                                                            const int* __restrict__ yi, const short* __restrict__ yt, int band) {
+  __shared__ int hbuf[kLzRows][kLzTileW * 3];
+  __shared__ short sxt[kLzTileW * 8];
+  __shared__ int sxi[kLzTileW];
+  const int x0 = blockIdx.x * kLzTileW, y0 = blockIdx.y * band, y1 = min(y0 + band, oh);
+  const int tw = min(kLzTileW, ow - x0);
+  src += (size_t)blockIdx.z * h * w * 3;
+  dst += (size_t)blockIdx.z * oh * ow * 3;
+  const int rlo = yi[y0] - 3, span = yi[y1 - 1] + 4 - rlo + 1;
+  for (int i = threadIdx.x; i < tw * 8; i += 256) sxt[i] = xt[(size_t)x0 * 8 + i];
+  for (int i = threadIdx.x; i < tw; i += 256) sxi[i] = xi[x0 + i];
+  __syncthreads();
+  for (int i = threadIdx.x; i < span * tw; i += 256) {
+    const int r = i / tw, xl = i - r * tw;
+    const uint8_t* row = src + (size_t)min(max(rlo + r, 0), h - 1) * w * 3;
+    const int s = sxi[xl] - 3;
+    int a0 = 0, a1 = 0, a2 = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const uint8_t* p = row + min(max(s + k, 0), w - 1) * 3;
+      const int c = sxt[xl * 8 + k];
+      a0 += p[0] * c; a1 += p[1] * c; a2 += p[2] * c;
+    }
+    hbuf[r][xl * 3] = a0; hbuf[r][xl * 3 + 1] = a1; hbuf[r][xl * 3 + 2] = a2;
+  }
+  __syncthreads();
+  const int te = tw * 3;
+  for (int i = threadIdx.x; i < (y1 - y0) * te; i += 256) {
+    const int yl = i / te, e = i - yl * te, y = y0 + yl, r0 = yi[y] - 3 - rlo;
+    int acc = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc += hbuf[r0 + k][e] * yt[y * 8 + k];
+    dst[((size_t)y * ow + x0) * 3 + e] = (uint8_t)min(max((acc + (1 << 21)) >> 22, 0), 255);
+  }
+}
+
+// ---- the gray branch of add_restored_face ----------------------------------------------------------------------
+constexpr int kGraySlices = 64;
+
+__device__ __forceinline__ double bgr2gray(const uint8_t* p) {      // 0.2989 r + 0.5870 g + 0.1140 b, left to right
+  return __dadd_rn(__dadd_rn(__dmul_rn(0.2989, (double)p[2]), __dmul_rn(0.5870, (double)p[1])), __dmul_rn(0.1140, (double)p[0]));
+}
+
+// partial sums over slice blockIdx.x of face blockIdx.y of q = {gray(restored), cropped b, g, r}: the values (stats == NULL)
+// or their squared deviations from the means in stats[face][0 / 2][.].  Fixed order: strided per thread, then a tree.
+__global__ void k_gray_partial(const uint8_t* __restrict__ restored, const uint8_t* __restrict__ cropped, int npx,
+                               const double* __restrict__ stats, double* __restrict__ partial) {
+  const int f = blockIdx.y;
+  const uint8_t* r = restored + (size_t)f * npx * 3;
+  const uint8_t* c = cropped + (size_t)f * npx * 3;
+  double mean[4] = {0., 0., 0., 0.};
+  if (stats) {
+    mean[0] = stats[f * 12];
+    for (int k = 0; k < 3; ++k) mean[1 + k] = stats[f * 12 + 6 + k];
+  }
+  const int per = (npx + gridDim.x - 1) / gridDim.x, lo = blockIdx.x * per, hi = min(lo + per, npx);
+  double s[4] = {0., 0., 0., 0.};
+  for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+    const double q[4] = {bgr2gray(r + (size_t)i * 3), (double)c[(size_t)i * 3], (double)c[(size_t)i * 3 + 1], (double)c[(size_t)i * 3 + 2]};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const double d = __dsub_rn(q[k], mean[k]);
+      s[k] = __dadd_rn(s[k], stats ? __dmul_rn(d, d) : q[k]);
+    }
+  }
+  __shared__ double red[4][256];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) red[k][threadIdx.x] = s[k];
+  __syncthreads();
+  for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o)
+      for (int k = 0; k < 4; ++k) red[k][threadIdx.x] = __dadd_rn(red[k][threadIdx.x], red[k][threadIdx.x + o]);
+    __syncthreads();
+  }
+  if (threadIdx.x < 4) partial[((size_t)f * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = red[threadIdx.x][0];
+}
+
+// the slices of a face summed in order: stats[face] = {content mean, content std, style mean, style std} x 3 channels (the
+// three content channels are the same gray).  pass 0 writes the means, pass 1 sqrt(var + 1e-5).
+__global__ void k_gray_stats(const double* __restrict__ partial, int slices, int npx, int pass, double* __restrict__ stats) {
+  const int f = blockIdx.x, k = threadIdx.x;
+  if (k >= 4) return;
+  double s = 0.;
+  for (int i = 0; i < slices; ++i) s = __dadd_rn(s, partial[((size_t)f * slices + i) * 4 + k]);
+  s = __ddiv_rn(s, (double)npx);
+  if (pass) s = sqrt(__dadd_rn(s, 1e-5));
+  double* o = stats + f * 12 + pass * 3;
+  if (k == 0) o[0] = o[1] = o[2] = s;
+  else o[6 + k - 1] = s;
+}
+
+// (gray - content mean) / content std * style std + style mean
+__global__ void k_gray_apply(const uint8_t* __restrict__ restored, int npx, const double* __restrict__ stats, double* __restrict__ out) {
+  const int f = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npx) return;
+  const double* st = stats + f * 12;
+  const double nrm = __ddiv_rn(__dsub_rn(bgr2gray(restored + ((size_t)f * npx + i) * 3), st[0]), st[3]);
+  double* o = out + ((size_t)f * npx + i) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c] = __dadd_rn(__dmul_rn(nrm, st[9 + c]), st[6 + c]);
+}
+
+// the parse network's input of a float64 face: astype(float32) / 255, BGR -> RGB, (x - 0.5) / 0.5, HWC -> NCHW
+__global__ void k_f64_to_input(const double* __restrict__ img, float* __restrict__ x, int64_t hw, int64_t total) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int64_t n = i / (3 * hw), r = i - n * 3 * hw;
+  const int c = (int)(r / hw);
+  const int64_t px = r - (int64_t)c * hw;
+  const float t = __fdiv_rn(__double2float_rn(img[(n * hw + px) * 3 + (2 - c)]), 255.f);
+  x[i] = __fdiv_rn(__fsub_rn(t, 0.5f), 0.5f);
 }
 
 }  // namespace
@@ -809,6 +1070,119 @@ int cfb_paste_faces(uint8_t* canvas, int32_t h_up, int32_t w_up, const uint8_t* 
                                    debug_canvas, w_edge_out, (char*)workspace, workspace_bytes, st);
   return cfb::paste_impl<float>(canvas, 1, nullptr, h_up, w_up, faces, n, face_size, nullptr, inverse_affines, upscale,
                                 debug_canvas, w_edge_out, (char*)workspace, workspace_bytes, st);
+  API_END(1)
+}
+
+
+void cfb_lanczos4_table(int32_t src_len, int32_t dst_len, int32_t* idx, int16_t* coef) {
+  if (src_len > 0 && dst_len > 0 && idx && coef) cfb::lanczos4_table(src_len, dst_len, idx, coef);
+}
+
+int cfb_resize_lanczos4_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_resize_lanczos4_u8: bad size");
+  CFB_REQUIRE(n <= 65535, "cfb_resize_lanczos4_u8: at most 65535 images per call");
+  CFB_REQUIRE(n == 0 || (src && dst), "cfb_resize_lanczos4_u8: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h == out_h && w == out_w) {                  // cv2.resize to the same size is a copy
+    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  // one host block: xi[ow] yi[oh] (int32) then xt[ow * 8] yt[oh * 8] (int16)
+  const size_t ni = (size_t)out_w + out_h;
+  std::vector<char> host(ni * 4 + ni * 16);
+  int32_t* xi = (int32_t*)host.data();
+  int32_t* yi = xi + out_w;
+  int16_t* xt = (int16_t*)(host.data() + ni * 4);
+  int16_t* yt = xt + (size_t)out_w * 8;
+  cfb::lanczos4_table(w, out_w, xi, xt);
+  cfb::lanczos4_table(h, out_h, yi, yt);
+  int band = 16;                                   // the tallest band whose source rows fit the shared rows
+  for (;; band /= 2) {
+    int span = 0;
+    for (int y0 = 0; y0 < out_h; y0 += band) span = std::max(span, yi[std::min(y0 + band, out_h) - 1] - yi[y0] + 8);
+    if (span <= cfb::kLzRows) break;               // a band of one row needs eight
+  }
+  CFB_REQUIRE((out_h + band - 1) / band <= 65535, "cfb_resize_lanczos4_u8: output too tall");
+  char* dtab = nullptr;
+  CFB_CUDA(cudaMallocAsync((void**)&dtab, host.size(), st));
+  CFB_CUDA(cudaMemcpyAsync(dtab, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  const int* dxi = (const int*)dtab;
+  const short* dxt = (const short*)(dtab + ni * 4);
+  cfb::k_resize_lanczos4_u8<<<dim3((out_w + cfb::kLzTileW - 1) / cfb::kLzTileW, (out_h + band - 1) / band, n), 256, 0, st>>>(
+      src, h, w, dst, out_h, out_w, dxi, dxt, dxi + out_w, dxt + (size_t)out_w * 8, band);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(dtab, st));
+  return 0;
+  API_END(1)
+}
+
+int cfb_gray_adain_faces(const uint8_t* restored, const uint8_t* cropped, int32_t n, int32_t face_size, double* out, double* stats,
+                         void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && face_size > 0 && face_size <= 8192, "cfb_gray_adain_faces: bad size");
+  CFB_REQUIRE(n <= 65535, "cfb_gray_adain_faces: at most 65535 faces per call");
+  CFB_REQUIRE(n == 0 || (restored && cropped && out), "cfb_gray_adain_faces: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int npx = face_size * face_size;
+  double* tmp = nullptr;                           // partial[n][slices][4], then stats[n][12] when the caller wants none
+  const size_t np = (size_t)n * cfb::kGraySlices * 4;
+  CFB_CUDA(cudaMallocAsync((void**)&tmp, (np + (size_t)n * 12) * 8, st));
+  double* dstats = stats ? stats : tmp + np;
+  const dim3 g(cfb::kGraySlices, n);
+  for (int pass = 0; pass < 2; ++pass) {           // means first, then the squared deviations from them
+    cfb::k_gray_partial<<<g, 256, 0, st>>>(restored, cropped, npx, pass ? dstats : nullptr, tmp);
+    CFB_LAUNCH_CHECK();
+    cfb::k_gray_stats<<<n, 32, 0, st>>>(tmp, cfb::kGraySlices, npx, pass, dstats);
+    CFB_LAUNCH_CHECK();
+  }
+  cfb::k_gray_apply<<<dim3((npx + 255) / 256, n), 256, 0, st>>>(restored, npx, dstats, out);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(tmp, st));
+  return 0;
+  API_END(1)
+}
+
+int cfb_f64_to_input(const double* img_bgr_hwc, float* x_nchw, int32_t n, int32_t hw, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && hw > 0, "cfb_f64_to_input: bad size");
+  CFB_REQUIRE(n == 0 || (img_bgr_hwc && x_nchw), "cfb_f64_to_input: NULL argument");
+  const int64_t total = (int64_t)n * 3 * hw;
+  if (total == 0) return 0;
+  cfb::k_f64_to_input<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(img_bgr_hwc, x_nchw, hw, total);
+  CFB_LAUNCH_CHECK();
+  return 0;
+  API_END(1)
+}
+
+int64_t cfb_paste_faces_f64_workspace_bytes(int32_t n_img, int32_t h_up, int32_t w_up, int32_t n, int32_t face_size,
+                                            int32_t use_parse, const double* inverse_affines) {
+  if (n_img <= 0 || h_up <= 0 || w_up <= 0 || n < 0 || face_size <= 0 || (n > 0 && !inverse_affines)) {
+    cfb::set_error("cfb_paste_faces_f64_workspace_bytes: bad argument");
+    return -1;
+  }
+  cfb::Plan P;
+  cfb::make_plan(h_up, w_up, n, face_size, inverse_affines, P);
+  return (int64_t)cfb::layout(h_up, w_up, n, face_size, use_parse != 0, P, cfb::max_gauss_floats(P), n_img, true).total;
+}
+
+int cfb_paste_faces_f64(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_t w_up, const double* faces, int32_t n,
+                        int32_t face_size, const uint8_t* parse_masks, const double* inverse_affines, const int32_t* img_index,
+                        double upscale, uint16_t* canvases_u16, int32_t* wide_out, int32_t* w_edge_out, void* workspace,
+                        int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n_img > 0 && n_img <= 65535 && h_up > 0 && w_up > 0 && n >= 0 && face_size > 0 && upscale > 0, "cfb_paste_faces_f64: bad size");
+  CFB_REQUIRE(canvases && workspace && (n == 0 || (faces && inverse_affines && img_index)), "cfb_paste_faces_f64: NULL argument");
+  CFB_REQUIRE(!canvases_u16 || wide_out, "cfb_paste_faces_f64: canvases_u16 needs wide_out");
+  for (int i = 0; i < n; ++i)
+    CFB_REQUIRE(img_index[i] >= 0 && img_index[i] < n_img, "cfb_paste_faces_f64: image index out of range");
+  const int64_t need = cfb_paste_faces_f64_workspace_bytes(n_img, h_up, w_up, n, face_size, parse_masks != nullptr, inverse_affines);
+  CFB_REQUIRE(need > 0 && workspace_bytes >= need, "cfb_paste_faces_f64: workspace too small (cfb_paste_faces_f64_workspace_bytes)");
+  return cfb::paste_impl<double, double>(canvases, n_img, img_index, h_up, w_up, faces, n, face_size, parse_masks,
+                                         inverse_affines, upscale, nullptr, w_edge_out, (char*)workspace, workspace_bytes,
+                                         (cudaStream_t)stream, canvases_u16, wide_out);
   API_END(1)
 }
 

@@ -219,28 +219,32 @@ class RealESRGANer:
             out += [(th, tw, rows[i:i + k]) for i in range(0, len(rows), k)]
         return out
 
-    def _device_path(self, outscale):
-        """enhance / enhance_batch run on the device: the model is this package's 3-channel RRDBNet, no LANCZOS resize."""
+    def _device_path(self, outscale=None):
+        """enhance / enhance_batch run on the device: the model is this package's 3-channel RRDBNet (any ``outscale``)."""
         m = self.model
-        return (isinstance(m, RRDBNet) and m.num_in_ch == 3 and m.num_out_ch == 3 and
-                (outscale is None or outscale == float(self.scale)))
+        return isinstance(m, RRDBNet) and m.num_in_ch == 3 and m.num_out_ch == 3
 
     @torch.no_grad()
-    def enhance_batch(self, images, outscale=None, max_tiles=None):
+    def enhance_batch(self, images, outscale=None, max_tiles=None, lanczos=False):
         """``enhance`` of every image of ``images`` (CUDA uint8 [B,H,W,3] BGR) on the device, as CUDA uint8
-        [B,H*scale,W*scale,3] BGR; each image equals ``enhance(img)[0]`` byte for byte.  The tiles of all images are grouped
+        [B,H*scale,W*scale,3] BGR; each image equals ``enhance(img)[0]`` byte for byte.  With ``lanczos=True`` an ``outscale``
+        other than ``scale`` resizes the network's output to (int(W*outscale), int(H*outscale)) with cv2's INTER_LANCZOS4 on
+        the device (``resize_lanczos4``, realesrgan_utils.py:245-250), one launch for the batch, as ``enhance`` does; without
+        it such an ``outscale`` is refused, so that a caller who sized its buffers for ``scale`` never gets another size.  The tiles of all images are grouped
         by input-window shape (``tile_groups``) and every group runs as forwards of at most ``max_tiles`` tiles (default:
         as many as ``WORKSPACE_BUDGET`` holds) that read the uint8 images and write the uint8 result directly.  Keeps no
         state on ``self``: threads may share one upsampler.
 
-        Raises NotImplementedError for ``outscale`` other than None / ``scale`` (the reference's INTER_LANCZOS4 resize is
-        not built), for images that are not uint8 with 3 channels and for models other than a 3-channel
-        ``codeformer_b200.RRDBNet``; RuntimeError for CPU tensors and for pads not smaller than the dimension they reflect;
+        Raises NotImplementedError for ``outscale`` other than None / ``scale`` without ``lanczos=True``, for images that are
+        not uint8 with 3 channels and for models other than a 3-channel ``codeformer_b200.RRDBNet``; ValueError for an
+        ``outscale`` that is not positive; RuntimeError for CPU tensors and for pads not smaller than the dimension they reflect;
         AssertionError, as RRDBNet.forward, for tiles whose size is not a multiple of the pixel-unshuffle factor."""
-        if outscale is not None and outscale != float(self.scale):
-            raise NotImplementedError(f'RealESRGANer.enhance_batch: outscale {outscale} != scale {self.scale} needs the '
-                                      'reference\'s INTER_LANCZOS4 resize, which is not built')
-        if not self._device_path(None):
+        if outscale is not None and outscale != float(self.scale) and not lanczos:
+            raise NotImplementedError(f'RealESRGANer.enhance_batch: outscale {outscale} != scale {self.scale} changes the output '
+                                      'size; pass lanczos=True for the reference\'s INTER_LANCZOS4 resize')
+        if outscale is not None and not outscale > 0:
+            raise ValueError(f'RealESRGANer.enhance_batch: outscale must be positive, got {outscale}')
+        if not self._device_path():
             raise NotImplementedError('RealESRGANer.enhance_batch: built for a codeformer_b200.RRDBNet with 3 input and 3 output '
                                       f'channels, got {type(self.model).__name__}')
         if not torch.is_tensor(images):
@@ -252,6 +256,12 @@ class RealESRGANer:
                                       f'images go through enhance), got {images.dtype} {tuple(images.shape)}')
         B, H, W, _ = images.shape
         sc = self.scale
+        if outscale is not None and outscale != float(sc):
+            from .pasteback import resize_lanczos4
+            size = (int(W * outscale), int(H * outscale))
+            if B == 0 or H == 0 or W == 0 or size[0] == 0 or size[1] == 0:
+                return torch.empty((B, size[1], size[0], 3), dtype=torch.uint8, device=images.device)
+            return resize_lanczos4(self.enhance_batch(images, max_tiles=max_tiles), size)
         out = torch.empty((B, H * sc, W * sc, 3), dtype=torch.uint8, device=images.device)
         if B == 0 or H == 0 or W == 0:
             return out
@@ -297,12 +307,19 @@ class RealESRGANer:
 
     @torch.no_grad()
     def enhance(self, img, outscale=None, alpha_upsampler='realesrgan'):
-        """The reference's ``enhance``.  uint8 3-channel images with this package's RRDBNet and no LANCZOS resize go through
-        ``enhance_batch`` (the same bytes); every other case through pre_process / tile_process / post_process."""
-        import cv2
-        if img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and self._device_path(outscale):
+        """The reference's ``enhance``.  uint8 3-channel images with this package's RRDBNet go through ``enhance_batch``,
+        the INTER_LANCZOS4 resize of ``outscale != scale`` included (the same bytes); every other case through pre_process /
+        tile_process / post_process and cv2 on the host."""
+        if img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and self._device_path():
             x = torch.from_numpy(np.ascontiguousarray(img)).to(self.device)
-            return self.enhance_batch(x[None])[0].cpu().numpy(), 'RGB'
+            return self.enhance_batch(x[None], outscale=outscale, lanczos=True)[0].cpu().numpy(), 'RGB'
+        return self._enhance_host(img, outscale, alpha_upsampler)
+
+    @torch.no_grad()
+    def _enhance_host(self, img, outscale=None, alpha_upsampler='realesrgan'):
+        """``enhance`` through pre_process / tile_process / post_process with cv2 on the host: every dtype and channel count
+        the reference takes."""
+        import cv2
         h_input, w_input = img.shape[0:2]
         img = img.astype(np.float32)
         max_range = 65535 if np.max(img) > 256 else 255              # :193-199

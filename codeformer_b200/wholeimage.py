@@ -14,7 +14,13 @@ and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of im
   * the paste-back runs once per chunk of images (``cfb_paste_faces_multi``), one read-back of the erosion areas.
 
   * a ``codeformer_b200.RealESRGANer`` background / face upsampler whose scale is ``upscale`` runs once per chunk on the
-    device (``enhance_batch``): the chunk's images, then its restored faces, each as one batch of tiles.
+    device (``enhance_batch``): the chunk's images, then its restored faces, each as one batch of tiles.  With another scale
+    it is called per image / per face through ``enhance(img, outscale=upscale)``, which runs the network and cv2's
+    INTER_LANCZOS4 on the device.  A background whose size is not the output's (``read_image`` enlarged the image, or any
+    other upsampler's result) goes through INTER_LANCZOS4 on the device (``resize_lanczos4``), as the reference's paste does;
+  * gray images (``is_gray``) take the gray branch of ``add_restored_face`` for their own faces: one ``gray_adain_faces``
+    call over the chunk's gray faces, then the float64 paste (``cfb_paste_faces_f64``) over the gray images' canvases after
+    the uint8 paste of the colour images' faces.  A chunk may mix gray and colour images; the colour ones are untouched.
 
 What stays on the host, as in the reference: the NMS and the landmark filter, ``get_center_face``,
 ``cv2.estimateAffinePartial2D(LMEDS)`` (cv2 is imported lazily, as ``align_warp_face`` does), and the ``enhance`` of any
@@ -27,8 +33,8 @@ from . import _lib
 from .detection import RetinaFace, cuda_u8_image
 from .detection import finish_detections as retinaface_finish
 from .upsampler import RealESRGANer
-from .pasteback import (_paste_multi, adjust_inverse_affines, parse_masks, resize_area, resize_linear, resize_linear_factor,
-                        warp_faces_multi)
+from .pasteback import (_paste_multi, adjust_inverse_affines, gray_adain_faces, parse_masks, resize_area, resize_lanczos4,
+                        resize_linear, resize_linear_factor, warp_faces_multi)
 from .yolov5face import YoloDetector, _resize_u8, letterbox_geometry
 from .yolov5face import finish_detections as yolo_finish
 
@@ -150,8 +156,8 @@ def _restore(net, crops, w, max_batch, errors):
 
 
 def _on_device(upsampler, upscale):
-    """The upsampler runs through ``enhance_batch``: this package's RealESRGANer over its RRDBNet, no LANCZOS resize."""
-    return isinstance(upsampler, RealESRGANer) and upsampler._device_path(upscale)
+    """The upsampler runs through ``enhance_batch``: this package's RealESRGANer over its 3-channel RRDBNet at its own scale."""
+    return isinstance(upsampler, RealESRGANer) and upsampler._device_path() and upscale == float(upsampler.scale)
 
 
 def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_center_face=False, detection_resize=640,
@@ -161,10 +167,14 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
     (``init_parsing_model()``) or None for use_parse=False.  ``bg_upsampler`` / ``face_upsampler``: objects with
     ``enhance(img, outscale=upscale)`` (``RealESRGANer``).  A ``codeformer_b200.RealESRGANer`` over ``RRDBNet`` with
     ``scale == upscale`` runs on the device, once per chunk of images for the backgrounds and once for the restored faces
-    (``enhance_batch``); any other upsampler is called per image / per face on the host.
+    (``enhance_batch``); any other upsampler is called per image / per face through ``enhance`` (for this package's
+    RealESRGANer at another scale that call runs the network and the INTER_LANCZOS4 resize on the device).  The float64 faces of gray images always go to ``face_upsampler.enhance`` on the host, one by one, and come back
+    uint8 as in the reference (a face above 256 is 16-bit to ``enhance``: NotImplementedError).
 
     Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
-    also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted.  Each image equals the
+    also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted (float64 for a gray image
+    without a face upsampler, as the reference's ``restored_faces`` holds them).  A gray image whose pasted canvas exceeds
+    256 comes back uint16, as in the reference.  Each image equals the
     reference loop body on that image alone, whatever ``max_batch`` is.  ``self.last_restore_errors`` of the reference's
     fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back."""
     import cv2    # estimateAffinePartial2D(LMEDS) / invertAffineTransform stay on the host, as in the reference
@@ -196,62 +206,90 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
             for landmark in lm:
                 affines.append(cv2.estimateAffinePartial2D(landmark, FACE_TEMPLATE, method=cv2.LMEDS)[0])
                 owner.append(k)
-            if lm and gray[k]:
-                raise NotImplementedError('restore_images: the gray branch of add_restored_face gives float faces; the '
-                                          'paste-back of gray images stays caller-side')
         crops = warp_faces_multi(x, affines, owner, FACE_SIZE)
         with torch.no_grad():
             restored = _restore(net, crops, w, max_batch, errors)
+        owner = np.asarray(owner, np.int64)
+        # add_restored_face: the faces of gray images become adain_npy(bgr2gray(restored), cropped), float64
+        is_g = np.asarray([gray[k] for k in owner], bool)
+        gsel, csel = np.nonzero(is_g)[0], np.nonzero(~is_g)[0]
+        gt, ct = torch.from_numpy(gsel).to(dev), torch.from_numpy(csel).to(dev)
+        gray_faces = gray_adain_faces(restored[gt], crops[gt]) if len(gsel) else None
         S = FACE_SIZE
         if face_upsampler is not None and len(affines):
-            if _on_device(face_upsampler, upscale):
-                restored = face_upsampler.enhance_batch(restored, outscale=upscale)
-            else:
-                host = restored.cpu().numpy()
-                up = [face_upsampler.enhance(f, outscale=upscale)[0] for f in host]
-                restored = torch.from_numpy(np.ascontiguousarray(np.stack(up))).to(dev)
-            S = FACE_SIZE * upscale
-            if restored.shape[1] != S or restored.shape[2] != S:
-                raise RuntimeError(f'restore_images: the face upsampler returned {tuple(restored.shape[1:3])}, expected {S}x{S}')
+            S = int(FACE_SIZE * upscale)
+            up = torch.empty((len(affines), S, S, 3), dtype=torch.uint8, device=dev)
+
+            def host_faces(faces):
+                res = [np.asarray(face_upsampler.enhance(f, outscale=upscale)[0]) for f in faces]
+                if any(r.dtype != np.uint8 for r in res):
+                    raise NotImplementedError('restore_images: the face upsampler returned a 16-bit face (a gray face above 256 '
+                                              'is 16-bit to RealESRGANer.enhance); 16-bit faces are not pasted')
+                if any(r.shape != (S, S, 3) for r in res):
+                    raise RuntimeError(f'restore_images: the face upsampler returned {res[0].shape[:2]}, expected {S}x{S}')
+                return torch.from_numpy(np.ascontiguousarray(np.stack(res))).to(dev)
+            if len(csel):
+                if _on_device(face_upsampler, upscale):
+                    up[ct] = face_upsampler.enhance_batch(restored[ct], outscale=upscale)
+                else:
+                    up[ct] = host_faces(restored[ct].cpu().numpy())
+            if len(gsel):          # enhance takes the float64 faces on the host and returns uint8, as in the reference
+                up[gt] = host_faces(gray_faces.cpu().numpy())
+            restored, gray_faces = up, None
         h_up, w_up = int(h * upscale), int(wd * upscale)
         if bg_upsampler is not None and _on_device(bg_upsampler, upscale):
             canvases = bg_upsampler.enhance_batch(torch.stack([inputs[i][0] for i in idx]), outscale=upscale)
-            if canvases.shape[1:3] != (h_up, w_up):
-                raise NotImplementedError(f'restore_images: the background upsampler returned {tuple(canvases.shape[1:3])}, the '
-                                          f'output is {h_up}x{w_up}; the reference resizes it with INTER_LANCZOS4, which is not built')
         elif bg_upsampler is not None:
             bgs = []
             for i in idx:
                 src = inputs[i][1] if inputs[i][2] else inputs[i][0].cpu().numpy()
                 bg = np.asarray(bg_upsampler.enhance(src, outscale=upscale)[0])
-                if bg.shape[:2] != (h_up, w_up):
-                    raise NotImplementedError(f'restore_images: the background upsampler returned {bg.shape[:2]}, the output '
-                                              f'is {h_up}x{w_up}; the reference resizes it with INTER_LANCZOS4, which is not built')
+                if bg.dtype != np.uint8 or bg.ndim != 3 or bg.shape[2] != 3:
+                    raise NotImplementedError(f'restore_images: the background upsampler returned {bg.dtype} {bg.shape}; only '
+                                              'uint8 BGR backgrounds are pasted')
                 bgs.append(torch.from_numpy(np.ascontiguousarray(bg)))
             canvases = torch.stack(bgs).to(dev)
         else:
             canvases = resize_linear(x, (w_up, h_up))
+        if tuple(canvases.shape[1:3]) != (h_up, w_up):      # paste_faces_to_input_image: INTER_LANCZOS4 to the output size
+            canvases = resize_lanczos4(canvases, (w_up, h_up))
         invs = []
         for a in affines:
             inv = cv2.invertAffineTransform(a)
             inv *= upscale
             invs.append(inv)
         adjust_inverse_affines(invs, upscale, face_upsampler is not None)
-        masks = None
-        if parser is not None and restored.shape[0] > 0:
+
+        def masks_of(faces):
+            if parser is None or faces.shape[0] == 0:
+                return None
             with torch.no_grad():
-                masks = torch.cat([parse_masks(restored[lo:lo + max_batch], parser)
-                                   for lo in range(0, restored.shape[0], max_batch)])
-        out, _ = _paste_multi(canvases, restored, invs, owner, upscale, masks)
-        owner = np.asarray(owner, np.int64)
+                return torch.cat([parse_masks(faces[lo:lo + max_batch], parser) for lo in range(0, faces.shape[0], max_batch)])
+        wide = {}
+        if gray_faces is None:
+            out, _ = _paste_multi(canvases, restored, invs, owner, upscale, masks_of(restored))
+        else:
+            # the uint8 paste for the colour images' faces, then the float64 paste over the gray images' canvases alone
+            out, _ = _paste_multi(canvases, restored[ct], [invs[j] for j in csel], owner[csel], upscale, masks_of(restored[ct]))
+            gk = np.unique(owner[gsel])
+            gkt = torch.from_numpy(gk).to(dev)
+            gw = {}
+            out_g, _ = _paste_multi(out[gkt], gray_faces, [invs[j] for j in gsel], np.searchsorted(gk, owner[gsel]), upscale,
+                                    masks_of(gray_faces), gw)
+            out[gkt] = out_g
+            wide = {int(gk[k]): v for k, v in gw.items()}
         for k, i in enumerate(idx):
             sel = torch.from_numpy(np.nonzero(owner == k)[0]).to(dev)
+            res = wide.get(k, out[k])
+            faces = restored[sel]
+            if gray_faces is not None and gray[k]:
+                faces = gray_faces[torch.from_numpy(np.searchsorted(gsel, np.nonzero(owner == k)[0])).to(dev)]
             if inputs[i][2]:
-                results[i] = out[k].cpu().numpy()
-                crops_out[i], faces_out[i] = crops[sel].cpu().numpy(), restored[sel].cpu().numpy()
+                results[i] = res.cpu().numpy()
+                crops_out[i], faces_out[i] = crops[sel].cpu().numpy(), faces.cpu().numpy()
             else:
-                results[i] = out[k]
-                crops_out[i], faces_out[i] = crops[sel], restored[sel]
+                results[i] = res
+                crops_out[i], faces_out[i] = crops[sel], faces
     restore_images.last_errors = errors
     if return_faces:
         return results, crops_out, faces_out

@@ -422,6 +422,35 @@ int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_
                           int32_t face_size, const uint8_t* parse_masks, const double* inverse_affines, const int32_t* img_index,
                           double upscale, int32_t* w_edge_out, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- whole-image mode: any output scale, and gray images ----
+ * cfb_resize_lanczos4_u8: cv2.resize(src[i], (out_w, out_h), INTER_LANCZOS4) for n images [n,h,w,3], any factors, byte for byte:
+ *   what RealESRGANer.enhance does for outscale != scale (realesrgan_utils.py:245-250) and paste_faces_to_input_image does to
+ *   the upsampled background (face_restoration_helper.py:381).  The tap tables are built on the host per call.
+ * cfb_lanczos4_table: those tables for one axis (host only, no device needed): idx[dst_len] = floor of the source coordinate
+ *   (taps at idx-3 .. idx+4, clamped to the image), coef[dst_len*8] = the weights * 2048 as int16.
+ * cfb_gray_adain_faces: add_restored_face on a gray image (face_restoration_helper.py:364-369): out[i] [S,S,3] float64 =
+ *   adain_npy(bgr2gray(restored[i]), cropped[i]) (facelib/utils/misc.py:169-202), both inputs uint8 [n,S,S,3] BGR.  stats
+ *   (optional, device double [n,4,3]) receives content mean, content std, style mean, style std per channel.  float64, two-pass
+ *   variance, fixed summation order (equal to numpy's up to rounding; the same on every run, whatever n is).
+ * cfb_f64_to_input: cfb_u8_to_input for float64 faces: astype(float32) / 255, BGR -> RGB, (x - 0.5) / 0.5 (:459-461).
+ * cfb_paste_faces_f64: cfb_paste_faces_multi for float64 faces [n,S,S,3] (the restored faces of a gray image): warpAffine as
+ *   cv2 runs it on CV_64F (the fixed-point coordinates, float32 weights, sums in double) and a float64 canvas from the first
+ *   face on.  wide_out (optional, host int32[n_img]) tells which canvases exceed 256, where the reference returns
+ *   astype(np.uint16) (:496-499); canvases_u16 (optional, needs wide_out) receives that cast of every canvas when any does.
+ *   `canvases` always receives astype(np.uint8). */
+int cfb_resize_lanczos4_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
+                           void* stream);
+void cfb_lanczos4_table(int32_t src_len, int32_t dst_len, int32_t* idx, int16_t* coef);
+int cfb_gray_adain_faces(const uint8_t* restored, const uint8_t* cropped, int32_t n, int32_t face_size, double* out, double* stats,
+                         void* stream);
+int cfb_f64_to_input(const double* img_bgr_hwc, float* x_nchw, int32_t n, int32_t hw, void* stream);
+int64_t cfb_paste_faces_f64_workspace_bytes(int32_t n_img, int32_t h_up, int32_t w_up, int32_t n, int32_t face_size,
+                                            int32_t use_parse, const double* inverse_affines);
+int cfb_paste_faces_f64(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_t w_up, const double* faces, int32_t n,
+                        int32_t face_size, const uint8_t* parse_masks, const double* inverse_affines, const int32_t* img_index,
+                        double upscale, uint16_t* canvases_u16, int32_t* wide_out, int32_t* w_edge_out, void* workspace,
+                        int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
