@@ -87,6 +87,8 @@ SIGNATURES = {
     'cfb_parsenet_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32]),
     'cfb_parsenet_forward': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_parse_argmax': (c_int, [_P, _P, _P, c_int32, c_int32, c_int64, _P]),
+    'cfb_parsenet_set_precision': (c_int, [_P, c_int32]),
+    'cfb_parsenet_masks_u8': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_conv2d_gen_workspace_bytes': (c_int64, [c_int32, c_int32]),
     'cfb_conv2d_gen_nhwc': (c_int, [_P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                     c_int32, c_int32, c_int32, _P, c_int32, _P, c_int32, c_float, _P, c_int64, _P]),

@@ -217,6 +217,12 @@ int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w
                           cudaStream_t st);
 int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
                            unsigned char* canvas_bgr_hwc, int out_h, int out_w, int N, int H, int W, cudaStream_t st);
+// ParseNet's ends for cfb_parsenet_masks_u8: the input conv reads uint8 HWC BGR faces [N, H, W, 3] (the value of
+// u8_to_input); the output conv writes the argmax classes and / or the 0/255 face mask, uint8 [N, H, W] (either may be NULL)
+int conv_thin_in_u8_faces(const unsigned char* faces_bgr_hwc, const float* wgt_tck, const float* bias, float* out, int N, int H, int W,
+                          int pad_mode, int out_pitch, int out_c0, cudaStream_t st);
+int conv_thin_out_argmax(const float* in_nhwc64, const float* wgt_tcp, const float* bias, unsigned char* cls, unsigned char* mask,
+                         int N, int H, int W, int Cout, int pad_mode, cudaStream_t st);
 int relayout_thin_out(const float* oihw, float* out, int Cout, cudaStream_t st);
 int fold_bn(const float* w, const float* gamma, const float* beta, const float* mean, const float* var, float eps, float* wout,
             float* bout, int Cout, int per_out, cudaStream_t st);

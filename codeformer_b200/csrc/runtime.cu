@@ -1519,6 +1519,7 @@ struct cfb_parsenet : cfb::NetCore {
   std::vector<cfb::PnBlock> blocks;       // encoder[1:], body, decoder in order
   int n_enc = 0, n_body = 0, n_dec = 0, head_ch = 64;
   float *first_w = nullptr, *first_b = nullptr, *mask_w = nullptr, *mask_b = nullptr, *img_w = nullptr, *img_b = nullptr;
+  int precision = 0;                     // GEN convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
 };
 namespace cfb {
 
@@ -1599,8 +1600,12 @@ static int pn_prepare(cfb_parsenet* n, cudaStream_t st) {
   return 0;
 }
 
+// The uint8 ends of cfb_parsenet_masks_u8: encoder.0 reads the faces, out_mask_conv writes classes / mask; out_img_conv is
+// not run (the caller drops out_img, face_restoration_helper.py:464).
+struct PnU8Io { const unsigned char* faces; unsigned char* cls; unsigned char* mask; };
+
 static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* out_img, int N, int H, int W, void* ws, int64_t ws_bytes,
-                      cudaStream_t st, bool dry) {
+                      cudaStream_t st, bool dry, const PnU8Io* u8 = nullptr) {
   CFB_CHECK(n->begin_forward(dry));
   const int div = 1 << n->n_enc;
   CFB_REQUIRE(H % div == 0 && W % div == 0 && H >= 2 * div && W >= 2 * div, "ParseNet: H and W must be multiples of 2^down_steps");
@@ -1610,7 +1615,12 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
   float* t = nullptr;
   int h = H, w = W, c = 64;
   CFB_CHECK(n->alloc(&t, (size_t)N * h * w * 64));
-  if (!dry) CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, t, N, h, w, 3, 1, 1, 64, 0, st));
+  if (!dry) {
+    if (u8) CFB_CHECK(conv_thin_in_u8_faces(u8->faces, n->first_w, n->first_b, t, N, h, w, 1, 64, 0, st));
+    else CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, t, N, h, w, 3, 1, 1, 64, 0, st));
+  }
+  // every GEN conv runs in the handle's precision; encoder.0 and the heads are the fp32 SIMT thin convs in both
+  auto conv = [&](GenLaunch& g) { g.single_pass = n->precision == 1; return gen_conv(g, n->sm_count, st); };
   float* feat = nullptr;           // encoder output, added back after the body (parsenet.py:190)
   for (size_t i = 0; i < n->blocks.size(); ++i) {
     const PnBlock& b = n->blocks[i];
@@ -1625,13 +1635,13 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
       CFB_CHECK(n->alloc(&s, (size_t)N * ho * wo * b.cout));
       GenLaunch g{&b.sc, t, b.cin, h, w, N, s, b.cout, 0, OUT_NONE};
       g.pad_mode = b.kind == 2 ? 2 : 1; g.sub = b.kind == 1;
-      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+      if (!dry) CFB_CHECK(conv(g));
     }
     CFB_CHECK(n->alloc(&c1, (size_t)N * h1 * w1 * b.cout));
     {
       GenLaunch g{&b.c1, t, b.cin, h, w, N, c1, b.cout, 0, OUT_LRELU};
       g.pad_mode = b.kind == 2 ? 2 : 1;
-      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+      if (!dry) CFB_CHECK(conv(g));
     }
     CFB_CHECK(n->alloc(&o, (size_t)N * ho * wo * b.cout));
     {
@@ -1639,7 +1649,7 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
       g.pad_mode = 1; g.sub = b.kind == 1;
       g.res = b.kind ? s : t; g.res_pitch = b.cout;
       if (last_body) { g.res2 = feat; g.res2_pitch = b.cout; g.post = 1.f; }      // x = feat + body(feat)
-      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+      if (!dry) CFB_CHECK(conv(g));
     }
     ar.release(c1);
     if (s) ar.release(s);
@@ -1650,8 +1660,12 @@ static int pn_forward(cfb_parsenet* n, const float* x, float* out_mask, float* o
   if (n->n_body == 0) feat = nullptr;
   CFB_REQUIRE(c == 64, "ParseNet: head must have 64 channels");
   if (!dry) {
-    CFB_CHECK(conv_thin_out(t, n->mask_w, n->mask_b, out_mask, N, h, w, n->parsing_ch, 1, st));
-    if (out_img) CFB_CHECK(conv_thin_out(t, n->img_w, n->img_b, out_img, N, h, w, 3, 1, st));
+    if (u8) {
+      CFB_CHECK(conv_thin_out_argmax(t, n->mask_w, n->mask_b, u8->cls, u8->mask, N, h, w, n->parsing_ch, 1, st));
+    } else {
+      CFB_CHECK(conv_thin_out(t, n->mask_w, n->mask_b, out_mask, N, h, w, n->parsing_ch, 1, st));
+      if (out_img) CFB_CHECK(conv_thin_out(t, n->img_w, n->img_b, out_img, N, h, w, 3, 1, st));
+    }
   }
   ar.release(t);
   return 0;
@@ -2242,6 +2256,25 @@ int cfb_parsenet_forward(cfb_parsenet* n, const float* x, float* out_mask, float
   CFB_REQUIRE(n && (batch == 0 || (x && out_mask && workspace)), "cfb_parsenet_forward: NULL argument");
   std::lock_guard<std::mutex> lk(n->mu);
   return cfb::pn_forward(n, x, out_mask, out_img, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_parsenet_set_precision(cfb_parsenet* n, int32_t precision) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_parsenet_set_precision: NULL net");
+  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_parsenet_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
+  std::lock_guard<std::mutex> lk(n->mu);
+  n->precision = precision;
+  return 0;
+  API_END(1)
+}
+int cfb_parsenet_masks_u8(cfb_parsenet* n, const uint8_t* faces_bgr, uint8_t* classes, uint8_t* mask, int32_t batch, int32_t h,
+                          int32_t w, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (classes || mask) && (batch == 0 || (faces_bgr && workspace)), "cfb_parsenet_masks_u8: NULL argument");
+  CFB_REQUIRE(batch >= 0 && h > 0 && w > 0, "cfb_parsenet_masks_u8: bad face batch");
+  std::lock_guard<std::mutex> lk(n->mu);
+  const cfb::PnU8Io io{faces_bgr, classes, mask};
+  return cfb::pn_forward(n, nullptr, nullptr, nullptr, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream, false, &io);
   API_END(1)
 }
 int cfb_parse_argmax(const float* logits_nchw, uint8_t* classes, uint8_t* mask, int32_t batch, int32_t channels, int64_t hw, void* stream) {

@@ -1547,6 +1547,15 @@ struct U8TileSrc {
   }
 };
 
+// ParseNet's input read from uint8 HWC BGR faces [N, H, W, 3] (cfb_parsenet_masks_u8): img2tensor(face / 255.) + normalize(0.5,
+// 0.5) of face_restoration_helper.py:458-460, BGR -> RGB, the value cfb_u8_to_input writes (u8_to_model_input).
+struct U8FaceSrc {
+  const unsigned char* img; int H, W;
+  __device__ __forceinline__ float operator()(int n, int c, int y, int x_) const {
+    return u8_to_model_input(__ldg(img + (((int64_t)n * H + y) * W + x_) * 3 + (2 - c)));
+  }
+};
+
 // x [N, Cimg, H*us, W*us] (read through Src) -> out [N, H, W, out_pitch] (channels out_c0 .. out_c0+63), 3x3 pad 1.
 // us > 1: pixel_unshuffle(x, us) first -- channel c*us*us + dy*us + dx of the conv input is x[c][y*us+dy][x*us+dx].
 // weights: [tap][cin][64] (relayout_oihw_to_tck).
@@ -1612,6 +1621,10 @@ int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w
   const U8TileSrc x{img_bgr_hwc, img_h, img_w, img_h + pre_pad, img_w + pre_pad, tiles};
   return launch_thin_in(x, wgt_tck, bias, out, N, H, W, 3, us, 0, out_pitch, out_c0, st);
 }
+int conv_thin_in_u8_faces(const unsigned char* faces_bgr_hwc, const float* wgt_tck, const float* bias, float* out, int N, int H, int W,
+                          int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
+  return launch_thin_in(U8FaceSrc{faces_bgr_hwc, H, W}, wgt_tck, bias, out, N, H, W, 3, 1, pad_mode, out_pitch, out_c0, st);
+}
 
 // Destinations of conv_thin_out: `wants` selects the output pixels to compute, `store` writes one pixel's Cout values.
 struct NchwDst {                 // out [N, Cout, H, W] fp32
@@ -1644,6 +1657,25 @@ struct U8CanvasDst {
     unsigned char* px = canvas + (((int64_t)tab.t[n].img * out_h + Y) * out_w + X) * 3;
 #pragma unroll
     for (int c = 0; c < 3; ++c) px[2 - c] = (unsigned char)rintf(__fmul_rn(fminf(fmaxf(acc[c], 0.f), 1.f), 255.f));
+  }
+};
+
+// ParseNet's logits reduced in registers (cfb_parsenet_masks_u8): out.argmax(dim=1) and the MASK_COLORMAP byte of
+// face_restoration_helper.py:463-468, uint8 [N, H, W] each (either may be NULL).  The comparison and tie rule are
+// parse_argmax_kernel's (first maximum, strict >; a NaN first logit stays class 0), so the bytes equal the unfused chain's.
+struct ArgmaxU8Dst {
+  unsigned char* cls; unsigned char* mask;
+  __device__ __forceinline__ bool wants(int, int, int) const { return true; }
+  template <int CP>
+  __device__ __forceinline__ void store(int n, int oy, int ox, int H, int W, int Cout, const float (&acc)[CP]) const {
+    float best = acc[0];
+    int bi = 0;
+#pragma unroll
+    for (int c = 1; c < CP; ++c)
+      if (c < Cout && acc[c] > best) { best = acc[c]; bi = c; }
+    const int64_t i = ((int64_t)n * H + oy) * W + ox;
+    if (cls) cls[i] = (unsigned char)bi;
+    if (mask) mask[i] = ((bi >= 1 && bi <= 13) || bi == 15) ? 255 : 0;      // MASK_COLORMAP = [0, 255 x13, 0, 255, 0, 0, 0]
   }
 };
 
@@ -1715,6 +1747,21 @@ int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const f
   if (M == 0) return 0;
   const U8CanvasDst dst{canvas_bgr_hwc, out_h, out_w, tiles};
   conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, 3, 0);
+  CFB_LAUNCH_CHECK();
+  return 0;
+}
+int conv_thin_out_argmax(const float* in_nhwc64, const float* wgt_tcp, const float* bias, unsigned char* cls, unsigned char* mask,
+                         int N, int H, int W, int Cout, int pad_mode, cudaStream_t st) {
+  CFB_REQUIRE(Cout >= 1 && Cout <= 20, "conv_thin_out_argmax: at most 20 output channels");
+  const int64_t M = (int64_t)N * H * W;
+  if (M == 0) return 0;
+  // the weights' column padding (relayout_thin_out) picks the instantiation, as in conv_thin_out; both fit the default
+  // 48 KB of dynamic shared memory
+  const ArgmaxU8Dst dst{cls, mask};
+  if (Cout <= 4)
+    conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, Cout, pad_mode);
+  else
+    conv_thin_out_kernel<20><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 20 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, Cout, pad_mode);
   CFB_LAUNCH_CHECK();
   return 0;
 }

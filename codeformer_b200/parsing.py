@@ -112,6 +112,30 @@ class ParseNet(NativeNet):
         super().__init__('parsenet', (in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, int(ch_range[0]), int(ch_range[1])),
                          parsenet_spec(in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, tuple(ch_range)), _parsenet_init)
         self.res_depth, self.parsing_ch = res_depth, parsing_ch
+        self.in_size, self.min_feat_size = in_size, min_feat_size
+        object.__setattr__(self, '_precision', 'fp32')
+
+    PRECISIONS = {'fp32': 0, 'fp16': 1}
+
+    @property
+    def precision(self):
+        """``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core product
+        per k-step, fp32 accumulation and fp32 activations, for the shortcut, conv1 and conv2 of every encoder, body and
+        decoder block.  encoder.0 and the two heads stay fp32 in both."""
+        return self._precision
+
+    def set_precision(self, precision):
+        """Select the conv precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and re-preparation;
+        switching never re-prepares the weights.  Returns the module."""
+        if precision not in self.PRECISIONS:
+            raise ValueError(f"ParseNet.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
+        object.__setattr__(self, '_precision', precision)
+        return self
+
+    def _begin(self, dev):
+        """Under the lock: prepare the native copy and hand the precision on."""
+        self._prepare(dev)
+        _lib.check(_lib.load().cfb_parsenet_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_parsenet_set_precision')
 
     def forward(self, x, return_img=True):
         """x [B,3,H,W] fp32 CUDA -> (out_mask [B,parsing_ch,H,W], out_img [B,3,H,W])  (parsenet.py:188-194)."""
@@ -124,7 +148,7 @@ class ParseNet(NativeNet):
         B, _, H, W = x.shape
         dev = x.device
         with self._lock, torch.cuda.device(dev):
-            self._prepare(dev)
+            self._begin(dev)
             mask = torch.empty((B, self.parsing_ch, H, W), dtype=torch.float32, device=dev)
             img = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev) if return_img else None
             ws = self._workspace(B, H, W, dev)
@@ -132,6 +156,33 @@ class ParseNet(NativeNet):
                                                 ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                        'cfb_parsenet_forward')
         return mask, img
+
+    def masks_u8(self, faces):
+        """The parse step of paste_faces_to_input_image:458-468 straight from uint8 faces: CUDA uint8 [N,H,W,3] BGR ->
+        (classes, mask), CUDA uint8 [N,H,W] each -- byte-equal to ``face_parse_mask(self(x)[0])`` with x the normalised
+        input of the same faces (``cfb_parsenet_masks_u8``: no fp32 input, logits or out_img in between).  H and W must be
+        multiples of 2^down_steps (in_size / min_feat_size) and at least twice that."""
+        if not (torch.is_tensor(faces) and faces.is_cuda):
+            raise RuntimeError('ParseNet.masks_u8: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
+        if faces.dtype != torch.uint8 or faces.dim() != 4 or faces.shape[3] != 3:
+            raise RuntimeError(f'ParseNet.masks_u8: expected uint8 [N,H,W,3] BGR faces, got {faces.dtype} {tuple(faces.shape)}')
+        N, H, W, _ = faces.shape
+        div = 2 ** int(np.log2(self.in_size // min(self.in_size, self.min_feat_size)))
+        if H % div or W % div or H < 2 * div or W < 2 * div:
+            raise RuntimeError(f'ParseNet.masks_u8: H and W must be multiples of {div} and at least {2 * div}, got {H}x{W}')
+        lib = _lib.load()
+        faces = faces.contiguous()
+        dev = faces.device
+        with self._lock, torch.cuda.device(dev):
+            self._begin(dev)
+            cls = torch.empty((N, H, W), dtype=torch.uint8, device=dev)
+            mask = torch.empty((N, H, W), dtype=torch.uint8, device=dev)
+            if N:
+                ws = self._workspace(N, H, W, dev)
+                _lib.check(lib.cfb_parsenet_masks_u8(self._net, _lib.ptr(faces), _lib.ptr(cls), _lib.ptr(mask), N, H, W, _lib.ptr(ws),
+                                                     ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                           'cfb_parsenet_masks_u8')
+        return cls, mask
 
 
 def face_parse_mask(out_mask):

@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .parsing import face_parse_mask
+from .parsing import ParseNet, face_parse_mask
 
 BORDER_MODES = {'constant': 0, 'reflect': 2, 'reflect101': 4}
 PARSE_SIZE = 512
@@ -288,11 +288,19 @@ def adjust_inverse_affines(inverse_affines, upscale, upsampled):
 def parse_masks(restored, face_parse):
     """The parse masks of paste_faces_to_input_image:458-468 for all faces at once: resize to 512 (INTER_LINEAR),
     img2tensor + normalize, ``face_parse(x)[0]``, argmax + MASK_COLORMAP.  -> CUDA uint8 [N,512,512] (0/255).  float64 faces
-    (gray images) are 512 wide -- a face upsampler returns uint8 -- and convert with ``cfb_f64_to_input``."""
+    (gray images) are 512 wide -- a face upsampler returns uint8 -- and convert with ``cfb_f64_to_input``.  uint8 faces and
+    this package's ``ParseNet`` take ``ParseNet.masks_u8`` (same bytes, no fp32 tensor in between); in its fp16 precision
+    the status word is checked after the parse, so an fp16 range overflow raises instead of giving masks."""
     f64 = restored.dtype == torch.float64
     if f64 and restored.shape[1] != PARSE_SIZE:
         raise NotImplementedError(f'parse_masks: float64 faces must be {PARSE_SIZE} wide, got {restored.shape[1]}')
     faces = restored if restored.shape[1] == PARSE_SIZE else resize_linear(restored, (PARSE_SIZE, PARSE_SIZE))
+    if not f64 and isinstance(face_parse, ParseNet):
+        mask = face_parse.masks_u8(faces)[1]
+        if face_parse.precision == 'fp16':
+            torch.cuda.current_stream(faces.device).synchronize()
+            _lib.check(_lib.load().cfb_check_async_status(), 'parse_masks')
+        return mask
     n = faces.shape[0]
     x = torch.empty((n, 3, PARSE_SIZE, PARSE_SIZE), dtype=torch.float32, device=faces.device)
     lib = _lib.load()

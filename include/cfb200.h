@@ -277,6 +277,17 @@ int       cfb_parsenet_forward(cfb_parsenet* net, const float* x, float* out_mas
                                void* workspace, int64_t workspace_bytes, void* stream);
 int       cfb_parse_argmax(const float* logits_nchw, uint8_t* classes, uint8_t* mask, int32_t batch, int32_t channels, int64_t hw,
                            void* stream);
+/* Precision of the GEN convs (shortcut, conv1 and conv2 of every encoder, body and decoder block; encoder.0 and the two heads
+ * stay fp32 in both): 0 = fp32 (default; split fp16 x3 operands, fp32 parity), 1 = fp16 (fp16 operands, one tensor-core
+ * product per k-step, fp32 accumulation and fp32 activations).  Other values are an error.  Takes effect at the next forward;
+ * no re-prepare.  Honoured by cfb_parsenet_forward and cfb_parsenet_masks_u8. */
+int       cfb_parsenet_set_precision(cfb_parsenet* net, int32_t precision);
+/* The parse masks straight from uint8 faces: faces_bgr [batch, h, w, 3] HWC BGR (the value cfb_u8_to_input makes of them)
+ * -> classes and / or mask, uint8 [batch, h, w] (either may be NULL, not both), byte-equal to cfb_u8_to_input +
+ * cfb_parsenet_forward + cfb_parse_argmax.  out_img_conv is not run.  workspace: cfb_parsenet_workspace_bytes(net, batch,
+ * h, w). */
+int       cfb_parsenet_masks_u8(cfb_parsenet* net, const uint8_t* faces_bgr, uint8_t* classes, uint8_t* mask, int32_t batch,
+                                int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* One 3x3 conv of the generalised fused-transform engine (the building block of RRDBNet / ParseNet; test entry point).
  * in: NHWC buffer of in_pitch channels per pixel, channels [0, cin) are read; any h x w.  upsample != 0: nearest x2 first.
