@@ -9,6 +9,8 @@ import ctypes
 import os
 from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libcfb200.so')
 
@@ -187,3 +189,8 @@ def check(status, what=''):
 def ptr(t):
     """Device/host pointer of a torch tensor (None -> NULL)."""
     return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+def stream(device=None):
+    """The current CUDA stream of ``device`` (default: the current device), as the ``void* stream`` argument."""
+    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)

@@ -29,7 +29,7 @@ from torch import nn
 
 from . import _lib
 from . import spec as S
-from .native import upload_params
+from .native import NativeHandle, Precision
 from .registry import ARCH_REGISTRY
 
 
@@ -139,10 +139,6 @@ class _Embedding(_ParamsOnly):
         nn.init.uniform_(self.weight, -1.0 / k, 1.0 / k)          # vqgan_arch.py:31
 
 
-def _stream_ptr(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 def _require_cuda(x, what):
     if not (torch.is_tensor(x) and x.is_cuda):
         raise RuntimeError(f'{what}: codeformer_b200 runs on a CUDA device only (got {getattr(x, "device", type(x))}); '
@@ -181,7 +177,7 @@ class VectorQuantizer(nn.Module):
             ws = torch.empty(int(wsb), dtype=torch.uint8, device=z.device)
             _lib.check(lib.cfb_vq_nearest(_lib.ptr(z), _lib.ptr(E), B, H, W, D, self.codebook_size, float(self.beta),
                                           _lib.ptr(zq), _lib.ptr(idx), _lib.ptr(stats), _lib.ptr(onehot),
-                                          _lib.ptr(ws), wsb, _stream_ptr(z.device)), 'cfb_vq_nearest')
+                                          _lib.ptr(ws), wsb, _lib.stream(z.device)), 'cfb_vq_nearest')
         return zq, stats[0], {'perplexity': stats[1], 'min_encodings': onehot,
                               'min_encoding_indices': idx, 'mean_distance': stats[2]}
 
@@ -197,7 +193,7 @@ class VectorQuantizer(nn.Module):
         sig = (w.data_ptr(), w._version, str(dev))
         if cache.get('sig') != sig:
             prep = torch.empty(int(lib.cfb_vq_prepared_bytes(K, D)), dtype=torch.uint8, device=dev)
-            _lib.check(lib.cfb_vq_prepare(_lib.ptr(E), K, D, _lib.ptr(prep), prep.numel(), _stream_ptr(dev)), 'cfb_vq_prepare')
+            _lib.check(lib.cfb_vq_prepare(_lib.ptr(E), K, D, _lib.ptr(prep), prep.numel(), _lib.stream(dev)), 'cfb_vq_prepare')
             cache.clear()
             cache.update(sig=sig, prep=prep, E=E)
         prep, E = cache['prep'], cache['E']
@@ -217,7 +213,7 @@ class VectorQuantizer(nn.Module):
         onehot = torch.empty((T, K), dtype=torch.float32, device=dev) if return_min_encodings else None
         _lib.check(lib.cfb_vq_nearest_fast(_lib.ptr(z), _lib.ptr(E), _lib.ptr(prep), B, H, W, D, K, float(self.beta),
                                            _lib.ptr(zq), _lib.ptr(idx), _lib.ptr(stats), _lib.ptr(onehot), _lib.ptr(ws),
-                                           ws.numel(), _stream_ptr(dev)), 'cfb_vq_nearest_fast')
+                                           ws.numel(), _lib.stream(dev)), 'cfb_vq_nearest_fast')
         return zq, stats[0], {'perplexity': stats[1], 'min_encodings': onehot, 'min_encoding_indices': idx, 'mean_distance': stats[2]}
 
     def get_codebook_feat(self, indices, shape):
@@ -236,13 +232,18 @@ class VectorQuantizer(nn.Module):
         with torch.cuda.device(idx.device):
             out = torch.empty((B, self.emb_dim, H, W), dtype=torch.float32, device=idx.device)
             _lib.check(lib.cfb_codebook_lookup(_lib.ptr(idx), _lib.ptr(E), B, H, W, self.emb_dim, self.codebook_size,
-                                               _lib.ptr(out), _stream_ptr(idx.device)), 'cfb_codebook_lookup')
+                                               _lib.ptr(out), _lib.stream(idx.device)), 'cfb_codebook_lookup')
         return out.view(B, self.emb_dim) if shape is None else out
 
 
 @ARCH_REGISTRY.register()
-class VQAutoEncoder(nn.Module):
-    """Mirror of ``VQAutoEncoder`` (vqgan_arch.py:326-389), quantizer='nearest'."""
+class VQAutoEncoder(Precision, NativeHandle):
+    """Mirror of ``VQAutoEncoder`` (vqgan_arch.py:326-389), quantizer='nearest'.
+
+    ``set_precision`` selects the precision of the decoder convs -- the generator's and the Fuse_sft_blocks' (not the
+    AttnBlocks', not the last conv).  The encoder, the Transformer and the quantizer are the same in both precisions, so
+    ``logits``, ``lq_feat`` and the code indices are bit-identical; only the decoded image changes.  'fp16' needs the
+    tensor-core engine ('auto' or 'tc'): with ``set_engine('f32')`` the forward raises."""
 
     _KIND = 0
     stream_lanes = 1                  # >1: sub-batches run on separate CUDA streams; the persistent conv CTAs already own every
@@ -252,7 +253,9 @@ class VQAutoEncoder(nn.Module):
     def __init__(self, img_size, nf, ch_mult, quantizer='nearest', res_blocks=2, attn_resolutions=[16],
                  codebook_size=1024, emb_dim=256, beta=0.25, gumbel_straight_through=False, gumbel_kl_weight=1e-8,
                  model_path=None):
-        super().__init__()
+        super().__init__('net')
+        object.__setattr__(self, '_cfb_ws', {})
+        object.__setattr__(self, '_cfb_graphs', {})
         if quantizer != 'nearest':
             raise NotImplementedError("codeformer_b200 builds the 'nearest' quantizer only (the Gumbel quantizer is "
                                       'training-only in the reference, SURVEY.md §2.1)')
@@ -269,7 +272,6 @@ class VQAutoEncoder(nn.Module):
         self.beta = beta
         self.quantize = VectorQuantizer(codebook_size, emb_dim, beta)
         self.generator = _BlockStack(S.generator_plan(nf, ch_mult, res_blocks, img_size, attn_resolutions, emb_dim))
-        self._cfb_init()
         if model_path is not None:                                   # vqgan_arch.py:373-382
             chkpt = torch.load(model_path, map_location='cpu')
             if 'params_ema' in chkpt:
@@ -279,16 +281,7 @@ class VQAutoEncoder(nn.Module):
             else:
                 raise ValueError('Wrong params!')
 
-    # ---- native handle management -------------------------------------------------------------
-    def _cfb_init(self):
-        object.__setattr__(self, '_cfb_lock', threading.Lock())
-        object.__setattr__(self, '_cfb_net', None)
-        object.__setattr__(self, '_cfb_sig', None)
-        object.__setattr__(self, '_cfb_keep', None)
-        object.__setattr__(self, '_cfb_ws', {})
-        object.__setattr__(self, '_cfb_graphs', {})
-        object.__setattr__(self, '_cfb_precision', 'fp32')
-
+    # ---- native handle: what differs from NativeHandle ----------------------------------------------
     def _cfb_config(self) -> '_lib.CfbConfig':
         c = _lib.CfbConfig()
         c.kind = self._KIND
@@ -302,28 +295,20 @@ class VQAutoEncoder(nn.Module):
         c.codebook_size, c.emb_dim, c.beta = self.codebook_size, self.embed_dim, float(self.beta)
         return c
 
-    def _cfb_prepare(self, device):
-        """(Re)build the native weight copies when parameters were loaded, moved or modified; hand the precision on."""
-        lib = _lib.load()
-        params = list(self.state_dict(keep_vars=True).items())
-        sig = tuple((k, v.data_ptr(), v._version, str(v.device)) for k, v in params)
-        if self._cfb_net is None or sig != self._cfb_sig:
-            self._cfb_prepare_weights(lib, params, sig, device)
-        _lib.check(lib.cfb_net_set_precision(self._cfb_net, self.PRECISIONS[self._cfb_precision]), 'cfb_net_set_precision')
+    def _create_args(self):
+        return (ctypes.byref(self._cfb_config()),)
 
-    def _cfb_prepare_weights(self, lib, params, sig, device):
-        if self._cfb_net is None:
-            cfg = self._cfb_config()
-            h = lib.cfb_net_create(ctypes.byref(cfg))
-            if not h:
-                _lib.check(1, 'cfb_net_create')
-            object.__setattr__(self, '_cfb_net', ctypes.c_void_p(h))
-            _lib.check(lib.cfb_net_set_engine(self._cfb_net, getattr(self, '_cfb_engine', 0)), 'cfb_net_set_engine')
-        keep = upload_params(lib, 'net', self._cfb_net, params, device)
-        _lib.check(lib.cfb_net_prepare(self._cfb_net, _stream_ptr(device)), 'cfb_net_prepare')
-        object.__setattr__(self, '_cfb_sig', sig)
-        self._cfb_graphs.clear()                       # captured launch sequences bake in the old weight copies
-        object.__setattr__(self, '_cfb_keep', keep)
+    def _handle(self):
+        if self._net is None:
+            super()._handle()
+            _lib.check(_lib.load().cfb_net_set_engine(self._net, getattr(self, '_cfb_engine', 0)), 'cfb_net_set_engine')
+        return self._net
+
+    def _prepare(self, device):
+        prepared = super()._prepare(device)
+        if prepared:
+            self._cfb_graphs.clear()                   # captured launch sequences bake in the old weight copies
+        return prepared
 
     def _cfb_side_streams(self, device, count):
         pool = self._cfb_ws.setdefault(('streams', device.index), [])
@@ -334,7 +319,7 @@ class VQAutoEncoder(nn.Module):
     def _cfb_workspace(self, device, batch, lane=0):
         lib = _lib.load()
         key = (device.index, torch.cuda.current_stream(device).cuda_stream, lane)
-        need = lib.cfb_workspace_bytes(self._cfb_net, batch)
+        need = lib.cfb_workspace_bytes(self._net, batch)
         if need < 0:
             _lib.check(1, 'cfb_workspace_bytes')
         ws = self._cfb_ws.get(key)
@@ -343,13 +328,6 @@ class VQAutoEncoder(nn.Module):
             ws = torch.empty(int(need), dtype=torch.uint8, device=device)   # owned by the module (the caller may
             self._cfb_ws[key] = ws                                          # empty_cache() after every face)
         return ws
-
-    def __del__(self):
-        try:
-            if getattr(self, '_cfb_net', None) is not None:
-                _lib.load().cfb_net_destroy(self._cfb_net)
-        except Exception:
-            pass
 
     def _check_input(self, x):
         _require_cuda(x, type(self).__name__ + '.forward')
@@ -363,42 +341,23 @@ class VQAutoEncoder(nn.Module):
         code = {'auto': 0, 'f32': 1, 'tc': 2}[engine]
         object.__setattr__(self, '_cfb_engine', code)
         self._cfb_graphs.clear()
-        if self._cfb_net is not None:
-            _lib.check(_lib.load().cfb_net_set_engine(self._cfb_net, code), 'cfb_net_set_engine')
-
-    PRECISIONS = {'fp32': 0, 'fp16': 1}
-
-    @property
-    def precision(self):
-        """Precision of the decoder convs -- the generator's and the Fuse_sft_blocks' (not the AttnBlocks', not the last
-        conv).  ``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core
-        product per k-step, fp32 accumulation and fp32 activations.  The encoder, the Transformer and the quantizer are the
-        same in both, so ``logits``, ``lq_feat`` and the code indices are bit-identical; only the decoded image changes."""
-        return self._cfb_precision
-
-    def set_precision(self, precision):
-        """Select the decoder precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and
-        re-preparation; switching never re-prepares the weights.  'fp16' needs the tensor-core engine ('auto' or 'tc'):
-        with ``set_engine('f32')`` the forward raises.  Returns the module."""
-        if precision not in self.PRECISIONS:
-            raise ValueError(f"{type(self).__name__}.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
-        object.__setattr__(self, '_cfb_precision', precision)
-        return self
+        if self._net is not None:
+            _lib.check(_lib.load().cfb_net_set_engine(self._net, code), 'cfb_net_set_engine')
 
     def capture(self, stage: str, dst: Optional[torch.Tensor]):
         """Parity hook (cfb_net_capture): copy the NHWC activation after ``stage`` into ``dst`` on the next forwards."""
-        if self._cfb_net is None:
+        if self._net is None:
             raise RuntimeError('capture: run one forward (or load weights on the device) first')
         hooks = getattr(self, '_cfb_hooks', set())
         (hooks.add if dst is not None else hooks.discard)(stage)
         object.__setattr__(self, '_cfb_hooks', hooks)
         self._cfb_graphs.clear()                       # hooks add copies to the launch sequence
-        _lib.check(_lib.load().cfb_net_capture(self._cfb_net, stage.encode(), _lib.ptr(dst),
+        _lib.check(_lib.load().cfb_net_capture(self._net, stage.encode(), _lib.ptr(dst),
                                                0 if dst is None else dst.numel()), 'cfb_net_capture')
 
     @property
     def last_launch_count(self) -> int:
-        return 0 if self._cfb_net is None else int(_lib.load().cfb_last_launch_count(self._cfb_net))
+        return 0 if self._net is None else int(_lib.load().cfb_last_launch_count(self._net))
 
     # ---- VQAutoEncoder.forward  vqgan_arch.py:385-389 -------------------------------------------
     def forward(self, x, return_min_encodings=True):
@@ -409,8 +368,8 @@ class VQAutoEncoder(nn.Module):
         lib = _lib.load()
         B = x.shape[0]
         dev = x.device
-        with self._cfb_lock, torch.cuda.device(dev):
-            self._cfb_prepare(dev)
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
             ws = self._cfb_workspace(dev, B)
             out = torch.empty_like(x)
             n_tok = B * (self.resolution >> (len(self.ch_mult) - 1)) ** 2
@@ -418,8 +377,8 @@ class VQAutoEncoder(nn.Module):
             stats = torch.empty(4, dtype=torch.float32, device=dev)
             onehot = torch.empty((n_tok, self.codebook_size), dtype=torch.float32, device=dev) \
                 if return_min_encodings else None
-            _lib.check(lib.cfb_vqae_forward(self._cfb_net, _lib.ptr(x), _lib.ptr(out), _lib.ptr(idx), _lib.ptr(stats),
-                                            _lib.ptr(onehot), B, _lib.ptr(ws), ws.numel(), _stream_ptr(dev)),
+            _lib.check(lib.cfb_vqae_forward(self._net, _lib.ptr(x), _lib.ptr(out), _lib.ptr(idx), _lib.ptr(stats),
+                                            _lib.ptr(onehot), B, _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                        'cfb_vqae_forward')
         return out, stats[0], {'perplexity': stats[1], 'min_encodings': onehot,
                                'min_encoding_indices': idx, 'mean_distance': stats[2]}
@@ -521,13 +480,21 @@ class CodeFormer(VQAutoEncoder):
         lib = _lib.load()
         B = x.shape[0]
         dev = x.device
-        with self._cfb_lock, torch.cuda.device(dev):
-            self._cfb_prepare(dev)
-            if 0 < B <= self.cuda_graph_max_batch and os.environ.get('CFB_CUDA_GRAPH', '1') != '0' \
-                    and not getattr(self, '_cfb_hooks', None) and not torch.cuda.is_current_stream_capturing():
-                res = self._cfb_forward_graphed(x, float(w), bool(adain), bool(code_only))
-                if res is not None:
-                    return res
+        w, adain, code_only = float(w), bool(adain), bool(code_only)
+
+        def launch(src, logits, lq_feat, out, ws):
+            _lib.check(lib.cfb_codeformer_forward(self._net, _lib.ptr(src), _lib.ptr(out), _lib.ptr(logits), _lib.ptr(lq_feat), None,
+                                                  src.shape[0], w, int(adain), int(code_only), _lib.ptr(ws), ws.numel(),
+                                                  _lib.stream(dev)), 'cfb_codeformer_forward')
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            bufs = self._graphed((dev.index, B, w, adain, code_only, self._precision), x, lambda: (
+                torch.empty_like(x), torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev),
+                torch.empty((B, 256, 16, 16), dtype=torch.float32, device=dev), None if code_only else torch.empty_like(x),
+                torch.empty(int(lib.cfb_workspace_bytes(self._net, B)), dtype=torch.uint8, device=dev)), launch)
+            if bufs is not None:
+                _, logits, lq, out, _ = bufs
+                return (logits.clone(), lq.clone()) if code_only else (out.clone(), logits.clone(), lq.clone())
             logits = torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev)
             lq_feat = torch.empty((B, 256, 16, 16), dtype=torch.float32, device=dev)
             out = None if code_only else torch.empty_like(x)
@@ -546,12 +513,8 @@ class CodeFormer(VQAutoEncoder):
                 if li > 0:
                     st.wait_stream(cur)                       # inputs / weights produced on the caller's stream
                 with torch.cuda.stream(st):
-                    ws = self._cfb_workspace(dev, hi - lo, lane=li)
-                    _lib.check(lib.cfb_codeformer_forward(
-                        self._cfb_net, _lib.ptr(x[lo:hi]), None if out is None else _lib.ptr(out[lo:hi]),
-                        _lib.ptr(logits[lo:hi]), _lib.ptr(lq_feat[lo:hi]), None, hi - lo, float(w), int(bool(adain)),
-                        int(bool(code_only)), _lib.ptr(ws), ws.numel(), ctypes.c_void_p(st.cuda_stream)),
-                        'cfb_codeformer_forward')
+                    launch(x[lo:hi], logits[lo:hi], lq_feat[lo:hi], None if out is None else out[lo:hi],
+                           self._cfb_workspace(dev, hi - lo, lane=li))
             for li in range(1, lanes):
                 cur.wait_stream(side[li - 1])                 # results are ordered on the caller's stream again
         if code_only:
@@ -564,45 +527,36 @@ class CodeFormer(VQAutoEncoder):
     cuda_graph_max_batch = 4
     cuda_graph_cache_size = 6
 
-    def _cfb_forward_graphed(self, x, w, adain, code_only):
-        lib = _lib.load()
-        dev = x.device
-        B = x.shape[0]
-        key = (dev.index, B, w, adain, code_only, self._cfb_precision)      # the launch sequence depends on the precision
+    def _graphed(self, key, x, buffers, launch):
+        """``launch(*bufs)`` replayed from the CUDA graph cached under ``key`` (the key holds the precision: the launch
+        sequence depends on it).  On a miss ``buffers()`` makes the static buffers, the first of which is the input, and the
+        graph is captured.  ``x`` is copied into the input before every run.  Returns the buffers after the replay (the
+        caller clones what it returns), or None where the plain launch path runs instead."""
+        if not 0 < x.shape[0] <= self.cuda_graph_max_batch or os.environ.get('CFB_CUDA_GRAPH', '1') == '0' \
+                or getattr(self, '_cfb_hooks', None) or torch.cuda.is_current_stream_capturing():
+            return None
         ent = self._cfb_graphs.pop(key, None)              # re-inserted below: dict order = least recently used first
         if ent is None:
             while len(self._cfb_graphs) >= self.cuda_graph_cache_size:      # callers sweep w (Gradio slider): evict the LRU
                 self._cfb_graphs.pop(next(iter(self._cfb_graphs)))          # entry only; each pins one workspace
-            sx = torch.empty_like(x)
-            logits = torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev)
-            lq = torch.empty((B, 256, 16, 16), dtype=torch.float32, device=dev)
-            out = None if code_only else torch.empty_like(x)
-            ws = torch.empty(int(lib.cfb_workspace_bytes(self._cfb_net, B)), dtype=torch.uint8, device=dev)
-
-            def launch():
-                _lib.check(lib.cfb_codeformer_forward(self._cfb_net, _lib.ptr(sx), _lib.ptr(out), _lib.ptr(logits), _lib.ptr(lq),
-                                                      None, B, w, int(adain), int(code_only), _lib.ptr(ws), ws.numel(),
-                                                      _stream_ptr(dev)), 'cfb_codeformer_forward')
-            sx.copy_(x)
-            launch()                                         # eager warm-up: one-time function attributes, lazy module load
-            torch.cuda.current_stream(dev).synchronize()
+            bufs = buffers()
+            bufs[0].copy_(x)
+            launch(*bufs)                                    # eager warm-up: one-time function attributes, lazy module load
+            torch.cuda.current_stream(x.device).synchronize()
             g = torch.cuda.CUDAGraph()
             try:
                 with torch.cuda.graph(g):
-                    launch()
+                    launch(*bufs)
+                ent = (g, bufs)
             except Exception:                                # capture not possible here: keep the plain launch path
-                self._cfb_graphs[key] = False
-                return None
-            ent = (g, sx, out, logits, lq, ws)
+                ent = False
         self._cfb_graphs[key] = ent
         if ent is False:
             return None
-        g, sx, out, logits, lq, ws = ent
-        sx.copy_(x)
+        g, bufs = ent
+        bufs[0].copy_(x)
         g.replay()
-        if code_only:
-            return logits.clone(), lq.clone()
-        return out.clone(), logits.clone(), lq.clone()
+        return bufs
 
     # ---- SURVEY.md section 8 rows f1 / f2: the caller's plumbing and per-face loop ----------------------------------
     def forward_u8(self, faces_bgr, w=0.5, adain=True):
@@ -618,41 +572,20 @@ class CodeFormer(VQAutoEncoder):
         faces_bgr = faces_bgr.contiguous()
         B, dev = faces_bgr.shape[0], faces_bgr.device
         w, adain = float(w), bool(adain)
-        with self._cfb_lock, torch.cuda.device(dev):
-            self._cfb_prepare(dev)
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
             if B == 0:
                 return torch.empty_like(faces_bgr)
 
             def launch(src, dst, ws):
-                _lib.check(lib.cfb_codeformer_forward_u8(self._cfb_net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w,
-                                                         int(adain), _lib.ptr(ws), ws.numel(), _stream_ptr(dev)),
+                _lib.check(lib.cfb_codeformer_forward_u8(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w,
+                                                         int(adain), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                            'cfb_codeformer_forward_u8')
-            graph_ok = B <= self.cuda_graph_max_batch and os.environ.get('CFB_CUDA_GRAPH', '1') != '0' \
-                and not getattr(self, '_cfb_hooks', None) and not torch.cuda.is_current_stream_capturing()
-            if graph_ok:
-                key = ('u8', dev.index, B, w, adain, self._cfb_precision)
-                ent = self._cfb_graphs.pop(key, None)
-                if ent is None:
-                    while len(self._cfb_graphs) >= self.cuda_graph_cache_size:
-                        self._cfb_graphs.pop(next(iter(self._cfb_graphs)))
-                    src, dst = torch.empty_like(faces_bgr), torch.empty_like(faces_bgr)
-                    ws = torch.empty(int(lib.cfb_workspace_bytes(self._cfb_net, B)), dtype=torch.uint8, device=dev)
-                    src.copy_(faces_bgr)
-                    launch(src, dst, ws)                          # eager warm-up before capture
-                    torch.cuda.current_stream(dev).synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    try:
-                        with torch.cuda.graph(g):
-                            launch(src, dst, ws)
-                        ent = (g, src, dst, ws)
-                    except Exception:
-                        ent = False
-                self._cfb_graphs[key] = ent
-                if ent:
-                    g, src, dst, _ = ent
-                    src.copy_(faces_bgr)
-                    g.replay()
-                    return dst.clone()
+            bufs = self._graphed(('u8', dev.index, B, w, adain, self._precision), faces_bgr, lambda: (
+                torch.empty_like(faces_bgr), torch.empty_like(faces_bgr),
+                torch.empty(int(lib.cfb_workspace_bytes(self._net, B)), dtype=torch.uint8, device=dev)), launch)
+            if bufs is not None:
+                return bufs[1].clone()
             out = torch.empty_like(faces_bgr)
             launch(faces_bgr, out, self._cfb_workspace(dev, B))
         return out
@@ -739,10 +672,10 @@ class CodeFormer(VQAutoEncoder):
         dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         x_host = x_host.contiguous()
         B = x_host.shape[0]
-        with self._cfb_lock, torch.cuda.device(dev):
-            self._cfb_prepare(dev)
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
             ws = self._cfb_workspace(dev, B)
-            iob = lib.cfb_host_io_bytes(self._cfb_net, B)
+            iob = lib.cfb_host_io_bytes(self._net, B)
             key = ('io', dev.index)
             io = self._cfb_ws.get(key)
             if io is None or io.numel() < iob:
@@ -751,8 +684,8 @@ class CodeFormer(VQAutoEncoder):
             out = torch.empty(x_host.shape, dtype=torch.float32, pin_memory=True)
             logits = torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, pin_memory=True)
             lq = torch.empty((B, 256, 16, 16), dtype=torch.float32, pin_memory=True)
-            _lib.check(lib.cfb_codeformer_forward_host(self._cfb_net, _lib.ptr(x_host), _lib.ptr(out), _lib.ptr(logits),
+            _lib.check(lib.cfb_codeformer_forward_host(self._net, _lib.ptr(x_host), _lib.ptr(out), _lib.ptr(logits),
                                                        _lib.ptr(lq), B, float(w), int(bool(adain)), _lib.ptr(io),
-                                                       io.numel(), _lib.ptr(ws), ws.numel(), _stream_ptr(dev)),
+                                                       io.numel(), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                        'cfb_codeformer_forward_host')
         return out, logits, lq

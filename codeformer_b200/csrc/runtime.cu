@@ -141,8 +141,8 @@ class Arena {
 
 // ---- what every network handle shares ----------------------------------------------------------------
 // The parameters the caller registered (device pointers it keeps alive), the slab with the prepared weights on the device
-// that was current at prepare time, and the workspace arena.  `label` names the network in error messages, `api` is the
-// infix of its C functions (cfb_<api>_prepare, ...).
+// that was current at prepare time, the workspace arena and the conv precision.  `label` names the network in error
+// messages, `api` is the infix of its C functions (cfb_<api>_prepare, ...).
 struct NetCore {
   std::mutex mu;
   std::unordered_map<std::string, std::pair<const float*, int64_t>> raw;
@@ -151,6 +151,7 @@ struct NetCore {
   int device = -1;                    // CUDA device the slab / prepared weights live on
   int sm_count = 148;
   bool prepared = false;
+  int precision = 0;                  // of the convs each forward names: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
   Arena arena;
   const char* label;
   const char* api;
@@ -162,6 +163,15 @@ struct NetCore {
     std::lock_guard<std::mutex> lk(mu);
     raw[name] = {dev_ptr, numel};
     prepared = false;
+    return 0;
+  }
+
+  // cfb_<api>_set_precision: host state only, read by the next forward
+  int set_precision(int32_t precision) {
+    CFB_REQUIRE(precision == 0 || precision == 1,
+                "cfb_" + std::string(api) + "_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
+    std::lock_guard<std::mutex> lk(mu);
+    this->precision = precision;
     return 0;
   }
 
@@ -303,7 +313,6 @@ struct cfb_net : cfb::NetCore {
   int gn_ctr_pos = 0;
   std::map<int, int64_t> ws_memo;     // batch -> cfb_workspace_bytes (16 host-side dry runs per miss)
   int engine = 0;                     // 0 auto (wgmma where the shape allows), 1 fp32 CUDA cores, 2 wgmma only
-  int precision = 0;                  // generator + fusion convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
   std::map<std::string, std::pair<float*, int64_t>> captures;   // stage name -> (device dst, capacity in floats)
 };
 
@@ -1275,7 +1284,6 @@ struct cfb_rrdb : cfb::NetCore {
   std::vector<cfb::GenConv> convs;      // [blocks*15] dense convs, then conv_body, conv_up1, conv_up2, conv_hr
   float* first_w = nullptr; float* first_b = nullptr;   // conv_first  [tap][cin][64]
   float* last_w = nullptr; float* last_b = nullptr;     // conv_last   [tap][64][4]
-  int precision = 0;                                    // GEN convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
 };
 
 namespace cfb {
@@ -1519,7 +1527,6 @@ struct cfb_parsenet : cfb::NetCore {
   std::vector<cfb::PnBlock> blocks;       // encoder[1:], body, decoder in order
   int n_enc = 0, n_body = 0, n_dec = 0, head_ch = 64;
   float *first_w = nullptr, *first_b = nullptr, *mask_w = nullptr, *mask_b = nullptr, *img_w = nullptr, *img_b = nullptr;
-  int precision = 0;                     // GEN convs: 0 split fp16 x3 (fp32 parity), 1 single-pass fp16
 };
 namespace cfb {
 
@@ -2189,10 +2196,7 @@ int cfb_rrdb_prepare(cfb_rrdb* n, void* stream) {
 int cfb_rrdb_set_precision(cfb_rrdb* n, int32_t precision) {
   API_BEGIN
   CFB_REQUIRE(n, "cfb_rrdb_set_precision: NULL net");
-  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_rrdb_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->precision = precision;
-  return 0;
+  return n->set_precision(precision);
   API_END(1)
 }
 int64_t cfb_rrdb_workspace_bytes(cfb_rrdb* n, int32_t batch, int32_t h, int32_t w) {
@@ -2261,10 +2265,7 @@ int cfb_parsenet_forward(cfb_parsenet* n, const float* x, float* out_mask, float
 int cfb_parsenet_set_precision(cfb_parsenet* n, int32_t precision) {
   API_BEGIN
   CFB_REQUIRE(n, "cfb_parsenet_set_precision: NULL net");
-  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_parsenet_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->precision = precision;
-  return 0;
+  return n->set_precision(precision);
   API_END(1)
 }
 int cfb_parsenet_masks_u8(cfb_parsenet* n, const uint8_t* faces_bgr, uint8_t* classes, uint8_t* mask, int32_t batch, int32_t h,
@@ -2598,10 +2599,7 @@ int cfb_net_set_engine(cfb_net* n, int32_t engine) {
 int cfb_net_set_precision(cfb_net* n, int32_t precision) {
   API_BEGIN
   CFB_REQUIRE(n, "cfb_net_set_precision: NULL net");
-  CFB_REQUIRE(precision == 0 || precision == 1, "cfb_net_set_precision: precision must be 0 (fp32, split) or 1 (fp16)");
-  std::lock_guard<std::mutex> lk(n->mu);
-  n->precision = precision;
-  return 0;
+  return n->set_precision(precision);
   API_END(1)
 }
 

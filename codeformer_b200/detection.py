@@ -8,7 +8,6 @@ BatchNorm buffers, so ``detection_Resnet50_Final.pth`` loads strictly), same ``f
 (``cfb_retinaface_*``); one small device-to-host copy brings back the candidates, and the sort and the NMS run on the host
 as in the reference.  No CPU fallback; inference only.  The package imports neither torchvision nor cv2.
 """
-import ctypes
 from collections import OrderedDict
 
 import numpy as np
@@ -195,7 +194,7 @@ class RetinaFace(NativeNet):
             ws = self._workspace(B, H, W, dev)
             fn = lib.cfb_retinaface_forward_u8 if u8 else lib.cfb_retinaface_forward
             _lib.check(fn(self._net, _lib.ptr(x), _lib.ptr(loc), _lib.ptr(conf), _lib.ptr(landms), B, H, W, _lib.ptr(ws),
-                          ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'cfb_retinaface_forward')
+                          ws.numel(), _lib.stream(dev)), 'cfb_retinaface_forward')
         return loc, conf, landms
 
     def forward(self, inputs):
@@ -228,8 +227,7 @@ class RetinaFace(NativeNet):
             counts = torch.empty((B,), dtype=torch.int32, device=dev)
             _lib.check(lib.cfb_retinaface_candidates(_lib.ptr(loc.contiguous()), _lib.ptr(conf.contiguous()), _lib.ptr(landms.contiguous()),
                                                      B, h, w, float(conf_threshold), _lib.ptr(rows), _lib.ptr(counts),
-                                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                       'cfb_retinaface_candidates')
+                                                     _lib.stream(dev)), 'cfb_retinaface_candidates')
             n = counts.cpu().tolist()
         return [rows[b, :n[b]] for b in range(B)]
 

@@ -8,14 +8,12 @@ constructor, same ``state_dict`` (238 entries incl. the BatchNorm buffers -- a r
 the conv weights when the native copy is prepared.  ``face_parse_mask`` is the caller's step right after the network
 (argmax over the 19 classes + MASK_COLORMAP) on the device.  No CPU fallback; inference only (BatchNorm uses running stats).
 """
-import ctypes
-
 import numpy as np
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .native import NativeNet
+from .native import NativeNet, Precision
 
 
 def parsenet_plan(in_size=512, out_size=512, min_feat_size=32, base_ch=64, res_depth=10, ch_range=(32, 256)):
@@ -102,8 +100,10 @@ def _parsenet_init(name, entry, g):
     return nn.Parameter(torch.ones(shape) if name.endswith('norm.weight') else torch.zeros(shape))
 
 
-class ParseNet(NativeNet):
-    """Parameter holder with the reference's ``state_dict`` + ``forward`` on the wgmma conv engine."""
+class ParseNet(Precision, NativeNet):
+    """Parameter holder with the reference's ``state_dict`` + ``forward`` on the wgmma conv engine.  ``set_precision('fp16')``
+    covers the shortcut, conv1 and conv2 of every encoder, body and decoder block; encoder.0 and the two heads stay fp32 in
+    both precisions."""
 
     def __init__(self, in_size=128, out_size=128, min_feat_size=32, base_ch=64, parsing_ch=19, res_depth=10,
                  relu_type='LeakyReLU', norm_type='bn', ch_range=[32, 256]):
@@ -113,29 +113,6 @@ class ParseNet(NativeNet):
                          parsenet_spec(in_size, out_size, min_feat_size, base_ch, parsing_ch, res_depth, tuple(ch_range)), _parsenet_init)
         self.res_depth, self.parsing_ch = res_depth, parsing_ch
         self.in_size, self.min_feat_size = in_size, min_feat_size
-        object.__setattr__(self, '_precision', 'fp32')
-
-    PRECISIONS = {'fp32': 0, 'fp16': 1}
-
-    @property
-    def precision(self):
-        """``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core product
-        per k-step, fp32 accumulation and fp32 activations, for the shortcut, conv1 and conv2 of every encoder, body and
-        decoder block.  encoder.0 and the two heads stay fp32 in both."""
-        return self._precision
-
-    def set_precision(self, precision):
-        """Select the conv precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and re-preparation;
-        switching never re-prepares the weights.  Returns the module."""
-        if precision not in self.PRECISIONS:
-            raise ValueError(f"ParseNet.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
-        object.__setattr__(self, '_precision', precision)
-        return self
-
-    def _begin(self, dev):
-        """Under the lock: prepare the native copy and hand the precision on."""
-        self._prepare(dev)
-        _lib.check(_lib.load().cfb_parsenet_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_parsenet_set_precision')
 
     def forward(self, x, return_img=True):
         """x [B,3,H,W] fp32 CUDA -> (out_mask [B,parsing_ch,H,W], out_img [B,3,H,W])  (parsenet.py:188-194)."""
@@ -148,13 +125,12 @@ class ParseNet(NativeNet):
         B, _, H, W = x.shape
         dev = x.device
         with self._lock, torch.cuda.device(dev):
-            self._begin(dev)
+            self._prepare(dev)
             mask = torch.empty((B, self.parsing_ch, H, W), dtype=torch.float32, device=dev)
             img = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev) if return_img else None
             ws = self._workspace(B, H, W, dev)
             _lib.check(lib.cfb_parsenet_forward(self._net, _lib.ptr(x), _lib.ptr(mask), _lib.ptr(img), B, H, W, _lib.ptr(ws),
-                                                ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                       'cfb_parsenet_forward')
+                                                ws.numel(), _lib.stream(dev)), 'cfb_parsenet_forward')
         return mask, img
 
     def masks_u8(self, faces):
@@ -174,14 +150,13 @@ class ParseNet(NativeNet):
         faces = faces.contiguous()
         dev = faces.device
         with self._lock, torch.cuda.device(dev):
-            self._begin(dev)
+            self._prepare(dev)
             cls = torch.empty((N, H, W), dtype=torch.uint8, device=dev)
             mask = torch.empty((N, H, W), dtype=torch.uint8, device=dev)
             if N:
                 ws = self._workspace(N, H, W, dev)
                 _lib.check(lib.cfb_parsenet_masks_u8(self._net, _lib.ptr(faces), _lib.ptr(cls), _lib.ptr(mask), N, H, W, _lib.ptr(ws),
-                                                     ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                           'cfb_parsenet_masks_u8')
+                                                     ws.numel(), _lib.stream(dev)), 'cfb_parsenet_masks_u8')
         return cls, mask
 
 
@@ -197,7 +172,7 @@ def face_parse_mask(out_mask):
         cls = torch.empty((B, H, W), dtype=torch.uint8, device=out_mask.device)
         mask = torch.empty((B, H, W), dtype=torch.uint8, device=out_mask.device)
         _lib.check(lib.cfb_parse_argmax(_lib.ptr(out_mask), _lib.ptr(cls), _lib.ptr(mask), B, C, H * W,
-                                        ctypes.c_void_p(torch.cuda.current_stream(out_mask.device).cuda_stream)), 'cfb_parse_argmax')
+                                        _lib.stream(out_mask.device)), 'cfb_parse_argmax')
     return cls, mask
 
 

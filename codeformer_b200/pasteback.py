@@ -37,10 +37,6 @@ def invert_affine(M):
     return np.array([[A11, A12, -A11 * M[0, 2] - A12 * M[1, 2]], [A21, A22, -A21 * M[0, 2] - A22 * M[1, 2]]], np.float64)
 
 
-def _stream(dev):
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _check_image(x, name, ndim=3):
     if not torch.is_tensor(x) or not x.is_cuda:
         raise RuntimeError(f'{name}: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
@@ -72,7 +68,7 @@ def warp_faces(img, affines, face_size=512, border_mode='constant', border_value
     with torch.cuda.device(img.device):
         _lib.check(_lib.load().cfb_warp_affine_u8(_lib.ptr(img), h, w, m.ctypes.data_as(ctypes.c_void_p), n, _lib.ptr(out),
                                                   face_size, face_size, BORDER_MODES[border_mode], bv[0], bv[1], bv[2],
-                                                  _stream(img.device)), 'cfb_warp_affine_u8')
+                                                  _lib.stream(img.device)), 'cfb_warp_affine_u8')
     return out
 
 
@@ -84,7 +80,7 @@ def resize_linear(img, size):
     n, h, w = x.shape[:3]
     out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint8, device=img.device)
     with torch.cuda.device(img.device):
-        _lib.check(_lib.load().cfb_resize_linear_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _stream(img.device)),
+        _lib.check(_lib.load().cfb_resize_linear_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _lib.stream(img.device)),
                    'cfb_resize_linear_u8')
     return out if batched else out[0]
 
@@ -100,7 +96,7 @@ def resize_area(img, size):
         raise NotImplementedError(f'resize_area shrinks only ({w}x{h} -> {size[0]}x{size[1]}); use resize_linear to enlarge')
     out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint8, device=img.device)
     with torch.cuda.device(img.device):
-        _lib.check(_lib.load().cfb_resize_area_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _stream(img.device)),
+        _lib.check(_lib.load().cfb_resize_area_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _lib.stream(img.device)),
                    'cfb_resize_area_u8')
     return out if batched else out[0]
 
@@ -114,7 +110,7 @@ def resize_lanczos4(img, size):
     n, h, w = x.shape[:3]
     out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint8, device=img.device)
     with torch.cuda.device(img.device):
-        _lib.check(_lib.load().cfb_resize_lanczos4_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _stream(img.device)),
+        _lib.check(_lib.load().cfb_resize_lanczos4_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _lib.stream(img.device)),
                    'cfb_resize_lanczos4_u8')
     return out if batched else out[0]
 
@@ -136,7 +132,7 @@ def gray_adain_faces(restored, cropped, with_stats=False):
     stats = torch.empty((n, 4, 3), dtype=torch.float64, device=restored.device)
     with torch.cuda.device(restored.device):
         _lib.check(_lib.load().cfb_gray_adain_faces(_lib.ptr(restored), _lib.ptr(cropped), n, S, _lib.ptr(out), _lib.ptr(stats),
-                                                    _stream(restored.device)), 'cfb_gray_adain_faces')
+                                                    _lib.stream(restored.device)), 'cfb_gray_adain_faces')
     return (out, stats) if with_stats else out
 
 
@@ -170,7 +166,7 @@ def resize_linear_factor(img, f):
     out = torch.empty((n, oh, ow, 3), dtype=torch.uint8, device=img.device)
     with torch.cuda.device(img.device):
         _lib.check(_lib.load().cfb_resize_linear_scale_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), oh, ow, float(f), float(f),
-                                                          _stream(img.device)), 'cfb_resize_linear_scale_u8')
+                                                          _lib.stream(img.device)), 'cfb_resize_linear_scale_u8')
     return out if batched else out[0]
 
 
@@ -199,7 +195,7 @@ def warp_faces_multi(imgs, affines, img_index, face_size=512, border_mode='const
         _lib.check(_lib.load().cfb_warp_affine_multi_u8(_lib.ptr(imgs), B, h, w, m.ctypes.data_as(ctypes.c_void_p),
                                                         idx.ctypes.data_as(ctypes.c_void_p), n, _lib.ptr(out), face_size,
                                                         face_size, BORDER_MODES[border_mode], bv[0], bv[1], bv[2],
-                                                        _stream(imgs.device)), 'cfb_warp_affine_multi_u8')
+                                                        _lib.stream(imgs.device)), 'cfb_warp_affine_multi_u8')
     return out
 
 
@@ -237,14 +233,14 @@ def _paste_multi(canvases, restored, inverse_affines, img_index, upscale, masks,
             _lib.check(lib.cfb_paste_faces_f64(_lib.ptr(canvases), B, h_up, w_up, _lib.ptr(restored), n, S, _lib.ptr(masks), mp,
                                                idx.ctypes.data_as(ctypes.c_void_p), float(upscale), _lib.ptr(u16),
                                                is_wide.ctypes.data_as(ctypes.c_void_p), w_edge.ctypes.data_as(ctypes.c_void_p),
-                                               _lib.ptr(ws), ws.numel(), _stream(dev)), 'cfb_paste_faces_f64')
+                                               _lib.ptr(ws), ws.numel(), _lib.stream(dev)), 'cfb_paste_faces_f64')
         if wide is not None:
             wide.update({int(k): u16[k] for k in np.nonzero(is_wide)[0]})
         return canvases, w_edge[:n]
     with torch.cuda.device(dev):
         _lib.check(lib.cfb_paste_faces_multi(_lib.ptr(canvases), B, h_up, w_up, _lib.ptr(restored), n, S, _lib.ptr(masks), mp,
                                              idx.ctypes.data_as(ctypes.c_void_p), float(upscale),
-                                             w_edge.ctypes.data_as(ctypes.c_void_p), _lib.ptr(ws), ws.numel(), _stream(dev)),
+                                             w_edge.ctypes.data_as(ctypes.c_void_p), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                    'cfb_paste_faces_multi')
     return canvases, w_edge[:n]
 
@@ -306,7 +302,7 @@ def parse_masks(restored, face_parse):
     lib = _lib.load()
     with torch.cuda.device(faces.device):
         _lib.check((lib.cfb_f64_to_input if f64 else lib.cfb_u8_to_input)(_lib.ptr(faces.contiguous()), _lib.ptr(x), n,
-                                                                         PARSE_SIZE * PARSE_SIZE, _stream(faces.device)),
+                                                                         PARSE_SIZE * PARSE_SIZE, _lib.stream(faces.device)),
                    'cfb_f64_to_input' if f64 else 'cfb_u8_to_input')
     with torch.no_grad():
         logits = face_parse(x)[0]
@@ -346,7 +342,7 @@ def _paste(img, restored, inverse_affines, upscale, face_size, masks, upsample_i
     with torch.cuda.device(dev):
         _lib.check(lib.cfb_paste_faces(_lib.ptr(canvas), h_up, w_up, _lib.ptr(restored), n, S, _lib.ptr(masks),
                                        m.ctypes.data_as(ctypes.c_void_p), float(upscale), _lib.ptr(dbg),
-                                       w_edge.ctypes.data_as(ctypes.c_void_p), _lib.ptr(ws), ws.numel(), _stream(dev)),
+                                       w_edge.ctypes.data_as(ctypes.c_void_p), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                    'cfb_paste_faces')
     return (canvas, w_edge[:n], dbg) if debug else (canvas, w_edge[:n])
 

@@ -19,7 +19,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import spec as S
-from .native import NativeNet
+from .native import NativeNet, Precision
 from .registry import ARCH_REGISTRY
 
 
@@ -32,8 +32,10 @@ def _rrdbnet_init(name, shape, g):
 
 
 @ARCH_REGISTRY.register()
-class RRDBNet(NativeNet):
-    """Parameters of the reference's RRDBNet (identical ``state_dict``) with ``forward`` on the wgmma conv engine."""
+class RRDBNet(Precision, NativeNet):
+    """Parameters of the reference's RRDBNet (identical ``state_dict``) with ``forward`` on the wgmma conv engine.
+    ``set_precision('fp16')`` is what the reference computes with ``half=True``; conv_first and conv_last stay fp32 in both
+    precisions."""
 
     train = nn.Module.train          # no BatchNorm: training mode changes nothing here
 
@@ -44,24 +46,6 @@ class RRDBNet(NativeNet):
                          S.rrdbnet_spec(num_in_ch, num_out_ch, scale, num_feat, num_block, num_grow_ch), _rrdbnet_init)
         self.scale, self.num_in_ch, self.num_out_ch = scale, num_in_ch, num_out_ch
         self.num_feat, self.num_block, self.num_grow_ch = num_feat, num_block, num_grow_ch
-        object.__setattr__(self, '_precision', 'fp32')
-
-    PRECISIONS = {'fp32': 0, 'fp16': 1}
-
-    @property
-    def precision(self):
-        """``'fp32'`` (default): split-fp16 x3 operands, fp32 parity.  ``'fp16'``: fp16 operands with one tensor-core product
-        per k-step, fp32 accumulation and fp32 activations -- what the reference computes with ``half=True``.  conv_first and
-        conv_last stay fp32 in both."""
-        return self._precision
-
-    def set_precision(self, precision):
-        """Select the conv precision (see ``precision``).  Kept across ``load_state_dict``, ``.to()`` and re-preparation;
-        switching never re-prepares the weights.  Returns the module."""
-        if precision not in self.PRECISIONS:
-            raise ValueError(f"RRDBNet.set_precision: expected one of {sorted(self.PRECISIONS)}, got {precision!r}")
-        object.__setattr__(self, '_precision', precision)
-        return self
 
     def forward(self, x):
         """x [B, num_in_ch, H, W] fp32 CUDA -> [B, num_out_ch, H*scale, W*scale] (rrdbnet_arch.py:103-119)."""
@@ -81,11 +65,10 @@ class RRDBNet(NativeNet):
         dev = x.device
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
-            _lib.check(lib.cfb_rrdb_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_rrdb_set_precision')
             out = torch.empty((B, self.num_out_ch, H // us * 4, W // us * 4), dtype=torch.float32, device=dev)
             ws = self._workspace(B, H, W, dev)
             _lib.check(lib.cfb_rrdb_forward(self._net, _lib.ptr(x), _lib.ptr(out), B, H, W, _lib.ptr(ws), ws.numel(),
-                                            ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), 'cfb_rrdb_forward')
+                                            _lib.stream(dev)), 'cfb_rrdb_forward')
         return out
 
 
@@ -100,12 +83,10 @@ class RRDBNet(NativeNet):
         dev = images.device
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
-            _lib.check(lib.cfb_rrdb_set_precision(self._net, self.PRECISIONS[self._precision]), 'cfb_rrdb_set_precision')
             ws = self._workspace(rows.shape[0], tile_h, tile_w, dev)
             _lib.check(lib.cfb_rrdb_forward_u8_tiles(self._net, _lib.ptr(images), B, H, W, pre_pad,
                                                      rows.ctypes.data_as(ctypes.c_void_p), rows.shape[0], tile_h, tile_w,
-                                                     _lib.ptr(out), _lib.ptr(ws), ws.numel(),
-                                                     ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                                                     _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                        'cfb_rrdb_forward_u8_tiles')
         return out
 

@@ -8,7 +8,6 @@ resize, the network, the Detect decode and the objectness threshold run on the G
 device-to-host copy brings back the candidates, and the NMS, the coordinate scaling and the int conversion run on the host
 as in the reference.  No CPU fallback; inference only.  The package imports neither torchvision, cv2 nor yaml.
 """
-import ctypes
 import math
 import os
 from collections import OrderedDict
@@ -230,7 +229,7 @@ class YOLOv5lFace(NativeNet):
             raws = [torch.empty((B, 3, H // s, W // s, 16), dtype=torch.float32, device=dev) for s in STRIDES] if raw else []
             rp = [_lib.ptr(r) for r in raws] if raw else [None] * 3
             ws = self._workspace(B, H, W, dev)
-            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            st = _lib.stream(dev)
             if u8 is None:
                 _lib.check(lib.cfb_yolov5face_forward(self._net, _lib.ptr(x), _lib.ptr(pred), *rp, B, H, W, _lib.ptr(ws),
                                                       ws.numel(), st), 'cfb_yolov5face_forward')
@@ -269,7 +268,7 @@ class YOLOv5lFace(NativeNet):
             rows = torch.empty((B, P, 16), dtype=torch.float32, device=dev)
             counts = torch.empty((B,), dtype=torch.int32, device=dev)
             _lib.check(lib.cfb_yolov5face_candidates(_lib.ptr(pred.contiguous()), B, h, w, float(conf_thres), _lib.ptr(rows),
-                                                     _lib.ptr(counts), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                                                     _lib.ptr(counts), _lib.stream(dev)),
                        'cfb_yolov5face_candidates')
             n = counts.cpu().tolist()
         return [rows[b, :n[b]].cpu() for b in range(B)]
@@ -280,7 +279,7 @@ def _resize_u8(x, h, w):
     lib = _lib.load()
     out = torch.empty((x.shape[0], h, w, 3), dtype=torch.uint8, device=x.device)
     _lib.check(lib.cfb_resize_linear_u8(_lib.ptr(x), x.shape[0], x.shape[1], x.shape[2], _lib.ptr(out), h, w,
-                                        ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), 'cfb_resize_linear_u8')
+                                        _lib.stream(x.device)), 'cfb_resize_linear_u8')
     return out
 
 

@@ -331,7 +331,7 @@ def test_precision_errors(net_main):
     lib = _lib.load()
     net_main(faces_input(slice(0, 1)).cuda(), w=0.5, adain=True)      # the handle exists
     with pytest.raises(RuntimeError, match='precision'):
-        _lib.check(lib.cfb_net_set_precision(net_main._cfb_net, 2), 'cfb_net_set_precision')
+        _lib.check(lib.cfb_net_set_precision(net_main._net, 2), 'cfb_net_set_precision')
     net = cb.CodeFormer().cuda().eval()
     net.load_state_dict(S.random_state_dict(S.codeformer_spec(), 1))
     net.set_engine('f32')

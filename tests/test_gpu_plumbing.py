@@ -122,10 +122,10 @@ def test_restore_host_c_entry(net_main):
     want = net_main.forward_u8(torch.from_numpy(f).cuda(), w=0.5, adain=True).cpu().numpy()
     hin = torch.from_numpy(f).pin_memory()
     hout = torch.empty_like(hin).pin_memory()
-    iob = lib.cfb_host_io_bytes(net_main._cfb_net, 2)
+    iob = lib.cfb_host_io_bytes(net_main._net, 2)
     io = torch.empty(int(iob), dtype=torch.uint8, device='cuda')
-    wsb = lib.cfb_workspace_bytes(net_main._cfb_net, 2)
+    wsb = lib.cfb_workspace_bytes(net_main._net, 2)
     ws = torch.empty(int(wsb), dtype=torch.uint8, device='cuda')
-    _lib.check(lib.cfb_codeformer_restore_host(net_main._cfb_net, _lib.ptr(hin), _lib.ptr(hout), 2, 0.5, 1, _lib.ptr(io), iob,
+    _lib.check(lib.cfb_codeformer_restore_host(net_main._net, _lib.ptr(hin), _lib.ptr(hout), 2, 0.5, 1, _lib.ptr(io), iob,
                                                _lib.ptr(ws), wsb, _stream()), 'cfb_codeformer_restore_host')
     assert np.array_equal(hout.numpy(), want)
