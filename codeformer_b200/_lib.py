@@ -42,6 +42,7 @@ SIGNATURES = {
     'cfb_host_io_bytes': (c_int64, [_P, c_int32]),
     'cfb_codeformer_forward_host': (c_int, [_P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P, c_int64, _P]),
     'cfb_codeformer_forward_u8': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P]),
+    'cfb_codeformer_inpaint_u8': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_restore_host': (c_int, [_P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P, c_int64, _P]),
     'cfb_u8_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_output_to_u8': (c_int, [_P, _P, c_int32, c_int32, _P]),
@@ -140,6 +141,7 @@ SIGNATURES = {
     'cfb_resize_lanczos4_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
     'cfb_lanczos4_table': (None, [c_int32, c_int32, _P, _P]),
     'cfb_gray_adain_faces': (c_int, [_P, _P, c_int32, c_int32, _P, _P, _P]),
+    'cfb_is_gray_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, _P]),
     'cfb_f64_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_paste_faces_f64_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P]),
     'cfb_paste_faces_f64': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, _P, c_double, _P, _P, _P, _P,

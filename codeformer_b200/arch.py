@@ -559,11 +559,15 @@ class CodeFormer(VQAutoEncoder):
         return bufs
 
     # ---- SURVEY.md section 8 rows f1 / f2: the caller's plumbing and per-face loop ----------------------------------
-    def forward_u8(self, faces_bgr, w=0.5, adain=True):
+    def forward_u8(self, faces_bgr, w=0.5, adain=True, inpaint=False):
         """``cfb_codeformer_forward_u8``: DEVICE uint8 [B,512,512,3] HWC BGR faces (``face_helper.cropped_faces`` as they
         are) -> restored faces, same layout and dtype.  Bit-for-bit the reference chain img2tensor(face/255.) ->
         normalize(.5,.5) -> net(x, w, adain)[0] -> tensor2img(rgb2bgr, min_max=(-1,1)).astype(uint8)
-        (inference_codeformer.py:199-213) with the conversions fused into the first and last conv."""
+        (inference_codeformer.py:199-213) with the conversions fused into the first and last conv.
+
+        ``inpaint=True`` (``cfb_codeformer_inpaint_u8``) is inference_inpainting.py:64-75 (there ``w=1, adain=False`` on the
+        codebook-512, 3-connect net): the output keeps the input face except where the face is white (255, 255, 255), the mask
+        the script builds, i.e. ``(1-mask)*input + mask*output`` before ``tensor2img``, fused into the last conv."""
         if not torch.is_tensor(faces_bgr) or not faces_bgr.is_cuda or faces_bgr.dtype != torch.uint8:
             raise RuntimeError('forward_u8 expects a CUDA uint8 tensor')
         if faces_bgr.dim() != 4 or tuple(faces_bgr.shape[1:]) != (512, 512, 3):
@@ -571,17 +575,18 @@ class CodeFormer(VQAutoEncoder):
         lib = _lib.load()
         faces_bgr = faces_bgr.contiguous()
         B, dev = faces_bgr.shape[0], faces_bgr.device
-        w, adain = float(w), bool(adain)
+        w, adain, inpaint = float(w), bool(adain), bool(inpaint)
+        name = 'cfb_codeformer_inpaint_u8' if inpaint else 'cfb_codeformer_forward_u8'
+        fn = getattr(lib, name)
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
             if B == 0:
                 return torch.empty_like(faces_bgr)
 
             def launch(src, dst, ws):
-                _lib.check(lib.cfb_codeformer_forward_u8(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w,
-                                                         int(adain), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
-                           'cfb_codeformer_forward_u8')
-            bufs = self._graphed(('u8', dev.index, B, w, adain, self._precision), faces_bgr, lambda: (
+                _lib.check(fn(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w, int(adain), _lib.ptr(ws), ws.numel(),
+                              _lib.stream(dev)), name)
+            bufs = self._graphed(('u8', dev.index, B, w, adain, inpaint, self._precision), faces_bgr, lambda: (
                 torch.empty_like(faces_bgr), torch.empty_like(faces_bgr),
                 torch.empty(int(lib.cfb_workspace_bytes(self._net, B)), dtype=torch.uint8, device=dev)), launch)
             if bufs is not None:
@@ -590,13 +595,14 @@ class CodeFormer(VQAutoEncoder):
             launch(faces_bgr, out, self._cfb_workspace(dev, B))
         return out
 
-    def restore_faces(self, faces, w=0.5, adain=True, max_batch=32, device=None, on_error='input'):
+    def restore_faces(self, faces, w=0.5, adain=True, max_batch=32, device=None, on_error='input', inpaint=False):
         """Batched front-end for the caller loop ``for cropped_face in face_helper.cropped_faces`` of
         inference_codeformer.py:197-214 (one face per call there).  ``faces``: a list of uint8 [512,512,3] BGR arrays (or one
         [B,512,512,3] array / CPU uint8 tensor).  Returns the list of restored uint8 BGR faces in order -- what the loop
         passes to ``face_helper.add_restored_face``.  Faces go through pinned uint8 staging (0.79 MB per face each way)
         in chunks of ``max_batch``.  ``on_error='input'`` mirrors the reference's fallback (:209-211: on any failure the
-        restored face is the input face); ``'raise'`` re-raises."""
+        restored face is the input face); ``'raise'`` re-raises.  ``inpaint=True`` is the loop of inference_inpainting.py
+        (``forward_u8(inpaint=True)``; its fallback, :78-80, is the input face as well)."""
         if torch.is_tensor(faces):
             arr = faces.detach().cpu().numpy()
         elif isinstance(faces, np.ndarray):
@@ -647,7 +653,7 @@ class CodeFormer(VQAutoEncoder):
                         self._cfb_ws[key] = pin
                     drain(1)                           # the buffers of chunk k-2 (same parity) are free again
                     pin[0].copy_(torch.from_numpy(np.ascontiguousarray(arr[lo:hi])))
-                    out = self.forward_u8(pin[0].to(dev, non_blocking=True), w=w, adain=adain)
+                    out = self.forward_u8(pin[0].to(dev, non_blocking=True), w=w, adain=adain, inpaint=inpaint)
                     pin[1].copy_(out, non_blocking=True)
                     ev = torch.cuda.Event()
                     ev.record(torch.cuda.current_stream(dev))

@@ -192,6 +192,11 @@ int conv_first_u8(const unsigned char* x_bgr_hwc, const float* wgt, const float*
                   int Cout, cudaStream_t st, float* gn_part = nullptr);
 int conv_last_u8(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
                  unsigned char* out_bgr_hwc, int N, int H, int W, int Cin, cudaStream_t st);
+// conv_last_u8 with the inpainting blend of inference_inpainting.py:68-75 before the conversion: where the normalised input
+// face (the forward's own uint8 input, face_bgr_hwc) sums to 3 over its channels the output is the network's, elsewhere the input
+int conv_last_u8_inpaint(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
+                         const unsigned char* face_bgr_hwc, unsigned char* out_bgr_hwc, int N, int H, int W, int Cin,
+                         cudaStream_t st);
 int u8_to_input(const unsigned char* img_bgr_hwc, float* x_nchw, int N, int64_t HW, cudaStream_t st);
 int output_to_u8(const float* x_nchw, unsigned char* img_bgr_hwc, int N, int64_t HW, cudaStream_t st);
 

@@ -867,6 +867,36 @@ __global__ void k_gray_apply(const uint8_t* __restrict__ restored, int npx, cons
   for (int c = 0; c < 3; ++c) o[c] = __dadd_rn(__dmul_rn(nrm, st[9 + c]), st[6 + c]);
 }
 
+// ---- is_gray (facelib/utils/misc.py:146-158) of a batch: the exact moments of the three channel differences ---------------
+// Image blockIdx.y, pixels strided over the x blocks.  sums[img] = {Σd, Σd²} for d = B-G, G-R, R-B (int64, zeroed by the
+// caller); integer adds are exact, so the result does not depend on the order of the atomics.
+constexpr int kGrayTestBlocks = 512;     // blocks over all images: about four per SM
+
+__global__ void __launch_bounds__(256) k_is_gray_sums(const uint8_t* __restrict__ img, int64_t npx,
+                                                      unsigned long long* __restrict__ sums) {
+  const uint8_t* p = img + (size_t)blockIdx.y * npx * 3;
+  long long s[6] = {0, 0, 0, 0, 0, 0};
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < npx; i += (int64_t)gridDim.x * blockDim.x) {
+    const int b = p[i * 3], g = p[i * 3 + 1], r = p[i * 3 + 2];
+    const int d[3] = {b - g, g - r, r - b};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { s[k] += d[k]; s[3 + k] += d[k] * d[k]; }
+  }
+#pragma unroll
+  for (int k = 0; k < 6; ++k)
+    for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+  __shared__ long long red[8][6];
+  const int warp = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0)
+    for (int k = 0; k < 6; ++k) red[warp][k] = s[k];
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    long long t = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w][threadIdx.x];
+    atomicAdd(sums + (size_t)blockIdx.y * 6 + threadIdx.x, (unsigned long long)t);   // two's complement: signed sums too
+  }
+}
+
 // the parse network's input of a float64 face: astype(float32) / 255, BGR -> RGB, (x - 0.5) / 0.5, HWC -> NCHW
 __global__ void k_f64_to_input(const double* __restrict__ img, float* __restrict__ x, int64_t hw, int64_t total) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1141,6 +1171,22 @@ int cfb_gray_adain_faces(const uint8_t* restored, const uint8_t* cropped, int32_
   cfb::k_gray_apply<<<dim3((npx + 255) / 256, n), 256, 0, st>>>(restored, npx, dstats, out);
   CFB_LAUNCH_CHECK();
   CFB_CUDA(cudaFreeAsync(tmp, st));
+  return 0;
+  API_END(1)
+}
+
+int cfb_is_gray_u8(const uint8_t* images, int32_t n, int32_t h, int32_t w, int64_t* sums, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n >= 0 && n <= 65535 && h > 0 && w > 0, "cfb_is_gray_u8: bad size");
+  CFB_REQUIRE(n == 0 || (images && sums), "cfb_is_gray_u8: NULL argument");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t npx = (int64_t)h * w;
+  const int64_t want = (npx + 2047) / 2048;        // at least 8 pixels per thread
+  const int bx = (int)std::max<int64_t>(1, std::min<int64_t>(want, std::max(1, cfb::kGrayTestBlocks / n)));
+  CFB_CUDA(cudaMemsetAsync(sums, 0, (size_t)n * 6 * sizeof(int64_t), st));
+  cfb::k_is_gray_sums<<<dim3(bx, n), 256, 0, st>>>(images, npx, reinterpret_cast<unsigned long long*>(sums));
+  CFB_LAUNCH_CHECK();
   return 0;
   API_END(1)
 }

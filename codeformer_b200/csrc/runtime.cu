@@ -588,6 +588,7 @@ struct Fwd {
   // caller-side image plumbing fused into the first / last conv (cfb_codeformer_forward_u8): uint8 HWC BGR faces
   const unsigned char* in_u8 = nullptr;
   unsigned char* out_u8 = nullptr;
+  bool inpaint = false;       // conv_last blends out_u8 with in_u8 as inference_inpainting.py does (cfb_codeformer_inpaint_u8)
   bool single_pass = false;   // the convs issued now run single-pass fp16 (ConvArgs::single_pass): set by generator()
 
   int alloc(Tensor& t, int N, int H, int W, int C) {
@@ -934,7 +935,9 @@ struct Fwd {
         case B_CONV:
           if (i + 1 == n->gen.size()) {
             if (!dry) {
-              if (out_u8) CFB_CHECK(conv_last_u8(x.p, ps, ph, b.conv.w_f32, b.conv.bias, out_u8, x.N, x.H, x.W, x.C, st));
+              if (out_u8 && inpaint)
+                CFB_CHECK(conv_last_u8_inpaint(x.p, ps, ph, b.conv.w_f32, b.conv.bias, in_u8, out_u8, x.N, x.H, x.W, x.C, st));
+              else if (out_u8) CFB_CHECK(conv_last_u8(x.p, ps, ph, b.conv.w_f32, b.conv.bias, out_u8, x.N, x.H, x.W, x.C, st));
               else CFB_CHECK(conv_last(x.p, ps, ph, b.conv.w_f32, b.conv.bias, out_nchw, x.N, x.H, x.W, x.C, st));
             }
             if (ps) { release_raw(ps); release_raw(ph); ps = ph = nullptr; }
@@ -1092,7 +1095,7 @@ static std::vector<int> tap_blocks_of(const cfb_config& c, bool encoder) {
 static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float* logits, float* lq_feat,
                                    int64_t* top_idx, int B, float w, int adain, int code_only, void* ws, int64_t ws_bytes,
                                    cudaStream_t st, bool dry, const unsigned char* x_u8 = nullptr,
-                                   unsigned char* out_u8 = nullptr) {
+                                   unsigned char* out_u8 = nullptr, bool inpaint = false) {
   CFB_REQUIRE(n->cfg.kind == 1, "net was created as VQAutoEncoder");
   CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
   if (!dry) CFB_CHECK(check_device(n));
@@ -1102,7 +1105,7 @@ static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float
   if (B == 0) return 0;
   n->arena.reset(ws, (size_t)ws_bytes, dry);
   Fwd f{n, st, n->arena, dry, n->engine};
-  f.in_u8 = x_u8; f.out_u8 = out_u8;
+  f.in_u8 = x_u8; f.out_u8 = out_u8; f.inpaint = inpaint;
   const cfb_config& c = n->cfg;
   std::map<int, Tensor> taps;
   Tensor lq;
@@ -2630,19 +2633,35 @@ int cfb_codeformer_forward(cfb_net* n, const float* x, float* out, float* logits
   API_END(1)
 }
 
+static int codeformer_u8(const char* what, cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits,
+                         float* lq_feat, int64_t* top_idx, int32_t batch, float w, int32_t adain, void* workspace,
+                         int64_t workspace_bytes, void* stream, bool inpaint) {
+  CFB_REQUIRE(n, std::string(what) + ": NULL net");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(faces_bgr && restored_bgr, std::string(what) + ": NULL image pointer");
+  std::lock_guard<std::mutex> lk(n->mu);
+  const int64_t before = cfb::launch_count();
+  const int rc = cfb::codeformer_forward_impl(n, nullptr, nullptr, logits, lq_feat, top_idx, batch, w, adain, 0, workspace,
+                                              workspace_bytes, (cudaStream_t)stream, false, faces_bgr, restored_bgr, inpaint);
+  n->last_launches = cfb::launch_count() - before;
+  return rc;
+}
+
 int cfb_codeformer_forward_u8(cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
                               int64_t* top_idx, int32_t batch, float w, int32_t adain, void* workspace,
                               int64_t workspace_bytes, void* stream) {
   API_BEGIN
-  CFB_REQUIRE(n, "cfb_codeformer_forward_u8: NULL net");
-  if (batch == 0) return 0;
-  CFB_REQUIRE(faces_bgr && restored_bgr, "cfb_codeformer_forward_u8: NULL image pointer");
-  std::lock_guard<std::mutex> lk(n->mu);
-  const int64_t before = cfb::launch_count();
-  const int rc = cfb::codeformer_forward_impl(n, nullptr, nullptr, logits, lq_feat, top_idx, batch, w, adain, 0, workspace,
-                                              workspace_bytes, (cudaStream_t)stream, false, faces_bgr, restored_bgr);
-  n->last_launches = cfb::launch_count() - before;
-  return rc;
+  return codeformer_u8("cfb_codeformer_forward_u8", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, w, adain,
+                       workspace, workspace_bytes, stream, false);
+  API_END(1)
+}
+
+int cfb_codeformer_inpaint_u8(cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                              int64_t* top_idx, int32_t batch, float w, int32_t adain, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  return codeformer_u8("cfb_codeformer_inpaint_u8", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, w, adain,
+                       workspace, workspace_bytes, stream, true);
   API_END(1)
 }
 

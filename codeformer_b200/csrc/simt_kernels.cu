@@ -373,11 +373,14 @@ constexpr int CL_PH = CL_TH + 2, CL_PW = CL_TW + 2;  // input patch
 constexpr int CL_MAX_CIN = 128;                      // shared memory: 9*Cin*16 + 6*66*Cin*4 bytes <= 227 KB
 static size_t conv_last_smem(int Cin) { return (size_t)(9 * Cin * 4 + CL_PH * CL_PW * Cin) * sizeof(float); }
 
-template <bool U8>
+// INPAINT (with U8): the blend of inference_inpainting.py:68-75 before the uint8 conversion.  face is the forward's own uint8
+// HWC BGR input [N][H][W][3]; only that instantiation reads it.
+template <bool U8, bool INPAINT = false>
 __global__ void __launch_bounds__(256) conv_last_kernel(const float* __restrict__ in, const float* __restrict__ in_scale,
                                                         const float* __restrict__ in_shift, const float* __restrict__ wgt,
                                                         const float* __restrict__ bias, float* __restrict__ out, int N,
-                                                        int H, int W, int Cin) {
+                                                        int H, int W, int Cin, const unsigned char* __restrict__ face) {
+  static_assert(U8 || !INPAINT, "conv_last: the inpainting blend writes uint8");
   extern __shared__ __align__(16) float sm[];
   float* ws = sm;                 // [9][Cin][3] padded -> [9][Cin][4]
   // [CL_PH][CL_PW][Cin/4] float4: normalised patch, zero outside the image.  Channel quad q of patch column pc is stored at
@@ -435,6 +438,16 @@ __global__ void __launch_bounds__(256) conv_last_kernel(const float* __restrict_
   }
   if (y >= H || x >= W) return;
   const int64_t HW = (int64_t)H * W, pix = (int64_t)y * W + x;
+  if constexpr (INPAINT) {
+    // mask = (R + G + B of the normalised input == 3), summed in the reference's RGB order; then (1-m)*in + m*out per
+    // channel as two fp32 products and one add (no FMA: the reference multiplies and adds separate tensors)
+    const unsigned char* f8 = face + ((int64_t)n * HW + pix) * 3;
+    const float xi[3] = {u8_to_model_input(__ldg(f8 + 2)), u8_to_model_input(__ldg(f8 + 1)), u8_to_model_input(__ldg(f8 + 0))};
+    const float m = __fadd_rn(__fadd_rn(xi[0], xi[1]), xi[2]) == 3.f ? 1.f : 0.f;
+    const float keep = __fsub_rn(1.f, m);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) acc[k] = __fadd_rn(__fmul_rn(keep, xi[k]), __fmul_rn(m, acc[k]));
+  }
   if constexpr (U8) {
     // uint8 HWC BGR
     unsigned char* o8 = reinterpret_cast<unsigned char*>(out) + ((int64_t)n * HW + pix) * 3;
@@ -447,9 +460,9 @@ __global__ void __launch_bounds__(256) conv_last_kernel(const float* __restrict_
   }
 }
 
-template <bool U8>
+template <bool U8, bool INPAINT = false>
 static int launch_conv_last(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
-                            float* out, int N, int H, int W, int Cin, cudaStream_t st) {
+                            float* out, int N, int H, int W, int Cin, cudaStream_t st, const unsigned char* face = nullptr) {
   CFB_REQUIRE(Cin % 32 == 0 && Cin <= CL_MAX_CIN, "conv_last: Cin must be a multiple of 32 and at most 128");
   if (N == 0 || H == 0 || W == 0) return 0;
   // the patch needs more than the default 48 KB of dynamic shared memory: a per-device property of the function
@@ -458,13 +471,14 @@ static int launch_conv_last(const float* in, const float* in_scale, const float*
   CFB_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_last_kernel<U8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_last_smem(CL_MAX_CIN)));
+    CFB_CUDA(cudaFuncSetAttribute(conv_last_kernel<U8, INPAINT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)conv_last_smem(CL_MAX_CIN)));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   const int64_t tiles = (int64_t)N * ((H + CL_TH - 1) / CL_TH) * ((W + CL_TW - 1) / CL_TW);
   CFB_REQUIRE(tiles <= 0x7fffffffLL, "conv_last: too many tiles");
-  CFB_LAUNCH_PDL(conv_last_kernel<U8>, dim3((unsigned)tiles), dim3(256), conv_last_smem(Cin), st, in, in_scale, in_shift, wgt, bias,
-                 out, N, H, W, Cin);
+  CFB_LAUNCH_PDL((conv_last_kernel<U8, INPAINT>), dim3((unsigned)tiles), dim3(256), conv_last_smem(Cin), st, in, in_scale, in_shift,
+                 wgt, bias, out, N, H, W, Cin, face);
   return 0;
 }
 
@@ -475,6 +489,13 @@ int conv_last(const float* in, const float* in_scale, const float* in_shift, con
 int conv_last_u8(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
                  unsigned char* out_bgr_hwc, int N, int H, int W, int Cin, cudaStream_t st) {
   return launch_conv_last<true>(in, in_scale, in_shift, wgt, bias, reinterpret_cast<float*>(out_bgr_hwc), N, H, W, Cin, st);
+}
+int conv_last_u8_inpaint(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
+                         const unsigned char* face_bgr_hwc, unsigned char* out_bgr_hwc, int N, int H, int W, int Cin,
+                         cudaStream_t st) {
+  CFB_REQUIRE(face_bgr_hwc != nullptr, "conv_last: the inpainting blend needs the input faces");
+  return launch_conv_last<true, true>(in, in_scale, in_shift, wgt, bias, reinterpret_cast<float*>(out_bgr_hwc), N, H, W, Cin, st,
+                                      face_bgr_hwc);
 }
 
 // stand-alone plumbing (unit parity + callers that want the fp32 tensor): uint8 HWC BGR <-> fp32 NCHW RGB in [-1,1]

@@ -121,7 +121,7 @@ def gray_adain_faces(restored, cropped, with_stats=False):
     also CUDA float64 [N,4,3]: content mean, content std, style mean, style std per channel.  The statistics are two-pass
     float64 sums in a fixed order: within 1e-13 relative of the exact statistics and 1e-10 of numpy's (whose own float64 sums
     carry a few 1e-12), identical on every run and for a face alone or inside a batch.  The result goes to ``paste_faces`` / ``paste_faces_multi`` as it is.
-    ``CodeFormer.restore_faces`` (the aligned-faces loop) does not call this; gray aligned faces can."""
+    ``CodeFormer.restore_faces`` does not call this; ``restore_aligned`` (the ``--has_aligned`` loop) does for gray crops."""
     restored = _check_image(restored, 'gray_adain_faces: restored faces', 4)
     cropped = _check_image(cropped, 'gray_adain_faces: cropped faces', 4)
     if restored.shape != cropped.shape or restored.shape[1] != restored.shape[2] or restored.device != cropped.device:

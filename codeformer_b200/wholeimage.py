@@ -22,6 +22,10 @@ and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of im
     call over the chunk's gray faces, then the float64 paste (``cfb_paste_faces_f64``) over the gray images' canvases after
     the uint8 paste of the colour images' faces.  A chunk may mix gray and colour images; the colour ones are untouched.
 
+``restore_aligned`` is the ``--has_aligned`` loop of the same script (:180-213) over already aligned crops of any size: the
+INTER_LINEAR resize to 512x512, the gray test of all crops in one launch (``cfb_is_gray_u8``), CodeFormer in batches and the
+gray crops' colour transfer, all on the device.
+
 What stays on the host, as in the reference: the NMS and the landmark filter, ``get_center_face``,
 ``cv2.estimateAffinePartial2D(LMEDS)`` (cv2 is imported lazily, as ``align_warp_face`` does), and the ``enhance`` of any
 other upsampler, per image.  Every result is per image: batching and chunking do not change any byte.
@@ -51,16 +55,31 @@ def is_gray(img, threshold=10):
     return bool(diff <= threshold)
 
 
-def _device_is_gray(img, threshold=10):
-    """``is_gray`` of a CUDA image from exact integer moments (the variances numpy computes, up to its rounding)."""
-    x = img.to(torch.int64)
-    n = x.shape[0] * x.shape[1]
-    total = 0.0
-    for a, b in ((0, 1), (1, 2), (2, 0)):
-        d = x[:, :, a] - x[:, :, b]
-        s, s2 = int(d.sum()), int((d * d).sum())
-        total += (n * s2 - s * s) / (n * n)
-    return bool(total / 3.0 <= threshold)
+def _gray_sums(x):
+    """``cfb_is_gray_u8``: CUDA uint8 [N,h,w,3] -> host int64 [N,6], {Σd1, Σd2, Σd3, Σd1², Σd2², Σd3²} of the channel
+    differences d1 = B-G, d2 = G-R, d3 = R-B of each image: one launch, one read-back."""
+    x = x.contiguous()
+    n, h, w = x.shape[:3]
+    sums = torch.empty((n, 6), dtype=torch.int64, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().cfb_is_gray_u8(_lib.ptr(x), n, h, w, _lib.ptr(sums), _lib.stream(x.device)), 'cfb_is_gray_u8')
+    return sums.cpu().numpy()
+
+
+def _device_is_gray(imgs, threshold=10):
+    """``is_gray`` of a CUDA image [h,w,3] (a bool) or of a batch [N,h,w,3] (a list of N) from exact integer moments (the
+    variances numpy computes, up to its rounding)."""
+    batched = imgs.dim() == 4
+    x = imgs if batched else imgs[None]
+    n = x.shape[1] * x.shape[2]
+    flags = []
+    for row in _gray_sums(x):
+        total = 0.0
+        for k in range(3):
+            s, s2 = int(row[k]), int(row[3 + k])
+            total += (n * s2 - s * s) / (n * n)
+        flags.append(bool(total / 3.0 <= threshold))
+    return flags if batched else flags[0]
 
 
 def get_center_face(det_faces, h=0, w=0):
@@ -123,21 +142,21 @@ def _chunks(images, max_batch):
     return out
 
 
-def _as_input(img, dev):
+def _as_input(img, dev, name='restore_images'):
     """-> (CUDA uint8 [h,w,3], host array or None, came from the host)."""
     if isinstance(img, np.ndarray):
         if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
-            raise NotImplementedError(f'restore_images takes uint8 HWC BGR images with 3 channels (gray, alpha and 16-bit '
+            raise NotImplementedError(f'{name} takes uint8 HWC BGR images with 3 channels (gray, alpha and 16-bit '
                                       f'images stay caller-side), got {img.dtype} {img.shape}')
-        return cuda_u8_image(img, dev, 'restore_images'), img, True
+        return cuda_u8_image(img, dev, name), img, True
     if torch.is_tensor(img):
         if not img.is_cuda:
-            raise RuntimeError('restore_images: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
-        return cuda_u8_image(img, dev, 'restore_images').contiguous(), None, False
-    raise NotImplementedError(f'restore_images takes numpy arrays or CUDA tensors, got {type(img).__name__}')
+            raise RuntimeError(f'{name}: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
+        return cuda_u8_image(img, dev, name).contiguous(), None, False
+    raise NotImplementedError(f'{name} takes numpy arrays or CUDA tensors, got {type(img).__name__}')
 
 
-def _restore(net, crops, w, max_batch, errors):
+def _restore(net, crops, w, max_batch, errors, adain=True, name='restore_images'):
     """CodeFormer over the crops in batches of <= max_batch; a failed batch gives its input faces back (the reference's
     per-face fallback, inference_codeformer.py:208-210)."""
     out = torch.empty_like(crops)
@@ -145,9 +164,9 @@ def _restore(net, crops, w, max_batch, errors):
     for lo in range(0, crops.shape[0], max_batch):
         hi = min(crops.shape[0], lo + max_batch)
         try:
-            res = net.forward_u8(crops[lo:hi], w=w, adain=True)
+            res = net.forward_u8(crops[lo:hi], w=w, adain=adain)
             torch.cuda.current_stream(dev).synchronize()
-            _lib.check(_lib.load().cfb_check_async_status(), 'restore_images')
+            _lib.check(_lib.load().cfb_check_async_status(), name)
             out[lo:hi] = res
         except RuntimeError as err:
             errors.append((lo, str(err)))
@@ -190,7 +209,11 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
         x = torch.stack([inputs[i][0] for i in idx])
         h0, w0 = x.shape[1:3]
         # read_image: gray test, then an INTER_LINEAR enlargement (fx = fy) when the short side is below 512
-        gray = [is_gray(inputs[i][1]) if inputs[i][2] else _device_is_gray(inputs[i][0]) for i in idx]
+        gray = [is_gray(inputs[i][1]) if inputs[i][2] else None for i in idx]
+        on_dev = [k for k, i in enumerate(idx) if not inputs[i][2]]
+        if on_dev:                                          # the CUDA images of the chunk in one launch
+            for k, g in zip(on_dev, _device_is_gray(x if len(on_dev) == len(idx) else x[on_dev])):
+                gray[k] = g
         if min(h0, w0) < 512:
             x = resize_linear_factor(x, 512.0 / min(h0, w0))
         h, wd = x.shape[1:3]
@@ -297,3 +320,57 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
 
 
 restore_images.last_errors = []
+
+
+def restore_aligned(faces, net, w=0.5, adain=True, max_batch=32, return_crops=False):
+    """The ``--has_aligned`` loop of inference_codeformer.py:180-213 over already cropped and aligned faces.  ``faces``: a
+    list of uint8 HWC BGR crops of any size (numpy arrays or CUDA tensors); ``net``: a ``CodeFormer``.  Per crop, as the
+    reference does for one: ``cv2.resize(img, (512, 512), INTER_LINEAR)`` (``resize_linear``, one launch per crop size),
+    ``is_gray(img, threshold=10)`` of the resized crop, CodeFormer with ``w`` / ``adain`` (``forward_u8`` over all crops in
+    batches of ``max_batch``; a failed batch gives its input crops back, as the reference's per-face fallback does, and
+    ``restore_aligned.last_errors`` lists (crop offset, message) of each) and ``add_restored_face``: the gray crops become
+    ``adain_npy(bgr2gray(restored), cropped)`` in float64 (``gray_adain_faces``).
+
+    The gray test runs on the device for all crops at once (``cfb_is_gray_u8``): exact integer moments, so it decides as the
+    reference's numpy variances do except for a crop whose score is within numpy's rounding of the threshold.
+
+    Returns, per crop, what the reference's ``face_helper.restored_faces`` holds: uint8 [512,512,3], or float64 for a gray
+    crop; host arrays for host inputs and CUDA tensors for CUDA inputs.  With ``return_crops`` also the resized crops
+    (CUDA uint8 [N,512,512,3]) and the gray flags.  Results do not depend on ``max_batch``."""
+    faces = list(faces)
+    dev = next(net.parameters()).device
+    if dev.type != 'cuda':
+        raise RuntimeError('restore_aligned: the network is not on a CUDA device; there is no CPU fallback')
+    max_batch = max(1, int(max_batch))
+    inputs = [_as_input(f, dev, 'restore_aligned') for f in faces]
+    n = len(inputs)
+    crops = torch.empty((n, FACE_SIZE, FACE_SIZE, 3), dtype=torch.uint8, device=dev)
+    groups = {}
+    for i, (t, _, _) in enumerate(inputs):
+        groups.setdefault(tuple(t.shape), []).append(i)
+    for shape, idx in groups.items():
+        x = torch.stack([inputs[i][0] for i in idx])
+        if shape[:2] != (FACE_SIZE, FACE_SIZE):        # cv2.resize to the same size is a copy
+            x = resize_linear(x, (FACE_SIZE, FACE_SIZE))
+        crops[torch.tensor(idx, device=dev)] = x
+    gray = _device_is_gray(crops) if n else []
+    errors = []
+    with torch.no_grad():
+        restored = _restore(net, crops, w, max_batch, errors, adain=adain, name='restore_aligned')
+    gsel = np.nonzero(np.asarray(gray, bool))[0]
+    gray_faces = None
+    if len(gsel):
+        gt = torch.from_numpy(gsel).to(dev)
+        gray_faces = gray_adain_faces(restored[gt], crops[gt])
+    pos = {int(i): k for k, i in enumerate(gsel)}
+    results = []
+    for i in range(n):
+        face = gray_faces[pos[i]] if i in pos else restored[i]
+        results.append(face.cpu().numpy() if inputs[i][2] else face)
+    restore_aligned.last_errors = errors
+    if return_crops:
+        return results, crops, gray
+    return results
+
+
+restore_aligned.last_errors = []

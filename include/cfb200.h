@@ -109,6 +109,13 @@ int cfb_codeformer_forward_host(cfb_net* net, const float* x_host, float* out_ho
 int cfb_codeformer_forward_u8(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
                               int64_t* top_idx, int32_t batch, float w, int32_t adain,
                               void* workspace, int64_t workspace_bytes, void* stream);
+/* cfb_codeformer_forward_u8 for face inpainting (inference_inpainting.py:64-75; there w = 1, adain = 0 on the codebook-512,
+ * 3-connect net): same arguments, launches and precision, but before the uint8 conversion every pixel where the normalised input
+ * face sums to 3 over its channels (only (255,255,255)) takes the network's output and every other pixel keeps the input:
+ * (1-mask)*input + mask*output in fp32, then tensor2img.  Restored faces are the script's save_face, byte for byte. */
+int cfb_codeformer_inpaint_u8(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                              int64_t* top_idx, int32_t batch, float w, int32_t adain,
+                              void* workspace, int64_t workspace_bytes, void* stream);
 /* the same with HOST uint8 buffers (0.79 MB per face each way instead of 3.1 MB): H2D, forward, D2H, stream sync.
  * dev_scratch >= cfb_host_io_bytes(net, batch). */
 int cfb_codeformer_restore_host(cfb_net* net, const uint8_t* faces_host, uint8_t* restored_host, int32_t batch, float w,
@@ -443,6 +450,9 @@ int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_
  *   adain_npy(bgr2gray(restored[i]), cropped[i]) (facelib/utils/misc.py:169-202), both inputs uint8 [n,S,S,3] BGR.  stats
  *   (optional, device double [n,4,3]) receives content mean, content std, style mean, style std per channel.  float64, two-pass
  *   variance, fixed summation order (equal to numpy's up to rounding; the same on every run, whatever n is).
+ * cfb_is_gray_u8: the moments behind is_gray(img, threshold) (facelib/utils/misc.py:146-158) of n images [n,h,w,3] BGR in one
+ *   launch: sums (device int64 [n][6]) = {Σd1, Σd2, Σd3, Σd1², Σd2², Σd3²} for d1 = B-G, d2 = G-R, d3 = R-B, exact.  The caller
+ *   decides: mean over k of (h*w*Σdk² - (Σdk)²) / (h*w)² <= threshold.
  * cfb_f64_to_input: cfb_u8_to_input for float64 faces: astype(float32) / 255, BGR -> RGB, (x - 0.5) / 0.5 (:459-461).
  * cfb_paste_faces_f64: cfb_paste_faces_multi for float64 faces [n,S,S,3] (the restored faces of a gray image): warpAffine as
  *   cv2 runs it on CV_64F (the fixed-point coordinates, float32 weights, sums in double) and a float64 canvas from the first
@@ -454,6 +464,7 @@ int cfb_resize_lanczos4_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, 
 void cfb_lanczos4_table(int32_t src_len, int32_t dst_len, int32_t* idx, int16_t* coef);
 int cfb_gray_adain_faces(const uint8_t* restored, const uint8_t* cropped, int32_t n, int32_t face_size, double* out, double* stats,
                          void* stream);
+int cfb_is_gray_u8(const uint8_t* images, int32_t n, int32_t h, int32_t w, int64_t* sums, void* stream);
 int cfb_f64_to_input(const double* img_bgr_hwc, float* x_nchw, int32_t n, int32_t hw, void* stream);
 int64_t cfb_paste_faces_f64_workspace_bytes(int32_t n_img, int32_t h_up, int32_t w_up, int32_t n, int32_t face_size,
                                             int32_t use_parse, const double* inverse_affines);
