@@ -43,6 +43,9 @@ SIGNATURES = {
     'cfb_codeformer_forward_host': (c_int, [_P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P, c_int64, _P]),
     'cfb_codeformer_forward_u8': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_inpaint_u8': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P]),
+    'cfb_codeformer_forward_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_codeformer_forward_u8_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, _P, c_int64, _P]),
+    'cfb_codeformer_inpaint_u8_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_restore_host': (c_int, [_P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P, c_int64, _P]),
     'cfb_u8_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_output_to_u8': (c_int, [_P, _P, c_int32, c_int32, _P]),
@@ -71,6 +74,9 @@ SIGNATURES = {
     'cfb_debug_conv_tc_prec': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                       _P, _P, c_int32, _P, _P, _P, c_float, _P, _P, _P, c_int64, _P, POINTER(c_int32), c_int32,
                                       c_int32, c_int32]),
+    'cfb_debug_conv_tc_prec_wv': (c_int, [_P, _P, c_int32, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                         _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, POINTER(c_int32), c_int32,
+                                         c_int32, c_int32]),
     'cfb_debug_gn_partials_workspace_bytes': (c_int64, [c_int32, c_int32]),
     'cfb_debug_gn_coef_from_partials': (c_int, [_P, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, c_int64, _P]),
     'cfb_debug_gn_cat_partials': (c_int, [_P, _P, _P, c_int64, c_int32, _P]),

@@ -418,6 +418,40 @@ class _FuseSft(_ParamsOnly):
         self.shift = nn.ModuleDict({'0': _Conv(c, c, 3), '2': _Conv(c, c, 3)})
 
 
+def fidelity_weights(w, n, device=None):
+    """The fidelity weight ``w`` of the CodeFormer forwards for ``n`` faces.  A number (anything ``float()`` takes, a 0-d array
+    or tensor included) is one weight for every face and comes back as a float: the scalar path.  One weight per face -- a
+    sequence of n numbers, a floating numpy array or a floating tensor of shape [n], on the host or on the CUDA ``device`` --
+    comes back as a contiguous float32 tensor [n] where it was given.  A wrong length or shape, or a CUDA tensor on another
+    device than ``device``, raises RuntimeError; a non-floating array or tensor (or a sequence of non-numbers) ValueError."""
+    if torch.is_tensor(w):
+        if w.dim() == 0:
+            return float(w)
+        if not w.dtype.is_floating_point:
+            raise ValueError(f'w: per-face fidelity weights must be floating point, got a {w.dtype} tensor')
+        if w.is_cuda and device is not None and w.device != torch.device(device):
+            raise RuntimeError(f'w: per-face fidelity weights are on {w.device}, the faces on {torch.device(device)}')
+        t = w.detach()
+    elif isinstance(w, (np.ndarray, list, tuple)):
+        a = np.asarray(w)
+        if a.ndim == 0:
+            return float(a)
+        ok = 'f' if isinstance(w, np.ndarray) else 'fiub'          # a sequence may hold Python ints
+        if a.dtype.kind not in ok:
+            raise ValueError(f'w: per-face fidelity weights must be floating point, got {a.dtype}')
+        t = torch.from_numpy(a.astype(np.float32))
+    else:
+        return float(w)
+    if t.dim() != 1 or t.shape[0] != n:
+        raise RuntimeError(f'w: expected one fidelity weight per face, shape [{n}], got {tuple(t.shape)}')
+    return t.to(torch.float32).contiguous()
+
+
+def _weights_on(w, dev):
+    """A per-face weight tensor of fidelity_weights on CUDA device ``dev`` (host values go through pinned memory: no sync)."""
+    return w if w.is_cuda else w.pin_memory().to(dev, non_blocking=True)
+
+
 def restore_chunks(n_faces, max_batch):
     """Chunk plan of ``CodeFormer.restore_faces``: consecutive [lo, hi) ranges of <= max_batch faces; a chunk of >= 16 faces
     is split in two so the host-side staging of one half overlaps the GPU work of the other."""
@@ -475,25 +509,41 @@ class CodeFormer(VQAutoEncoder):
 
     def forward(self, x, w=0, detach_16=True, code_only=False, adain=False):
         """-> (out [B,3,512,512], logits [B,256,K], lq_feat [B,256,16,16]); ``code_only`` -> (logits, lq_feat).
-        ``detach_16`` only affects autograd in the reference (:263-264) and is accepted for signature parity."""
+        ``detach_16`` only affects autograd in the reference (:263-264) and is accepted for signature parity.
+        ``w`` is one fidelity weight, or one per face (``fidelity_weights``): face i then equals the call on that face alone
+        with ``w[i]``, bit for bit (``cfb_codeformer_forward_wv``)."""
         x = self._check_input(x)
         lib = _lib.load()
         B = x.shape[0]
         dev = x.device
-        w, adain, code_only = float(w), bool(adain), bool(code_only)
+        w, adain, code_only = fidelity_weights(w, B, dev), bool(adain), bool(code_only)
+        per_face = torch.is_tensor(w)
 
-        def launch(src, logits, lq_feat, out, ws):
-            _lib.check(lib.cfb_codeformer_forward(self._net, _lib.ptr(src), _lib.ptr(out), _lib.ptr(logits), _lib.ptr(lq_feat), None,
-                                                  src.shape[0], w, int(adain), int(code_only), _lib.ptr(ws), ws.numel(),
-                                                  _lib.stream(dev)), 'cfb_codeformer_forward')
+        def launch(src, wv, logits, lq_feat, out, ws):
+            if wv is None:
+                _lib.check(lib.cfb_codeformer_forward(self._net, _lib.ptr(src), _lib.ptr(out), _lib.ptr(logits), _lib.ptr(lq_feat),
+                                                      None, src.shape[0], w, int(adain), int(code_only), _lib.ptr(ws), ws.numel(),
+                                                      _lib.stream(dev)), 'cfb_codeformer_forward')
+            else:
+                _lib.check(lib.cfb_codeformer_forward_wv(self._net, _lib.ptr(src), _lib.ptr(out), _lib.ptr(logits),
+                                                         _lib.ptr(lq_feat), None, src.shape[0], _lib.ptr(wv), int(adain),
+                                                         int(code_only), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
+                           'cfb_codeformer_forward_wv')
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
-            bufs = self._graphed((dev.index, B, w, adain, code_only, self._precision), x, lambda: (
-                torch.empty_like(x), torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev),
+            # per-face weights are data: one graph per batch size serves every w vector (copied in before each replay)
+            if per_face:
+                w = _weights_on(w, dev)
+                key, inputs = ('wv', dev.index, B, adain, code_only, self._precision), (x, w)
+            else:
+                key, inputs = (dev.index, B, w, adain, code_only, self._precision), (x,)
+            bufs = self._graphed(key, inputs, lambda: (
+                torch.empty_like(x), torch.empty_like(w) if per_face else None,
+                torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev),
                 torch.empty((B, 256, 16, 16), dtype=torch.float32, device=dev), None if code_only else torch.empty_like(x),
                 torch.empty(int(lib.cfb_workspace_bytes(self._net, B)), dtype=torch.uint8, device=dev)), launch)
             if bufs is not None:
-                _, logits, lq, out, _ = bufs
+                _, _, logits, lq, out, _ = bufs
                 return (logits.clone(), lq.clone()) if code_only else (out.clone(), logits.clone(), lq.clone())
             logits = torch.empty((B, self.latent_size, self.codebook_size), dtype=torch.float32, device=dev)
             lq_feat = torch.empty((B, 256, 16, 16), dtype=torch.float32, device=dev)
@@ -513,8 +563,8 @@ class CodeFormer(VQAutoEncoder):
                 if li > 0:
                     st.wait_stream(cur)                       # inputs / weights produced on the caller's stream
                 with torch.cuda.stream(st):
-                    launch(x[lo:hi], logits[lo:hi], lq_feat[lo:hi], None if out is None else out[lo:hi],
-                           self._cfb_workspace(dev, hi - lo, lane=li))
+                    launch(x[lo:hi], w[lo:hi] if per_face else None, logits[lo:hi], lq_feat[lo:hi],
+                           None if out is None else out[lo:hi], self._cfb_workspace(dev, hi - lo, lane=li))
             for li in range(1, lanes):
                 cur.wait_stream(side[li - 1])                 # results are ordered on the caller's stream again
         if code_only:
@@ -523,15 +573,17 @@ class CodeFormer(VQAutoEncoder):
 
     # The reference's callers feed ONE face per call (inference_codeformer.py:197-206); at that size the forward is ~440
     # small launches and launch latency dominates.  Small batches are therefore replayed from a CUDA graph captured once
-    # per (batch, w, adain, code_only, precision): static input/output buffers, same kernels, same results.
+    # per (batch, w, adain, code_only, precision): static input/output buffers, same kernels, same results.  Per-face weights
+    # are an input buffer like the faces, so their key holds no w and one graph serves every w vector.
     cuda_graph_max_batch = 4
     cuda_graph_cache_size = 6
 
-    def _graphed(self, key, x, buffers, launch):
+    def _graphed(self, key, inputs, buffers, launch):
         """``launch(*bufs)`` replayed from the CUDA graph cached under ``key`` (the key holds the precision: the launch
-        sequence depends on it).  On a miss ``buffers()`` makes the static buffers, the first of which is the input, and the
-        graph is captured.  ``x`` is copied into the input before every run.  Returns the buffers after the replay (the
-        caller clones what it returns), or None where the plain launch path runs instead."""
+        sequence depends on it).  On a miss ``buffers()`` makes the static buffers, the first ``len(inputs)`` of which are the
+        inputs, and the graph is captured.  ``inputs`` (the faces first) are copied into them before every run.  Returns the
+        buffers after the replay (the caller clones what it returns), or None where the plain launch path runs instead."""
+        x = inputs[0]
         if not 0 < x.shape[0] <= self.cuda_graph_max_batch or os.environ.get('CFB_CUDA_GRAPH', '1') == '0' \
                 or getattr(self, '_cfb_hooks', None) or torch.cuda.is_current_stream_capturing():
             return None
@@ -540,7 +592,8 @@ class CodeFormer(VQAutoEncoder):
             while len(self._cfb_graphs) >= self.cuda_graph_cache_size:      # callers sweep w (Gradio slider): evict the LRU
                 self._cfb_graphs.pop(next(iter(self._cfb_graphs)))          # entry only; each pins one workspace
             bufs = buffers()
-            bufs[0].copy_(x)
+            for b, t in zip(bufs, inputs):
+                b.copy_(t)
             launch(*bufs)                                    # eager warm-up: one-time function attributes, lazy module load
             torch.cuda.current_stream(x.device).synchronize()
             g = torch.cuda.CUDAGraph()
@@ -554,7 +607,8 @@ class CodeFormer(VQAutoEncoder):
         if ent is False:
             return None
         g, bufs = ent
-        bufs[0].copy_(x)
+        for b, t in zip(bufs, inputs):
+            b.copy_(t)
         g.replay()
         return bufs
 
@@ -567,7 +621,12 @@ class CodeFormer(VQAutoEncoder):
 
         ``inpaint=True`` (``cfb_codeformer_inpaint_u8``) is inference_inpainting.py:64-75 (there ``w=1, adain=False`` on the
         codebook-512, 3-connect net): the output keeps the input face except where the face is white (255, 255, 255), the mask
-        the script builds, i.e. ``(1-mask)*input + mask*output`` before ``tensor2img``, fused into the last conv."""
+        the script builds, i.e. ``(1-mask)*input + mask*output`` before ``tensor2img``, fused into the last conv.
+
+        ``w`` is one fidelity weight, or one per face (``fidelity_weights``; ``cfb_codeformer_forward_u8_wv`` /
+        ``cfb_codeformer_inpaint_u8_wv``): face i equals the call on that face alone with ``w[i]``, byte for byte.  With per-face
+        weights the Fuse_sft_blocks run for every face (a face with w <= 0 blends with 0), so in fp16 precision their operand
+        range guard can fail a batch whose scalar calls would have skipped them."""
         if not torch.is_tensor(faces_bgr) or not faces_bgr.is_cuda or faces_bgr.dtype != torch.uint8:
             raise RuntimeError('forward_u8 expects a CUDA uint8 tensor')
         if faces_bgr.dim() != 4 or tuple(faces_bgr.shape[1:]) != (512, 512, 3):
@@ -575,24 +634,30 @@ class CodeFormer(VQAutoEncoder):
         lib = _lib.load()
         faces_bgr = faces_bgr.contiguous()
         B, dev = faces_bgr.shape[0], faces_bgr.device
-        w, adain, inpaint = float(w), bool(adain), bool(inpaint)
-        name = 'cfb_codeformer_inpaint_u8' if inpaint else 'cfb_codeformer_forward_u8'
+        w, adain, inpaint = fidelity_weights(w, B, dev), bool(adain), bool(inpaint)
+        per_face = torch.is_tensor(w)
+        name = ('cfb_codeformer_inpaint_u8' if inpaint else 'cfb_codeformer_forward_u8') + ('_wv' if per_face else '')
         fn = getattr(lib, name)
         with self._lock, torch.cuda.device(dev):
             self._prepare(dev)
             if B == 0:
                 return torch.empty_like(faces_bgr)
 
-            def launch(src, dst, ws):
-                _lib.check(fn(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w, int(adain), _lib.ptr(ws), ws.numel(),
-                              _lib.stream(dev)), name)
-            bufs = self._graphed(('u8', dev.index, B, w, adain, inpaint, self._precision), faces_bgr, lambda: (
-                torch.empty_like(faces_bgr), torch.empty_like(faces_bgr),
+            def launch(src, wv, dst, ws):
+                _lib.check(fn(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, w if wv is None else _lib.ptr(wv),
+                              int(adain), _lib.ptr(ws), ws.numel(), _lib.stream(dev)), name)
+            if per_face:
+                w = _weights_on(w, dev)
+                key, inputs = ('u8wv', dev.index, B, adain, inpaint, self._precision), (faces_bgr, w)
+            else:
+                key, inputs = ('u8', dev.index, B, w, adain, inpaint, self._precision), (faces_bgr,)
+            bufs = self._graphed(key, inputs, lambda: (
+                torch.empty_like(faces_bgr), torch.empty_like(w) if per_face else None, torch.empty_like(faces_bgr),
                 torch.empty(int(lib.cfb_workspace_bytes(self._net, B)), dtype=torch.uint8, device=dev)), launch)
             if bufs is not None:
-                return bufs[1].clone()
+                return bufs[2].clone()
             out = torch.empty_like(faces_bgr)
-            launch(faces_bgr, out, self._cfb_workspace(dev, B))
+            launch(faces_bgr, w if per_face else None, out, self._cfb_workspace(dev, B))
         return out
 
     def restore_faces(self, faces, w=0.5, adain=True, max_batch=32, device=None, on_error='input', inpaint=False):
@@ -602,7 +667,9 @@ class CodeFormer(VQAutoEncoder):
         passes to ``face_helper.add_restored_face``.  Faces go through pinned uint8 staging (0.79 MB per face each way)
         in chunks of ``max_batch``.  ``on_error='input'`` mirrors the reference's fallback (:209-211: on any failure the
         restored face is the input face); ``'raise'`` re-raises.  ``inpaint=True`` is the loop of inference_inpainting.py
-        (``forward_u8(inpaint=True)``; its fallback, :78-80, is the input face as well)."""
+        (``forward_u8(inpaint=True)``; its fallback, :78-80, is the input face as well).  ``w``: one fidelity weight or one per
+        face (``fidelity_weights``), each chunk taking its faces' weights; a chunk that fails (in fp16 precision the
+        Fuse_sft_blocks of per-face weights run even for faces with w <= 0) falls back on its own."""
         if torch.is_tensor(faces):
             arr = faces.detach().cpu().numpy()
         elif isinstance(faces, np.ndarray):
@@ -617,6 +684,9 @@ class CodeFormer(VQAutoEncoder):
         if on_error not in ('input', 'raise'):
             raise RuntimeError("on_error must be 'input' or 'raise'")
         dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        w = fidelity_weights(w, arr.shape[0], dev)
+        if torch.is_tensor(w):
+            w = _weights_on(w, dev)                    # once: the chunks take device slices (no host sync per chunk)
         max_batch = max(1, int(max_batch))
         self.last_restore_errors = []
         # chunks of <= max_batch faces; a chunk of >= 16 is split in two so that the host-side staging copies of one half
@@ -653,7 +723,8 @@ class CodeFormer(VQAutoEncoder):
                         self._cfb_ws[key] = pin
                     drain(1)                           # the buffers of chunk k-2 (same parity) are free again
                     pin[0].copy_(torch.from_numpy(np.ascontiguousarray(arr[lo:hi])))
-                    out = self.forward_u8(pin[0].to(dev, non_blocking=True), w=w, adain=adain, inpaint=inpaint)
+                    out = self.forward_u8(pin[0].to(dev, non_blocking=True), w=w[lo:hi] if torch.is_tensor(w) else w,
+                                          adain=adain, inpaint=inpaint)
                     pin[1].copy_(out, non_blocking=True)
                     ev = torch.cuda.Event()
                     ev.record(torch.cuda.current_stream(dev))

@@ -582,6 +582,7 @@ struct TcParams {
   __half* pl_lo;
   float* gn_part;           // optional GroupNorm(32) partials of `out`: [m_tile*4 + warp][32][mean, M2]
   int gn_cpg;               // channels per group = Cout/32
+  const float* sft_wv;      // [N] per-image w in place of sft_w | null (ConvArgs::sft_wv; raw-input kernels only, !XF)
 #if CFB_TC_STAMPS
   long long* dbg;           // diagnostics (cfb_debug_set_stamps): CTA 0 writes clock64() at its role hand-offs; null in production
 #endif
@@ -1378,8 +1379,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           if (p.sft_dec && inside[k]) {
             const float4 d = __ldg(reinterpret_cast<const float4*>(p.sft_dec + off));
             const float4 sc = __ldg(reinterpret_cast<const float4*>(p.sft_scale + off));
-            v.x = d.x + p.sft_w * (d.x * sc.x + v.x); v.y = d.y + p.sft_w * (d.y * sc.y + v.y);
-            v.z = d.z + p.sft_w * (d.z * sc.z + v.z); v.w = d.w + p.sft_w * (d.w * sc.w + v.w);
+            float sw = p.sft_w;     // per image (a tile never spans two): max(w, 0), so w <= 0 or NaN leaves dec unchanged
+            if constexpr (!XF) { if (p.sft_wv) { const float t = __ldg(p.sft_wv + n); sw = t > 0.f ? t : 0.f; } }
+            v.x = d.x + sw * (d.x * sc.x + v.x); v.y = d.y + sw * (d.y * sc.y + v.y);
+            v.z = d.z + sw * (d.z * sc.z + v.z); v.w = d.w + sw * (d.w * sc.w + v.w);
           }
           if (!inside[k]) v = make_float4(0.f, 0.f, 0.f, 0.f);          // outside the image: no store, no statistics
           if (p.out && inside[k]) *reinterpret_cast<float4*>(p.out + off) = v;      // null: only the operand planes are consumed
@@ -1838,7 +1841,10 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(a.in2 == nullptr, "conv_tc: a two-source input needs the fused operand transform");
   }
   p.bias = a.bias; p.residual = a.residual; p.out_act = a.out_act;
-  p.sft_dec = a.sft_dec; p.sft_scale = a.sft_scale; p.sft_w = a.sft_w; p.wscale_inv = a.wscale_inv;
+  // per-image SFT weights are read by the raw-input kernels only (the Fuse_sft_block's shift.2 conv reads shift.0's planes): the
+  // fused-transform variants keep their register budgets
+  CFB_REQUIRE(!a.sft_wv || (a.sft_dec && !a.xform), "conv_tc: per-image SFT weights need the SFT epilogue of a raw-input conv");
+  p.sft_dec = a.sft_dec; p.sft_scale = a.sft_scale; p.sft_w = a.sft_w; p.sft_wv = a.sft_wv; p.wscale_inv = a.wscale_inv;
   p.out = a.gen || !a.out ? a.out : a.out + a.out_c0;      // per-tap engine: the slice offset is folded into the base pointer
   p.gn_part = a.gn_part; p.gn_cpg = a.Cout / 32;
   p.pl_hi = (__half*)a.out_planes;
@@ -1911,7 +1917,7 @@ int bmm_tc(const BmmArgs& g, int sm_count, cudaStream_t st) {
 #endif
   p.Hin = 16; p.Win = 16; p.pad_mode = 0; p.sub = 0; p.out_pitch = out_pitch; p.out_c0 = 0; p.cout_valid = out_pitch; p.res_pitch = out_pitch;
   p.residual2 = nullptr; p.res2_pitch = out_pitch; p.post_scale = 1.f;
-  p.bias = nullptr; p.residual = nullptr; p.out_act = OUT_NONE; p.sft_dec = nullptr; p.sft_scale = nullptr; p.sft_w = 0.f;
+  p.bias = nullptr; p.residual = nullptr; p.out_act = OUT_NONE; p.sft_dec = nullptr; p.sft_scale = nullptr; p.sft_w = 0.f; p.sft_wv = nullptr;
   p.wscale_inv = g.scale_dev; p.out = g.out;
   p.gn_part = nullptr; p.gn_cpg = 0;
   p.pl_hi = (__half*)g.out_planes;

@@ -147,6 +147,7 @@ struct ConvArgs {
   const float* sft_dec = nullptr;
   const float* sft_scale = nullptr;
   float sft_w = 0.f;
+  const float* sft_wv = nullptr;    // [N] per-image w (device) in place of sft_w | null; w <= 0 or NaN blends with 0 (out = dec)
   float* out = nullptr;             // [N,Ho,Wo,Cout]
   // tensor-core engine only: GroupNorm(32) partials of `out`, [N*tiles_per_image*4][32 groups][mean, M2] floats
   float* gn_part = nullptr;

@@ -628,6 +628,7 @@ struct Fwd {
     const float* in_scale = nullptr; const float* in_shift = nullptr; int in_act = IN_NONE;
     const float* residual = nullptr; int out_act = OUT_NONE;
     const float* sft_dec = nullptr; const float* sft_scale = nullptr; float sft_w = 0.f;
+    const float* sft_wv = nullptr;   // [N] per-image w on the device in place of sft_w
     float* out_ptr = nullptr;   // write into caller memory instead of the arena
     bool want_stats = false;    // consumer is a GroupNorm: let the tensor-core epilogue emit the partial sums
     bool want_planes = false;   // a following conv reads this output raw: emit its fp16 hi/lo operand planes too
@@ -643,7 +644,7 @@ struct Fwd {
     a.in = in.p; a.N = in.N; a.H = in.H; a.W = in.W; a.Cin = in.C; a.Ho = Ho; a.Wo = Wo; a.Cout = w.cout;
     a.ksize = w.k; a.mode = o.mode; a.wgt_f32 = w.w_f32; a.wgt_hi = w.w_hi; a.wgt_lo = w.w_lo; a.wscale_inv = w.wscale + 1; a.bias = w.bias;
     a.in_scale = o.in_scale; a.in_shift = o.in_shift; a.in_act = o.in_act; a.residual = o.residual;
-    a.out_act = o.out_act; a.sft_dec = o.sft_dec; a.sft_scale = o.sft_scale; a.sft_w = o.sft_w;
+    a.out_act = o.out_act; a.sft_dec = o.sft_dec; a.sft_scale = o.sft_scale; a.sft_w = o.sft_w; a.sft_wv = o.sft_wv;
     bool use_tc = engine == 2 || (engine == 0 && n->tc_ok && tc_tiles_exact(a));
     CFB_REQUIRE(dry || !single_pass || use_tc, "conv: precision fp16 runs on the wgmma engine only: " + w.name);
     a.single_pass = single_pass;
@@ -796,8 +797,8 @@ struct Fwd {
     return 0;
   }
 
-  // Fuse_sft_block.forward  codeformer_arch.py:151-157
-  int fuse(const FuseW& f, const Tensor& enc_feat, const Tensor& dec, float wgt, Tensor& y) {
+  // Fuse_sft_block.forward  codeformer_arch.py:151-157; wv: per-image w (device, [N]) in place of wgt, or null
+  int fuse(const FuseW& f, const Tensor& enc_feat, const Tensor& dec, float wgt, const float* wv, Tensor& y) {
     Tensor cat;
     const bool stats_from_parts = enc_feat.gn_part && dec.gn_part && enc_feat.gn_slots == dec.gn_slots && enc_feat.C == dec.C;
     bool two_src = false;
@@ -842,7 +843,7 @@ struct Fwd {
     release(s0);
     CFB_CHECK(conv(f.h0, e, h0, ol));
     release(e);
-    ConvOpt of; of.sft_dec = dec.p; of.sft_scale = sc.p; of.sft_w = wgt; of.want_stats = true; of.want_planes = true;
+    ConvOpt of; of.sft_dec = dec.p; of.sft_scale = sc.p; of.sft_w = wgt; of.sft_wv = wv; of.want_stats = true; of.want_planes = true;
     CFB_CHECK(conv(f.h2, h0, y, of));
     release(h0); release(sc);
     return 0;
@@ -913,8 +914,11 @@ struct Fwd {
     return 0;
   }
 
-  // Generator.forward with the SFT fusion of codeformer_arch.py:272-277; writes NCHW into out_nchw
-  int generator(Tensor x, float* out_nchw, std::map<int, Tensor>* taps, const std::vector<int>& fuse_blocks, float w) {
+  // Generator.forward with the SFT fusion of codeformer_arch.py:272-277; writes NCHW into out_nchw.  wv (device, [N]): one w
+  // per image; the fusion then runs whatever the values, and an image with w <= 0 (or NaN) blends with 0, i.e. keeps dec
+  int generator(Tensor x, float* out_nchw, std::map<int, Tensor>* taps, const std::vector<int>& fuse_blocks, float w,
+                const float* wv = nullptr) {
+    const bool fusing = taps && (w > 0.f || wv);
     // fp16 precision: the convs of every generator block and of the fusion run single pass, except the AttnBlocks' q,k,v and
     // proj_out (about 2 of 586 GF per face); conv_last is the fp32 SIMT conv in both precisions
     const bool p1 = n->precision == 1;
@@ -923,7 +927,7 @@ struct Fwd {
       const Block& b = n->gen[i];
       single_pass = p1 && b.kind != B_ATTN;
       bool pl = next_takes_planes(n->gen, i);
-      if (taps && w > 0.f)
+      if (fusing)
         for (int fb : fuse_blocks)
           if ((int)i == fb) pl = false;      // consumed by the fusion (concat + SFT read fp32); the fused output emits its own
       Tensor y;
@@ -954,7 +958,7 @@ struct Fwd {
       release(x);
       x = y;
       CFB_CHECK(capture("gen." + std::to_string(i), x));
-      if (taps && w > 0.f)
+      if (fusing)
         for (int fb : fuse_blocks)
           if ((int)i == fb) {
             auto it = taps->find(x.W);
@@ -963,7 +967,7 @@ struct Fwd {
             CFB_REQUIRE(fw != n->fuse.end(), "fusion: no Fuse_sft_block for this size");
             Tensor fz;
             single_pass = p1;
-            CFB_CHECK(fuse(fw->second, it->second, x, w, fz));
+            CFB_CHECK(fuse(fw->second, it->second, x, w, wv, fz));
             release(x);
             release(it->second);
             x = fz;
@@ -1095,7 +1099,7 @@ static std::vector<int> tap_blocks_of(const cfb_config& c, bool encoder) {
 static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float* logits, float* lq_feat,
                                    int64_t* top_idx, int B, float w, int adain, int code_only, void* ws, int64_t ws_bytes,
                                    cudaStream_t st, bool dry, const unsigned char* x_u8 = nullptr,
-                                   unsigned char* out_u8 = nullptr, bool inpaint = false) {
+                                   unsigned char* out_u8 = nullptr, bool inpaint = false, const float* w_dev = nullptr) {
   CFB_REQUIRE(n->cfg.kind == 1, "net was created as VQAutoEncoder");
   CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
   if (!dry) CFB_CHECK(check_device(n));
@@ -1109,7 +1113,8 @@ static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float
   const cfb_config& c = n->cfg;
   std::map<int, Tensor> taps;
   Tensor lq;
-  const bool want_taps = (w > 0.f) && !code_only;   // codeformer_arch.py:276 -- features are only consumed when w>0
+  // codeformer_arch.py:276 -- features are only consumed when w>0; a per-image w (w_dev) always runs the fusion
+  const bool want_taps = (w > 0.f || w_dev) && !code_only;
   CFB_CHECK(f.encoder(x, B, lq, want_taps ? &taps : nullptr, tap_blocks_of(c, true)));
   const int T = B * lq.H * lq.W;
   float* logits_buf = logits;
@@ -1134,7 +1139,7 @@ static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float
   }
   CFB_CHECK(f.capture("quant", quant));
   f.release(lq);
-  CFB_CHECK(f.generator(quant, out, want_taps ? &taps : nullptr, tap_blocks_of(c, false), w));
+  CFB_CHECK(f.generator(quant, out, want_taps ? &taps : nullptr, tap_blocks_of(c, false), w, w_dev));
   return 0;
 }
 
@@ -2617,32 +2622,50 @@ int cfb_net_capture(cfb_net* n, const char* stage, float* dst, int64_t capacity)
   API_END(1)
 }
 
+static int codeformer_f32(const char* what, cfb_net* n, const float* x, float* out, float* logits, float* lq_feat,
+                          int64_t* top_idx, int32_t batch, float w, const float* w_dev, int32_t adain, int32_t code_only,
+                          void* workspace, int64_t workspace_bytes, void* stream) {
+  CFB_REQUIRE(n, std::string(what) + ": NULL net");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(x, std::string(what) + ": NULL input");
+  std::lock_guard<std::mutex> lk(n->mu);   // two caller threads may share one net (web-demos/hugging_face/app.py:282)
+  const int64_t before = cfb::launch_count();
+  const int rc = cfb::codeformer_forward_impl(n, x, out, logits, lq_feat, top_idx, batch, w, adain, code_only, workspace,
+                                              workspace_bytes, (cudaStream_t)stream, false, nullptr, nullptr, false, w_dev);
+  n->last_launches = cfb::launch_count() - before;
+  return rc;
+}
+
 int cfb_codeformer_forward(cfb_net* n, const float* x, float* out, float* logits, float* lq_feat, int64_t* top_idx,
                            int32_t batch, float w, int32_t adain, int32_t code_only, void* workspace,
                            int64_t workspace_bytes, void* stream) {
   API_BEGIN
-  CFB_REQUIRE(n, "cfb_codeformer_forward: NULL net");
-  if (batch == 0) return 0;
-  CFB_REQUIRE(x, "cfb_codeformer_forward: NULL input");
-  std::lock_guard<std::mutex> lk(n->mu);   // two caller threads may share one net (web-demos/hugging_face/app.py:282)
-  const int64_t before = cfb::launch_count();
-  const int rc = cfb::codeformer_forward_impl(n, x, out, logits, lq_feat, top_idx, batch, w, adain, code_only, workspace,
-                                              workspace_bytes, (cudaStream_t)stream, false);
-  n->last_launches = cfb::launch_count() - before;
-  return rc;
+  return codeformer_f32("cfb_codeformer_forward", n, x, out, logits, lq_feat, top_idx, batch, w, nullptr, adain, code_only,
+                        workspace, workspace_bytes, stream);
+  API_END(1)
+}
+
+int cfb_codeformer_forward_wv(cfb_net* n, const float* x, float* out, float* logits, float* lq_feat, int64_t* top_idx,
+                              int32_t batch, const float* w_dev, int32_t adain, int32_t code_only, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(w_dev || batch == 0, "cfb_codeformer_forward_wv: NULL w_dev");
+  return codeformer_f32("cfb_codeformer_forward_wv", n, x, out, logits, lq_feat, top_idx, batch, 0.f, w_dev, adain, code_only,
+                        workspace, workspace_bytes, stream);
   API_END(1)
 }
 
 static int codeformer_u8(const char* what, cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits,
                          float* lq_feat, int64_t* top_idx, int32_t batch, float w, int32_t adain, void* workspace,
-                         int64_t workspace_bytes, void* stream, bool inpaint) {
+                         int64_t workspace_bytes, void* stream, bool inpaint, const float* w_dev = nullptr) {
   CFB_REQUIRE(n, std::string(what) + ": NULL net");
   if (batch == 0) return 0;
   CFB_REQUIRE(faces_bgr && restored_bgr, std::string(what) + ": NULL image pointer");
   std::lock_guard<std::mutex> lk(n->mu);
   const int64_t before = cfb::launch_count();
   const int rc = cfb::codeformer_forward_impl(n, nullptr, nullptr, logits, lq_feat, top_idx, batch, w, adain, 0, workspace,
-                                              workspace_bytes, (cudaStream_t)stream, false, faces_bgr, restored_bgr, inpaint);
+                                              workspace_bytes, (cudaStream_t)stream, false, faces_bgr, restored_bgr, inpaint,
+                                              w_dev);
   n->last_launches = cfb::launch_count() - before;
   return rc;
 }
@@ -2662,6 +2685,26 @@ int cfb_codeformer_inpaint_u8(cfb_net* n, const uint8_t* faces_bgr, uint8_t* res
   API_BEGIN
   return codeformer_u8("cfb_codeformer_inpaint_u8", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, w, adain,
                        workspace, workspace_bytes, stream, true);
+  API_END(1)
+}
+
+int cfb_codeformer_forward_u8_wv(cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                                 int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(w_dev || batch == 0, "cfb_codeformer_forward_u8_wv: NULL w_dev");
+  return codeformer_u8("cfb_codeformer_forward_u8_wv", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, 0.f, adain,
+                       workspace, workspace_bytes, stream, false, w_dev);
+  API_END(1)
+}
+
+int cfb_codeformer_inpaint_u8_wv(cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                                 int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(w_dev || batch == 0, "cfb_codeformer_inpaint_u8_wv: NULL w_dev");
+  return codeformer_u8("cfb_codeformer_inpaint_u8_wv", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, 0.f, adain,
+                       workspace, workspace_bytes, stream, true, w_dev);
   API_END(1)
 }
 
@@ -2950,13 +2993,12 @@ int cfb_debug_conv_tc(const float* in, const float* in2, int32_t cin1, const flo
                                 tile_n, 3, cfb::OUT_NONE, 0);
 }
 
-int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
-                           float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
-                           const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
-                           const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
-                           void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
-                           int32_t out_act, int32_t precision) {
-  API_BEGIN
+static int debug_conv_tc(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                         float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                         const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                         const float* sft_dec, const float* sft_scale, float sft_w, const float* sft_wv, void* out_planes,
+                         float* gn_part, void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
+                         int32_t out_act, int32_t precision) {
   CFB_REQUIRE(in && weight_oihw && out && workspace && tile_n, "cfb_debug_conv_tc: NULL argument");
   CFB_REQUIRE(mode == cfb::CONV_SAME || mode == cfb::CONV_UP, "cfb_debug_conv_tc: mode must be 0 or 2");
   CFB_REQUIRE(ksize == 3 || (ksize == 1 && mode == cfb::CONV_SAME && !xform), "cfb_debug_conv_tc_prec: ksize 3, or 1 (raw, mode 0)");
@@ -2970,7 +3012,7 @@ int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, cons
   a.Ho = mode == cfb::CONV_UP ? h * 2 : h;
   a.Wo = mode == cfb::CONV_UP ? w * 2 : w;
   a.bias = bias; a.in_scale = in_scale; a.in_shift = in_shift; a.in_act = in_act; a.residual = residual; a.out = out;
-  a.sft_dec = sft_dec; a.sft_scale = sft_scale; a.sft_w = sft_w; a.out_planes = out_planes; a.gn_part = gn_part;
+  a.sft_dec = sft_dec; a.sft_scale = sft_scale; a.sft_w = sft_w; a.sft_wv = sft_wv; a.out_planes = out_planes; a.gn_part = gn_part;
   a.in2 = in2; a.Cin1 = in2 ? cin1 : 0;
   a.out_act = out_act; a.single_pass = precision == 1;
   CFB_REQUIRE(cfb::tc_supported(a), "cfb_debug_conv_tc: shape not on the wgmma engine");
@@ -2994,6 +3036,32 @@ int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, cons
   *tile_n = cfb::tc_tile_n(a);
   CFB_CHECK(cfb::conv_tc(a, p, sms, st));
   return 0;
+}
+
+int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                           float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                           const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                           const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
+                           void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
+                           int32_t out_act, int32_t precision) {
+  API_BEGIN
+  return debug_conv_tc(in, in2, cin1, weight_oihw, bias, out, n, h, w, cin, cout, mode, xform, in_scale, in_shift, in_act, residual,
+                       sft_dec, sft_scale, sft_w, nullptr, out_planes, gn_part, workspace, workspace_bytes, stream, tile_n, ksize,
+                       out_act, precision);
+  API_END(1)
+}
+
+int cfb_debug_conv_tc_prec_wv(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                              float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                              const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                              const float* sft_dec, const float* sft_scale, const float* sft_wv, void* out_planes,
+                              float* gn_part, void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n,
+                              int32_t ksize, int32_t out_act, int32_t precision) {
+  API_BEGIN
+  CFB_REQUIRE(sft_wv || !sft_dec, "cfb_debug_conv_tc_prec_wv: NULL sft_wv with an SFT epilogue");
+  return debug_conv_tc(in, in2, cin1, weight_oihw, bias, out, n, h, w, cin, cout, mode, xform, in_scale, in_shift, in_act, residual,
+                       sft_dec, sft_scale, 0.f, sft_wv, out_planes, gn_part, workspace, workspace_bytes, stream, tile_n, ksize,
+                       out_act, precision);
   API_END(1)
 }
 int cfb_debug_time_conv(const float* in, const float* weight_oihw, float* out, int32_t n, int32_t h, int32_t w, int32_t cin,

@@ -195,8 +195,10 @@ __global__ void __launch_bounds__(256) conv_f32_kernel(ConvArgs a) {
       if (a.sft_dec) {
         const float4 d = __ldg(reinterpret_cast<const float4*>(a.sft_dec + off));
         const float4 s = __ldg(reinterpret_cast<const float4*>(a.sft_scale + off));
-        v.x = d.x + a.sft_w * (d.x * s.x + v.x); v.y = d.y + a.sft_w * (d.y * s.y + v.y);
-        v.z = d.z + a.sft_w * (d.z * s.z + v.z); v.w = d.w + a.sft_w * (d.w * s.w + v.w);
+        float sw = a.sft_w;
+        if (a.sft_wv) { const float t = __ldg(a.sft_wv + m / ((int64_t)a.Ho * a.Wo)); sw = t > 0.f ? t : 0.f; }
+        v.x = d.x + sw * (d.x * s.x + v.x); v.y = d.y + sw * (d.y * s.y + v.y);
+        v.z = d.z + sw * (d.z * s.z + v.z); v.w = d.w + sw * (d.w * s.w + v.w);
       }
       *reinterpret_cast<float4*>(a.out + off) = v;
     }

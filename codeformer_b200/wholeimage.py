@@ -34,6 +34,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .arch import fidelity_weights
 from .detection import RetinaFace, cuda_u8_image
 from .detection import finish_detections as retinaface_finish
 from .upsampler import RealESRGANer
@@ -157,14 +158,14 @@ def _as_input(img, dev, name='restore_images'):
 
 
 def _restore(net, crops, w, max_batch, errors, adain=True, name='restore_images'):
-    """CodeFormer over the crops in batches of <= max_batch; a failed batch gives its input faces back (the reference's
-    per-face fallback, inference_codeformer.py:208-210)."""
+    """CodeFormer over the crops in batches of <= max_batch (``w``: a float, or a float32 tensor of one weight per crop); a
+    failed batch gives its input faces back (the reference's per-face fallback, inference_codeformer.py:208-210)."""
     out = torch.empty_like(crops)
     dev = crops.device
     for lo in range(0, crops.shape[0], max_batch):
         hi = min(crops.shape[0], lo + max_batch)
         try:
-            res = net.forward_u8(crops[lo:hi], w=w, adain=adain)
+            res = net.forward_u8(crops[lo:hi], w=w[lo:hi] if torch.is_tensor(w) else w, adain=adain)
             torch.cuda.current_stream(dev).synchronize()
             _lib.check(_lib.load().cfb_check_async_status(), name)
             out[lo:hi] = res
@@ -195,12 +196,18 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
     without a face upsampler, as the reference's ``restored_faces`` holds them).  A gray image whose pasted canvas exceeds
     256 comes back uint16, as in the reference.  Each image equals the
     reference loop body on that image alone, whatever ``max_batch`` is.  ``self.last_restore_errors`` of the reference's
-    fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back."""
+    fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back.
+
+    ``w``: one fidelity weight, or one per image (``fidelity_weights`` over the images): every face of image i is restored
+    with ``w[i]``, and faces of images with different weights still share CodeFormer batches."""
     import cv2    # estimateAffinePartial2D(LMEDS) / invertAffineTransform stay on the host, as in the reference
     images = list(images)
     dev = next(net.parameters()).device
     if dev.type != 'cuda':
         raise RuntimeError('restore_images: the network is not on a CUDA device; there is no CPU fallback')
+    w = fidelity_weights(w, len(images), dev)
+    if torch.is_tensor(w):
+        w = w.cpu()                                    # picked per face on the host, moved with each chunk's faces
     max_batch = max(1, int(max_batch))
     inputs = [_as_input(im, dev) for im in images]
     results, crops_out, faces_out = [None] * len(images), [None] * len(images), [None] * len(images)
@@ -230,8 +237,9 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
                 affines.append(cv2.estimateAffinePartial2D(landmark, FACE_TEMPLATE, method=cv2.LMEDS)[0])
                 owner.append(k)
         crops = warp_faces_multi(x, affines, owner, FACE_SIZE)
+        wf = w[torch.as_tensor(np.asarray(idx, np.int64)[np.asarray(owner, np.int64)])].to(dev) if torch.is_tensor(w) else w
         with torch.no_grad():
-            restored = _restore(net, crops, w, max_batch, errors)
+            restored = _restore(net, crops, wf, max_batch, errors)
         owner = np.asarray(owner, np.int64)
         # add_restored_face: the faces of gray images become adain_npy(bgr2gray(restored), cropped), float64
         is_g = np.asarray([gray[k] for k in owner], bool)
@@ -329,7 +337,8 @@ def restore_aligned(faces, net, w=0.5, adain=True, max_batch=32, return_crops=Fa
     ``is_gray(img, threshold=10)`` of the resized crop, CodeFormer with ``w`` / ``adain`` (``forward_u8`` over all crops in
     batches of ``max_batch``; a failed batch gives its input crops back, as the reference's per-face fallback does, and
     ``restore_aligned.last_errors`` lists (crop offset, message) of each) and ``add_restored_face``: the gray crops become
-    ``adain_npy(bgr2gray(restored), cropped)`` in float64 (``gray_adain_faces``).
+    ``adain_npy(bgr2gray(restored), cropped)`` in float64 (``gray_adain_faces``).  ``w``: one fidelity weight, or one per
+    crop (``fidelity_weights``).
 
     The gray test runs on the device for all crops at once (``cfb_is_gray_u8``): exact integer moments, so it decides as the
     reference's numpy variances do except for a crop whose score is within numpy's rounding of the threshold.
@@ -342,6 +351,9 @@ def restore_aligned(faces, net, w=0.5, adain=True, max_batch=32, return_crops=Fa
     if dev.type != 'cuda':
         raise RuntimeError('restore_aligned: the network is not on a CUDA device; there is no CPU fallback')
     max_batch = max(1, int(max_batch))
+    w = fidelity_weights(w, len(faces), dev)
+    if torch.is_tensor(w):
+        w = w.to(dev)
     inputs = [_as_input(f, dev, 'restore_aligned') for f in faces]
     n = len(inputs)
     crops = torch.empty((n, FACE_SIZE, FACE_SIZE, 3), dtype=torch.uint8, device=dev)

@@ -91,6 +91,13 @@ int64_t  cfb_last_launch_count(cfb_net* net);
 int cfb_codeformer_forward(cfb_net* net, const float* x, float* out, float* logits, float* lq_feat,
                            int64_t* top_idx, int32_t batch, float w, int32_t adain, int32_t code_only,
                            void* workspace, int64_t workspace_bytes, void* stream);
+/* Per-face fidelity weights: the *_wv entry points take w_dev, a DEVICE float [batch] (one w per face, on `stream`), in place of
+ * `w`.  Face i equals the scalar call on that face alone with w = w_dev[i], bit for bit; a face with w_dev[i] <= 0 or NaN gets
+ * the skipped-fusion result of w <= 0.  The Fuse_sft_blocks run for every face whatever the values (their blend multiplies by
+ * max(w, 0)), so in fp16 precision their operand range guard may also fail a batch whose faces all have w <= 0. */
+int cfb_codeformer_forward_wv(cfb_net* net, const float* x, float* out, float* logits, float* lq_feat,
+                              int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain, int32_t code_only,
+                              void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Same call with HOST buffers (pinned recommended): H2D of x, forward, D2H of out/logits/lq_feat,
  * all on `stream`, then one stream synchronise.  dev_scratch must hold the device copies:
@@ -116,6 +123,13 @@ int cfb_codeformer_forward_u8(cfb_net* net, const uint8_t* faces_bgr, uint8_t* r
 int cfb_codeformer_inpaint_u8(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
                               int64_t* top_idx, int32_t batch, float w, int32_t adain,
                               void* workspace, int64_t workspace_bytes, void* stream);
+/* the two uint8 forwards with one w per face (w_dev: DEVICE float [batch], see cfb_codeformer_forward_wv) */
+int cfb_codeformer_forward_u8_wv(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                                 int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
+int cfb_codeformer_inpaint_u8_wv(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                                 int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
 /* the same with HOST uint8 buffers (0.79 MB per face each way instead of 3.1 MB): H2D, forward, D2H, stream sync.
  * dev_scratch >= cfb_host_io_bytes(net, batch). */
 int cfb_codeformer_restore_host(cfb_net* net, const uint8_t* faces_host, uint8_t* restored_host, int32_t batch, float w,
@@ -221,6 +235,14 @@ int cfb_debug_conv_tc_prec(const float* in, const float* in2, int32_t cin1, cons
                            const float* sft_dec, const float* sft_scale, float sft_w, void* out_planes, float* gn_part,
                            void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n, int32_t ksize,
                            int32_t out_act, int32_t precision);
+/* cfb_debug_conv_tc_prec with one SFT weight per image: sft_wv (DEVICE float [n], required with sft_dec) in place of sft_w;
+ * image i blends with max(sft_wv[i], 0) (NaN: 0). */
+int cfb_debug_conv_tc_prec_wv(const float* in, const float* in2, int32_t cin1, const float* weight_oihw, const float* bias,
+                              float* out, int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t mode, int32_t xform,
+                              const float* in_scale, const float* in_shift, int32_t in_act, const float* residual,
+                              const float* sft_dec, const float* sft_scale, const float* sft_wv, void* out_planes,
+                              float* gn_part, void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n,
+                              int32_t ksize, int32_t out_act, int32_t precision);
 /* diagnostics / tests: the GroupNorm(32) finalize of the forward on partials in the layout cfb_debug_conv_tc writes (slots of
  * 32 pixels, [n][slots][32 groups][2] floats): scale[n,c] = rstd*gamma, shift[n,c] = beta - mean*rstd*gamma over hw pixels
  * of c channels.  The workspace (>= cfb_debug_gn_partials_workspace_bytes) holds the split-finalize scratch and the ticket
