@@ -403,6 +403,10 @@ __device__ __forceinline__ void wg_mma_64x128(float (&d)[64], uint64_t da, uint6
       : "memory");
 }
 __device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// Per-warpgroup register limit (.sync.aligned: every thread of the warpgroup executes it).  `inc` blocks until other
+// warpgroups have released enough registers with `dec`.
+template <int N> __device__ __forceinline__ void wg_regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void wg_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // Warpgroup-uniform decision (named barrier `bar_id` over the 128 threads of one MMA warpgroup: 2 for physical warps 0..3, 3
 // for warps 4..7): true when `v` holds in any thread.  The wgmma instructions are .sync.aligned over the warpgroup, so after a
@@ -486,11 +490,13 @@ __device__ __forceinline__ void xf_chunk(const uint4& a, const uint4& b, const f
   if constexpr (LO) lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
 }
 // One patch: RPP rows per pass (8 lanes per row), two passes in flight per iteration.  LO = false: the hi plane only.
+// The 2 transform warps of the 128-wide tiles (RPP = 8) run on 96 registers: their 12 iterations stay a loop, which
+// ptxas would otherwise interleave into spills.
 template <int MODE, int RPP, int NPASS, int PW, int ROWS, bool LO = true>
 __device__ __forceinline__ void xf_patch(uint32_t src_base, uint32_t hi_base, uint32_t lo_base, int c0, int j, int rsub,
                                          const float (&sc)[8], const float (&sh)[8], bool border, int y0, int x0, int Hin,
                                          int Win, float& amax) {
-#pragma unroll
+#pragma unroll (RPP >= 16 ? 64 : 1)
   for (int it = 0; it < NPASS; it += 2) {
     uint4 a[2], b[2];
     bool act[2];
@@ -603,24 +609,28 @@ constexpr int TC_A_BYTES = 128 * 128;                 // 128 pixels x 64 fp16
 //   BN = 64 (every engine): one MMA warpgroup issues the wgmma of the whole 128-row tile into 2 x 32 fp32 registers per thread
 //     and hands every partial sum to 8 epilogue warps (4 row quadrants x 2 column halves), which fold it into registers.
 //   BN = 128 (halo engine, 3x3 and Upsample convs with Cout % 128 == 0): two MMA warpgroups, one per 64-pixel half, issue
-//     m64n128k16 into 64 fp32 registers per thread and fold their partial sums themselves into the shared fp32 tile slot;
-//     4 epilogue warps (one per row quadrant, all 128 columns) read the finished tile from the slot.  A 64-channel patch is
-//     transformed once per 128 output channels instead of once per 64, and each A byte read from shared memory feeds twice
-//     the MACs.  16 warps (8 MMA, TMA, 4 epilogue, 2 transform, patch loader) leave 128 registers per thread.
+//     m64n128k16 into 64 fp32 registers per thread and fold their partial sums themselves into a 64-float running sum in
+//     registers; the finished tile goes through the shared fp32 tile slot once, and 4 epilogue warps (one per row quadrant,
+//     all 128 columns) read it from there.  A 64-channel patch is transformed once per 128 output channels instead of once
+//     per 64, and each A byte read from shared memory feeds twice the MACs.  16 warps (8 MMA, TMA, 4 epilogue, 2 transform,
+//     patch loader; without the transform 3 idle warps) in 4 warpgroups: the MMA warpgroups run on 160 registers, the
+//     others on 96 (setmaxnreg).
 template <int BN>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128, "the wgmma engine runs 64- or 128-wide n-tiles");
   static constexpr bool WIDE = BN == 128;
   static constexpr int MMA_WARPS = WIDE ? 8 : 4;
   static constexpr int EPI_WARPS = WIDE ? 4 : 8;
-  static constexpr int THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS);   // MMA warpgroup(s), TMA warp, epilogue warps
+  // MMA warpgroup(s), TMA warp, epilogue warps; BN = 128 runs whole warpgroups (setmaxnreg), padded with 3 idle warps
+  static constexpr int THREADS = WIDE ? 512 : 32 * (MMA_WARPS + 1 + EPI_WARPS);
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * TC_A_BYTES + 2 * B_BYTES;
   static constexpr int STAGES = 3;
   // Partial-sum hand-off (128 rows, padded by 4 floats against bank conflicts).  BN = 64: the MMA warpgroup stores each
   // partial sum here and goes on with the next chunk while the epilogue warps fold the slot into their fp32 registers with
-  // round-to-nearest adds.  BN = 128: the MMA warpgroups keep the running sum here (first chunk stored, later chunks added with
-  // round-to-nearest adds: the same sums in the same order), the epilogue reads the tile once.
+  // round-to-nearest adds.  BN = 128: the MMA warpgroups store the finished tile here once (their running sum in registers:
+  // first chunk 0 + sum, later chunks added with round-to-nearest adds, the same sums in the same order), the epilogue reads
+  // it once.
   static constexpr int SLOT_PITCH = BN + 4;
   static constexpr int SLOT_BYTES = 128 * SLOT_PITCH * 4;
   static constexpr int SLOTS = 1;
@@ -638,7 +648,8 @@ struct TcCfg {
   // fused operand transform (XF, halo engine only): the A patches arrive as the RAW fp32 activation (two 32-channel planes per
   // slot) and the transform warps apply GroupNorm-affine + SiLU + the hi/lo split in place before the MMAs read them
   static constexpr int XF_WARPS = WIDE ? 2 : 4;             // a BN = 128 patch feeds twice the MMA time of a BN = 64 one
-  static constexpr int XF_THREADS = THREADS + 32 * XF_WARPS + 32;
+  static constexpr int XF_THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS + XF_WARPS + 1);
+  static_assert(!WIDE || XF_THREADS == THREADS, "the 128-wide transform variant fills the pad warps exactly");
   static constexpr int X_A_SLOTS = 2;
   static constexpr int X_A_PLANE2 = H_A_PLANE + XF_SKEW;   // second plane of an XF slot (ends at 46720 <= H_A_SLOT)
   static constexpr int X_B_SLOTS = H_B_SLOTS;
@@ -706,6 +717,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   const int warp = pwarp < MMA_WARPS ? 1 : (ridx == 0 ? 0 : ridx + 1);
   const int lane = threadIdx.x & 31;
   bool aborted = false;      // set when a barrier wait timed out anywhere on the device: leave the role loop (see mbar_wait)
+  if constexpr (WIDE) {
+    // 16 warps cap every thread at 128 registers; the MMA warpgroups (0-1) hold 64 accumulators and the 64-float running sum
+    // of their tile, so they take 160 (`inc` at the top of the MMA role) from warpgroups 2-3 (TMA, epilogue, transform,
+    // patch loader or idle pad warps), which give theirs back here, before the first barrier of the kernel, and run on 96:
+    // 2 x 128 x 160 + 2 x 128 x 96 = 65 536.  `inc` never waits on a warpgroup that is itself waiting (abort path included).
+    if (pwarp >= MMA_WARPS) wg_regs_dec<96>();
+  }
   if (threadIdx.x == 0) TC_STAMP(0);
 
   if (warp == 0 && lane == 0) {
@@ -826,6 +844,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // the TMA unit used when it wrote the buffer.
     // CM: the same descriptor is the B operand and spans the whole 128-pixel tile: its 16 core-matrix groups are the 16 patch
     // rows, PW*128 B apart, and the second 64-row half starts a_half = 8 groups in.
+    if constexpr (WIDE) wg_regs_inc<160>();
     {
       constexpr bool N128 = WIDE || CM;                 // m64n128k16 issue: one accumulator of 64 fp32 per thread
       constexpr int MH = N128 ? 1 : 2;                  // 64-row halves issued by this warpgroup
@@ -845,8 +864,37 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       if constexpr (N128) {
         // BN = 128 and CM: per chunk of k-blocks, every k-block's group is committed with one earlier group still in flight
         // (wait_group 1, a fixed depth), after which the weight slot (and, after its last tap, the patch) of the PREVIOUS
-        // k-block is released; wait_group 0 only after the chunk's last k-block, where the partial sum is folded (BN = 128)
-        // or handed to the epilogue warps (CM).
+        // k-block is released; wait_group 0 only after the chunk's last k-block, where the partial sum is folded into the
+        // running sum in registers (BN = 128) or handed to the epilogue warps (CM).
+        // BN = 128: `run` is the tile's running sum (first chunk 0 + sum, later chunks added with round-to-nearest: the sums
+        // of the 128 x 64 path in the same order).  A finished tile is stored into the slot once, after the next tile's first
+        // k-block has been issued, so the store runs under that k-block's MMAs and the epilogue has a whole tile of MMA time
+        // to drain the slot.
+        float run[64];                                               // BN = 128 only (CM never touches it)
+        // run -> slot [row][SLOT_PITCH] -> epilogue warps; true when the wait for the slot was abandoned (abort)
+        auto hand_off = [&]() -> bool {
+          mbar_wait(smem_u32(cempty + slot), slot_phase ^ 1, aborted);
+          if (wg_any(aborted, bar_id)) return true;
+          const int row = wg * 64 + wq * 16 + (lane >> 2);
+          // this thread's first slot element, formed anew per hand-off (opaque move): otherwise the compiler keeps the 32
+          // store addresses live across the tile loop and spills them; this way they are immediate offsets of one register
+          uint32_t e0;
+          asm volatile("mov.b32 %0, %1;" : "=r"(e0)
+                       : "r"(slot_base + (uint32_t)(slot * Cfg::SLOT_BYTES) + (uint32_t)((row * Cfg::SLOT_PITCH + 2 * (lane & 3)) * 4)));
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int h8 = 0; h8 < 2; ++h8) {
+              const uint32_t e = e0 + (uint32_t)((8 * h8 * Cfg::SLOT_PITCH + 8 * j) * 4);
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(e), "f"(run[4 * j + 2 * h8]), "f"(run[4 * j + 2 * h8 + 1])
+                           : "memory");
+            }
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
+          if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+          return false;
+        };
         for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
           const int par = p.up4 ? ((tile / p.n_tiles) & 3) : 0;    // output parity of this tile
           const int par_y = par >> 1, par_x = par & 1;
@@ -889,6 +937,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 }
               }
               wg_commit();
+              if constexpr (WIDE) {
+                if (it == 0 && tile != first_tile) {                 // previous tile -> slot under this k-block's MMAs
+                  if (hand_off()) { wg_wait_all(); aborted = true; goto teardown; }
+                }
+              }
               wg_wait_1();
               __syncwarp();
               mbar_arrive_if(prev_empty, lane == 0 && prev_empty != 0);
@@ -926,33 +979,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
               continue;
             }
-            // fold into the tile slot: the first chunk of a tile waits until the epilogue has read the previous tile and
-            // stores 0 + sum (the epilogue's fold starts from 0), later chunks add with round-to-nearest
-            const bool first_chunk = c0 == 0;
-            if (first_chunk) {
-              mbar_wait(smem_u32(cempty + slot), slot_phase ^ 1, aborted);
-              if (wg_any(aborted, bar_id)) { aborted = true; goto teardown; }
-            }
-            const uint32_t sbase = slot_base + (uint32_t)(slot * Cfg::SLOT_BYTES);
-            const int row = wg * 64 + wq * 16 + (lane >> 2);
+            if constexpr (WIDE) {      // fold: the first chunk gives 0 + sum (+0 for a -0 sum, as the epilogue's fold from 0 would)
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-#pragma unroll
-              for (int h8 = 0; h8 < 2; ++h8) {
-                const uint32_t e = sbase + (uint32_t)(((row + 8 * h8) * Cfg::SLOT_PITCH + 8 * j + 2 * (lane & 3)) * 4);
-                float x = 0.f, y = 0.f;
-                if (!first_chunk) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x), "=f"(y) : "r"(e) : "memory");
-                x = __fadd_rn(x, acc[0][4 * j + 2 * h8]);
-                y = __fadd_rn(y, acc[0][4 * j + 2 * h8 + 1]);
-                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(e), "f"(x), "f"(y) : "memory");
-              }
+              for (int i = 0; i < 64; ++i) run[i] = __fadd_rn(c0 == 0 ? 0.f : run[i], acc[0][i]);
             }
           }
-          if constexpr (!CM) {
-            __syncwarp();                                            // tile complete -> epilogue warps
-            if (lane == 0) mbar_arrive(smem_u32(cfull + slot));
-            if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
-          }
+        }
+        if constexpr (WIDE) {
+          if (first_tile < total_tiles && hand_off()) { aborted = true; goto teardown; }      // the last tile
         }
       } else {
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
@@ -1065,7 +1099,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
       }
     }
-  } else if (XF && warp >= 2 + EPI_WARPS) {
+  } else if ((XF || WIDE) && warp >= 2 + EPI_WARPS) {        // BN = 128 without XF: the 3 pad warps have no role
+
     // ============================ XF: operand transform (warps 10..) ============================
     // raw fp32 patch (zero outside the image: TMA out-of-bounds fill) -> y = act(x * scale[n,c] + shift[n,c]) (GroupNorm folded
     // into scale/shift, vqgan_arch.py:14-20,153-160) -> fp16 hi = rn(y), lo = rn(y - hi), written back IN PLACE in the
@@ -1228,7 +1263,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       }
       float acc[WIDE ? 1 : HC];
       if constexpr (WIDE) {
-        // the MMA warpgroups have folded every partial sum of this tile into the slot; it is read by the store loop below
+        // the MMA warpgroups have stored the finished tile (every partial sum folded) into the slot; the store loop reads it
         mbar_wait<250>(smem_u32(cfull + slot), slot_phase, aborted); if (aborted) goto teardown;
       } else {
 #pragma unroll
@@ -1329,8 +1364,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
         if (p.bias) bv = __ldg(reinterpret_cast<const float4*>(p.bias + colq));
         // global offsets of the (row, chunk) items of this lane, then their residual loads in flight at once: all 8 rows, or two
-        // batches of 4 in the register-capped (96-register) BN = 64 transform variants
-        constexpr int RB = (XF && !WIDE) ? 4 : 8;
+        // batches of 4 in the register-capped (96-register) transform variants
+        constexpr int RB = (XF || WIDE) ? 4 : 8;
         // GroupNorm partials: sums of deviations from the first value of the group this lane sees (k0, k1), so that a large
         // group mean does not cancel against the sum of squares (statistics need whole tiles: every value is inside)
         float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f, k0 = 0.f, k1 = 0.f;
