@@ -89,6 +89,8 @@ SIGNATURES = {
     'cfb_rrdb_forward': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_rrdb_forward_u8_tiles': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, _P, c_int32, c_int32, c_int32, _P, _P,
                                           c_int64, _P]),
+    'cfb_rrdb_forward_tiles': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, _P, c_int32, c_int32, c_int32, _P,
+                                       c_int32, _P, _P, c_int64, _P]),
     'cfb_parsenet_create': (c_void_p, [c_int32] * 8),
     'cfb_parsenet_destroy': (None, [_P]),
     'cfb_parsenet_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
@@ -146,6 +148,8 @@ SIGNATURES = {
     'cfb_paste_faces_multi': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P, _P, _P, c_double, _P, _P, c_int64, _P]),
     'cfb_resize_lanczos4_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
     'cfb_lanczos4_table': (None, [c_int32, c_int32, _P, _P]),
+    'cfb_resize_lanczos4_u16': (c_int, [_P, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'cfb_lanczos4_table_f32': (None, [c_int32, c_int32, _P, _P]),
     'cfb_gray_adain_faces': (c_int, [_P, _P, c_int32, c_int32, _P, _P, _P]),
     'cfb_is_gray_u8': (c_int, [_P, c_int32, c_int32, c_int32, _P, _P]),
     'cfb_f64_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),

@@ -206,7 +206,7 @@ int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, f
                  int pad_mode, int out_pitch, int out_c0, cudaStream_t st);
 int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bias, float* out_nchw, int N, int H, int W, int Cout,
                   int pad_mode, cudaStream_t st);
-// RRDBNet's tiles read from / written to uint8 images (cfb_rrdb_forward_u8_tiles): one row of its tile table.  The table of
+// RRDBNet's tiles read from / written to images (cfb_rrdb_forward_u8_tiles, cfb_rrdb_forward_tiles): one row of its tile table.  The table of
 // one launch travels by value in the kernel parameters (9 * 4 * 64 bytes, under the 4 KB parameter limit).
 struct RrdbU8Tile {
   int img;                       // source image / canvas index
@@ -218,11 +218,19 @@ struct RrdbU8Tiles {
   static constexpr int kMax = 64;
   RrdbU8Tile t[kMax];
 };
-int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w, int pre_pad, const RrdbU8Tiles& tiles,
-                          const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us, int out_pitch, int out_c0,
-                          cudaStream_t st);
-int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
-                           unsigned char* canvas_bgr_hwc, int out_h, int out_w, int N, int H, int W, cudaStream_t st);
+// Element type of the images those tiles are read from and written to (the CFB_IMG_* values of include/cfb200.h).
+enum ImgKind { IMG_U8 = 0, IMG_U16 = 1, IMG_F32 = 2, IMG_F64 = 3 };
+// max_range: the reference's per-image divisor, device int32 [images] from image_max_range, or nullptr for 255 (uint8 images).
+// The input is float32(v) / max_range, the output clamp(v, 0, 1) * max_range rounded half to even (saturated in a uint8 canvas).
+int conv_thin_in_tiles(const void* img_bgr_hwc, int in_kind, const int* max_range, int img_h, int img_w, int pre_pad,
+                       const RrdbU8Tiles& tiles, const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us,
+                       int out_pitch, int out_c0, cudaStream_t st);
+int conv_thin_out_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
+                        void* canvas_bgr_hwc, int out_kind, const int* max_range, int out_h, int out_w, int N, int H, int W,
+                        cudaStream_t st);
+// RealESRGANer.enhance's `max_range = 65535 if np.max(img.astype(np.float32)) > 256 else 255` of each of n images of `count`
+// elements, into device int32 max_range[n]; a NaN makes np.max NaN, hence 255.  No host synchronisation.
+int image_max_range(const void* images, int kind, int n, int64_t count, int* max_range, cudaStream_t st);
 // ParseNet's ends for cfb_parsenet_masks_u8: the input conv reads uint8 HWC BGR faces [N, H, W, 3] (the value of
 // u8_to_input); the output conv writes the argmax classes and / or the 0/255 face mask, uint8 [N, H, W] (either may be NULL)
 int conv_thin_in_u8_faces(const unsigned char* faces_bgr_hwc, const float* wgt_tck, const float* bias, float* out, int N, int H, int W,

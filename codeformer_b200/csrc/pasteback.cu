@@ -758,16 +758,71 @@ void lanczos4_table(int ssize, int dsize, int32_t* idx, int16_t* coef) {
   }
 }
 
+// cv2's float path (CV_16U): interpolateLanczos4 as resize builds float weights -- x + 3 summed in float32, each tap's
+// y = -((x + 3) - i) pi / 4 in double from the float32 (x + 3) - i, a tap at |(x + 3) - i| < 1e-6 set to 1e30 before the
+// normalisation (so x = 0 leaves the unit tap and neighbours of about 1e-31).
+void lanczos4_coeffs_f32(float x, float* cf) {
+  static const double s45 = 0.70710678118654752440084436210485;
+  static const double cs[8][2] = {{1, 0}, {-s45, -s45}, {0, 1}, {s45, -s45}, {-1, 0}, {s45, s45}, {0, -1}, {-s45, s45}};
+  const double pi = 3.1415926535897932384626433832795;
+  const float x3 = x + 3.f;
+  const double y0 = -(double)x3 * pi * 0.25, s0 = std::sin(y0), c0 = std::cos(y0);
+  float sum = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    const float t = x3 - (float)i;
+    if (std::fabs(t) >= 1e-6f) {
+      const double y = -(double)t * pi * 0.25;
+      cf[i] = (float)((cs[i][0] * s0 + cs[i][1] * c0) / (y * y));
+    } else {
+      cf[i] = 1e30f;
+    }
+    sum += cf[i];
+  }
+  sum = 1.f / sum;
+  for (int i = 0; i < 8; ++i) cf[i] *= sum;
+}
+
+void lanczos4_table_f32(int ssize, int dsize, int32_t* idx, float* coef) {
+  const double scale = 1. / ((double)dsize / ssize);
+  for (int d = 0; d < dsize; ++d) {
+    float f = (float)((d + 0.5) * scale - 0.5);
+    const int s = (int)std::floor(f);
+    f -= s;
+    idx[d] = s;
+    lanczos4_coeffs_f32(f, coef + (size_t)d * 8);
+  }
+}
+
 constexpr int kLzTileW = 64;     // output columns of a block
 constexpr int kLzRows = 48;      // source rows a block may hold (the host picks the band height to fit)
 
+// The arithmetic of one element type: uint8 sums int16 taps in int32 and rounds with (v + 2^21) >> 22; uint16 sums float32
+// products left to right, every product and sum rounded on its own (cv2's SSE code has no fused multiply-add), then rint.
+template <class T> struct LzOps;
+template <> struct LzOps<uint8_t> {
+  using Coef = short;
+  using Acc = int;
+  static __device__ __forceinline__ int mac(int a, int v, short c) { return a + v * c; }
+  static __device__ __forceinline__ uint8_t out(int acc) { return (uint8_t)min(max((acc + (1 << 21)) >> 22, 0), 255); }
+};
+template <> struct LzOps<uint16_t> {
+  using Coef = float;
+  using Acc = float;
+  static __device__ __forceinline__ float mac(float a, float v, float c) { return __fadd_rn(a, __fmul_rn(v, c)); }
+  static __device__ __forceinline__ uint16_t out(float acc) { return (uint16_t)fminf(fmaxf(rintf(acc), 0.f), 65535.f); }
+};
+
 // one block: a band of `band` output rows x kLzTileW output columns of image blockIdx.z.  The horizontal pass of every
-// source row the band needs goes to shared memory as int32, the vertical pass reads it back: no intermediate image.
-__global__ void __launch_bounds__(256) k_resize_lanczos4_u8(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst,
-                                                            int oh, int ow, const int* __restrict__ xi, const short* __restrict__ xt,
-                                                            const int* __restrict__ yi, const short* __restrict__ yt, int band) {
-  __shared__ int hbuf[kLzRows][kLzTileW * 3];
-  __shared__ short sxt[kLzTileW * 8];
+// source row the band needs goes to shared memory, the vertical pass reads it back: no intermediate image.
+template <class T>
+__global__ void __launch_bounds__(256) k_resize_lanczos4(const T* __restrict__ src, int h, int w, T* __restrict__ dst, int oh,
+                                                         int ow, const int* __restrict__ xi, const typename LzOps<T>::Coef* __restrict__ xt,
+                                                         const int* __restrict__ yi, const typename LzOps<T>::Coef* __restrict__ yt,
+                                                         int band) {
+  using Op = LzOps<T>;
+  using Acc = typename Op::Acc;
+  __shared__ Acc hbuf[kLzRows][kLzTileW * 3];
+  __shared__ typename Op::Coef sxt[kLzTileW * 8];
   __shared__ int sxi[kLzTileW];
   const int x0 = blockIdx.x * kLzTileW, y0 = blockIdx.y * band, y1 = min(y0 + band, oh);
   const int tw = min(kLzTileW, ow - x0);
@@ -779,14 +834,14 @@ __global__ void __launch_bounds__(256) k_resize_lanczos4_u8(const uint8_t* __res
   __syncthreads();
   for (int i = threadIdx.x; i < span * tw; i += 256) {
     const int r = i / tw, xl = i - r * tw;
-    const uint8_t* row = src + (size_t)min(max(rlo + r, 0), h - 1) * w * 3;
+    const T* row = src + (size_t)min(max(rlo + r, 0), h - 1) * w * 3;
     const int s = sxi[xl] - 3;
-    int a0 = 0, a1 = 0, a2 = 0;
+    Acc a0 = 0, a1 = 0, a2 = 0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const uint8_t* p = row + min(max(s + k, 0), w - 1) * 3;
-      const int c = sxt[xl * 8 + k];
-      a0 += p[0] * c; a1 += p[1] * c; a2 += p[2] * c;
+      const T* p = row + min(max(s + k, 0), w - 1) * 3;
+      const auto c = sxt[xl * 8 + k];
+      a0 = Op::mac(a0, p[0], c); a1 = Op::mac(a1, p[1], c); a2 = Op::mac(a2, p[2], c);
     }
     hbuf[r][xl * 3] = a0; hbuf[r][xl * 3 + 1] = a1; hbuf[r][xl * 3 + 2] = a2;
   }
@@ -794,11 +849,52 @@ __global__ void __launch_bounds__(256) k_resize_lanczos4_u8(const uint8_t* __res
   const int te = tw * 3;
   for (int i = threadIdx.x; i < (y1 - y0) * te; i += 256) {
     const int yl = i / te, e = i - yl * te, y = y0 + yl, r0 = yi[y] - 3 - rlo;
-    int acc = 0;
+    Acc acc = 0;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) acc += hbuf[r0 + k][e] * yt[y * 8 + k];
-    dst[((size_t)y * ow + x0) * 3 + e] = (uint8_t)min(max((acc + (1 << 21)) >> 22, 0), 255);
+    for (int k = 0; k < 8; ++k) acc = Op::mac(acc, hbuf[r0 + k][e], yt[y * 8 + k]);
+    dst[((size_t)y * ow + x0) * 3 + e] = Op::out(acc);
   }
+}
+
+// cfb_resize_lanczos4_u8 / _u16: tap tables of both axes built on the host (`table`), one launch for the n images
+template <class T, class Coef>
+int resize_lanczos4(const T* src, int n, int h, int w, T* dst, int out_h, int out_w, void (*table)(int, int, int32_t*, Coef*),
+                    const char* fn, cudaStream_t st) {
+  const std::string f(fn);
+  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, f + ": bad size");
+  CFB_REQUIRE(n <= 65535, f + ": at most 65535 images per call");
+  CFB_REQUIRE(n == 0 || (src && dst), f + ": NULL argument");
+  if (n == 0) return 0;
+  if (h == out_h && w == out_w) {                  // cv2.resize to the same size is a copy
+    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3 * sizeof(T), cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  // one host block: xi[ow] yi[oh] (int32) then xt[ow * 8] yt[oh * 8] (Coef)
+  const size_t ni = (size_t)out_w + out_h;
+  std::vector<char> host(ni * 4 + ni * 8 * sizeof(Coef));
+  int32_t* xi = (int32_t*)host.data();
+  int32_t* yi = xi + out_w;
+  Coef* xt = (Coef*)(host.data() + ni * 4);
+  Coef* yt = xt + (size_t)out_w * 8;
+  table(w, out_w, xi, xt);
+  table(h, out_h, yi, yt);
+  int band = 16;                                   // the tallest band whose source rows fit the shared rows
+  for (;; band /= 2) {
+    int span = 0;
+    for (int y0 = 0; y0 < out_h; y0 += band) span = std::max(span, yi[std::min(y0 + band, out_h) - 1] - yi[y0] + 8);
+    if (span <= kLzRows) break;                    // a band of one row needs eight
+  }
+  CFB_REQUIRE((out_h + band - 1) / band <= 65535, f + ": output too tall");
+  char* dtab = nullptr;
+  CFB_CUDA(cudaMallocAsync((void**)&dtab, host.size(), st));
+  CFB_CUDA(cudaMemcpyAsync(dtab, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  const int* dxi = (const int*)dtab;
+  const Coef* dxt = (const Coef*)(dtab + ni * 4);
+  k_resize_lanczos4<T><<<dim3((out_w + kLzTileW - 1) / kLzTileW, (out_h + band - 1) / band, n), 256, 0, st>>>(
+      src, h, w, dst, out_h, out_w, dxi, dxt, dxi + out_w, dxt + (size_t)out_w * 8, band);
+  CFB_LAUNCH_CHECK();
+  CFB_CUDA(cudaFreeAsync(dtab, st));
+  return 0;
 }
 
 // ---- the gray branch of add_restored_face ----------------------------------------------------------------------
@@ -1110,41 +1206,20 @@ void cfb_lanczos4_table(int32_t src_len, int32_t dst_len, int32_t* idx, int16_t*
 
 int cfb_resize_lanczos4_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w, void* stream) {
   API_BEGIN
-  CFB_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "cfb_resize_lanczos4_u8: bad size");
-  CFB_REQUIRE(n <= 65535, "cfb_resize_lanczos4_u8: at most 65535 images per call");
-  CFB_REQUIRE(n == 0 || (src && dst), "cfb_resize_lanczos4_u8: NULL argument");
-  if (n == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (h == out_h && w == out_w) {                  // cv2.resize to the same size is a copy
-    CFB_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st));
-    return 0;
-  }
-  // one host block: xi[ow] yi[oh] (int32) then xt[ow * 8] yt[oh * 8] (int16)
-  const size_t ni = (size_t)out_w + out_h;
-  std::vector<char> host(ni * 4 + ni * 16);
-  int32_t* xi = (int32_t*)host.data();
-  int32_t* yi = xi + out_w;
-  int16_t* xt = (int16_t*)(host.data() + ni * 4);
-  int16_t* yt = xt + (size_t)out_w * 8;
-  cfb::lanczos4_table(w, out_w, xi, xt);
-  cfb::lanczos4_table(h, out_h, yi, yt);
-  int band = 16;                                   // the tallest band whose source rows fit the shared rows
-  for (;; band /= 2) {
-    int span = 0;
-    for (int y0 = 0; y0 < out_h; y0 += band) span = std::max(span, yi[std::min(y0 + band, out_h) - 1] - yi[y0] + 8);
-    if (span <= cfb::kLzRows) break;               // a band of one row needs eight
-  }
-  CFB_REQUIRE((out_h + band - 1) / band <= 65535, "cfb_resize_lanczos4_u8: output too tall");
-  char* dtab = nullptr;
-  CFB_CUDA(cudaMallocAsync((void**)&dtab, host.size(), st));
-  CFB_CUDA(cudaMemcpyAsync(dtab, host.data(), host.size(), cudaMemcpyHostToDevice, st));
-  const int* dxi = (const int*)dtab;
-  const short* dxt = (const short*)(dtab + ni * 4);
-  cfb::k_resize_lanczos4_u8<<<dim3((out_w + cfb::kLzTileW - 1) / cfb::kLzTileW, (out_h + band - 1) / band, n), 256, 0, st>>>(
-      src, h, w, dst, out_h, out_w, dxi, dxt, dxi + out_w, dxt + (size_t)out_w * 8, band);
-  CFB_LAUNCH_CHECK();
-  CFB_CUDA(cudaFreeAsync(dtab, st));
-  return 0;
+  return cfb::resize_lanczos4<uint8_t, int16_t>(src, n, h, w, dst, out_h, out_w, cfb::lanczos4_table, "cfb_resize_lanczos4_u8",
+                                                (cudaStream_t)stream);
+  API_END(1)
+}
+
+void cfb_lanczos4_table_f32(int32_t src_len, int32_t dst_len, int32_t* idx, float* coef) {
+  if (src_len > 0 && dst_len > 0 && idx && coef) cfb::lanczos4_table_f32(src_len, dst_len, idx, coef);
+}
+
+int cfb_resize_lanczos4_u16(const uint16_t* src, int32_t n, int32_t h, int32_t w, uint16_t* dst, int32_t out_h, int32_t out_w,
+                            void* stream) {
+  API_BEGIN
+  return cfb::resize_lanczos4<uint16_t, float>(src, n, h, w, dst, out_h, out_w, cfb::lanczos4_table_f32, "cfb_resize_lanczos4_u16",
+                                               (cudaStream_t)stream);
   API_END(1)
 }
 

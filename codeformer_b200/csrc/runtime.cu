@@ -1396,12 +1396,14 @@ static size_t rrdb_ws_bytes(const cfb_rrdb* n, int N, int H, int W) {
   return (px * (64 + 3 * 192 + 64) + px * 4 * 64 + px * 16 * 64 * 2) * sizeof(float) + 8 * 1024;
 }
 
-// The uint8 ends of cfb_rrdb_forward_u8_tiles: conv_first reads the tiles from the source images, conv_last writes their crops
-// into the canvases; the launches take the host tile table in slices of RrdbU8Tiles::kMax tiles.
-struct RrdbU8Io {
-  const unsigned char* img; int img_h, img_w, pre_pad;
+// The image ends of cfb_rrdb_forward_u8_tiles / cfb_rrdb_forward_tiles: conv_first reads the tiles from the source images,
+// conv_last writes their crops into the canvases; the launches take the host tile table in slices of RrdbU8Tiles::kMax tiles.
+// range: the per-image max_range (device), nullptr for the uint8 entry point (255).
+struct RrdbTileIo {
+  const void* img; int in_kind, img_h, img_w, pre_pad;
   const RrdbU8Tile* tiles;
-  unsigned char* canvas; int out_h, out_w;
+  void* canvas; int out_kind, out_h, out_w;
+  const int* range;
   template <class F>
   int each_slice(int N, F f) const {
     for (int t0 = 0; t0 < N; t0 += RrdbU8Tiles::kMax) {
@@ -1415,7 +1417,7 @@ struct RrdbU8Io {
 };
 
 static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, int W, void* ws, int64_t ws_bytes, cudaStream_t st,
-                        const RrdbU8Io* u8 = nullptr) {
+                        const RrdbTileIo* io = nullptr) {
   CFB_CHECK(n->begin_forward(false));
   const int us = n->scale == 2 ? 2 : (n->scale == 1 ? 4 : 1);
   CFB_REQUIRE(H % us == 0 && W % us == 0, "RRDBNet: H and W must be multiples of the pixel-unshuffle factor (arch_util.py:202)");
@@ -1432,13 +1434,13 @@ static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, i
   float* HR = p; p += px * 16 * 64;
   // dense buffers start at zero: every channel a conv window can touch is finite from the first launch on
   CFB_CUDA(cudaMemsetAsync(D[0], 0, px * 192 * 3 * sizeof(float), st));
-  if (u8) {
-    CFB_CHECK(u8->each_slice(N, [&](int t0, int cnt, const RrdbU8Tiles& tab) {
+  if (io) {
+    CFB_CHECK(io->each_slice(N, [&](int t0, int cnt, const RrdbU8Tiles& tab) {
       const size_t o = (size_t)t0 * h * w;
-      CFB_CHECK(conv_thin_in_u8_tiles(u8->img, u8->img_h, u8->img_w, u8->pre_pad, tab, n->first_w, n->first_b, F + o * 64, cnt, h, w,
-                                      us, 64, 0, st));
-      return conv_thin_in_u8_tiles(u8->img, u8->img_h, u8->img_w, u8->pre_pad, tab, n->first_w, n->first_b, D[0] + o * 192, cnt, h,
-                                   w, us, 192, 0, st);
+      CFB_CHECK(conv_thin_in_tiles(io->img, io->in_kind, io->range, io->img_h, io->img_w, io->pre_pad, tab, n->first_w, n->first_b,
+                                   F + o * 64, cnt, h, w, us, 64, 0, st));
+      return conv_thin_in_tiles(io->img, io->in_kind, io->range, io->img_h, io->img_w, io->pre_pad, tab, n->first_w, n->first_b,
+                                D[0] + o * 192, cnt, h, w, us, 192, 0, st);
     }));
   } else {
     CFB_CHECK(conv_thin_in(x, n->first_w, n->first_b, F, N, h, w, n->in_ch, us, 0, 64, 0, st));
@@ -1471,29 +1473,31 @@ static int rrdb_forward(cfb_rrdb* n, const float* x, float* out, int N, int H, i
   { GenLaunch g{&n->convs[nb + 1], Bd, 64, h, w, N, U1, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
   { GenLaunch g{&n->convs[nb + 2], U1, 64, 2 * h, 2 * w, N, U2, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
   { GenLaunch g{&n->convs[nb + 3], U2, 64, 4 * h, 4 * w, N, HR, 64, 0, OUT_LRELU}; CFB_CHECK(conv(g)); }
-  if (u8)
-    return u8->each_slice(N, [&](int t0, int cnt, const RrdbU8Tiles& tab) {
-      return conv_thin_out_u8_tiles(HR + (size_t)t0 * 16 * h * w * 64, n->last_w, n->last_b, tab, u8->canvas, u8->out_h, u8->out_w,
-                                    cnt, 4 * h, 4 * w, st);
+  if (io)
+    return io->each_slice(N, [&](int t0, int cnt, const RrdbU8Tiles& tab) {
+      return conv_thin_out_tiles(HR + (size_t)t0 * 16 * h * w * 64, n->last_w, n->last_b, tab, io->canvas, io->out_kind, io->range,
+                                 io->out_h, io->out_w, cnt, 4 * h, 4 * w, st);
     });
   CFB_CHECK(conv_thin_out(HR, n->last_w, n->last_b, out, N, 4 * h, 4 * w, n->out_ch, 0, st));
   return 0;
 }
 
-// Checks of cfb_rrdb_forward_u8_tiles before any launch: the reflect pads of pre_process must be valid (each pad smaller than
-// the dimension it reflects, as F.pad requires), every tile window must lie in the padded image and every crop in the tile's
-// output, so that no launch reads or writes outside the images.
-static int rrdb_u8_tiles(cfb_rrdb* n, const uint8_t* images, int B, int H, int W, int pre_pad, const int32_t* tiles, int T, int th,
-                         int tw, uint8_t* out, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  CFB_REQUIRE(n->in_ch == 3 && n->out_ch == 3, "cfb_rrdb_forward_u8_tiles: built for 3 image channels in and out");
-  CFB_REQUIRE(B >= 0 && H > 0 && W > 0 && T >= 0, "cfb_rrdb_forward_u8_tiles: bad image batch");
+// Checks of cfb_rrdb_forward_u8_tiles / cfb_rrdb_forward_tiles (`fn`) before any launch: the reflect pads of pre_process must be
+// valid (each pad smaller than the dimension it reflects, as F.pad requires), every tile window must lie in the padded image and
+// every crop in the tile's output, so that no launch reads or writes outside the images.  range (device int32 [B]) is filled
+// by image_max_range first, or nullptr: 255 for every image (the uint8 entry point).
+static int rrdb_tiles(const char* fn, cfb_rrdb* n, const void* images, int in_kind, int B, int H, int W, int pre_pad,
+                      const int32_t* tiles, int T, int th, int tw, void* out, int out_kind, int* range, void* ws, int64_t ws_bytes,
+                      cudaStream_t st) {
+  const std::string f(fn);
+  CFB_REQUIRE(n->in_ch == 3 && n->out_ch == 3, f + ": built for 3 image channels in and out");
+  CFB_REQUIRE(B >= 0 && H > 0 && W > 0 && T >= 0, f + ": bad image batch");
   CFB_REQUIRE(pre_pad >= 0 && pre_pad < H && pre_pad < W,
-              "cfb_rrdb_forward_u8_tiles: pre_pad must be smaller than the image height and width (reflect pad)");
+              f + ": pre_pad must be smaller than the image height and width (reflect pad)");
   const int us = n->scale == 2 ? 2 : (n->scale == 1 ? 4 : 1);
   const int Hp = H + pre_pad, Wp = W + pre_pad;
   const int mh = (us - Hp % us) % us, mw = (us - Wp % us) % us;
-  CFB_REQUIRE(mh < Hp && mw < Wp, "cfb_rrdb_forward_u8_tiles: the pad to the pixel-unshuffle multiple must be smaller than the "
-                                   "padded image (reflect pad)");
+  CFB_REQUIRE(mh < Hp && mw < Wp, f + ": the pad to the pixel-unshuffle multiple must be smaller than the padded image (reflect pad)");
   CFB_REQUIRE(th > 0 && tw > 0 && th % us == 0 && tw % us == 0,
               "RRDBNet: H and W must be multiples of the pixel-unshuffle factor (arch_util.py:202)");
   const int Hm = Hp + mh, Wm = Wp + mw, oth = th * n->scale, otw = tw * n->scale;
@@ -1502,15 +1506,15 @@ static int rrdb_u8_tiles(cfb_rrdb* n, const uint8_t* images, int B, int H, int W
     const int32_t* r = tiles + (size_t)i * 9;
     RrdbU8Tile& t = tab[i];
     t = RrdbU8Tile{r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8]};
-    CFB_REQUIRE(t.img >= 0 && t.img < B, "cfb_rrdb_forward_u8_tiles: tile image index out of range");
-    CFB_REQUIRE(t.in_y >= 0 && t.in_x >= 0 && t.in_y + th <= Hm && t.in_x + tw <= Wm,
-                "cfb_rrdb_forward_u8_tiles: tile window outside the padded image");
+    CFB_REQUIRE(t.img >= 0 && t.img < B, f + ": tile image index out of range");
+    CFB_REQUIRE(t.in_y >= 0 && t.in_x >= 0 && t.in_y + th <= Hm && t.in_x + tw <= Wm, f + ": tile window outside the padded image");
     CFB_REQUIRE(t.crop_y >= 0 && t.crop_x >= 0 && t.crop_h >= 0 && t.crop_w >= 0 && t.crop_y + t.crop_h <= oth &&
                 t.crop_x + t.crop_w <= otw && t.out_y >= 0 && t.out_x >= 0,
-                "cfb_rrdb_forward_u8_tiles: tile crop outside the tile's output or negative output origin");
+                f + ": tile crop outside the tile's output or negative output origin");
   }
   if (T == 0) return 0;
-  const RrdbU8Io io{images, H, W, pre_pad, tab.data(), out, H * n->scale, W * n->scale};
+  if (range) CFB_CHECK(image_max_range(images, in_kind, B, (int64_t)H * W * 3, range, st));
+  const RrdbTileIo io{images, in_kind, H, W, pre_pad, tab.data(), out, out_kind, H * n->scale, W * n->scale, range};
   return rrdb_forward(n, nullptr, nullptr, T, th, tw, ws, ws_bytes, st, &io);
 }
 
@@ -2225,8 +2229,22 @@ int cfb_rrdb_forward_u8_tiles(cfb_rrdb* n, const uint8_t* images_bgr, int32_t nu
   API_BEGIN
   CFB_REQUIRE(n && (num_tiles <= 0 || (images_bgr && tiles && out_bgr && workspace)), "cfb_rrdb_forward_u8_tiles: NULL argument");
   std::lock_guard<std::mutex> lk(n->mu);
-  return cfb::rrdb_u8_tiles(n, images_bgr, num_images, img_h, img_w, pre_pad, tiles, num_tiles, tile_h, tile_w, out_bgr, workspace,
-                            workspace_bytes, (cudaStream_t)stream);
+  return cfb::rrdb_tiles("cfb_rrdb_forward_u8_tiles", n, images_bgr, cfb::IMG_U8, num_images, img_h, img_w, pre_pad, tiles,
+                         num_tiles, tile_h, tile_w, out_bgr, cfb::IMG_U8, nullptr, workspace, workspace_bytes, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_rrdb_forward_tiles(cfb_rrdb* n, const void* images_bgr, int32_t in_kind, int32_t num_images, int32_t img_h, int32_t img_w,
+                           int32_t pre_pad, const int32_t* tiles, int32_t num_tiles, int32_t tile_h, int32_t tile_w, void* out_bgr,
+                           int32_t out_kind, int32_t* max_range, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (num_tiles <= 0 || (images_bgr && tiles && out_bgr && max_range && workspace)),
+              "cfb_rrdb_forward_tiles: NULL argument");
+  CFB_REQUIRE(in_kind >= CFB_IMG_U8 && in_kind <= CFB_IMG_F64, "cfb_rrdb_forward_tiles: in_kind must be a CFB_IMG_* value");
+  CFB_REQUIRE(out_kind == CFB_IMG_U8 || out_kind == CFB_IMG_U16, "cfb_rrdb_forward_tiles: out_kind must be CFB_IMG_U8 or CFB_IMG_U16");
+  CFB_REQUIRE(num_images <= 65535, "cfb_rrdb_forward_tiles: at most 65535 images per call");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::rrdb_tiles("cfb_rrdb_forward_tiles", n, images_bgr, in_kind, num_images, img_h, img_w, pre_pad, tiles, num_tiles,
+                         tile_h, tile_w, out_bgr, out_kind, max_range, workspace, workspace_bytes, (cudaStream_t)stream);
   API_END(1)
 }
 

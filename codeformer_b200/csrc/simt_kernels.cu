@@ -1557,16 +1557,26 @@ struct NchwSrc {                 // x [N, Cimg, Hi, Wi] fp32
 // Index of row / column i of an image of n rows after F.pad(.., (0, p), 'reflect') (p < n): the bottom / right pad only.
 __device__ __forceinline__ int reflect_tail(int i, int n) { return i < n ? i : 2 * (n - 1) - i; }
 
-// The tiles of RealESRGANer.pre_process + tile_process read from uint8 HWC BGR source images (realesrgan_utils.py:71-175):
-// element n is the window at (in_y, in_x) of image `img` after the pre_pad reflect pad (bottom / right) and the reflect pad
-// to the pixel-unshuffle multiple; the value is the reference's float32 img / 255 (an IEEE division), BGR -> RGB.
-struct U8TileSrc {
-  const unsigned char* img; int H, W, Hp, Wp;        // source size, size after the pre_pad (Hp = H + pre_pad)
+// img.astype(np.float32) of one element of a uint8 / uint16 / float32 / float64 image (float64: round to nearest)
+__device__ __forceinline__ float img_f32(unsigned char v) { return (float)v; }
+__device__ __forceinline__ float img_f32(unsigned short v) { return (float)v; }
+__device__ __forceinline__ float img_f32(float v) { return v; }
+__device__ __forceinline__ float img_f32(double v) { return __double2float_rn(v); }
+
+// The tiles of RealESRGANer.pre_process + tile_process read from HWC BGR source images of element type T
+// (realesrgan_utils.py:71-175): element n is the window at (in_y, in_x) of image `img` after the pre_pad reflect pad (bottom /
+// right) and the reflect pad to the pixel-unshuffle multiple; the value is the reference's float32 img / max_range (an IEEE
+// division), BGR -> RGB.  range: per-image max_range (image_max_range), or nullptr for 255.
+template <class T>
+struct TileSrc {
+  const T* img; int H, W, Hp, Wp;                    // source size, size after the pre_pad (Hp = H + pre_pad)
+  const int* range;
   RrdbU8Tiles tab;                                   // by value: the table travels in the launch's parameters
   __device__ __forceinline__ float operator()(int n, int c, int y, int x_) const {
     const RrdbU8Tile& t = tab.t[n];
     const int sy = reflect_tail(reflect_tail(t.in_y + y, Hp), H), sx = reflect_tail(reflect_tail(t.in_x + x_, Wp), W);
-    return __fdiv_rn((float)__ldg(img + (((int64_t)t.img * H + sy) * W + sx) * 3 + (2 - c)), 255.f);
+    const float div = range ? (float)__ldg(range + t.img) : 255.f;
+    return __fdiv_rn(img_f32(__ldg(img + (((int64_t)t.img * H + sy) * W + sx) * 3 + (2 - c))), div);
   }
 };
 
@@ -1637,12 +1647,68 @@ int conv_thin_in(const float* x_nchw, const float* wgt_tck, const float* bias, f
                  int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
   return launch_thin_in(NchwSrc{x_nchw, Cimg, H * us, W * us}, wgt_tck, bias, out, N, H, W, Cimg, us, pad_mode, out_pitch, out_c0, st);
 }
-int conv_thin_in_u8_tiles(const unsigned char* img_bgr_hwc, int img_h, int img_w, int pre_pad, const RrdbU8Tiles& tiles,
-                          const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us, int out_pitch, int out_c0,
-                          cudaStream_t st) {
-  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_in_u8_tiles: too many tiles for one launch");
-  const U8TileSrc x{img_bgr_hwc, img_h, img_w, img_h + pre_pad, img_w + pre_pad, tiles};
+template <class T>
+static int thin_in_tiles(const void* img, const int* range, int img_h, int img_w, int pre_pad, const RrdbU8Tiles& tiles,
+                         const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us, int out_pitch, int out_c0,
+                         cudaStream_t st) {
+  const TileSrc<T> x{(const T*)img, img_h, img_w, img_h + pre_pad, img_w + pre_pad, range, tiles};
   return launch_thin_in(x, wgt_tck, bias, out, N, H, W, 3, us, 0, out_pitch, out_c0, st);
+}
+int conv_thin_in_tiles(const void* img_bgr_hwc, int in_kind, const int* max_range, int img_h, int img_w, int pre_pad,
+                       const RrdbU8Tiles& tiles, const float* wgt_tck, const float* bias, float* out, int N, int H, int W, int us,
+                       int out_pitch, int out_c0, cudaStream_t st) {
+  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_in_tiles: too many tiles for one launch");
+  CFB_REQUIRE(in_kind >= IMG_U8 && in_kind <= IMG_F64, "conv_thin_in_tiles: unknown image kind");
+  switch (in_kind) {
+    case IMG_U8: return thin_in_tiles<unsigned char>(img_bgr_hwc, max_range, img_h, img_w, pre_pad, tiles, wgt_tck, bias, out, N, H,
+                                                     W, us, out_pitch, out_c0, st);
+    case IMG_U16: return thin_in_tiles<unsigned short>(img_bgr_hwc, max_range, img_h, img_w, pre_pad, tiles, wgt_tck, bias, out, N,
+                                                       H, W, us, out_pitch, out_c0, st);
+    case IMG_F32: return thin_in_tiles<float>(img_bgr_hwc, max_range, img_h, img_w, pre_pad, tiles, wgt_tck, bias, out, N, H, W, us,
+                                              out_pitch, out_c0, st);
+    default: return thin_in_tiles<double>(img_bgr_hwc, max_range, img_h, img_w, pre_pad, tiles, wgt_tck, bias, out, N, H, W, us,
+                                          out_pitch, out_c0, st);
+  }
+}
+
+// max_range of image_max_range: bit 0 of flags[i] = some element of image i above 256, bit 1 = some NaN
+template <class T>
+__global__ void __launch_bounds__(256) image_range_flags_kernel(const T* __restrict__ img, int64_t count, int* __restrict__ flags) {
+  const T* p = img + (int64_t)blockIdx.y * count;
+  bool big = false, nan = false;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < count; i += (int64_t)gridDim.x * 256) {
+    const float v = img_f32(__ldg(p + i));
+    big |= v > 256.f;
+    nan |= v != v;
+  }
+  big = __any_sync(0xffffffffu, big);
+  nan = __any_sync(0xffffffffu, nan);
+  if ((threadIdx.x & 31) == 0 && (big || nan)) atomicOr(flags + blockIdx.y, (big ? 1 : 0) | (nan ? 2 : 0));
+}
+__global__ void image_range_finish_kernel(int* r, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) r[i] = r[i] == 1 ? 65535 : 255;
+}
+template <class T>
+static void launch_range_flags(const void* img, int n, int64_t count, int* flags, cudaStream_t st) {
+  const unsigned gx = (unsigned)std::min<int64_t>((count + 256 * 8 - 1) / (256 * 8), 256);
+  image_range_flags_kernel<T><<<dim3(gx, n), 256, 0, st>>>((const T*)img, count, flags);
+}
+int image_max_range(const void* images, int kind, int n, int64_t count, int* max_range, cudaStream_t st) {
+  CFB_REQUIRE(n >= 0 && n <= 65535 && count > 0, "image_max_range: bad image batch");
+  CFB_REQUIRE(kind >= IMG_U8 && kind <= IMG_F64, "image_max_range: unknown image kind");
+  if (n == 0) return 0;
+  CFB_CUDA(cudaMemsetAsync(max_range, 0, (size_t)n * sizeof(int), st));
+  switch (kind) {
+    case IMG_U8: launch_range_flags<unsigned char>(images, n, count, max_range, st); break;
+    case IMG_U16: launch_range_flags<unsigned short>(images, n, count, max_range, st); break;
+    case IMG_F32: launch_range_flags<float>(images, n, count, max_range, st); break;
+    default: launch_range_flags<double>(images, n, count, max_range, st); break;
+  }
+  CFB_LAUNCH_CHECK();
+  image_range_finish_kernel<<<(n + 255) / 256, 256, 0, st>>>(max_range, n);
+  CFB_LAUNCH_CHECK();
+  return 0;
 }
 int conv_thin_in_u8_faces(const unsigned char* faces_bgr_hwc, const float* wgt_tck, const float* bias, float* out, int N, int H, int W,
                           int pad_mode, int out_pitch, int out_c0, cudaStream_t st) {
@@ -1659,12 +1725,15 @@ struct NchwDst {                 // out [N, Cout, H, W] fp32
   }
 };
 
-// The crop-back of tile_process and post_process with the reference's uint8 conversion (realesrgan_utils.py:147-186,
-// 203-210): pixel (oy, ox) of tile n is kept when it lies in the tile's crop and its canvas position (out + offset into the
+// The crop-back of tile_process and post_process with the reference's integer conversion (realesrgan_utils.py:147-186,
+// 203-243): pixel (oy, ox) of tile n is kept when it lies in the tile's crop and its canvas position (out + offset into the
 // crop) lies inside the out_h x out_w canvas of image `img` (the mod pad and pre_pad rows / columns fall outside); it is
-// written as uint8 HWC BGR: clamp to [0, 1], float32 * 255, round half to even.
-struct U8CanvasDst {
-  unsigned char* canvas; int out_h, out_w;
+// written as HWC BGR of element type T: clamp to [0, 1], float32 * max_range, round half to even, saturated to T.
+// range: per-image max_range (image_max_range), or nullptr for 255.
+template <class T>
+struct TileDst {
+  T* canvas; int out_h, out_w;
+  const int* range;
   RrdbU8Tiles tab;
   __device__ __forceinline__ bool pos(int n, int oy, int ox, int& Y, int& X) const {
     const RrdbU8Tile& t = tab.t[n];
@@ -1677,9 +1746,12 @@ struct U8CanvasDst {
   __device__ __forceinline__ void store(int n, int oy, int ox, int, int, int, const float (&acc)[CP]) const {
     int Y, X;
     pos(n, oy, ox, Y, X);
-    unsigned char* px = canvas + (((int64_t)tab.t[n].img * out_h + Y) * out_w + X) * 3;
+    const int img = tab.t[n].img;
+    const float mul = range ? (float)__ldg(range + img) : 255.f;
+    const float top = sizeof(T) == 1 ? 255.f : 65535.f;
+    T* px = canvas + (((int64_t)img * out_h + Y) * out_w + X) * 3;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) px[2 - c] = (unsigned char)rintf(__fmul_rn(fminf(fmaxf(acc[c], 0.f), 1.f), 255.f));
+    for (int c = 0; c < 3; ++c) px[2 - c] = (T)fminf(rintf(__fmul_rn(fminf(fmaxf(acc[c], 0.f), 1.f), mul)), top);
   }
 };
 
@@ -1763,13 +1835,21 @@ int conv_thin_out(const float* in_nhwc64, const float* wgt_tcp, const float* bia
   CFB_LAUNCH_CHECK();
   return 0;
 }
-int conv_thin_out_u8_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
-                           unsigned char* canvas_bgr_hwc, int out_h, int out_w, int N, int H, int W, cudaStream_t st) {
-  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_out_u8_tiles: too many tiles for one launch");
+int conv_thin_out_tiles(const float* in_nhwc64, const float* wgt_tcp, const float* bias, const RrdbU8Tiles& tiles,
+                        void* canvas_bgr_hwc, int out_kind, const int* max_range, int out_h, int out_w, int N, int H, int W,
+                        cudaStream_t st) {
+  CFB_REQUIRE(N <= RrdbU8Tiles::kMax, "conv_thin_out_tiles: too many tiles for one launch");
+  CFB_REQUIRE(out_kind == IMG_U8 || out_kind == IMG_U16, "conv_thin_out_tiles: the output is uint8 or uint16");
   const int64_t M = (int64_t)N * H * W;
   if (M == 0) return 0;
-  const U8CanvasDst dst{canvas_bgr_hwc, out_h, out_w, tiles};
-  conv_thin_out_kernel<4><<<(unsigned)((M + 127) / 128), 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, 3, 0);
+  const unsigned grid = (unsigned)((M + 127) / 128);
+  if (out_kind == IMG_U8) {
+    const TileDst<unsigned char> dst{(unsigned char*)canvas_bgr_hwc, out_h, out_w, max_range, tiles};
+    conv_thin_out_kernel<4><<<grid, 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, 3, 0);
+  } else {
+    const TileDst<unsigned short> dst{(unsigned short*)canvas_bgr_hwc, out_h, out_w, max_range, tiles};
+    conv_thin_out_kernel<4><<<grid, 128, 9 * 64 * 4 * 4, st>>>(in_nhwc64, wgt_tcp, bias, dst, N, H, W, 3, 0);
+  }
   CFB_LAUNCH_CHECK();
   return 0;
 }

@@ -37,10 +37,10 @@ def invert_affine(M):
     return np.array([[A11, A12, -A11 * M[0, 2] - A12 * M[1, 2]], [A21, A22, -A21 * M[0, 2] - A22 * M[1, 2]]], np.float64)
 
 
-def _check_image(x, name, ndim=3):
+def _check_image(x, name, ndim=3, dtype=torch.uint8):
     if not torch.is_tensor(x) or not x.is_cuda:
         raise RuntimeError(f'{name}: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
-    if x.dtype != torch.uint8:
+    if x.dtype != dtype:
         raise NotImplementedError(f'{name}: only 8-bit images are supported, got {x.dtype}')
     if x.dim() != ndim or x.shape[-1] != 3:
         raise NotImplementedError(f'{name}: only 3-channel HWC images are supported, got shape {tuple(x.shape)}')
@@ -103,15 +103,19 @@ def resize_area(img, size):
 
 def resize_lanczos4(img, size):
     """``cv2.resize(img, size, interpolation=INTER_LANCZOS4)`` (size = (w, h), enlarging or shrinking, byte for byte) on CUDA
-    uint8 [h,w,3] or [N,h,w,3] (``cfb_resize_lanczos4_u8``); an [N,...] call is one launch and equals N single calls."""
+    uint8 or uint16 [h,w,3] or [N,h,w,3] (``cfb_resize_lanczos4_u8`` / ``cfb_resize_lanczos4_u16``: cv2's int16 taps for 8-bit
+    images, its float32 path for 16-bit ones); an [N,...] call is one launch and equals N single calls."""
     batched = img.dim() == 4
-    img = _check_image(img, 'resize_lanczos4', 4 if batched else 3)
+    wide = torch.is_tensor(img) and img.dtype == torch.uint16
+    # a 16-bit image is checked and made contiguous as int16, the same bytes (torch's uint16 has few kernels)
+    img = _check_image(img.view(torch.int16) if wide else img, 'resize_lanczos4', 4 if batched else 3,
+                       torch.int16 if wide else torch.uint8)
     x = img if batched else img[None]
     n, h, w = x.shape[:3]
-    out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint8, device=img.device)
+    out = torch.empty((n, size[1], size[0], 3), dtype=torch.uint16 if wide else torch.uint8, device=img.device)
+    fn = 'cfb_resize_lanczos4_u16' if wide else 'cfb_resize_lanczos4_u8'
     with torch.cuda.device(img.device):
-        _lib.check(_lib.load().cfb_resize_lanczos4_u8(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _lib.stream(img.device)),
-                   'cfb_resize_lanczos4_u8')
+        _lib.check(getattr(_lib.load(), fn)(_lib.ptr(x), n, h, w, _lib.ptr(out), size[1], size[0], _lib.stream(img.device)), fn)
     return out if batched else out[0]
 
 

@@ -90,6 +90,26 @@ class RRDBNet(Precision, NativeNet):
                        'cfb_rrdb_forward_u8_tiles')
         return out
 
+    # element kinds of cfb_rrdb_forward_tiles (CFB_IMG_* of include/cfb200.h)
+    IMAGE_KINDS = {torch.uint8: 0, torch.uint16: 1, torch.float32: 2, torch.float64: 3}
+
+    def forward_tiles(self, images, pre_pad, tiles, tile_h, tile_w, out, max_range):
+        """``forward_u8_tiles`` for CUDA uint8 / uint16 / float32 / float64 images [B,H,W,3] into a CUDA uint8 or uint16 ``out``
+        ([B,H*scale,W*scale,3]) with the reference's per-image ``max_range`` (``cfb_rrdb_forward_tiles``): the call fills
+        ``max_range`` (CUDA int32 [B]) with 255 or 65535 per image before the forward, on the device."""
+        B, H, W, _ = images.shape
+        rows = np.ascontiguousarray(np.asarray(tiles, dtype=np.int32).reshape(-1, 9))
+        lib = _lib.load()
+        dev = images.device
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            ws = self._workspace(rows.shape[0], tile_h, tile_w, dev)
+            _lib.check(lib.cfb_rrdb_forward_tiles(self._net, _lib.ptr(images), self.IMAGE_KINDS[images.dtype], B, H, W, pre_pad,
+                                                  rows.ctypes.data_as(ctypes.c_void_p), rows.shape[0], tile_h, tile_w,
+                                                  _lib.ptr(out), self.IMAGE_KINDS[out.dtype], _lib.ptr(max_range), _lib.ptr(ws),
+                                                  ws.numel(), _lib.stream(dev)), 'cfb_rrdb_forward_tiles')
+        return out
+
 
 def unshuffle_factor(scale):
     """pixel_unshuffle factor of RRDBNet's input, which is also pre_process's mod_scale (1: no mod pad)."""
@@ -110,7 +130,7 @@ def reflect_pad_index(n, pre_pad, scale):
 
 class RealESRGANer:
     """The reference's helper around the upsampling network (realesrgan_utils.py:14-250): ``enhance(img)`` takes an HWC
-    uint8 / uint16 BGR (or gray, or BGRA) image and returns ``(upsampled image, mode)``.  ``model`` is any module mapping
+    uint8 / uint16 / float BGR (or gray, or BGRA) image and returns ``(upsampled image, mode)``.  ``model`` is any module mapping
     [1,3,h,w] -> [1,3,h*scale,w*scale] on ``device`` (``codeformer_b200.RRDBNet`` in production; the tests also pass CPU
     stand-ins to compare the tiling against the reference's).  ``precision`` (not in the reference): ``None`` leaves the model
     as it is, a string is passed to ``model.set_precision`` -- the reference's ``half=use_half`` maps to
@@ -207,19 +227,23 @@ class RealESRGANer:
 
     @torch.no_grad()
     def enhance_batch(self, images, outscale=None, max_tiles=None, lanczos=False):
-        """``enhance`` of every image of ``images`` (CUDA uint8 [B,H,W,3] BGR) on the device, as CUDA uint8
-        [B,H*scale,W*scale,3] BGR; each image equals ``enhance(img)[0]`` byte for byte.  With ``lanczos=True`` an ``outscale``
-        other than ``scale`` resizes the network's output to (int(W*outscale), int(H*outscale)) with cv2's INTER_LANCZOS4 on
-        the device (``resize_lanczos4``, realesrgan_utils.py:245-250), one launch for the batch, as ``enhance`` does; without
-        it such an ``outscale`` is refused, so that a caller who sized its buffers for ``scale`` never gets another size.  The tiles of all images are grouped
-        by input-window shape (``tile_groups``) and every group runs as forwards of at most ``max_tiles`` tiles (default:
-        as many as ``WORKSPACE_BUDGET`` holds) that read the uint8 images and write the uint8 result directly.  Keeps no
-        state on ``self``: threads may share one upsampler.
+        """``enhance`` of every image of ``images`` (CUDA [B,H,W,3] BGR) on the device.  uint8 images give CUDA uint8
+        [B,H*scale,W*scale,3]; uint16, float32 and float64 images give a list of B CUDA tensors [H*scale,W*scale,3], each
+        uint16 where that image's float32 maximum exceeds 256 and uint8 otherwise, as ``enhance`` picks its dtype per image.
+        Each image equals ``enhance(img)[0]`` byte for byte.  With ``lanczos=True`` an ``outscale`` other than ``scale`` resizes
+        the network's output to (int(W*outscale), int(H*outscale)) with cv2's INTER_LANCZOS4 on the device
+        (``resize_lanczos4``, realesrgan_utils.py:245-250), one launch per output dtype, as ``enhance`` does; without it such an
+        ``outscale`` is refused, so that a caller who sized its buffers for ``scale`` never gets another size.  The tiles of all
+        images are grouped by input-window shape (``tile_groups``) and every group runs as forwards of at most ``max_tiles``
+        tiles (default: as many as ``WORKSPACE_BUDGET`` holds) that read the images and write the integer result directly
+        (``cfb_rrdb_forward_u8_tiles``, ``cfb_rrdb_forward_tiles`` for the other dtypes).  Keeps no state on ``self``: threads
+        may share one upsampler.
 
         Raises NotImplementedError for ``outscale`` other than None / ``scale`` without ``lanczos=True``, for images that are
-        not uint8 with 3 channels and for models other than a 3-channel ``codeformer_b200.RRDBNet``; ValueError for an
-        ``outscale`` that is not positive; RuntimeError for CPU tensors and for pads not smaller than the dimension they reflect;
-        AssertionError, as RRDBNet.forward, for tiles whose size is not a multiple of the pixel-unshuffle factor."""
+        not uint8 / uint16 / float32 / float64 with 3 channels and for models other than a 3-channel
+        ``codeformer_b200.RRDBNet``; ValueError for an ``outscale`` that is not positive; RuntimeError for CPU tensors and for
+        pads not smaller than the dimension they reflect; AssertionError, as RRDBNet.forward, for tiles whose size is not a
+        multiple of the pixel-unshuffle factor."""
         if outscale is not None and outscale != float(self.scale) and not lanczos:
             raise NotImplementedError(f'RealESRGANer.enhance_batch: outscale {outscale} != scale {self.scale} changes the output '
                                       'size; pass lanczos=True for the reference\'s INTER_LANCZOS4 resize')
@@ -229,34 +253,55 @@ class RealESRGANer:
             raise NotImplementedError('RealESRGANer.enhance_batch: built for a codeformer_b200.RRDBNet with 3 input and 3 output '
                                       f'channels, got {type(self.model).__name__}')
         if not torch.is_tensor(images):
-            raise NotImplementedError(f'RealESRGANer.enhance_batch takes a CUDA uint8 tensor, got {type(images).__name__}')
+            raise NotImplementedError(f'RealESRGANer.enhance_batch takes a CUDA tensor, got {type(images).__name__}')
         if not images.is_cuda:
             raise RuntimeError('RealESRGANer.enhance_batch: codeformer_b200 runs on a CUDA device only; there is no CPU fallback')
-        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
-            raise NotImplementedError(f'RealESRGANer.enhance_batch takes uint8 [B,H,W,3] BGR images (16-bit, gray and alpha '
-                                      f'images go through enhance), got {images.dtype} {tuple(images.shape)}')
+        if images.dtype not in RRDBNet.IMAGE_KINDS or images.dim() != 4 or images.shape[3] != 3:
+            raise NotImplementedError(f'RealESRGANer.enhance_batch takes uint8, uint16, float32 or float64 [B,H,W,3] BGR images '
+                                      f'(gray and alpha images go through enhance), got {images.dtype} {tuple(images.shape)}')
         B, H, W, _ = images.shape
         sc = self.scale
+        u8 = images.dtype == torch.uint8
         if outscale is not None and outscale != float(sc):
             from .pasteback import resize_lanczos4
             size = (int(W * outscale), int(H * outscale))
             if B == 0 or H == 0 or W == 0 or size[0] == 0 or size[1] == 0:
-                return torch.empty((B, size[1], size[0], 3), dtype=torch.uint8, device=images.device)
-            return resize_lanczos4(self.enhance_batch(images, max_tiles=max_tiles), size)
-        out = torch.empty((B, H * sc, W * sc, 3), dtype=torch.uint8, device=images.device)
+                out = torch.empty((B, size[1], size[0], 3), dtype=torch.uint8, device=images.device)
+                return out if u8 else list(out)
+            up = self.enhance_batch(images, max_tiles=max_tiles)
+            if u8:
+                return resize_lanczos4(up, size)
+            res = [None] * B
+            for dt in (torch.uint8, torch.uint16):          # one launch per output dtype; uint16 is stacked as int16
+                sel = [i for i in range(B) if up[i].dtype == dt]
+                if sel:
+                    batch = torch.stack([up[i].view(torch.int16) if dt == torch.uint16 else up[i] for i in sel])
+                    for i, r in zip(sel, resize_lanczos4(batch.view(dt), size)):
+                        res[i] = r
+            return res
+        out = torch.empty((B, H * sc, W * sc, 3), dtype=torch.uint8 if u8 else torch.uint16, device=images.device)
         if B == 0 or H == 0 or W == 0:
-            return out
-        images = images.contiguous()
+            return out if u8 else list(out.view(torch.int16).to(torch.uint8))
+        # made contiguous through an int16 view for uint16 (torch's uint16 has few kernels): the same bytes
+        images = images.view(torch.int16).contiguous().view(torch.uint16) if images.dtype == torch.uint16 else images.contiguous()
         us = unshuffle_factor(sc)
         lib = _lib.load()
+        max_range = None if u8 else torch.empty(B, dtype=torch.int32, device=images.device)
 
         def tile_bytes(n, th, tw):
             return lib.cfb_rrdb_workspace_bytes(self.model._handle(), n, th, tw)
         for th, tw, rows in self.tile_groups(B, H, W, max_tiles, tile_bytes):
             if th % us or tw % us:
                 raise AssertionError('pixel_unshuffle needs H and W divisible by the factor (arch_util.py:202)')
-            self.model.forward_u8_tiles(images, self.pre_pad, rows, th, tw, out)
-        return out
+            if u8:
+                self.model.forward_u8_tiles(images, self.pre_pad, rows, th, tw, out)
+            else:
+                self.model.forward_tiles(images, self.pre_pad, rows, th, tw, out, max_range)
+        if u8:
+            return out
+        wide = (max_range == 65535).tolist()                # the one read-back: each result's dtype
+        narrow = None if all(wide) else out.view(torch.int16).to(torch.uint8)
+        return [out[i] if wide[i] else narrow[i] for i in range(B)]
 
     def tile_process(self):
         b, c, height, width = self.img.shape
@@ -288,10 +333,11 @@ class RealESRGANer:
 
     @torch.no_grad()
     def enhance(self, img, outscale=None, alpha_upsampler='realesrgan'):
-        """The reference's ``enhance``.  uint8 3-channel images with this package's RRDBNet go through ``enhance_batch``,
-        the INTER_LANCZOS4 resize of ``outscale != scale`` included (the same bytes); every other case through pre_process /
-        tile_process / post_process and cv2 on the host."""
-        if img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and self._device_path():
+        """The reference's ``enhance``.  uint8, uint16, float32 and float64 3-channel images with this package's RRDBNet go
+        through ``enhance_batch``, the INTER_LANCZOS4 resize of ``outscale != scale`` included (the same bytes and dtype);
+        every other case (gray, alpha, other models) through pre_process / tile_process / post_process and cv2 on the host."""
+        if (img.dtype in (np.uint8, np.uint16, np.float32, np.float64) and img.ndim == 3 and img.shape[2] == 3
+                and self._device_path()):
             x = torch.from_numpy(np.ascontiguousarray(img)).to(self.device)
             return self.enhance_batch(x[None], outscale=outscale, lanczos=True)[0].cpu().numpy(), 'RGB'
         return self._enhance_host(img, outscale, alpha_upsampler)

@@ -14,7 +14,8 @@ and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of im
   * the paste-back runs once per chunk of images (``cfb_paste_faces_multi``), one read-back of the erosion areas.
 
   * a ``codeformer_b200.RealESRGANer`` background / face upsampler whose scale is ``upscale`` runs once per chunk on the
-    device (``enhance_batch``): the chunk's images, then its restored faces, each as one batch of tiles.  With another scale
+    device (``enhance_batch``): the chunk's images, then its restored faces (the colour faces as uint8, the gray images'
+    float64 faces as a second batch), each as one batch of tiles.  With another scale
     it is called per image / per face through ``enhance(img, outscale=upscale)``, which runs the network and cv2's
     INTER_LANCZOS4 on the device.  A background whose size is not the output's (``read_image`` enlarged the image, or any
     other upsampler's result) goes through INTER_LANCZOS4 on the device (``resize_lanczos4``), as the reference's paste does;
@@ -188,8 +189,9 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
     ``enhance(img, outscale=upscale)`` (``RealESRGANer``).  A ``codeformer_b200.RealESRGANer`` over ``RRDBNet`` with
     ``scale == upscale`` runs on the device, once per chunk of images for the backgrounds and once for the restored faces
     (``enhance_batch``); any other upsampler is called per image / per face through ``enhance`` (for this package's
-    RealESRGANer at another scale that call runs the network and the INTER_LANCZOS4 resize on the device).  The float64 faces of gray images always go to ``face_upsampler.enhance`` on the host, one by one, and come back
-    uint8 as in the reference (a face above 256 is 16-bit to ``enhance``: NotImplementedError).
+    RealESRGANer at another scale that call runs the network and the INTER_LANCZOS4 resize on the device).  The float64 faces
+    of gray images go with the colour ones: one ``enhance_batch`` of the chunk's gray faces on the device, or ``enhance`` per
+    face; they come back uint8 as in the reference (a face above 256 is 16-bit to ``enhance``: NotImplementedError).
 
     Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
     also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted (float64 for a gray image
@@ -251,11 +253,14 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
             S = int(FACE_SIZE * upscale)
             up = torch.empty((len(affines), S, S, 3), dtype=torch.uint8, device=dev)
 
-            def host_faces(faces):
-                res = [np.asarray(face_upsampler.enhance(f, outscale=upscale)[0]) for f in faces]
-                if any(r.dtype != np.uint8 for r in res):
+            def no_16bit(wide):
+                if any(wide):
                     raise NotImplementedError('restore_images: the face upsampler returned a 16-bit face (a gray face above 256 '
                                               'is 16-bit to RealESRGANer.enhance); 16-bit faces are not pasted')
+
+            def host_faces(faces):
+                res = [np.asarray(face_upsampler.enhance(f, outscale=upscale)[0]) for f in faces]
+                no_16bit([r.dtype != np.uint8 for r in res])
                 if any(r.shape != (S, S, 3) for r in res):
                     raise RuntimeError(f'restore_images: the face upsampler returned {res[0].shape[:2]}, expected {S}x{S}')
                 return torch.from_numpy(np.ascontiguousarray(np.stack(res))).to(dev)
@@ -264,8 +269,13 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
                     up[ct] = face_upsampler.enhance_batch(restored[ct], outscale=upscale)
                 else:
                     up[ct] = host_faces(restored[ct].cpu().numpy())
-            if len(gsel):          # enhance takes the float64 faces on the host and returns uint8, as in the reference
-                up[gt] = host_faces(gray_faces.cpu().numpy())
+            if len(gsel):          # the float64 faces come back uint8, as enhance returns them in the reference
+                if _on_device(face_upsampler, upscale):
+                    res = face_upsampler.enhance_batch(gray_faces, outscale=upscale)
+                    no_16bit([r.dtype != torch.uint8 for r in res])
+                    up[gt] = torch.stack(res)
+                else:
+                    up[gt] = host_faces(gray_faces.cpu().numpy())
             restored, gray_faces = up, None
         h_up, w_up = int(h * upscale), int(wd * upscale)
         if bg_upsampler is not None and _on_device(bg_upsampler, upscale):

@@ -286,6 +286,22 @@ int       cfb_rrdb_forward(cfb_rrdb* net, const float* x, float* out, int32_t ba
 int       cfb_rrdb_forward_u8_tiles(cfb_rrdb* net, const uint8_t* images_bgr, int32_t num_images, int32_t img_h, int32_t img_w,
                                     int32_t pre_pad, const int32_t* tiles, int32_t num_tiles, int32_t tile_h, int32_t tile_w,
                                     uint8_t* out_bgr, void* workspace, int64_t workspace_bytes, void* stream);
+/* cfb_rrdb_forward_u8_tiles for the other images RealESRGANer.enhance takes (realesrgan_utils.py:190-243): images_bgr of element
+ * type in_kind (uint8, uint16, float32 or float64), out_bgr of out_kind (CFB_IMG_U8 or CFB_IMG_U16); the same tile table, pads,
+ * checks and workspace.  Per image, as the reference: img.astype(np.float32) (float64 rounded to nearest first),
+ * max_range = 65535 if its float32 maximum exceeds 256 else 255 (a NaN makes numpy's maximum NaN: 255), the input value
+ * float32 v / max_range (an IEEE division), the output clamp(v, 0, 1) * max_range in float32 rounded half to even (saturated
+ * to 255 in a uint8 canvas).  max_range: device int32 [num_images], written by the call (a device reduction over every image,
+ * before the forward; no host synchronisation) when num_tiles > 0 -- the caller reads it back to pick each result's dtype
+ * (uint16 where it is 65535).  num_images <= 65535. */
+#define CFB_IMG_U8  0
+#define CFB_IMG_U16 1
+#define CFB_IMG_F32 2
+#define CFB_IMG_F64 3
+int       cfb_rrdb_forward_tiles(cfb_rrdb* net, const void* images_bgr, int32_t in_kind, int32_t num_images, int32_t img_h,
+                                 int32_t img_w, int32_t pre_pad, const int32_t* tiles, int32_t num_tiles, int32_t tile_h, int32_t tile_w,
+                                 void* out_bgr, int32_t out_kind, int32_t* max_range, void* workspace, int64_t workspace_bytes,
+                                 void* stream);
 
 /* ---- ParseNet (SURVEY.md section 8 row f3): face parsing of the restored face for the paste-back blend ----
  * /root/reference/facelib/parsing/parsenet.py:140-194; built by init_parsing_model('parsenet') as ParseNet(in_size=512,
@@ -468,6 +484,10 @@ int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_
  *   the upsampled background (face_restoration_helper.py:381).  The tap tables are built on the host per call.
  * cfb_lanczos4_table: those tables for one axis (host only, no device needed): idx[dst_len] = floor of the source coordinate
  *   (taps at idx-3 .. idx+4, clamped to the image), coef[dst_len*8] = the weights * 2048 as int16.
+ * cfb_resize_lanczos4_u16: cv2.resize on CV_16U [n,h,w,3], byte for byte: cv2's float path, not the int16 taps of uint8 --
+ *   float32 weights, a horizontal then a vertical pass of float32 products summed left to right (no fused multiply-add),
+ *   rounded half to even and saturated.  What enhance does to a 16-bit result for outscale != scale.
+ * cfb_lanczos4_table_f32: its tables for one axis (host only): idx as above, coef[dst_len*8] the float32 weights.
  * cfb_gray_adain_faces: add_restored_face on a gray image (face_restoration_helper.py:364-369): out[i] [S,S,3] float64 =
  *   adain_npy(bgr2gray(restored[i]), cropped[i]) (facelib/utils/misc.py:169-202), both inputs uint8 [n,S,S,3] BGR.  stats
  *   (optional, device double [n,4,3]) receives content mean, content std, style mean, style std per channel.  float64, two-pass
@@ -484,6 +504,9 @@ int cfb_paste_faces_multi(uint8_t* canvases, int32_t n_img, int32_t h_up, int32_
 int cfb_resize_lanczos4_u8(const uint8_t* src, int32_t n, int32_t h, int32_t w, uint8_t* dst, int32_t out_h, int32_t out_w,
                            void* stream);
 void cfb_lanczos4_table(int32_t src_len, int32_t dst_len, int32_t* idx, int16_t* coef);
+int cfb_resize_lanczos4_u16(const uint16_t* src, int32_t n, int32_t h, int32_t w, uint16_t* dst, int32_t out_h, int32_t out_w,
+                            void* stream);
+void cfb_lanczos4_table_f32(int32_t src_len, int32_t dst_len, int32_t* idx, float* coef);
 int cfb_gray_adain_faces(const uint8_t* restored, const uint8_t* cropped, int32_t n, int32_t face_size, double* out, double* stats,
                          void* stream);
 int cfb_is_gray_u8(const uint8_t* images, int32_t n, int32_t h, int32_t w, int64_t* sums, void* stream);
