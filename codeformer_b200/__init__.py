@@ -14,7 +14,7 @@ from .detection import RetinaFace, init_detection_model   # noqa: F401
 from .yolov5face import YOLOv5lFace, YoloDetector   # noqa: F401
 from .pasteback import resize_area, warp_faces_multi, paste_faces_multi   # noqa: F401
 from .pasteback import resize_lanczos4, gray_adain_faces, add_restored_face   # noqa: F401
-from .wholeimage import restore_images, restore_aligned   # noqa: F401
+from .wholeimage import restore_images, restore_images_sweep, restore_aligned   # noqa: F401
 
 
 def check_async_status():
@@ -28,4 +28,5 @@ def check_async_status():
 __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQuantizer', 'RRDBNet', 'RealESRGANer', 'ParseNet', 'face_parse_mask', 'init_parsing_model',
            'warp_faces', 'paste_faces', 'align_warp_face', 'paste_faces_to_input_image', 'RetinaFace', 'init_detection_model',
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
-           'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'check_async_status']
+           'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
+           'check_async_status']

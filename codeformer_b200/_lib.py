@@ -46,6 +46,8 @@ SIGNATURES = {
     'cfb_codeformer_forward_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_forward_u8_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_inpaint_u8_wv': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int32, _P, c_int64, _P]),
+    'cfb_sweep_workspace_bytes': (c_int64, [_P, c_int32, c_int32]),
+    'cfb_codeformer_sweep_u8': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, _P, c_int32, _P, c_int64, _P]),
     'cfb_codeformer_restore_host': (c_int, [_P, _P, _P, c_int32, c_float, c_int32, _P, c_int64, _P, c_int64, _P]),
     'cfb_u8_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_output_to_u8': (c_int, [_P, _P, c_int32, c_int32, _P]),

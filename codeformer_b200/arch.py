@@ -316,15 +316,16 @@ class VQAutoEncoder(Precision, NativeHandle):
             pool.append(torch.cuda.Stream(device=device))
         return pool
 
-    def _cfb_workspace(self, device, batch, lane=0):
+    def _cfb_workspace(self, device, batch, lane=0, sweep_k=0):
         lib = _lib.load()
         key = (device.index, torch.cuda.current_stream(device).cuda_stream, lane)
-        need = lib.cfb_workspace_bytes(self._net, batch)
+        need = lib.cfb_sweep_workspace_bytes(self._net, batch, sweep_k) if sweep_k else lib.cfb_workspace_bytes(self._net, batch)
         if need < 0:
-            _lib.check(1, 'cfb_workspace_bytes')
+            _lib.check(1, 'cfb_sweep_workspace_bytes' if sweep_k else 'cfb_workspace_bytes')
         ws = self._cfb_ws.get(key)
         if ws is None or ws.numel() < need:
             self._cfb_ws.pop(key, None)
+            ws = None                                  # the old buffer is free before the larger one is allocated
             ws = torch.empty(int(need), dtype=torch.uint8, device=device)   # owned by the module (the caller may
             self._cfb_ws[key] = ws                                          # empty_cache() after every face)
         return ws
@@ -445,6 +446,39 @@ def fidelity_weights(w, n, device=None):
     if t.dim() != 1 or t.shape[0] != n:
         raise RuntimeError(f'w: expected one fidelity weight per face, shape [{n}], got {tuple(t.shape)}')
     return t.to(torch.float32).contiguous()
+
+
+def sweep_weights(ws, device=None):
+    """The K fidelity weights of a sweep (``CodeFormer.forward_u8_sweep``, ``restore_images_sweep``): a 1-D sequence of
+    numbers, a floating numpy array or a floating tensor of K >= 1 values, on the host or on the CUDA ``device`` -> a contiguous
+    float32 tensor [K] where it was given.  An empty, 0-d or multi-dimensional ``ws``, a non-floating array or tensor or a
+    sequence of non-numbers raises ValueError; a CUDA tensor on another device than ``device`` RuntimeError."""
+    if torch.is_tensor(ws):
+        if not ws.dtype.is_floating_point:
+            raise ValueError(f'ws: fidelity weights must be floating point, got a {ws.dtype} tensor')
+        if ws.is_cuda and device is not None and ws.device != torch.device(device):
+            raise RuntimeError(f'ws: fidelity weights are on {ws.device}, the faces on {torch.device(device)}')
+        t = ws.detach()
+    elif isinstance(ws, (np.ndarray, list, tuple)):
+        try:
+            a = np.asarray(ws)
+        except ValueError as err:
+            raise ValueError(f'ws: expected a 1-D sequence of fidelity weights ({err})') from None
+        if a.dtype.kind not in ('f' if isinstance(ws, np.ndarray) else 'fiub'):
+            raise ValueError(f'ws: fidelity weights must be floating point, got {a.dtype}')
+        t = torch.from_numpy(a.astype(np.float32))
+    else:
+        raise ValueError(f'ws: expected a 1-D sequence, array or tensor of fidelity weights, got {type(ws).__name__}')
+    if t.dim() != 1 or t.shape[0] == 0:
+        raise ValueError(f'ws: expected K >= 1 fidelity weights in one dimension, got shape {tuple(t.shape)}')
+    return t.to(torch.float32).contiguous()
+
+
+def sweep_chunks(n_faces, k, max_batch):
+    """Chunk plan of a fidelity sweep over ``n_faces`` faces at ``k`` weights: consecutive [lo, hi) ranges of
+    ``max(1, max_batch // k)`` faces, so that the decoder batch (faces x k) stays within ``max_batch`` when k <= max_batch."""
+    step = max(1, int(max_batch) // max(1, int(k)))
+    return [(lo, min(n_faces, lo + step)) for lo in range(0, n_faces, step)]
 
 
 def _weights_on(w, dev):
@@ -658,6 +692,43 @@ class CodeFormer(VQAutoEncoder):
                 return bufs[2].clone()
             out = torch.empty_like(faces_bgr)
             launch(faces_bgr, w if per_face else None, out, self._cfb_workspace(dev, B))
+        return out
+
+    def forward_u8_sweep(self, faces_bgr, ws, adain=True):
+        """A fidelity sweep (``cfb_codeformer_sweep_u8``): DEVICE uint8 [B,512,512,3] HWC BGR faces, each restored at every
+        weight of ``ws`` (``sweep_weights``: K >= 1 values, shared by all faces) -> CUDA uint8 [B,K,512,512,3].  The encoder,
+        the Transformer, the code lookup and AdaIN run once per face; only the generator and the Fuse_sft_blocks run B*K
+        times.  ``[b, k]`` equals ``forward_u8(faces_bgr[b:b+1], w=ws[k], adain=adain)``, byte for byte; as with per-face
+        weights, the Fuse_sft_blocks run for every weight (w <= 0 or NaN blends with 0), so in fp16 precision their operand
+        range guard can fail a sweep whose scalar calls would have skipped them."""
+        if not torch.is_tensor(faces_bgr) or not faces_bgr.is_cuda or faces_bgr.dtype != torch.uint8:
+            raise RuntimeError('forward_u8_sweep expects a CUDA uint8 tensor')
+        if faces_bgr.dim() != 4 or tuple(faces_bgr.shape[1:]) != (512, 512, 3):
+            raise RuntimeError(f'forward_u8_sweep expects [B,512,512,3] HWC BGR faces, got {tuple(faces_bgr.shape)}')
+        lib = _lib.load()
+        faces_bgr = faces_bgr.contiguous()
+        B, dev = faces_bgr.shape[0], faces_bgr.device
+        ws, adain = sweep_weights(ws, dev), bool(adain)
+        K = ws.shape[0]
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            if B == 0:
+                return torch.empty((0, K, 512, 512, 3), dtype=torch.uint8, device=dev)
+            wv = _weights_on(ws, dev).repeat(B)           # [B*K], face-major: decoder face b*K + k takes ws[k]
+
+            def launch(src, wv, dst, ws_buf):
+                _lib.check(lib.cfb_codeformer_sweep_u8(self._net, _lib.ptr(src), _lib.ptr(dst), None, None, None, B, K,
+                                                       _lib.ptr(wv), int(adain), _lib.ptr(ws_buf), ws_buf.numel(),
+                                                       _lib.stream(dev)), 'cfb_codeformer_sweep_u8')
+            # the weights are a static input: one graph per (B, K) serves every ws
+            bufs = self._graphed(('u8sweep', dev.index, B, K, adain, self._precision), (faces_bgr, wv), lambda: (
+                torch.empty_like(faces_bgr), torch.empty_like(wv),
+                torch.empty((B, K, 512, 512, 3), dtype=torch.uint8, device=dev),
+                torch.empty(int(lib.cfb_sweep_workspace_bytes(self._net, B, K)), dtype=torch.uint8, device=dev)), launch)
+            if bufs is not None:
+                return bufs[2].clone()
+            out = torch.empty((B, K, 512, 512, 3), dtype=torch.uint8, device=dev)
+            launch(faces_bgr, wv, out, self._cfb_workspace(dev, B, sweep_k=K))
         return out
 
     def restore_faces(self, faces, w=0.5, adain=True, max_batch=32, device=None, on_error='input', inpaint=False):

@@ -296,6 +296,12 @@ int adain_nhwc(const float* content, const float* style, float* out, int B, int 
 int nchw_to_nhwc(const float* in, float* out, int N, int C, int HW, cudaStream_t st);
 int nhwc_to_nchw(const float* in, float* out, int N, int C, int HW, cudaStream_t st);
 int concat_channels(const float* a, const float* b, float* out, int64_t pixels, int Ca, int Cb, cudaStream_t st);
+// fidelity sweep (cfb_codeformer_sweep_u8): for each listed buffer of B faces of `bytes` each, face b is copied to faces
+// b*K .. b*K+K-1 of dst (face-major).  bytes, src and dst 16-byte aligned.
+constexpr int EXPAND_MAX = 16;
+struct ExpandCopy { const void* src; void* dst; int64_t bytes; };
+struct ExpandList { ExpandCopy d[EXPAND_MAX]; int n = 0; };
+int expand_faces(const ExpandList& L, int B, int K, cudaStream_t st);
 
 // VectorQuantizer.forward core on token-major z [T,D] (NHWC); writes idx, zq_st = z + (E[idx]-z) [T,D],
 // stats = {loss, perplexity, mean_distance, 0}; onehot optional [T,K]

@@ -312,6 +312,7 @@ struct cfb_net : cfb::NetCore {
   unsigned* gn_counters = nullptr;    // ticket-counter ring of the split GroupNorm finalize (in the slab, zero between uses)
   int gn_ctr_pos = 0;
   std::map<int, int64_t> ws_memo;     // batch -> cfb_workspace_bytes (16 host-side dry runs per miss)
+  std::map<std::pair<int, int>, int64_t> sweep_ws_memo;   // (batch, k) -> cfb_sweep_workspace_bytes
   int engine = 0;                     // 0 auto (wgmma where the shape allows), 1 fp32 CUDA cores, 2 wgmma only
   std::map<std::string, std::pair<float*, int64_t>> captures;   // stage name -> (device dst, capacity in floats)
 };
@@ -508,6 +509,7 @@ static int prepare(cfb_net* n, cudaStream_t st) {
   n->sm_count = sms > 0 ? sms : 148;
   n->tc_ok = (major == 9);
   n->ws_memo.clear();
+  n->sweep_ws_memo.clear();
   CFB_CHECK(async_status_init(st));
   char* p = (char*)n->slab;
   auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
@@ -849,6 +851,40 @@ struct Fwd {
     return 0;
   }
 
+  // Fidelity sweep: the decoder runs at batch N*K on the encoder results of N faces; decoder face b*K+k gets face b's
+  // generator input and encoder taps, in one expand_faces launch.  Of a tap, fuse() reads the fp32 activation p and, through
+  // stats_from_parts, gn_part / gn_slots; it never reads the tap's operand planes (the concatenation's planes are rebuilt
+  // from p), so those are not copied.  Every copied buffer is contiguous per face, which makes face b one run of bytes at
+  // b * bytes-per-face: p is NHWC [N][H][W][C]; gn_part is [N][gn_slots][64] (gn_coef_from_partials reads image n's slots at
+  // n * gn_slots).  The batch-N buffers are released here, the expanded taps after their fusion (generator()).
+  int expand_for_sweep(Tensor& quant, std::map<int, Tensor>& taps, int K) {
+    ExpandList L;
+    std::vector<std::pair<Tensor*, Tensor>> grown;      // (batch-N tensor, its expansion)
+    auto grow = [&](Tensor& t) -> int {
+      CFB_REQUIRE(t.p && !t.p2 && L.n + 2 <= EXPAND_MAX, "sweep: unexpected decoder input");
+      Tensor e;
+      CFB_CHECK(alloc(e, t.N * K, t.H, t.W, t.C));
+      L.d[L.n++] = {t.p, e.p, (int64_t)t.H * t.W * t.C * 4};
+      if (t.gn_part) {
+        const int64_t pb = (int64_t)t.gn_slots * 64 * sizeof(float);
+        e.gn_slots = t.gn_slots;
+        CFB_CHECK(alloc_raw((void**)&e.gn_part, (size_t)e.N * pb));
+        L.d[L.n++] = {t.gn_part, e.gn_part, pb};
+      }
+      grown.push_back({&t, e});
+      return 0;
+    };
+    const int N = quant.N;
+    CFB_CHECK(grow(quant));
+    for (auto& kv : taps) CFB_CHECK(grow(kv.second));
+    if (!dry) CFB_CHECK(expand_faces(L, N, K, st));
+    for (auto& g : grown) {       // the sources are free once their one reader is enqueued
+      release(*g.first);
+      *g.first = g.second;
+    }
+    return 0;
+  }
+
   // conv1 of a fused ResBlock at this shape: fused operand transform available?
   bool xf_ok(int N, int H, int W, const ConvW& w) const {
     if (!(engine == 2 || (engine == 0 && n->tc_ok))) return false;
@@ -1099,7 +1135,8 @@ static std::vector<int> tap_blocks_of(const cfb_config& c, bool encoder) {
 static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float* logits, float* lq_feat,
                                    int64_t* top_idx, int B, float w, int adain, int code_only, void* ws, int64_t ws_bytes,
                                    cudaStream_t st, bool dry, const unsigned char* x_u8 = nullptr,
-                                   unsigned char* out_u8 = nullptr, bool inpaint = false, const float* w_dev = nullptr) {
+                                   unsigned char* out_u8 = nullptr, bool inpaint = false, const float* w_dev = nullptr,
+                                   int sweep_k = 1) {
   CFB_REQUIRE(n->cfg.kind == 1, "net was created as VQAutoEncoder");
   CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
   if (!dry) CFB_CHECK(check_device(n));
@@ -1139,6 +1176,8 @@ static int codeformer_forward_impl(cfb_net* n, const float* x, float* out, float
   }
   CFB_CHECK(f.capture("quant", quant));
   f.release(lq);
+  // fidelity sweep (cfb_codeformer_sweep_u8): w_dev holds B*K weights, face-major; the decoder runs at batch B*K
+  if (sweep_k > 1) CFB_CHECK(f.expand_for_sweep(quant, taps, sweep_k));
   CFB_CHECK(f.generator(quant, out, want_taps ? &taps : nullptr, tap_blocks_of(c, false), w, w_dev));
   return 0;
 }
@@ -2610,6 +2649,33 @@ int64_t cfb_workspace_bytes(cfb_net* n, int32_t batch) {
   API_END(-1)
 }
 
+int64_t cfb_sweep_workspace_bytes(cfb_net* n, int32_t batch, int32_t k) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_sweep_workspace_bytes: NULL net"); return -1; }
+  if (n->cfg.kind != 1 || batch < 0 || k < 1 || (int64_t)batch * k > INT32_MAX) {
+    cfb::set_error("cfb_sweep_workspace_bytes: needs a CodeFormer net, batch >= 0 and k >= 1");
+    return -1;
+  }
+  std::lock_guard<std::mutex> lk(n->mu);
+  {
+    auto it = n->sweep_ws_memo.find({batch, k});
+    if (it != n->sweep_ws_memo.end()) return it->second;
+  }
+  // the worst of the flags a sweep takes: AdaIN on or off, caller-provided logits or not
+  size_t high = 0;
+  for (int m = 0; m < 4; ++m) {
+    float* lg = (m & 2) ? (float*)0x1000 : nullptr;
+    if (cfb::codeformer_forward_impl(n, nullptr, nullptr, lg, (float*)0x1000, nullptr, batch, 0.f, m & 1, 0, nullptr, 0, nullptr,
+                                     true, (const unsigned char*)0x1000, (unsigned char*)0x1000, false, (const float*)0x1000,
+                                     k) != 0)
+      return -1;
+    if (n->arena.high() > high) high = n->arena.high();
+  }
+  n->sweep_ws_memo[{batch, k}] = (int64_t)high + 4096;
+  return (int64_t)high + 4096;
+  API_END(-1)
+}
+
 int64_t cfb_last_launch_count(cfb_net* n) { return n ? n->last_launches : 0; }
 
 int cfb_net_set_engine(cfb_net* n, int32_t engine) {
@@ -2618,6 +2684,7 @@ int cfb_net_set_engine(cfb_net* n, int32_t engine) {
   std::lock_guard<std::mutex> lk(n->mu);
   n->engine = engine;
   n->ws_memo.clear();
+  n->sweep_ws_memo.clear();
   return 0;
   API_END(1)
 }
@@ -2636,6 +2703,7 @@ int cfb_net_capture(cfb_net* n, const char* stage, float* dst, int64_t capacity)
   if (dst) n->captures[stage] = {dst, capacity};
   else n->captures.erase(stage);
   n->ws_memo.clear();
+  n->sweep_ws_memo.clear();
   return 0;
   API_END(1)
 }
@@ -2675,7 +2743,7 @@ int cfb_codeformer_forward_wv(cfb_net* n, const float* x, float* out, float* log
 
 static int codeformer_u8(const char* what, cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits,
                          float* lq_feat, int64_t* top_idx, int32_t batch, float w, int32_t adain, void* workspace,
-                         int64_t workspace_bytes, void* stream, bool inpaint, const float* w_dev = nullptr) {
+                         int64_t workspace_bytes, void* stream, bool inpaint, const float* w_dev = nullptr, int sweep_k = 1) {
   CFB_REQUIRE(n, std::string(what) + ": NULL net");
   if (batch == 0) return 0;
   CFB_REQUIRE(faces_bgr && restored_bgr, std::string(what) + ": NULL image pointer");
@@ -2683,7 +2751,7 @@ static int codeformer_u8(const char* what, cfb_net* n, const uint8_t* faces_bgr,
   const int64_t before = cfb::launch_count();
   const int rc = cfb::codeformer_forward_impl(n, nullptr, nullptr, logits, lq_feat, top_idx, batch, w, adain, 0, workspace,
                                               workspace_bytes, (cudaStream_t)stream, false, faces_bgr, restored_bgr, inpaint,
-                                              w_dev);
+                                              w_dev, sweep_k);
   n->last_launches = cfb::launch_count() - before;
   return rc;
 }
@@ -2723,6 +2791,18 @@ int cfb_codeformer_inpaint_u8_wv(cfb_net* n, const uint8_t* faces_bgr, uint8_t* 
   CFB_REQUIRE(w_dev || batch == 0, "cfb_codeformer_inpaint_u8_wv: NULL w_dev");
   return codeformer_u8("cfb_codeformer_inpaint_u8_wv", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, 0.f, adain,
                        workspace, workspace_bytes, stream, true, w_dev);
+  API_END(1)
+}
+
+int cfb_codeformer_sweep_u8(cfb_net* n, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                            int64_t* top_idx, int32_t batch, int32_t k, const float* w_dev, int32_t adain, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(k >= 1, "cfb_codeformer_sweep_u8: k must be >= 1");
+  CFB_REQUIRE((int64_t)batch * k <= INT32_MAX, "cfb_codeformer_sweep_u8: batch * k too large");
+  CFB_REQUIRE(w_dev || batch == 0, "cfb_codeformer_sweep_u8: NULL w_dev");
+  return codeformer_u8("cfb_codeformer_sweep_u8", n, faces_bgr, restored_bgr, logits, lq_feat, top_idx, batch, 0.f, adain,
+                       workspace, workspace_bytes, stream, false, w_dev, k);
   API_END(1)
 }
 

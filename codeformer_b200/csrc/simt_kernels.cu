@@ -16,6 +16,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <math.h>
 #include <stdint.h>
@@ -1209,6 +1210,38 @@ int concat_channels(const float* a, const float* b, float* out, int64_t pixels, 
   concat_kernel<<<(unsigned)(blocks > 148 * 16 ? 148 * 16 : blocks), 256, 0, st>>>((const float4*)a, (const float4*)b,
                                                                                    (float4*)out, pixels, Ca / 4, Cb / 4);
   CFB_LAUNCH_CHECK();
+  return 0;
+}
+
+// Fidelity sweep: buffer d holds B faces of d.bytes each, back to back; face b goes to faces b*K .. b*K+K-1 of its
+// destination.  Each 16-byte vector is read once and stored K times.  grid: (x-stride over a face, buffer, source face).
+__global__ void expand_faces_kernel(const __grid_constant__ ExpandList L, int B, int K) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const ExpandCopy& d = L.d[blockIdx.y];
+  const int64_t nv = d.bytes / 16;
+  for (int b = blockIdx.z; b < B; b += gridDim.z) {
+    const uint4* src = (const uint4*)d.src + (int64_t)b * nv;
+    uint4* dst = (uint4*)d.dst + (int64_t)b * K * nv;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (int64_t)gridDim.x * blockDim.x) {
+      const uint4 v = __ldg(src + i);
+      for (int k = 0; k < K; ++k) dst[(int64_t)k * nv + i] = v;
+    }
+  }
+}
+int expand_faces(const ExpandList& L, int B, int K, cudaStream_t st) {
+  CFB_REQUIRE(L.n >= 0 && L.n <= EXPAND_MAX, "expand_faces: too many buffers");
+  if (B == 0 || L.n == 0) return 0;
+  int64_t big = 0;
+  for (int i = 0; i < L.n; ++i) {
+    const ExpandCopy& d = L.d[i];
+    CFB_REQUIRE(d.bytes % 16 == 0 && (uintptr_t)d.src % 16 == 0 && (uintptr_t)d.dst % 16 == 0,
+                "expand_faces: buffers must be 16-byte aligned, with a multiple of 16 bytes per face");
+    big = std::max(big, d.bytes / 16);
+  }
+  // about 8 vectors per thread of the largest buffer; the small buffers' surplus blocks exit at once
+  const int64_t gx = std::min<int64_t>(std::max<int64_t>((big + 2047) / 2048, 1), 512);
+  CFB_LAUNCH_PDL(expand_faces_kernel, dim3((unsigned)gx, (unsigned)L.n, (unsigned)std::min(B, 65535)), dim3(256), 0, st, L, B, K);
   return 0;
 }
 

@@ -23,6 +23,10 @@ and this package's drop-ins: read_image (with its INTER_LINEAR enlargement of im
     call over the chunk's gray faces, then the float64 paste (``cfb_paste_faces_f64``) over the gray images' canvases after
     the uint8 paste of the colour images' faces.  A chunk may mix gray and colour images; the colour ones are untouched.
 
+``restore_images_sweep`` gives ``restore_images`` at several fidelity weights from one pass of everything that does not
+depend on ``w``: detection, the crop warp and the background run once per chunk, each face's encoder and Transformer once
+(``CodeFormer.forward_u8_sweep``); the decoder, the gray colour transfer, the face upsampler, the masks and the paste per weight.
+
 ``restore_aligned`` is the ``--has_aligned`` loop of the same script (:180-213) over already aligned crops of any size: the
 INTER_LINEAR resize to 512x512, the gray test of all crops in one launch (``cfb_is_gray_u8``), CodeFormer in batches and the
 gray crops' colour transfer, all on the device.
@@ -35,7 +39,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .arch import fidelity_weights
+from .arch import fidelity_weights, sweep_chunks, sweep_weights
 from .detection import RetinaFace, cuda_u8_image
 from .detection import finish_detections as retinaface_finish
 from .upsampler import RealESRGANer
@@ -181,39 +185,43 @@ def _on_device(upsampler, upscale):
     return isinstance(upsampler, RealESRGANer) and upsampler._device_path() and upscale == float(upsampler.scale)
 
 
-def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_center_face=False, detection_resize=640,
-                   eye_dist_threshold=5, bg_upsampler=None, face_upsampler=None, max_batch=32, return_faces=False):
-    """Restore whole images in batches.  ``images``: a list of uint8 HWC BGR numpy arrays or CUDA tensors.  ``net``: a
-    ``CodeFormer``; ``detector``: ``init_detection_model('retinaface_resnet50' | 'YOLOv5l')``; ``parser``: a ParseNet
-    (``init_parsing_model()``) or None for use_parse=False.  ``bg_upsampler`` / ``face_upsampler``: objects with
-    ``enhance(img, outscale=upscale)`` (``RealESRGANer``).  A ``codeformer_b200.RealESRGANer`` over ``RRDBNet`` with
-    ``scale == upscale`` runs on the device, once per chunk of images for the backgrounds and once for the restored faces
-    (``enhance_batch``); any other upsampler is called per image / per face through ``enhance`` (for this package's
-    RealESRGANer at another scale that call runs the network and the INTER_LANCZOS4 resize on the device).  The float64 faces
-    of gray images go with the colour ones: one ``enhance_batch`` of the chunk's gray faces on the device, or ``enhance`` per
-    face; they come back uint8 as in the reference (a face above 256 is 16-bit to ``enhance``: NotImplementedError).
+def _restore_sweep(net, crops, ws, max_batch, errors, name='restore_images_sweep'):
+    """CodeFormer over the crops at each weight of ``ws`` (a float32 tensor [K]): ``forward_u8_sweep`` over chunks of
+    ``max(1, max_batch // K)`` crops.  Returns K tensors like ``crops``; a failed chunk gives its input faces back in every
+    variant (the reference's per-face fallback, inference_codeformer.py:208-210)."""
+    outs = [torch.empty_like(crops) for _ in range(ws.shape[0])]
+    dev = crops.device
+    for lo, hi in sweep_chunks(crops.shape[0], ws.shape[0], max_batch):
+        try:
+            res = net.forward_u8_sweep(crops[lo:hi], ws, adain=True)
+            torch.cuda.current_stream(dev).synchronize()
+            _lib.check(_lib.load().cfb_check_async_status(), name)
+            for k, o in enumerate(outs):
+                o[lo:hi] = res[:, k]
+        except RuntimeError as err:
+            errors.append((lo, str(err)))
+            for o in outs:
+                o[lo:hi] = crops[lo:hi]
+    return outs
 
-    Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
-    also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted (float64 for a gray image
-    without a face upsampler, as the reference's ``restored_faces`` holds them).  A gray image whose pasted canvas exceeds
-    256 comes back uint16, as in the reference.  Each image equals the
-    reference loop body on that image alone, whatever ``max_batch`` is.  ``self.last_restore_errors`` of the reference's
-    fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back.
 
-    ``w``: one fidelity weight, or one per image (``fidelity_weights`` over the images): every face of image i is restored
-    with ``w[i]``, and faces of images with different weights still share CodeFormer batches."""
-    import cv2    # estimateAffinePartial2D(LMEDS) / invertAffineTransform stay on the host, as in the reference
-    images = list(images)
+def _net_device(net, name):
     dev = next(net.parameters()).device
     if dev.type != 'cuda':
-        raise RuntimeError('restore_images: the network is not on a CUDA device; there is no CPU fallback')
-    w = fidelity_weights(w, len(images), dev)
-    if torch.is_tensor(w):
-        w = w.cpu()                                    # picked per face on the host, moved with each chunk's faces
-    max_batch = max(1, int(max_batch))
-    inputs = [_as_input(im, dev) for im in images]
-    results, crops_out, faces_out = [None] * len(images), [None] * len(images), [None] * len(images)
-    errors = []
+        raise RuntimeError(f'{name}: the network is not on a CUDA device; there is no CPU fallback')
+    return dev
+
+
+def _restore_pipeline(inputs, detector, parser, restore, upscale, only_center_face, detection_resize, eye_dist_threshold,
+                      bg_upsampler, face_upsampler, max_batch, dev):
+    """The body of ``restore_images`` with its CodeFormer stage as a parameter: ``restore(crops, idx, owner)`` gives the
+    restored faces of a chunk's crops as a list of V variants (V = 1 for ``restore_images``, one per weight for a sweep).  The
+    gray test, resizes, detection, landmark fits, crop warp, background and inverse affines run once per chunk; the gray
+    colour transfer, the face upsampler, the parse masks and the paste run per variant, each variant pasted on the one
+    background.  Returns (results[v][i], crops_out[i], faces_out[v][i])."""
+    import cv2    # estimateAffinePartial2D(LMEDS) / invertAffineTransform stay on the host, as in the reference
+    n_img = len(inputs)
+    results, crops_out, faces_out = None, [None] * n_img, None
     for idx in _chunks([t for t, _, _ in inputs], max_batch):
         x = torch.stack([inputs[i][0] for i in idx])
         h0, w0 = x.shape[1:3]
@@ -239,44 +247,49 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
                 affines.append(cv2.estimateAffinePartial2D(landmark, FACE_TEMPLATE, method=cv2.LMEDS)[0])
                 owner.append(k)
         crops = warp_faces_multi(x, affines, owner, FACE_SIZE)
-        wf = w[torch.as_tensor(np.asarray(idx, np.int64)[np.asarray(owner, np.int64)])].to(dev) if torch.is_tensor(w) else w
         with torch.no_grad():
-            restored = _restore(net, crops, wf, max_batch, errors)
+            restored_v = restore(crops, idx, owner)
+        if results is None:
+            results = [[None] * n_img for _ in restored_v]
+            faces_out = [[None] * n_img for _ in restored_v]
         owner = np.asarray(owner, np.int64)
         # add_restored_face: the faces of gray images become adain_npy(bgr2gray(restored), cropped), float64
         is_g = np.asarray([gray[k] for k in owner], bool)
         gsel, csel = np.nonzero(is_g)[0], np.nonzero(~is_g)[0]
         gt, ct = torch.from_numpy(gsel).to(dev), torch.from_numpy(csel).to(dev)
-        gray_faces = gray_adain_faces(restored[gt], crops[gt]) if len(gsel) else None
-        S = FACE_SIZE
-        if face_upsampler is not None and len(affines):
-            S = int(FACE_SIZE * upscale)
-            up = torch.empty((len(affines), S, S, 3), dtype=torch.uint8, device=dev)
+        variants = []
+        for restored in restored_v:
+            gray_faces = gray_adain_faces(restored[gt], crops[gt]) if len(gsel) else None
+            S = FACE_SIZE
+            if face_upsampler is not None and len(affines):
+                S = int(FACE_SIZE * upscale)
+                up = torch.empty((len(affines), S, S, 3), dtype=torch.uint8, device=dev)
 
-            def no_16bit(wide):
-                if any(wide):
-                    raise NotImplementedError('restore_images: the face upsampler returned a 16-bit face (a gray face above 256 '
-                                              'is 16-bit to RealESRGANer.enhance); 16-bit faces are not pasted')
+                def no_16bit(wide):
+                    if any(wide):
+                        raise NotImplementedError('restore_images: the face upsampler returned a 16-bit face (a gray face above '
+                                                  '256 is 16-bit to RealESRGANer.enhance); 16-bit faces are not pasted')
 
-            def host_faces(faces):
-                res = [np.asarray(face_upsampler.enhance(f, outscale=upscale)[0]) for f in faces]
-                no_16bit([r.dtype != np.uint8 for r in res])
-                if any(r.shape != (S, S, 3) for r in res):
-                    raise RuntimeError(f'restore_images: the face upsampler returned {res[0].shape[:2]}, expected {S}x{S}')
-                return torch.from_numpy(np.ascontiguousarray(np.stack(res))).to(dev)
-            if len(csel):
-                if _on_device(face_upsampler, upscale):
-                    up[ct] = face_upsampler.enhance_batch(restored[ct], outscale=upscale)
-                else:
-                    up[ct] = host_faces(restored[ct].cpu().numpy())
-            if len(gsel):          # the float64 faces come back uint8, as enhance returns them in the reference
-                if _on_device(face_upsampler, upscale):
-                    res = face_upsampler.enhance_batch(gray_faces, outscale=upscale)
-                    no_16bit([r.dtype != torch.uint8 for r in res])
-                    up[gt] = torch.stack(res)
-                else:
-                    up[gt] = host_faces(gray_faces.cpu().numpy())
-            restored, gray_faces = up, None
+                def host_faces(faces):
+                    res = [np.asarray(face_upsampler.enhance(f, outscale=upscale)[0]) for f in faces]
+                    no_16bit([r.dtype != np.uint8 for r in res])
+                    if any(r.shape != (S, S, 3) for r in res):
+                        raise RuntimeError(f'restore_images: the face upsampler returned {res[0].shape[:2]}, expected {S}x{S}')
+                    return torch.from_numpy(np.ascontiguousarray(np.stack(res))).to(dev)
+                if len(csel):
+                    if _on_device(face_upsampler, upscale):
+                        up[ct] = face_upsampler.enhance_batch(restored[ct], outscale=upscale)
+                    else:
+                        up[ct] = host_faces(restored[ct].cpu().numpy())
+                if len(gsel):          # the float64 faces come back uint8, as enhance returns them in the reference
+                    if _on_device(face_upsampler, upscale):
+                        res = face_upsampler.enhance_batch(gray_faces, outscale=upscale)
+                        no_16bit([r.dtype != torch.uint8 for r in res])
+                        up[gt] = torch.stack(res)
+                    else:
+                        up[gt] = host_faces(gray_faces.cpu().numpy())
+                restored, gray_faces = up, None
+            variants.append((restored, gray_faces))
         h_up, w_up = int(h * upscale), int(wd * upscale)
         if bg_upsampler is not None and _on_device(bg_upsampler, upscale):
             canvases = bg_upsampler.enhance_batch(torch.stack([inputs[i][0] for i in idx]), outscale=upscale)
@@ -306,31 +319,77 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
                 return None
             with torch.no_grad():
                 return torch.cat([parse_masks(faces[lo:lo + max_batch], parser) for lo in range(0, faces.shape[0], max_batch)])
-        wide = {}
-        if gray_faces is None:
-            out, _ = _paste_multi(canvases, restored, invs, owner, upscale, masks_of(restored))
-        else:
-            # the uint8 paste for the colour images' faces, then the float64 paste over the gray images' canvases alone
-            out, _ = _paste_multi(canvases, restored[ct], [invs[j] for j in csel], owner[csel], upscale, masks_of(restored[ct]))
-            gk = np.unique(owner[gsel])
-            gkt = torch.from_numpy(gk).to(dev)
-            gw = {}
-            out_g, _ = _paste_multi(out[gkt], gray_faces, [invs[j] for j in gsel], np.searchsorted(gk, owner[gsel]), upscale,
-                                    masks_of(gray_faces), gw)
-            out[gkt] = out_g
-            wide = {int(gk[k]): v for k, v in gw.items()}
-        for k, i in enumerate(idx):
-            sel = torch.from_numpy(np.nonzero(owner == k)[0]).to(dev)
-            res = wide.get(k, out[k])
-            faces = restored[sel]
-            if gray_faces is not None and gray[k]:
-                faces = gray_faces[torch.from_numpy(np.searchsorted(gsel, np.nonzero(owner == k)[0])).to(dev)]
-            if inputs[i][2]:
-                results[i] = res.cpu().numpy()
-                crops_out[i], faces_out[i] = crops[sel].cpu().numpy(), faces.cpu().numpy()
+        for v, (restored, gray_faces) in enumerate(variants):      # _paste_multi pastes on a copy of the canvases
+            wide = {}
+            if gray_faces is None:
+                out, _ = _paste_multi(canvases, restored, invs, owner, upscale, masks_of(restored))
             else:
-                results[i] = res
-                crops_out[i], faces_out[i] = crops[sel], faces
+                # the uint8 paste for the colour images' faces, then the float64 paste over the gray images' canvases alone
+                out, _ = _paste_multi(canvases, restored[ct], [invs[j] for j in csel], owner[csel], upscale,
+                                      masks_of(restored[ct]))
+                gk = np.unique(owner[gsel])
+                gkt = torch.from_numpy(gk).to(dev)
+                gw = {}
+                out_g, _ = _paste_multi(out[gkt], gray_faces, [invs[j] for j in gsel], np.searchsorted(gk, owner[gsel]),
+                                        upscale, masks_of(gray_faces), gw)
+                out[gkt] = out_g
+                wide = {int(gk[k]): val for k, val in gw.items()}
+            for k, i in enumerate(idx):
+                sel = torch.from_numpy(np.nonzero(owner == k)[0]).to(dev)
+                res = wide.get(k, out[k])
+                faces = restored[sel]
+                if gray_faces is not None and gray[k]:
+                    faces = gray_faces[torch.from_numpy(np.searchsorted(gsel, np.nonzero(owner == k)[0])).to(dev)]
+                if inputs[i][2]:
+                    results[v][i] = res.cpu().numpy()
+                    if v == 0:
+                        crops_out[i] = crops[sel].cpu().numpy()
+                    faces_out[v][i] = faces.cpu().numpy()
+                else:
+                    results[v][i] = res
+                    if v == 0:
+                        crops_out[i] = crops[sel]
+                    faces_out[v][i] = faces
+    return results, crops_out, faces_out
+
+
+def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_center_face=False, detection_resize=640,
+                   eye_dist_threshold=5, bg_upsampler=None, face_upsampler=None, max_batch=32, return_faces=False):
+    """Restore whole images in batches.  ``images``: a list of uint8 HWC BGR numpy arrays or CUDA tensors.  ``net``: a
+    ``CodeFormer``; ``detector``: ``init_detection_model('retinaface_resnet50' | 'YOLOv5l')``; ``parser``: a ParseNet
+    (``init_parsing_model()``) or None for use_parse=False.  ``bg_upsampler`` / ``face_upsampler``: objects with
+    ``enhance(img, outscale=upscale)`` (``RealESRGANer``).  A ``codeformer_b200.RealESRGANer`` over ``RRDBNet`` with
+    ``scale == upscale`` runs on the device, once per chunk of images for the backgrounds and once for the restored faces
+    (``enhance_batch``); any other upsampler is called per image / per face through ``enhance`` (for this package's
+    RealESRGANer at another scale that call runs the network and the INTER_LANCZOS4 resize on the device).  The float64 faces
+    of gray images go with the colour ones: one ``enhance_batch`` of the chunk's gray faces on the device, or ``enhance`` per
+    face; they come back uint8 as in the reference (a face above 256 is 16-bit to ``enhance``: NotImplementedError).
+
+    Returns the restored images (host uint8 arrays for host inputs, CUDA tensors for CUDA inputs); with ``return_faces``
+    also, per image, the cropped faces [n,512,512,3] and the restored faces as they were pasted (float64 for a gray image
+    without a face upsampler, as the reference's ``restored_faces`` holds them).  A gray image whose pasted canvas exceeds
+    256 comes back uint16, as in the reference.  Each image equals the
+    reference loop body on that image alone, whatever ``max_batch`` is.  ``self.last_restore_errors`` of the reference's
+    fallback is ``restore_images.last_errors``: (face offset, message) of each CodeFormer batch that fell back.
+
+    ``w``: one fidelity weight, or one per image (``fidelity_weights`` over the images): every face of image i is restored
+    with ``w[i]``, and faces of images with different weights still share CodeFormer batches."""
+    images = list(images)
+    dev = _net_device(net, 'restore_images')
+    w = fidelity_weights(w, len(images), dev)
+    if torch.is_tensor(w):
+        w = w.cpu()                                    # picked per face on the host, moved with each chunk's faces
+    max_batch = max(1, int(max_batch))
+    inputs = [_as_input(im, dev) for im in images]
+    errors = []
+
+    def restore(crops, idx, owner):
+        wf = w[torch.as_tensor(np.asarray(idx, np.int64)[np.asarray(owner, np.int64)])].to(dev) if torch.is_tensor(w) else w
+        return [_restore(net, crops, wf, max_batch, errors)]
+    results, crops_out, faces_out = _restore_pipeline(inputs, detector, parser, restore, upscale, only_center_face,
+                                                      detection_resize, eye_dist_threshold, bg_upsampler, face_upsampler,
+                                                      max_batch, dev)
+    results, faces_out = (results or [[]])[0], (faces_out or [[]])[0]
     restore_images.last_errors = errors
     if return_faces:
         return results, crops_out, faces_out
@@ -338,6 +397,37 @@ def restore_images(images, net, detector, parser=None, w=0.5, upscale=2, only_ce
 
 
 restore_images.last_errors = []
+
+
+def restore_images_sweep(images, net, detector, ws, parser=None, upscale=2, only_center_face=False, detection_resize=640,
+                         eye_dist_threshold=5, bg_upsampler=None, face_upsampler=None, max_batch=32, return_faces=False):
+    """``restore_images`` at several fidelity weights: ``results[k][i]`` equals ``restore_images(images, ..., w=ws[k])[i]``,
+    byte for byte and in dtype.  ``ws``: K >= 1 weights (``sweep_weights``), shared by all images.
+
+    Per chunk of images the gray test, the resizes, detection, the landmark fits, the crop warp and the background
+    upsample run once, and every face's encoder and Transformer run once (``CodeFormer.forward_u8_sweep`` over batches of
+    ``max(1, max_batch // K)`` faces).  Per weight: the gray colour transfer, the face upsampler, the parse masks (of the
+    restored faces) and the paste, each on the image's one background.  With ``return_faces`` also the cropped faces per
+    image (``crops[i]``) and the restored faces per weight (``faces[k][i]``).  A CodeFormer batch that fails gives its input
+    faces back in every variant; ``restore_images_sweep.last_errors`` lists (face offset, message) of each."""
+    images = list(images)
+    dev = _net_device(net, 'restore_images_sweep')
+    ws = sweep_weights(ws, dev).to(dev)
+    max_batch = max(1, int(max_batch))
+    inputs = [_as_input(im, dev, 'restore_images_sweep') for im in images]
+    errors = []
+    results, crops_out, faces_out = _restore_pipeline(
+        inputs, detector, parser, lambda crops, idx, owner: _restore_sweep(net, crops, ws, max_batch, errors), upscale,
+        only_center_face, detection_resize, eye_dist_threshold, bg_upsampler, face_upsampler, max_batch, dev)
+    if results is None:                                # no images
+        results = faces_out = [[] for _ in range(ws.shape[0])]
+    restore_images_sweep.last_errors = errors
+    if return_faces:
+        return results, crops_out, faces_out
+    return results
+
+
+restore_images_sweep.last_errors = []
 
 
 def restore_aligned(faces, net, w=0.5, adain=True, max_batch=32, return_crops=False):

@@ -130,6 +130,16 @@ int cfb_codeformer_forward_u8_wv(cfb_net* net, const uint8_t* faces_bgr, uint8_t
 int cfb_codeformer_inpaint_u8_wv(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
                                  int64_t* top_idx, int32_t batch, const float* w_dev, int32_t adain,
                                  void* workspace, int64_t workspace_bytes, void* stream);
+/* Fidelity sweep: `batch` faces, each at `k` fidelity weights, with one encoder / Transformer / code-lookup pass at batch
+ * `batch` and the decoder at batch batch*k.  w_dev: DEVICE float [batch*k], face-major (w_dev[b*k + j] is face b's j-th
+ * weight); restored_bgr: DEVICE uint8 [batch,k,512,512,3].  restored_bgr[b][j] equals cfb_codeformer_forward_u8_wv on face b
+ * alone with w = w_dev[b*k + j], byte for byte (so also cfb_codeformer_forward_u8 with that w); the fp16 caveat of the *_wv
+ * entry points applies.  logits / lq_feat / top_idx are optional and hold the batch-`batch` results.  No inpainting and no
+ * code_only.  workspace >= cfb_sweep_workspace_bytes(net, batch, k) (<0 on error). */
+int64_t cfb_sweep_workspace_bytes(cfb_net* net, int32_t batch, int32_t k);
+int cfb_codeformer_sweep_u8(cfb_net* net, const uint8_t* faces_bgr, uint8_t* restored_bgr, float* logits, float* lq_feat,
+                            int64_t* top_idx, int32_t batch, int32_t k, const float* w_dev, int32_t adain,
+                            void* workspace, int64_t workspace_bytes, void* stream);
 /* the same with HOST uint8 buffers (0.79 MB per face each way instead of 3.1 MB): H2D, forward, D2H, stream sync.
  * dev_scratch >= cfb_host_io_bytes(net, batch). */
 int cfb_codeformer_restore_host(cfb_net* net, const uint8_t* faces_host, uint8_t* restored_host, int32_t batch, float w,
