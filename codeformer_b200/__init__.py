@@ -15,6 +15,7 @@ from .yolov5face import YOLOv5lFace, YoloDetector   # noqa: F401
 from .pasteback import resize_area, warp_faces_multi, paste_faces_multi   # noqa: F401
 from .pasteback import resize_lanczos4, gray_adain_faces, add_restored_face   # noqa: F401
 from .wholeimage import restore_images, restore_images_sweep, restore_aligned   # noqa: F401
+from .arcface import ResNetArcFace, identity_similarity   # noqa: F401
 
 
 def check_async_status():
@@ -29,4 +30,4 @@ __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQua
            'warp_faces', 'paste_faces', 'align_warp_face', 'paste_faces_to_input_image', 'RetinaFace', 'init_detection_model',
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
-           'check_async_status']
+           'ResNetArcFace', 'identity_similarity', 'check_async_status']

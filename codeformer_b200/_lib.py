@@ -122,6 +122,15 @@ SIGNATURES = {
     'cfb_retinaface_forward': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_forward_u8': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_candidates': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, _P, _P]),
+    'cfb_arcface_create': (c_void_p, [c_int32, c_int32, c_int32, c_int32]),
+    'cfb_arcface_destroy': (None, [_P]),
+    'cfb_arcface_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
+    'cfb_arcface_prepare': (c_int, [_P, _P]),
+    'cfb_arcface_workspace_bytes': (c_int64, [_P, c_int32]),
+    'cfb_arcface_forward': (c_int, [_P, _P, _P, c_int32, _P, c_int64, _P]),
+    'cfb_arcface_forward_u8': (c_int, [_P, _P, _P, c_int32, _P, c_int64, _P]),
+    'cfb_debug_arcface_conv': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int32,
+                                       c_float, _P, _P, c_int64, _P]),
     'cfb_yolov5face_predictions': (c_int64, [c_int32, c_int32]),
     'cfb_yolov5face_create': (c_void_p, []),
     'cfb_yolov5face_destroy': (None, [_P]),

@@ -581,7 +581,10 @@ struct TcParams {
   int out_act;
   const float* sft_dec;
   const float* sft_scale;
-  float sft_w;
+  union {
+    float sft_w;
+    float prelu;            // PRELU kernels (ResNetArcFace, no SFT epilogue): the PReLU slope
+  };
   const float* wscale_inv;  // device scalar: 2^-k of the weight split
   float* out;
   __half* pl_hi;            // optional: `out` again as fp16 hi / lo planes (operand of a following raw-input conv)
@@ -670,13 +673,17 @@ struct TcCfg {
 // accumulation, chunked partial sums and their round-to-nearest folds are those of the split scheme, and wscale_inv undoes
 // 2^k exactly.  Built for GEN without SiLU (RRDBNet), the 128-wide and channel-major halo tiles and the per-tap engine
 // (CodeFormer's generator and Fuse_sft_block convs); K1 and the SiLU epilogue stay split.
+// PRELU: the epilogue activation is v > 0 ? v : p.prelu * v (ResNetArcFace); built for the generalised engine and the plain
+// per-tap engine, so that no other variant carries the branch.
 template <int BN, int CPG, bool HALO, bool XF, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false,
-          bool P1 = false>
+          bool P1 = false, bool PRELU = false>
 __global__ void __launch_bounds__(XF ? TcCfg<BN>::XF_THREADS : TcCfg<BN>::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, const TcParams p) {
   static_assert(!XF || HALO, "the fused operand transform exists for the halo engine only");
   static_assert(!GEN || (XF && CPG == 0), "the generalised addressing exists for the fused-transform engine only");
+  static_assert(!PRELU || (BN == 64 && CPG == 0 && !K1 && !CM && !SILU && !P1 && (GEN || !HALO)),
+                "the PReLU epilogue is built for the generalised and the per-tap engines");
   static_assert(!K1 || (XF && !GEN && CPG == 0), "K1 = fused transform of a 1x1 conv (patch = tile): its own instantiation");
   using Cfg = TcCfg<BN>;
   constexpr bool WIDE = Cfg::WIDE;
@@ -1329,7 +1336,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             const int r = it * 4 + rsub;
             float4 v = lds128f(stg + (uint32_t)(r * 128 + ((cch ^ (r & 7)) << 4)));
             v.x += bv.x + rres[it].x; v.y += bv.y + rres[it].y; v.z += bv.z + rres[it].z; v.w += bv.w + rres[it].w;
-            if (p.out_act == OUT_LRELU || p.out_act == OUT_RELU) {      // ReLU = slope 0 (a negative value becomes -0.0)
+            if constexpr (PRELU) {
+              v.x = v.x > 0.f ? v.x : p.prelu * v.x; v.y = v.y > 0.f ? v.y : p.prelu * v.y;
+              v.z = v.z > 0.f ? v.z : p.prelu * v.z; v.w = v.w > 0.f ? v.w : p.prelu * v.w;
+            } else if (p.out_act == OUT_LRELU || p.out_act == OUT_RELU) {      // ReLU = slope 0 (a negative value becomes -0.0)
               const float sl = p.out_act == OUT_LRELU ? 0.2f : 0.f;
               v.x = v.x > 0.f ? v.x : sl * v.x; v.y = v.y > 0.f ? v.y : sl * v.y;
               v.z = v.z > 0.f ? v.z : sl * v.z; v.w = v.w > 0.f ? v.w : sl * v.w;
@@ -1398,7 +1408,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           }
           const int64_t off = offs[k];
           v.x += bv.x + rres[k].x; v.y += bv.y + rres[k].y; v.z += bv.z + rres[k].z; v.w += bv.w + rres[k].w;
-          if (p.out_act == OUT_LRELU) {
+          if constexpr (PRELU) {
+            v.x = v.x > 0.f ? v.x : p.prelu * v.x; v.y = v.y > 0.f ? v.y : p.prelu * v.y;
+            v.z = v.z > 0.f ? v.z : p.prelu * v.z; v.w = v.w > 0.f ? v.w : p.prelu * v.w;
+          } else if (p.out_act == OUT_LRELU) {
             v.x = v.x > 0.f ? v.x : 0.2f * v.x; v.y = v.y > 0.f ? v.y : 0.2f * v.y;
             v.z = v.z > 0.f ? v.z : 0.2f * v.z; v.w = v.w > 0.f ? v.w : 0.2f * v.w;
           } else if (p.out_act == OUT_GELU) {
@@ -1629,7 +1642,7 @@ size_t tc_scratch_bytes(const ConvArgs& a) {
 struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
 
 template <int BN, int CPG, bool HALO, bool XF = false, bool GEN = false, bool K1 = false, bool CM = false, bool SILU = false,
-          bool P1 = false>
+          bool P1 = false, bool PRELU = false>
 static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int SMEM = XF ? Cfg::X_SMEM_BYTES : (HALO ? Cfg::H_SMEM_BYTES : Cfg::SMEM_BYTES);
@@ -1642,12 +1655,12 @@ static int launch_tc2(const TcMaps& m, const TcParams& p, int sm_count, cudaStre
   CFB_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    CFB_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1, PRELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count ? total : sm_count;
-  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st,
+  CFB_LAUNCH_PDL((conv_tc_kernel<BN, CPG, HALO, XF, GEN, K1, CM, SILU, P1, PRELU>), dim3((unsigned)grid), dim3(THREADS), (size_t)SMEM, st,
                  m.a_hi, m.a_lo, m.b_hi, m.b_lo, p);
   return 0;
 }
@@ -1693,6 +1706,14 @@ static int launch_tc(const TcMaps& m, const TcParams& p, int sm_count, cudaStrea
   // the SiLU epilogue (YOLOv5) is built into two variants only, so the others keep their register budgets
   CFB_REQUIRE(p.out_act != OUT_SILU || (CPG == 0 && (gen || (!p.xform && p.PW == 0))),
               "conv_tc: the SiLU epilogue is built for the per-tap and generalised engines without statistics");
+  if (p.out_act == OUT_PRELU) {     // ResNetArcFace: split precision, no statistics, no SFT / planes (conv_tc checks those)
+    CFB_REQUIRE(!single_pass && CPG == 0 && (gen || (!p.xform && p.PW == 0)),
+                "conv_tc: the PReLU epilogue is built for the split per-tap and generalised engines without statistics");
+    if constexpr (CPG == 0) {
+      if (gen) return launch_tc2<64, 0, true, true, true, false, false, false, false, true>(m, p, sm_count, st);
+      return launch_tc2<64, 0, false, false, false, false, false, false, false, true>(m, p, sm_count, st);
+    }
+  }
   if (single_pass) return launch_tc_p1<CPG>(m, p, sm_count, st, gen, tile);
   if (tile == TC_TILE_CM) {    // channel-major 128 x 64 tiles: conv_tc() only asks for them where tc_tile_kind() says so
     if constexpr (CPG <= 2) {
@@ -1851,8 +1872,9 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.cout_valid % 4 == 0 && p.res_pitch % 4 == 0 && p.res2_pitch % 4 == 0,
                 "conv_tc: channel pitches / offsets must be multiples of 4");
     CFB_REQUIRE(!a.subsample || (a.mode == CONV_SAME && a.Ho % 2 == 0 && a.Wo % 2 == 0), "conv_tc: subsampling needs even sizes");
-    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU || a.out_act == OUT_SILU,
-                "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU / SiLU epilogues");
+    CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU || a.out_act == OUT_SILU ||
+                    a.out_act == OUT_PRELU,
+                "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU / SiLU / PReLU epilogues");
   } else if (p.out_pitch != a.Cout || p.out_c0 != 0) {
     // per-tap engine writing a channel slice: the tile offsets use the destination pitch, which only the plain store follows
     CFB_REQUIRE(!geo.halo && p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.out_c0 + a.Cout <= p.out_pitch,
@@ -1880,6 +1902,11 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   // fused-transform variants keep their register budgets
   CFB_REQUIRE(!a.sft_wv || (a.sft_dec && !a.xform), "conv_tc: per-image SFT weights need the SFT epilogue of a raw-input conv");
   p.sft_dec = a.sft_dec; p.sft_scale = a.sft_scale; p.sft_w = a.sft_w; p.sft_wv = a.sft_wv; p.wscale_inv = a.wscale_inv;
+  if (a.out_act == OUT_PRELU) {
+    CFB_REQUIRE(!a.sft_dec && !a.gn_part && !a.out_planes && !a.residual2 && (a.gen || !geo.halo),
+                "conv_tc: the PReLU epilogue takes bias and residual only, on the generalised or the per-tap engine");
+    p.prelu = a.prelu_slope;
+  }
   p.out = a.gen || !a.out ? a.out : a.out + a.out_c0;      // per-tap engine: the slice offset is folded into the base pointer
   p.gn_part = a.gn_part; p.gn_cpg = a.Cout / 32;
   p.pl_hi = (__half*)a.out_planes;

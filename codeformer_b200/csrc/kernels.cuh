@@ -117,10 +117,16 @@ __device__ __forceinline__ void gn_merge_xor(float& mean, float& m2, int o, floa
   m2 = (m2 + oq) + (d * d) * (0.5f * n);
   mean = 0.5f * (mean + om);
 }
+// The caller's image plumbing of a uint8 face, bit for bit (inference_codeformer.py:199-200 + basicsr/utils/img_util.py:22-29):
+//   t = float32(u8 / 255.)  [numpy float64 division, then astype float32];  x = (t - 0.5) / 0.5  [torchvision normalize, fp32]
+__device__ __forceinline__ float u8_to_model_input(int u) {
+  const float t = (float)((double)u / 255.0);
+  return __fdiv_rn(__fsub_rn(t, 0.5f), 0.5f);
+}
 #endif
 
 enum InAct { IN_NONE = 0, IN_SILU = 1 };
-enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2, OUT_RELU = 3, OUT_SILU = 4 };
+enum OutAct { OUT_NONE = 0, OUT_LRELU = 1, OUT_GELU = 2, OUT_RELU = 3, OUT_SILU = 4, OUT_PRELU = 5 };
 enum ConvMode { CONV_SAME = 0, CONV_DOWN = 1, CONV_UP = 2 };
 
 // Convolution / linear layer as an implicit GEMM over NHWC fp32 activations.
@@ -149,6 +155,7 @@ struct ConvArgs {
   float sft_w = 0.f;
   const float* sft_wv = nullptr;    // [N] per-image w (device) in place of sft_w | null; w <= 0 or NaN blends with 0 (out = dec)
   float* out = nullptr;             // [N,Ho,Wo,Cout]
+  float prelu_slope = 0.f;          // OUT_PRELU (ResNetArcFace): out = v > 0 ? v : slope * v; generalised and per-tap engines
   // tensor-core engine only: GroupNorm(32) partials of `out`, [N*tiles_per_image*4][32 groups][mean, M2] floats
   float* gn_part = nullptr;
   // tensor-core engine only: also emit `out` as fp16 hi/lo operand planes for a following conv that consumes it raw
@@ -259,6 +266,21 @@ int yolo_copy(const float* src, int src_pitch, int src_c0, float* dst, int dst_p
 int yolo_decode(const float* const h[3], float* const raw[3], const int ny[3], const int nx[3], const float* anchor_grid, float* pred,
                 int N, int P, cudaStream_t st);
 int yolo_candidates(const float* pred, int N, int P, float thr, float* rows, int* counts, cudaStream_t st);
+// ResNetArcFace (arcface.cu): stem conv + PReLU + max pool (fp32 [N,1,128,128], or uint8 BGR 512 x 512 faces with the gray
+// resize fused) -> NHWC [N,64,64,64]; the per-image bn0 tables of the IRBlocks; the prepare-time BatchNorm folds
+int arc_stem(const float* x, const unsigned char* faces_bgr_hwc, const float* wt, const float* bias, float slope, float* out, int N,
+             cudaStream_t st);
+struct ArcBn0Table {               // block b's channels are [off[b], off[b + 1]) of the prepared per-channel tables
+  static constexpr int kMax = 128;
+  int blocks = 0;
+  int off[kMax + 1] = {};
+};
+int arc_bn0_tables(const float* scale, const float* shift, const ArcBn0Table& t, int N, float* dscale, float* dshift,
+                   cudaStream_t st);
+int arc_bn_affine(const float* g, const float* b, const float* m, const float* v, float eps, float* scale, float* shift, int C,
+                  cudaStream_t st);
+int arc_fold_fc(const float* w, const float* fc_b, const float* s4, const float* t4, const float* s5, const float* t5, int Cout, int C,
+                int HW, float* wout, float* bout, cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

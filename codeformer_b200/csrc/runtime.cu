@@ -1388,6 +1388,8 @@ struct GenLaunch {          // one generalised conv: src window -> destination s
   const float* res = nullptr; int res_pitch = 0; const float* res2 = nullptr; int res2_pitch = 0; float post = 1.f;
   int pad_mode = 0; bool sub = false;
   bool single_pass = false;   // fp16 operands, one product per k-step (ConvArgs::single_pass)
+  const float* in_scale = nullptr; const float* in_shift = nullptr;   // per-(image, channel) affine of the input (no activation)
+  float prelu = 0.f;          // act == OUT_PRELU: the slope
 };
 static int gen_conv(const GenLaunch& g, int sm_count, cudaStream_t st) {
   ConvArgs a;
@@ -1401,6 +1403,7 @@ static int gen_conv(const GenLaunch& g, int sm_count, cudaStream_t st) {
   a.out_pitch = g.out_pitch; a.out_c0 = g.out_c0; a.cout_valid = g.c->cout;
   a.res_pitch = g.res_pitch; a.residual2 = g.res2; a.res2_pitch = g.res2_pitch; a.post_scale = g.post;
   a.single_pass = g.single_pass;
+  a.in_scale = g.in_scale; a.in_shift = g.in_shift; a.prelu_slope = g.prelu;
   return conv_tc(a, nullptr, sm_count, st);
 }
 
@@ -1931,6 +1934,209 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
   }
   if (!dry) CFB_CHECK(rf_heads(hd, ch, cw, loc, conf, landms, N, (int)rf_priors(H, W), st));
   for (int k = 0; k < 3; ++k) ar.release(hd[k]);
+  return 0;
+}
+
+}  // namespace cfb
+
+// =========================================================================================================
+// ResNetArcFace('IRBlock', layers, use_se=False): identity embeddings of faces (scoring a fidelity sweep)
+//   /root/reference/basicsr/archs/arcface_arch.py:56-100 (IRBlock), 171-245 (ResNetArcFace); the gray 128 x 128 input of
+//   basicsr/models/codeformer_model.py:131-135 (gray_resize_for_identity).
+// Eval-mode BatchNorm after a conv is folded into its weights at prepare; the PReLU slopes (one scalar per module, shared by
+// both activations of an IRBlock) are read from the parameters at prepare.  Engines per conv form:
+//   stem (conv1 + bn1 + PReLU + MaxPool2d(2))          SIMT (arcface.cu), fp32 or uint8 BGR 512 x 512 faces (gray resize fused)
+//   IRBlock bn0 -> conv1 3x3 + bn1 + PReLU            generalised halo engine: bn0 is the fused operand transform (affine
+//                                                      without activation, applied inside the image only: the conv pads the
+//                                                      normalised tensor with zeros, which a weight fold would not), PReLU
+//                                                      epilogue
+//   conv2 3x3 + bn2 + residual + PReLU, stride 1      generalised halo engine, residual + PReLU epilogue
+//   conv2 3x3 stride 2 pad 1 (+ the same epilogue)    per-tap engine, PReLU epilogue
+//   downsample 1x1 stride 2 + BN                      per-tap engine
+//   bn4 -> flatten (NCHW) -> fc5 -> bn5               one linear (both BatchNorms folded, fc5's columns permuted to the NHWC
+//                                                      flatten at prepare) as a per-tap 1x1 conv over the B rows
+// 8 x 8 maps (layer4) are smaller than one 128-pixel tile: both engines run them as ragged tiles.
+// =========================================================================================================
+namespace cfb {
+struct ArcBlock {
+  int cin = 0, cout = 0, stride = 1;
+  GenConv c1, c2, ds;
+  bool has_ds = false;
+  float slope = 0.f;
+};
+}
+struct cfb_arcface : cfb::NetCore {
+  cfb_arcface() : NetCore("ResNetArcFace", "arcface") {}
+  int layers[4] = {2, 2, 2, 2};
+  std::vector<cfb::ArcBlock> blocks;
+  cfb::ArcBn0Table bn0;                    // channel offsets of each block's bn0 in bn0_scale / bn0_shift
+  float *bn0_scale = nullptr, *bn0_shift = nullptr;
+  float *stem_w = nullptr, *stem_b = nullptr;
+  float stem_slope = 0.f;
+  cfb::GenConv fc;                         // [512][8 * 8 * 512] on the NHWC flatten
+};
+namespace cfb {
+
+constexpr int ARC_FEAT = 8 * 8 * 512;      // fc5's input: layer4 at 8 x 8 for a 128 x 128 input
+
+static int arc_build(cfb_arcface* n) {     // ResNetArcFace.__init__ / _make_layer, arcface_arch.py:183-227
+  n->blocks.clear();
+  int inplanes = 64, total = 0;
+  for (int l = 0; l < 4; ++l) {
+    CFB_REQUIRE(n->layers[l] >= 1, "ResNetArcFace: every layer needs at least one block");
+    total += n->layers[l];
+  }
+  CFB_REQUIRE(total <= ArcBn0Table::kMax, "ResNetArcFace: at most " + std::to_string(ArcBn0Table::kMax) + " blocks");
+  n->bn0 = ArcBn0Table{};
+  for (int l = 0; l < 4; ++l) {
+    const int planes = 64 << l;
+    for (int b = 0; b < n->layers[l]; ++b) {
+      const std::string p = "layer" + std::to_string(l + 1) + "." + std::to_string(b) + ".";
+      ArcBlock k;
+      k.cin = inplanes; k.cout = planes; k.stride = (b == 0 && l > 0) ? 2 : 1;
+      k.c1 = plan_conv(p + "conv1.weight", inplanes, inplanes, 3, 1); k.c1.bn = p + "bn1.";
+      k.c2 = plan_conv(p + "conv2.weight", inplanes, planes, 3, k.stride); k.c2.bn = p + "bn2.";
+      k.has_ds = b == 0 && (k.stride != 1 || inplanes != planes);
+      if (k.has_ds) { k.ds = plan_conv(p + "downsample.0.weight", inplanes, planes, 1, k.stride); k.ds.bn = p + "downsample.1."; }
+      n->bn0.off[n->bn0.blocks + 1] = n->bn0.off[n->bn0.blocks] + inplanes;
+      ++n->bn0.blocks;
+      n->blocks.push_back(k);
+      inplanes = planes;
+    }
+  }
+  n->fc = plan_conv("fc5.weight", ARC_FEAT, 512, 1, 1);
+  return 0;
+}
+
+static int arc_prepare(cfb_arcface* n, cudaStream_t st) {
+  CFB_CHECK(n->begin_prepare(st));
+  CFB_CHECK(arc_build(n));
+  SlabPlan plan;
+  for (const ArcBlock& b : n->blocks) { plan.add(b.c1); plan.add(b.c2); if (b.has_ds) plan.add(b.ds); }
+  const int C0 = n->bn0.off[n->bn0.blocks];
+  const size_t fc_wn = (size_t)512 * ARC_FEAT;
+  CFB_CHECK(n->reserve_slab(plan.bytes() + 2 * align256((size_t)C0 * 4) + align256(64 * 9 * 4) + align256(64 * 4) +
+                            2 * align256(fc_wn * 2) + align256(512 * 4) + 256 + 4 * align256(512 * 4)));
+  WeightPrep wp(*n, plan, st);
+  n->bn0_scale = (float*)wp.take((size_t)C0 * 4); n->bn0_shift = (float*)wp.take((size_t)C0 * 4);
+  auto bn_affine = [&](const std::string& bn, int c, float* scale, float* shift) -> int {
+    const float* g = n->param(bn + "weight", c);
+    const float* be = n->param(bn + "bias", c);
+    const float* mu = n->param(bn + "running_mean", c);
+    const float* var = n->param(bn + "running_var", c);
+    if (!g || !be || !mu || !var) return 1;
+    return arc_bn_affine(g, be, mu, var, 1e-5f, scale, shift, c, st);      // nn.BatchNorm2d / BatchNorm1d default eps
+  };
+  std::vector<float> slopes(n->blocks.size() + 1, 0.f);
+  auto slope = [&](const std::string& name, float* dst) -> int {
+    const float* s = n->param(name, 1);
+    if (!s) return 1;
+    CFB_CUDA(cudaMemcpyAsync(dst, s, 4, cudaMemcpyDeviceToHost, st));
+    return 0;
+  };
+  auto folded = [&](GenConv& c) -> int {
+    CFB_CHECK(wp.fold(c.name, c.bn, c.cout, c.cin * c.k * c.k));
+    return wp.conv(c, wp.fold_w, wp.fold_b);
+  };
+  for (size_t i = 0; i < n->blocks.size(); ++i) {
+    ArcBlock& b = n->blocks[i];
+    const std::string p = b.c1.name.substr(0, b.c1.name.size() - std::string("conv1.weight").size());
+    CFB_CHECK(bn_affine(p + "bn0.", b.cin, n->bn0_scale + n->bn0.off[i], n->bn0_shift + n->bn0.off[i]));
+    CFB_CHECK(folded(b.c1));
+    CFB_CHECK(folded(b.c2));
+    if (b.has_ds) CFB_CHECK(folded(b.ds));
+    CFB_CHECK(slope(p + "prelu.weight", &slopes[i]));
+  }
+  n->stem_w = (float*)wp.take(64 * 9 * 4); n->stem_b = (float*)wp.take(64 * 4);
+  CFB_CHECK(wp.fold("conv1.weight", "bn1.", 64, 9));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, wp.fold_w, 64 * 9 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, wp.fold_b, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CHECK(slope("prelu.weight", &slopes.back()));
+  // the head: bn4 / bn5 as per-channel affines, folded with fc5 into a temporary fp32 weight, then split into the slab
+  GenConv& fc = n->fc;
+  fc.w_hi = (__half*)wp.take(fc_wn * 2); fc.w_lo = (__half*)wp.take(fc_wn * 2);
+  fc.bias = (float*)wp.take(512 * 4); fc.wscale = (float*)wp.take(8);
+  float* s4 = (float*)wp.take(512 * 4); float* t4 = (float*)wp.take(512 * 4);
+  float* s5 = (float*)wp.take(512 * 4); float* t5 = (float*)wp.take(512 * 4);
+  CFB_CHECK(bn_affine("bn4.", 512, s4, t4));
+  CFB_CHECK(bn_affine("bn5.", 512, s5, t5));
+  const float* w5 = n->param("fc5.weight", (int64_t)fc_wn);
+  const float* b5 = n->param("fc5.bias", 512);
+  if (!w5 || !b5) return 1;
+  float* tmp = nullptr;
+  CFB_CUDA(cudaMalloc((void**)&tmp, fc_wn * 4));
+  int rc = arc_fold_fc(w5, b5, s4, t4, s5, t5, 512, 512, 64, tmp, fc.bias, st);
+  if (rc == 0) rc = tc_split_weights(tmp, fc.w_hi, fc.w_lo, 512, ARC_FEAT, 1, fc.wscale, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  cudaFree(tmp);
+  if (rc) return rc;
+  CFB_REQUIRE(se == cudaSuccess, std::string("ResNetArcFace prepare: ") + cudaGetErrorString(se));
+  for (size_t i = 0; i < n->blocks.size(); ++i) n->blocks[i].slope = slopes[i];
+  n->stem_slope = slopes.back();
+  n->prepared = true;
+  return 0;
+}
+
+// x: fp32 [N,1,128,128] or faces: uint8 HWC BGR [N,512,512,3] -> emb [N,512]
+static int arc_forward(cfb_arcface* n, const float* x, const unsigned char* faces, float* emb, int N, void* ws, int64_t ws_bytes,
+                       cudaStream_t st, bool dry) {
+  CFB_CHECK(n->begin_forward(dry));
+  CFB_REQUIRE(N >= 0, "ResNetArcFace: negative batch");
+  if (N == 0) return 0;
+  if (n->blocks.empty()) CFB_CHECK(arc_build(n));
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  float *sc = nullptr, *sh = nullptr, *cur = nullptr;
+  CFB_CHECK(n->alloc(&sc, (size_t)N * n->bn0.off[n->bn0.blocks]));
+  CFB_CHECK(n->alloc(&sh, (size_t)N * n->bn0.off[n->bn0.blocks]));
+  if (!dry) CFB_CHECK(arc_bn0_tables(n->bn0_scale, n->bn0_shift, n->bn0, N, sc, sh, st));
+  CFB_CHECK(n->alloc(&cur, (size_t)N * 64 * 64 * 64));
+  if (!dry) CFB_CHECK(arc_stem(x, faces, n->stem_w, n->stem_b, n->stem_slope, cur, N, st));
+  int h = 64;
+  for (size_t i = 0; i < n->blocks.size(); ++i) {
+    const ArcBlock& b = n->blocks[i];
+    const int ho = b.stride == 2 ? h / 2 : h;
+    float *t1 = nullptr, *res = cur, *y = nullptr;
+    CFB_CHECK(n->alloc(&t1, (size_t)N * h * h * b.cin));
+    {   // prelu(bn1(conv1(bn0(x))))
+      GenLaunch g{&b.c1, cur, b.cin, h, h, N, t1, b.cin, 0, OUT_PRELU};
+      g.in_scale = sc + (size_t)N * n->bn0.off[i]; g.in_shift = sh + (size_t)N * n->bn0.off[i]; g.prelu = b.slope;
+      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+    }
+    if (b.has_ds) {
+      CFB_CHECK(n->alloc(&res, (size_t)N * ho * ho * b.cout));
+      CFB_CHECK(pertap_conv(*n, pertap_args(cur, N, h, h, b.cin, b.cout, 1, b.stride, res, 0, 0, OUT_NONE, nullptr), b.ds, dry, st));
+    }
+    CFB_CHECK(n->alloc(&y, (size_t)N * ho * ho * b.cout));
+    if (b.c2.gen) {   // prelu(bn2(conv2(.)) + residual)
+      GenLaunch g{&b.c2, t1, b.cin, h, h, N, y, b.cout, 0, OUT_PRELU};
+      g.res = res; g.res_pitch = b.cout; g.prelu = b.slope;
+      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+    } else {
+      ConvArgs a = pertap_args(t1, N, h, h, b.cin, b.cout, 3, 2, y, 0, 0, OUT_PRELU, res);
+      a.prelu_slope = b.slope;
+      CFB_CHECK(pertap_conv(*n, a, b.c2, dry, st));
+    }
+    ar.release(t1);
+    if (res != cur) ar.release(res);
+    ar.release(cur);
+    cur = y; h = ho;
+  }
+  CFB_REQUIRE(h == 8 && n->blocks.back().cout == 512, "ResNetArcFace: layer4 must end at 8 x 8 x 512");
+  // the head: the N flattened NHWC rows as one 1 x N image of ARC_FEAT channels; its operand planes are the plain fp16 split of
+  // the rows (concat_planes with one source), as the per-tap engine's own operand pass builds them for at most 2048 channels
+  ConvArgs a = pertap_args(cur, 1, 1, N, ARC_FEAT, 512, 1, 1, emb, 0, 0, OUT_NONE, nullptr);
+  a.wgt_hi = n->fc.w_hi; a.wgt_lo = n->fc.w_lo; a.wscale_inv = n->fc.wscale + 1; a.bias = n->fc.bias; a.skip_prep = true;
+  CFB_REQUIRE(tc_supported(a), "ResNetArcFace: head not supported by the wgmma engine");
+  void* planes = ar.alloc(tc_scratch_bytes(a));
+  CFB_REQUIRE(planes != nullptr, n->ws_error());
+  if (!dry) {
+    CFB_CHECK(concat_planes(cur, nullptr, planes, N, ARC_FEAT, 0, st));
+    CFB_CHECK(conv_tc(a, planes, n->sm_count, st));
+  }
+  ar.release(planes);
+  ar.release(cur);
+  ar.release(sc); ar.release(sh);
   return 0;
 }
 
@@ -2500,6 +2706,83 @@ int cfb_retinaface_candidates(const float* loc, const float* conf, const float* 
   CFB_REQUIRE(batch == 0 || (loc && conf && landms && rows && counts), "cfb_retinaface_candidates: NULL argument");
   CFB_REQUIRE(h >= 1 && w >= 1 && batch >= 0, "cfb_retinaface_candidates: empty image");
   return cfb::rf_candidates(loc, conf, landms, batch, h, w, conf_threshold, rows, counts, (cudaStream_t)stream);
+  API_END(1)
+}
+
+cfb_arcface* cfb_arcface_create(int32_t l1, int32_t l2, int32_t l3, int32_t l4) {
+  API_BEGIN
+  cfb_arcface* n = new cfb_arcface();
+  const int32_t l[4] = {l1, l2, l3, l4};
+  std::copy(l, l + 4, n->layers);
+  if (cfb::arc_build(n) != 0) { delete n; return nullptr; }
+  return n;
+  API_END(nullptr)
+}
+void cfb_arcface_destroy(cfb_arcface* n) { delete n; }
+int cfb_arcface_set_param(cfb_arcface* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_arcface_set_param: NULL argument");
+  return n->set_param(name, dev_ptr, numel);
+  API_END(1)
+}
+int cfb_arcface_prepare(cfb_arcface* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_arcface_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::arc_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_arcface_workspace_bytes(cfb_arcface* n, int32_t batch) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_arcface_workspace_bytes: NULL net"); return -1; }
+  return n->dry_run([&] { return cfb::arc_forward(n, (const float*)0x1000, nullptr, nullptr, batch, nullptr, 0, nullptr, true); });
+  API_END(-1)
+}
+int cfb_arcface_forward(cfb_arcface* n, const float* x, float* emb, int32_t batch, void* workspace, int64_t workspace_bytes,
+                        void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (x && emb && workspace)), "cfb_arcface_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::arc_forward(n, x, nullptr, emb, batch, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_arcface_forward_u8(cfb_arcface* n, const uint8_t* faces_bgr_hwc, float* emb, int32_t batch, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (faces_bgr_hwc && emb && workspace)), "cfb_arcface_forward_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::arc_forward(n, nullptr, faces_bgr_hwc, emb, batch, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_debug_arcface_conv(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h, int32_t w,
+                           int32_t cin, int32_t cout, int32_t ksize, int32_t stride, const float* in_scale, const float* in_shift,
+                           int32_t out_act, float prelu_slope, const float* residual, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(in && weight_oihw && out && workspace, "cfb_debug_arcface_conv: NULL argument");
+  CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_PRELU, "cfb_debug_arcface_conv: activation must be none or PReLU");
+  CFB_REQUIRE((in_scale != nullptr) == (in_shift != nullptr), "cfb_debug_arcface_conv: scale and shift go together");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ksize == 3 && stride == 1) {
+    CFB_REQUIRE(workspace_bytes >= cfb_conv2d_gen_workspace_bytes(cin, cout), "cfb_debug_arcface_conv: workspace too small");
+    CFB_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "cfb_debug_arcface_conv: channel counts must be multiples of 64");
+    CFB_CHECK(cfb::async_status_init(st));
+    int dev = 0, sms = 148;
+    CFB_CUDA(cudaGetDevice(&dev));
+    CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    cfb::GenConv c = cfb::plan_conv("", cin, cout);
+    char* p = (char*)(((uintptr_t)workspace + 255) / 256 * 256);
+    float* pad = (float*)p; p += align256((size_t)c.cout_p * c.cin_p * 9 * 4);
+    CFB_CHECK(cfb::prepare_conv(c, weight_oihw, bias, pad, p, st));
+    cfb::GenLaunch g{&c, in, cin, h, w, n, out, cout, 0, out_act};
+    g.res = residual; g.res_pitch = cout; g.in_scale = in_scale; g.in_shift = in_shift; g.prelu = prelu_slope;
+    return cfb::gen_conv(g, sms, st);
+  }
+  CFB_REQUIRE(in_scale == nullptr, "cfb_debug_arcface_conv: the input affine is built for 3x3 stride-1 convs");
+  CFB_REQUIRE(stride == 1 || stride == 2, "cfb_debug_arcface_conv: stride must be 1 or 2");
+  cfb::ConvArgs a = cfb::pertap_args(in, n, h, w, cin, cout, ksize, stride, out, 0, 0, out_act, residual);
+  a.prelu_slope = prelu_slope;
+  return pertap_nhwc("cfb_debug_arcface_conv", a, weight_oihw, bias, stride, workspace, workspace_bytes, st);
   API_END(1)
 }
 

@@ -228,12 +228,7 @@ int conv_f32(const ConvArgs& a, cudaStream_t st) {
 // =====================================================================================================
 // Thread = 4 horizontally adjacent pixels x COUT/4 channels (4 threads cover a pixel quad): every input value and every
 // weight read feeds 4 pixels; 16-byte coalesced NHWC stores.
-// The caller's image plumbing, bit for bit (inference_codeformer.py:199-200 + basicsr/utils/img_util.py:22-29):
-//   t = float32(u8 / 255.)  [numpy float64 division, then astype float32];  x = (t - 0.5) / 0.5  [torchvision normalize, fp32]
-__device__ __forceinline__ float u8_to_model_input(int u) {
-  const float t = (float)((double)u / 255.0);
-  return __fdiv_rn(__fsub_rn(t, 0.5f), 0.5f);
-}
+// The caller's image plumbing is u8_to_model_input (kernels.cuh),
 // and back (basicsr/utils/img_util.py:66-67,87-90 with min_max=(-1,1)): clamp, (x+1)/2, *255 in fp32, round half to even
 __device__ __forceinline__ unsigned model_output_to_u8(float v) {
   float t = fminf(fmaxf(v, -1.f), 1.f);

@@ -399,6 +399,32 @@ int       cfb_retinaface_forward_u8(cfb_retinaface* net, const uint8_t* img_bgr_
 int       cfb_retinaface_candidates(const float* loc, const float* conf, const float* landms, int32_t batch, int32_t h, int32_t w,
                                     float conf_threshold, float* rows, int32_t* counts, void* stream);
 
+/* ---- ResNetArcFace('IRBlock', layers, use_se=False) identity embeddings (basicsr/archs/arcface_arch.py; arcface.cu + the
+ * conv engine) ----
+ * create: the four block counts of `layers` (each >= 1).  Parameters by the reference's state-dict names (BatchNorm folded at
+ * prepare, the PReLU slopes read there).  forward: x fp32 [batch,1,128,128] (the gray identity input) -> emb [batch,512].
+ * forward_u8: uint8 HWC BGR faces [batch,512,512,3]; img2tensor(face / 255.) + normalize(0.5, 0.5), the gray conversion and the
+ * bilinear resize to 128 x 128 of gray_resize_for_identity are fused into the stem, and the result equals those steps as
+ * separate fp32 device passes followed by forward, bit for bit.  Workspace: cfb_arcface_workspace_bytes(net, batch).
+ * debug_conv (test entry point): one conv of the network's forms on NHWC fp32 -- 3x3 stride 1 on the generalised engine, with
+ * the optional per-(image, channel) input affine in_scale / in_shift [n][cin] (no activation; zero padding outside the image),
+ * or 1x1 / 3x3 stride 2 on the per-tap engine; out_act 0 none / 5 PReLU (prelu_slope), optional residual added before it.
+ * Workspace: cfb_conv2d_gen_workspace_bytes(cin, cout) for 3x3 stride 1, cfb_conv2d_pertap_workspace_bytes otherwise. */
+typedef struct cfb_arcface cfb_arcface;
+cfb_arcface* cfb_arcface_create(int32_t l1, int32_t l2, int32_t l3, int32_t l4);
+void         cfb_arcface_destroy(cfb_arcface* net);
+int          cfb_arcface_set_param(cfb_arcface* net, const char* name, const float* dev_ptr, int64_t numel);
+int          cfb_arcface_prepare(cfb_arcface* net, void* stream);
+int64_t      cfb_arcface_workspace_bytes(cfb_arcface* net, int32_t batch);
+int          cfb_arcface_forward(cfb_arcface* net, const float* x, float* emb, int32_t batch, void* workspace, int64_t workspace_bytes,
+                                 void* stream);
+int          cfb_arcface_forward_u8(cfb_arcface* net, const uint8_t* faces_bgr_hwc, float* emb, int32_t batch, void* workspace,
+                                    int64_t workspace_bytes, void* stream);
+int          cfb_debug_arcface_conv(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h,
+                                    int32_t w, int32_t cin, int32_t cout, int32_t ksize, int32_t stride, const float* in_scale,
+                                    const float* in_shift, int32_t out_act, float prelu_slope, const float* residual,
+                                    void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- YOLOv5l-face detector (facelib/detection/yolov5face, models/yolov5l.yaml; yolo.cu + the conv engine) ----
  * Parameters by the reference's state-dict names (BatchNorm folded at prepare; the Detect anchor_grid buffer gives the anchor
  * sizes in pixels).  h and w are multiples of 32; P = cfb_yolov5face_predictions(h, w) = 3 (hw/64 + hw/256 + hw/1024).
