@@ -9,6 +9,7 @@ from .registry import ARCH_REGISTRY, install          # noqa: F401
 from .arch import CodeFormer, VQAutoEncoder, VectorQuantizer   # noqa: F401
 from .upsampler import RRDBNet, RealESRGANer                   # noqa: F401
 from .parsing import ParseNet, face_parse_mask, init_parsing_model   # noqa: F401
+from .bisenet import BiSeNet   # noqa: F401
 from .pasteback import warp_faces, paste_faces, align_warp_face, paste_faces_to_input_image   # noqa: F401
 from .detection import RetinaFace, init_detection_model   # noqa: F401
 from .yolov5face import YOLOv5lFace, YoloDetector   # noqa: F401
@@ -26,7 +27,7 @@ def check_async_status():
     _lib.check(_lib.load().cfb_check_async_status(), 'check_async_status')
 
 
-__all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQuantizer', 'RRDBNet', 'RealESRGANer', 'ParseNet', 'face_parse_mask', 'init_parsing_model',
+__all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQuantizer', 'RRDBNet', 'RealESRGANer', 'ParseNet', 'BiSeNet', 'face_parse_mask', 'init_parsing_model',
            'warp_faces', 'paste_faces', 'align_warp_face', 'paste_faces_to_input_image', 'RetinaFace', 'init_detection_model',
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',

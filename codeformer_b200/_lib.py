@@ -122,6 +122,16 @@ SIGNATURES = {
     'cfb_retinaface_forward': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_forward_u8': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
     'cfb_retinaface_candidates': (c_int, [_P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, _P, _P]),
+    'cfb_bisenet_create': (c_void_p, [c_int32]),
+    'cfb_bisenet_destroy': (None, [_P]),
+    'cfb_bisenet_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
+    'cfb_bisenet_prepare': (c_int, [_P, _P]),
+    'cfb_bisenet_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32]),
+    'cfb_bisenet_forward': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_bisenet_masks_u8': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_debug_bisenet_bilinear': (c_int, [_P, c_int32, c_int32, c_int32, c_int32, c_int32, _P, c_int32, c_int32, _P]),
+    'cfb_debug_bisenet_attention': (c_int, [_P, c_int32, c_int32, c_int32, _P, _P, c_int32, c_int32, _P, _P, c_int32, c_int32, _P, _P,
+                                            _P]),
     'cfb_arcface_create': (c_void_p, [c_int32, c_int32, c_int32, c_int32]),
     'cfb_arcface_destroy': (None, [_P]),
     'cfb_arcface_set_param': (c_int, [_P, c_char_p, _P, c_int64]),

@@ -1,6 +1,7 @@
 // RetinaFace-ResNet50 (face detection of whole-image mode): the SIMT kernels around the conv engine.
 //   stem        torchvision resnet50 conv1 (7x7 s2 p3, 3 -> 64) + folded bn1 + ReLU; input fp32 NCHW or uint8 HWC BGR with the
-//               detector's (104, 117, 123) mean subtraction fused (facelib/detection/retinaface/retinaface.py:222)
+//               detector's (104, 117, 123) mean subtraction fused (facelib/detection/retinaface/retinaface.py:222), or with
+//               the face normalisation of u8_to_input fused (BiSeNet's ResNet18 has the same stem)
 //   maxpool     resnet50 maxpool (3x3 s2 p1, -inf padding)
 //   add_nearest FPN: output_k += F.interpolate(output_{k+1}, size=output_k.shape[2:], mode='nearest') (retinaface_net.py:84-94)
 //   heads       per-level head tensors [N,h,w,64] (bbox 8 | class 4 | landmark 20 | 0) -> loc / softmaxed conf / landms in
@@ -17,7 +18,9 @@ namespace cfb {
 
 // ---- stem: one thread per output pixel, all 64 channels; the folded OIHW weights [64][3][7][7] are read into shared memory
 // as [147 taps][64] ----
-template <bool U8>
+enum StemIn { STEM_F32 = 0, STEM_U8_DETECT = 1, STEM_U8_FACE = 2 };
+
+template <int IN>
 __global__ void __launch_bounds__(128) rf_stem_kernel(const float* __restrict__ x_nchw, const unsigned char* __restrict__ img,
                                                       const float* __restrict__ wt, const float* __restrict__ bias,
                                                       float* __restrict__ out, int H, int W, int Ho, int Wo) {
@@ -42,7 +45,8 @@ __global__ void __launch_bounds__(128) rf_stem_kernel(const float* __restrict__ 
         const int ix = 2 * ox - 3 + s;
         if ((unsigned)ix >= (unsigned)W) continue;
         float v;
-        if (U8) v = __fsub_rn((float)img[(((int64_t)n * H + iy) * W + ix) * 3 + ci], mean[ci]);   // exact in fp32
+        if (IN == STEM_U8_DETECT) v = __fsub_rn((float)img[(((int64_t)n * H + iy) * W + ix) * 3 + ci], mean[ci]);   // exact in fp32
+        else if (IN == STEM_U8_FACE) v = u8_to_model_input(img[(((int64_t)n * H + iy) * W + ix) * 3 + (2 - ci)]);   // RGB channel ci
         else v = __ldg(x_nchw + (((int64_t)n * 3 + ci) * H + iy) * W + ix);
         const float* wr = sw + ((ci * 7 + r) * 7 + s) * 64;
 #pragma unroll
@@ -58,12 +62,15 @@ __global__ void __launch_bounds__(128) rf_stem_kernel(const float* __restrict__ 
 }
 
 int rf_stem(const float* x_nchw, const unsigned char* img_bgr_hwc, const float* wt, const float* bias, float* out, int N, int H,
-            int W, cudaStream_t st) {
+            int W, cudaStream_t st, bool face_u8) {
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   if (N == 0) return 0;
   const dim3 grid((unsigned)((Wo + 127) / 128), (unsigned)Ho, (unsigned)N);
-  if (img_bgr_hwc) CFB_LAUNCH_PDL(rf_stem_kernel<true>, grid, dim3(128), 0, st, x_nchw, img_bgr_hwc, wt, bias, out, H, W, Ho, Wo);
-  else CFB_LAUNCH_PDL(rf_stem_kernel<false>, grid, dim3(128), 0, st, x_nchw, img_bgr_hwc, wt, bias, out, H, W, Ho, Wo);
+  if (img_bgr_hwc && face_u8)
+    CFB_LAUNCH_PDL(rf_stem_kernel<STEM_U8_FACE>, grid, dim3(128), 0, st, x_nchw, img_bgr_hwc, wt, bias, out, H, W, Ho, Wo);
+  else if (img_bgr_hwc)
+    CFB_LAUNCH_PDL(rf_stem_kernel<STEM_U8_DETECT>, grid, dim3(128), 0, st, x_nchw, img_bgr_hwc, wt, bias, out, H, W, Ho, Wo);
+  else CFB_LAUNCH_PDL(rf_stem_kernel<STEM_F32>, grid, dim3(128), 0, st, x_nchw, img_bgr_hwc, wt, bias, out, H, W, Ho, Wo);
   return 0;
 }
 

@@ -248,8 +248,10 @@ int relayout_thin_out(const float* oihw, float* out, int Cout, cudaStream_t st);
 int fold_bn(const float* w, const float* gamma, const float* beta, const float* mean, const float* var, float eps, float* wout,
             float* bout, int Cout, int per_out, cudaStream_t st);
 // RetinaFace-ResNet50 (detection.cu): stem conv + max-pool, FPN top-down add, head gather, candidate compaction
+// face_u8: the uint8 input is a BGR face normalised like u8_to_input (RGB, (x / 255 - 0.5) / 0.5; BiSeNet) instead of the
+// detector's mean-subtracted BGR image
 int rf_stem(const float* x_nchw, const unsigned char* img_bgr_hwc, const float* wt, const float* bias, float* out, int N, int H,
-            int W, cudaStream_t st);
+            int W, cudaStream_t st, bool face_u8 = false);
 int rf_maxpool(const float* in, float* out, int N, int H, int W, cudaStream_t st);
 int rf_add_nearest(float* fine, const float* coarse, int N, int Hf, int Wf, int Hc, int Wc, int C, cudaStream_t st);
 int rf_heads(const float* const h[3], const int hh[3], const int ww[3], float* loc, float* conf, float* landms, int N, int P,
@@ -281,6 +283,19 @@ int arc_bn_affine(const float* g, const float* b, const float* m, const float* v
                   cudaStream_t st);
 int arc_fold_fc(const float* w, const float* fc_b, const float* s4, const float* t4, const float* s5, const float* t5, int Cout, int C,
                 int HW, float* wout, float* bout, cudaStream_t st);
+// BiSeNet (bisenet.cu): whole-map mean of an NHWC tensor -> [N, C]; the 1x1 attention convs on it (one CTA per image); the
+// channel-scale combine; bilinear (align_corners=True) upsampling of the head logits, alone or fused with the parse argmax
+int bise_mean(const float* in, float* out, int N, int HW, int C, cudaStream_t st);
+struct BiseAttention {             // y = act1(w1 v + b1) [c0 -> c1], then z = act2(w2 y + b2) [c1 -> c2] when w2 is set
+  const float* w1; const float* b1; int c0, c1, act1;      // act: 0 none, 1 ReLU, 2 sigmoid; weights [cout][cin]
+  const float* w2; const float* b2; int c2, act2;
+};
+int bise_attention(const BiseAttention& a, const float* v, float* out, int N, cudaStream_t st);
+int bise_scale_add(const float* feat, const float* att, const float* add_vec, const float* add_t, float* out, int N, int64_t HW, int C,
+                   cudaStream_t st);
+int bise_bilinear(const float* in, int pitch, int h, int w, int C, float* out, int N, int H, int W, cudaStream_t st);
+int bise_bilinear_argmax(const float* in, int pitch, int h, int w, int C, unsigned char* cls, unsigned char* mask, int N, int H, int W,
+                         cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

@@ -1940,6 +1940,247 @@ static int rf_forward(cfb_retinaface* n, const float* x, const unsigned char* im
 }  // namespace cfb
 
 // =========================================================================================================
+// BiSeNet(num_class): the light face parser of the paste-back step (facelib's default parser)
+//   /root/reference/facelib/parsing/bisenet.py:104-140 (BiSeNet, ContextPath, ARM, FFM), resnet.py (ResNet18).
+// Eval-mode BatchNorm is folded into every conv at prepare (eps 1e-5).  H and W are multiples of 32, so every nearest resize of
+// the context path is an exact x2 or a broadcast of the 1 x 1 global average.  Engines per conv form:
+//   stem (7x7 s2 + bn1 + ReLU + max-pool)      SIMT (detection.cu, RetinaFace's), fp32 or uint8 BGR faces (normalisation fused)
+//   3x3 stride 1 (BasicBlock convs, ARM and    generalised halo engine: ReLU epilogue, residual + ReLU epilogue
+//     head ConvBNReLU)
+//   conv_head32 / conv_head16 on nearest x2   generalised halo engine, up form (four parity convs on the low-resolution map)
+//   3x3 stride 2, 1x1 downsample, FFM convblk, per-tap engine (conv_out zero-padded to 64 output channels)
+//     conv_out 1x1
+//   avg pool, attention vectors, feat * att + add, bilinear (+ argmax)    SIMT (bisenet.cu)
+// FFM's torch.cat([feat8, feat_cp8]) is one 256-channel buffer: conv_head16 writes channels [128, 256), feat8 is copied to
+// [0, 128) (layer3 reads feat8 dense on the per-tap engine, which has no input pitch), and conv_out16 reads [128, 256) in place.
+// =========================================================================================================
+struct cfb_bisenet : cfb::NetCore {
+  cfb_bisenet() : NetCore("BiSeNet", "bisenet") {}
+  int num_class = 19;
+  std::vector<cfb::GenConv> res;          // ResNet18 layer1..4: conv1, conv2[, downsample] per BasicBlock
+  cfb::GenConv arm[2], head32, head16, convblk, outc[3], outp[3];   // arm16, arm32; conv_out / 16 / 32: ConvBNReLU, conv_out
+  float *stem_w = nullptr, *stem_b = nullptr;
+  float *att_w[2] = {nullptr, nullptr}, *att_b[2] = {nullptr, nullptr};   // arm16 / arm32 conv_atten + bn_atten [128][128]
+  float *avg_w = nullptr, *avg_b = nullptr;                             // conv_avg + bn [128][512]
+  float *ffm_w1 = nullptr, *ffm_w2 = nullptr;                           // ffm.conv1 [64][256], ffm.conv2 [256][64]
+  std::vector<cfb::GenConv*> all() {
+    std::vector<cfb::GenConv*> v;
+    for (cfb::GenConv& c : res) v.push_back(&c);
+    for (cfb::GenConv* c : {&arm[0], &arm[1], &head32, &head16, &convblk, &outc[0], &outc[1], &outc[2], &outp[0], &outp[1], &outp[2]})
+      v.push_back(c);
+    return v;
+  }
+};
+namespace cfb {
+
+static void bs_build(cfb_bisenet* n) {
+  auto mk = [](const std::string& p, const std::string& bn, int cin, int cout, int k, int stride) {
+    GenConv c = plan_conv(p + "weight", cin, cout, k, stride);
+    c.bn = bn;
+    return c;
+  };
+  n->res.clear();
+  int cin = 64;
+  for (int l = 0; l < 4; ++l) {
+    const int cout = 64 << l;
+    for (int b = 0; b < 2; ++b) {
+      const std::string p = "cp.resnet.layer" + std::to_string(l + 1) + "." + std::to_string(b) + ".";
+      const int s = (b == 0 && l > 0) ? 2 : 1;
+      n->res.push_back(mk(p + "conv1.", p + "bn1.", cin, cout, 3, s));
+      n->res.push_back(mk(p + "conv2.", p + "bn2.", cout, cout, 3, 1));
+      if (cin != cout) n->res.push_back(mk(p + "downsample.0.", p + "downsample.1.", cin, cout, 1, s));
+      cin = cout;
+    }
+  }
+  n->arm[0] = mk("cp.arm16.conv.conv.", "cp.arm16.conv.bn.", 256, 128, 3, 1);
+  n->arm[1] = mk("cp.arm32.conv.conv.", "cp.arm32.conv.bn.", 512, 128, 3, 1);
+  n->head32 = mk("cp.conv_head32.conv.", "cp.conv_head32.bn.", 128, 128, 3, 1);
+  n->head16 = mk("cp.conv_head16.conv.", "cp.conv_head16.bn.", 128, 128, 3, 1);
+  n->head32.up = n->head16.up = true;
+  n->convblk = mk("ffm.convblk.conv.", "ffm.convblk.bn.", 256, 256, 1, 1);
+  const char* heads[3] = {"conv_out.", "conv_out16.", "conv_out32."};
+  const int hin[3] = {256, 128, 128}, mid[3] = {256, 64, 64};
+  for (int k = 0; k < 3; ++k) {
+    const std::string p = heads[k];
+    n->outc[k] = mk(p + "conv.conv.", p + "conv.bn.", hin[k], mid[k], 3, 1);
+    n->outp[k] = mk(p + "conv_out.", "", mid[k], n->num_class, 1, 1);
+  }
+}
+
+static int bs_prepare(cfb_bisenet* n, cudaStream_t st) {
+  CFB_CHECK(n->begin_prepare(st));
+  bs_build(n);
+  SlabPlan plan;
+  for (const GenConv* c : n->all()) plan.add(*c);
+  const size_t extra = align256((size_t)64 * 147 * 4) + align256(256) + 2 * (align256((size_t)128 * 128 * 4) + align256(128 * 4)) +
+                       align256((size_t)128 * 512 * 4) + align256(128 * 4) + 2 * align256((size_t)64 * 256 * 4);
+  CFB_CHECK(n->reserve_slab(plan.bytes() + extra));
+  WeightPrep wp(*n, plan, st);
+  for (GenConv* c : n->all()) {
+    if (c->bn.empty()) {       // conv_out: no BatchNorm, no bias
+      const float* w = n->param(c->name, (int64_t)c->cout * c->cin);
+      if (!w) return 1;
+      CFB_CHECK(wp.conv(*c, w, nullptr));
+    } else {
+      CFB_CHECK(wp.fold(c->name, c->bn, c->cout, c->cin * c->k * c->k));
+      CFB_CHECK(wp.conv(*c, wp.fold_w, wp.fold_b));
+    }
+  }
+  // a folded weight [cout][per_out] + bias kept in the slab
+  auto keep = [&](const std::string& w, const std::string& bn, int cout, int per_out, float*& wd, float*& bd) -> int {
+    CFB_CHECK(wp.fold(w, bn, cout, per_out));
+    wd = (float*)wp.take((size_t)cout * per_out * 4); bd = (float*)wp.take((size_t)std::max(cout, 64) * 4);
+    CFB_CUDA(cudaMemcpyAsync(wd, wp.fold_w, (size_t)cout * per_out * 4, cudaMemcpyDeviceToDevice, st));
+    CFB_CUDA(cudaMemcpyAsync(bd, wp.fold_b, (size_t)cout * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  };
+  CFB_CHECK(keep("cp.resnet.conv1.weight", "cp.resnet.bn1.", 64, 147, n->stem_w, n->stem_b));
+  CFB_CHECK(keep("cp.arm16.conv_atten.weight", "cp.arm16.bn_atten.", 128, 128, n->att_w[0], n->att_b[0]));
+  CFB_CHECK(keep("cp.arm32.conv_atten.weight", "cp.arm32.bn_atten.", 128, 128, n->att_w[1], n->att_b[1]));
+  CFB_CHECK(keep("cp.conv_avg.conv.weight", "cp.conv_avg.bn.", 128, 512, n->avg_w, n->avg_b));
+  for (int k = 0; k < 2; ++k) {
+    const float* w = n->param(k ? "ffm.conv2.weight" : "ffm.conv1.weight", 64 * 256);
+    if (!w) return 1;
+    float*& wd = k ? n->ffm_w2 : n->ffm_w1;
+    wd = (float*)wp.take((size_t)64 * 256 * 4);
+    CFB_CUDA(cudaMemcpyAsync(wd, w, (size_t)64 * 256 * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  CFB_CUDA(cudaStreamSynchronize(st));
+  n->prepared = true;
+  return 0;
+}
+
+// The uint8 ends of cfb_bisenet_masks_u8: the stem reads the faces, and the upsampling of `out` is fused with the argmax;
+// conv_out16 / conv_out32 are not run (the caller keeps `out` only, face_restoration_helper.py:462).
+struct BsU8Io { const unsigned char* faces; unsigned char* cls; unsigned char* mask; };
+
+static int bs_forward(cfb_bisenet* n, const float* x, float* const out[3], int N, int H, int W, void* ws, int64_t ws_bytes,
+                      cudaStream_t st, bool dry, const BsU8Io* u8 = nullptr) {
+  CFB_CHECK(n->begin_forward(dry));
+  CFB_REQUIRE(N >= 0 && H >= 32 && W >= 32 && H % 32 == 0 && W % 32 == 0, "BiSeNet: H and W must be positive multiples of 32");
+  if (N == 0) return 0;
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  // one conv of the plan: 3x3 stride 1 on the generalised engine (the up form for the heads of the context path), everything
+  // else on the per-tap engine.  h, w: the input resolution.
+  auto conv = [&](const GenConv& c, const float* in, int in_pitch, int h, int w, float* o, int out_pitch, int out_c0, int act,
+                  const float* resid) -> int {
+    if (c.gen) {
+      GenLaunch g{&c, in, in_pitch, h, w, N, o, out_pitch, out_c0, act};
+      g.res = resid; g.res_pitch = c.cout;
+      return dry ? 0 : gen_conv(g, n->sm_count, st);
+    }
+    return pertap_conv(*n, pertap_args(in, N, h, w, c.cin_p, c.cout_p, c.k, c.stride, o, out_pitch, out_c0, act, resid), c, dry, st);
+  };
+  auto px = [&](int h, int w) { return (size_t)N * h * w; };
+  const int H2 = H / 2, W2 = W / 2;
+  int h = H / 4, w = W / 4;
+  float *s0 = nullptr, *cur = nullptr;
+  CFB_CHECK(n->alloc(&s0, px(H2, W2) * 64));
+  if (!dry) CFB_CHECK(rf_stem(x, u8 ? u8->faces : nullptr, n->stem_w, n->stem_b, s0, N, H, W, st, true));
+  CFB_CHECK(n->alloc(&cur, px(h, w) * 64));
+  if (!dry) CFB_CHECK(rf_maxpool(s0, cur, N, H2, W2, st));
+  ar.release(s0);
+  // ResNet18: relu(shortcut + bn2(conv2(relu(bn1(conv1(x))))))
+  float* F[3] = {nullptr, nullptr, nullptr};      // feat8, feat16, feat32
+  int fh[3] = {0, 0, 0}, fw[3] = {0, 0, 0};
+  size_t ci = 0;
+  for (int l = 0; l < 4; ++l) {
+    for (int b = 0; b < 2; ++b) {
+      const GenConv& c1 = n->res[ci++];
+      const GenConv& c2 = n->res[ci++];
+      const GenConv* ds = c1.cin != c1.cout ? &n->res[ci++] : nullptr;
+      const int ho = c1.stride == 2 ? h / 2 : h, wo = c1.stride == 2 ? w / 2 : w;
+      float *t1 = nullptr, *sc = cur, *y = nullptr;
+      CFB_CHECK(n->alloc(&t1, px(ho, wo) * c1.cout));
+      CFB_CHECK(conv(c1, cur, c1.cin_p, h, w, t1, c1.cout, 0, OUT_RELU, nullptr));
+      if (ds) {
+        CFB_CHECK(n->alloc(&sc, px(ho, wo) * ds->cout));
+        CFB_CHECK(conv(*ds, cur, ds->cin_p, h, w, sc, ds->cout, 0, OUT_NONE, nullptr));
+      }
+      CFB_CHECK(n->alloc(&y, px(ho, wo) * c2.cout));
+      CFB_CHECK(conv(c2, t1, c2.cin_p, ho, wo, y, c2.cout, 0, OUT_RELU, sc));
+      ar.release(t1);
+      if (sc != cur) ar.release(sc);
+      if (l < 2 || b > 0) ar.release(cur);      // the inputs of layer3.0 / layer4.0 are feat8 / feat16, kept
+      cur = y; h = ho; w = wo;
+    }
+    if (l >= 1) { F[l - 1] = cur; fh[l - 1] = h; fw[l - 1] = w; }
+  }
+  const int h8 = fh[0], w8 = fw[0], h16 = fh[1], w16 = fw[1], h32 = fh[2], w32 = fw[2];
+  // ContextPath: avg = conv_avg(avg_pool(feat32)); feat32_sum = arm32(feat32) + avg_up; feat_cp16 = conv_head32(up(feat32_sum))
+  float *v512 = nullptr, *avg = nullptr, *m = nullptr, *att = nullptr;
+  CFB_CHECK(n->alloc(&v512, (size_t)N * 512));
+  CFB_CHECK(n->alloc(&avg, (size_t)N * 128));
+  CFB_CHECK(n->alloc(&m, (size_t)N * 256));
+  CFB_CHECK(n->alloc(&att, (size_t)N * 256));
+  if (!dry) {
+    CFB_CHECK(bise_mean(F[2], v512, N, h32 * w32, 512, st));
+    CFB_CHECK(bise_attention(BiseAttention{n->avg_w, n->avg_b, 512, 128, 1, nullptr, nullptr, 0, 0}, v512, avg, N, st));
+  }
+  // ARM k (0: arm16, 1: arm32) on its feature map, combined with `add_vec` or `add_t` in place
+  auto arm = [&](int k, const float* in, int hh, int ww, float* a, const float* add_vec, const float* add_t) -> int {
+    CFB_CHECK(conv(n->arm[k], in, n->arm[k].cin_p, hh, ww, a, 128, 0, OUT_RELU, nullptr));
+    if (dry) return 0;
+    CFB_CHECK(bise_mean(a, m, N, hh * ww, 128, st));
+    CFB_CHECK(bise_attention(BiseAttention{n->att_w[k], n->att_b[k], 128, 128, 2, nullptr, nullptr, 0, 0}, m, att, N, st));
+    return bise_scale_add(a, att, add_vec, add_t, a, N, (int64_t)hh * ww, 128, st);
+  };
+  float *a32 = nullptr, *cp16 = nullptr, *a16 = nullptr, *fcat = nullptr;
+  CFB_CHECK(n->alloc(&a32, px(h32, w32) * 128));
+  CFB_CHECK(arm(1, F[2], h32, w32, a32, avg, nullptr));
+  ar.release(F[2]); ar.release(v512); ar.release(avg);
+  CFB_CHECK(n->alloc(&cp16, px(h16, w16) * 128));
+  CFB_CHECK(conv(n->head32, a32, 128, h32, w32, cp16, 128, 0, OUT_RELU, nullptr));
+  ar.release(a32);
+  // feat16_sum = arm16(feat16) + feat32_up; feat_cp8 = conv_head16(up(feat16_sum)) -> fcat[128:256)
+  CFB_CHECK(n->alloc(&a16, px(h16, w16) * 128));
+  CFB_CHECK(arm(0, F[1], h16, w16, a16, nullptr, cp16));
+  ar.release(F[1]);
+  CFB_CHECK(n->alloc(&fcat, px(h8, w8) * 256));
+  CFB_CHECK(conv(n->head16, a16, 128, h16, w16, fcat, 256, 128, OUT_RELU, nullptr));
+  ar.release(a16);
+  if (!dry) CFB_CHECK(yolo_copy(F[0], 128, 0, fcat, 256, 0, N, h8, w8, 128, false, st));
+  ar.release(F[0]);
+  // FFM: feat = convblk(fcat); feat * sigmoid(conv2(relu(conv1(avg_pool(feat))))) + feat
+  float* ff = nullptr;
+  CFB_CHECK(n->alloc(&ff, px(h8, w8) * 256));
+  CFB_CHECK(conv(n->convblk, fcat, 256, h8, w8, ff, 256, 0, OUT_RELU, nullptr));
+  if (!dry) {
+    CFB_CHECK(bise_mean(ff, m, N, h8 * w8, 256, st));
+    CFB_CHECK(bise_attention(BiseAttention{n->ffm_w1, nullptr, 256, 64, 1, n->ffm_w2, nullptr, 256, 2}, m, att, N, st));
+    CFB_CHECK(bise_scale_add(ff, att, nullptr, nullptr, ff, N, (int64_t)h8 * w8, 256, st));
+  }
+  ar.release(m); ar.release(att);
+  // BiSeNetOutput k on `in`: ConvBNReLU 3x3, conv_out 1x1 (64 padded channels), bilinear to H x W
+  auto head = [&](int k, const float* in, int in_pitch, int hh, int ww) -> int {
+    const GenConv &c = n->outc[k], &p = n->outp[k];
+    float *t = nullptr, *lo = nullptr;
+    CFB_CHECK(n->alloc(&t, px(hh, ww) * c.cout));
+    CFB_CHECK(conv(c, in, in_pitch, hh, ww, t, c.cout, 0, OUT_RELU, nullptr));
+    CFB_CHECK(n->alloc(&lo, px(hh, ww) * p.cout_p));
+    CFB_CHECK(conv(p, t, p.cin_p, hh, ww, lo, p.cout_p, 0, OUT_NONE, nullptr));
+    ar.release(t);
+    if (!dry) {
+      if (u8) CFB_CHECK(bise_bilinear_argmax(lo, p.cout_p, hh, ww, n->num_class, u8->cls, u8->mask, N, H, W, st));
+      else CFB_CHECK(bise_bilinear(lo, p.cout_p, hh, ww, n->num_class, out[k], N, H, W, st));
+    }
+    ar.release(lo);
+    return 0;
+  };
+  CFB_CHECK(head(0, ff, 256, h8, w8));
+  ar.release(ff);
+  if (!u8) {
+    CFB_CHECK(head(1, fcat + 128, 256, h8, w8));
+    CFB_CHECK(head(2, cp16, 128, h16, w16));
+  }
+  ar.release(fcat); ar.release(cp16);
+  return 0;
+}
+
+}  // namespace cfb
+
+// =========================================================================================================
 // ResNetArcFace('IRBlock', layers, use_se=False): identity embeddings of faces (scoring a fidelity sweep)
 //   /root/reference/basicsr/archs/arcface_arch.py:56-100 (IRBlock), 171-245 (ResNetArcFace); the gray 128 x 128 input of
 //   basicsr/models/codeformer_model.py:131-135 (gray_resize_for_identity).
@@ -2706,6 +2947,75 @@ int cfb_retinaface_candidates(const float* loc, const float* conf, const float* 
   CFB_REQUIRE(batch == 0 || (loc && conf && landms && rows && counts), "cfb_retinaface_candidates: NULL argument");
   CFB_REQUIRE(h >= 1 && w >= 1 && batch >= 0, "cfb_retinaface_candidates: empty image");
   return cfb::rf_candidates(loc, conf, landms, batch, h, w, conf_threshold, rows, counts, (cudaStream_t)stream);
+  API_END(1)
+}
+
+cfb_bisenet* cfb_bisenet_create(int32_t num_class) {
+  API_BEGIN
+  if (num_class < 1 || num_class > 64) { cfb::set_error("cfb_bisenet_create: built for 1..64 classes"); return nullptr; }
+  cfb_bisenet* n = new cfb_bisenet();
+  n->num_class = num_class;
+  cfb::bs_build(n);
+  return n;
+  API_END(nullptr)
+}
+void cfb_bisenet_destroy(cfb_bisenet* n) { delete n; }
+int cfb_bisenet_set_param(cfb_bisenet* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_bisenet_set_param: NULL argument");
+  return n->set_param(name, dev_ptr, numel);
+  API_END(1)
+}
+int cfb_bisenet_prepare(cfb_bisenet* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_bisenet_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::bs_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_bisenet_workspace_bytes(cfb_bisenet* n, int32_t batch, int32_t h, int32_t w) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_bisenet_workspace_bytes: NULL net"); return -1; }
+  float* const outs[3] = {(float*)0x1000, (float*)0x1000, (float*)0x1000};
+  return n->dry_run([&] { return cfb::bs_forward(n, (const float*)0x1000, outs, batch, h, w, nullptr, 0, nullptr, true); });
+  API_END(-1)
+}
+int cfb_bisenet_forward(cfb_bisenet* n, const float* x_nchw, float* out, float* out16, float* out32, int32_t batch, int32_t h, int32_t w,
+                        void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (x_nchw && out && out16 && out32 && workspace)), "cfb_bisenet_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  float* const outs[3] = {out, out16, out32};
+  return cfb::bs_forward(n, x_nchw, outs, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_bisenet_masks_u8(cfb_bisenet* n, const uint8_t* faces_bgr, uint8_t* classes, uint8_t* mask, int32_t batch, int32_t h, int32_t w,
+                         void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (classes || mask) && (batch == 0 || (faces_bgr && workspace)), "cfb_bisenet_masks_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  float* const outs[3] = {nullptr, nullptr, nullptr};
+  const cfb::BsU8Io io{faces_bgr, classes, mask};
+  return cfb::bs_forward(n, nullptr, outs, batch, h, w, workspace, workspace_bytes, (cudaStream_t)stream, false, &io);
+  API_END(1)
+}
+int cfb_debug_bisenet_bilinear(const float* in_nhwc, int32_t pitch, int32_t n, int32_t h, int32_t w, int32_t c, float* out_nchw,
+                               int32_t out_h, int32_t out_w, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(in_nhwc && out_nchw, "cfb_debug_bisenet_bilinear: NULL argument");
+  CFB_REQUIRE(n >= 0 && h >= 1 && w >= 1 && c >= 1 && c <= pitch && out_h >= 1 && out_w >= 1, "cfb_debug_bisenet_bilinear: bad shape");
+  return cfb::bise_bilinear(in_nhwc, pitch, h, w, c, out_nchw, n, out_h, out_w, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_debug_bisenet_attention(const float* feat_nhwc, int32_t n, int32_t hw, int32_t c, const float* w1, const float* b1, int32_t c1,
+                                int32_t act1, const float* w2, const float* b2, int32_t c2, int32_t act2, float* mean, float* att,
+                                void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(feat_nhwc && w1 && mean && att, "cfb_debug_bisenet_attention: NULL argument");
+  CFB_REQUIRE(n >= 0 && hw >= 1 && c >= 1 && c1 >= 1 && (!w2 || c2 >= 1), "cfb_debug_bisenet_attention: bad shape");
+  const cudaStream_t st = (cudaStream_t)stream;
+  CFB_CHECK(cfb::bise_mean(feat_nhwc, mean, n, hw, c, st));
+  return cfb::bise_attention(cfb::BiseAttention{w1, b1, c, c1, act1, w2, b2, c2, act2}, mean, att, n, st);
   API_END(1)
 }
 

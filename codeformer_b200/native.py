@@ -1,5 +1,5 @@
 """What the modules whose forward is one libcfb200 network handle (``cfb_<api>_create`` / ``_set_param`` / ``_prepare`` /
-``_destroy``) share: CodeFormer / VQAutoEncoder, RRDBNet, ParseNet, RetinaFace and YOLOv5lFace.  The module owns the
+``_destroy``) share: CodeFormer / VQAutoEncoder, RRDBNet, ParseNet, BiSeNet, RetinaFace, YOLOv5lFace and ResNetArcFace.  The module owns the
 parameters under the reference's state-dict names; the handle holds device copies prepared from them, rebuilt whenever a
 parameter was loaded, moved or modified."""
 import ctypes

@@ -177,11 +177,16 @@ def face_parse_mask(out_mask):
 
 
 def init_parsing_model(model_name='parsenet', half=False, device='cuda', model_path=None):
-    """``facelib.parsing.init_parsing_model('parsenet')`` (facelib/parsing/__init__.py:8-23) without the download: pass the
-    checkpoint path (``parsing_parsenet.pth``) or load the state dict yourself."""
-    if model_name != 'parsenet':
-        raise NotImplementedError(f'{model_name} is not built (SURVEY.md section 8 f3 names ParseNet)')
-    model = ParseNet(in_size=512, out_size=512, parsing_ch=19)
+    """``facelib.parsing.init_parsing_model('parsenet' | 'bisenet')`` (facelib/parsing/__init__.py:8-23) without the download:
+    pass the checkpoint path (``parsing_parsenet.pth`` / ``parsing_bisenet.pth``, loaded strictly as is) or load the state
+    dict yourself."""
+    if model_name == 'parsenet':
+        model = ParseNet(in_size=512, out_size=512, parsing_ch=19)
+    elif model_name == 'bisenet':
+        from .bisenet import BiSeNet
+        model = BiSeNet(num_class=19)
+    else:
+        raise NotImplementedError(f'{model_name} is not built (codeformer_b200 builds parsenet and bisenet)')
     if model_path is not None:
         model.load_state_dict(torch.load(model_path, map_location='cpu'), strict=True)
     return model.eval().to(device)

@@ -399,6 +399,31 @@ int       cfb_retinaface_forward_u8(cfb_retinaface* net, const uint8_t* img_bgr_
 int       cfb_retinaface_candidates(const float* loc, const float* conf, const float* landms, int32_t batch, int32_t h, int32_t w,
                                     float conf_threshold, float* rows, int32_t* counts, void* stream);
 
+/* ---- BiSeNet(num_class) face parser (facelib/parsing/bisenet.py; bisenet.cu + the conv engine) ----
+ * Parameters by the reference's state-dict names (BatchNorm folded at prepare), 1 <= num_class <= 64.  h and w must be
+ * multiples of 32.  forward: x fp32 NCHW [batch,3,h,w] -> out, out16, out32, each fp32 NCHW [batch,num_class,h,w].
+ * masks_u8: uint8 HWC BGR faces [batch,h,w,3] (the normalisation of cfb_u8_to_input fused) -> classes = out.argmax(dim=1) and
+ * the 0/255 MASK_COLORMAP mask, uint8 [batch,h,w] each (either may be NULL), byte-equal to cfb_u8_to_input + forward +
+ * cfb_parse_argmax; out16 / out32 are not computed.  Workspace (both): cfb_bisenet_workspace_bytes.
+ * cfb_debug_bisenet_bilinear: NHWC [n,h,w,pitch] (first c channels) -> NCHW [n,c,out_h,out_w], bilinear, align_corners=True.
+ * cfb_debug_bisenet_attention: mean [n,c] of NHWC feat [n,hw,c], att = act2(w2 act1(w1 mean + b1) + b2) (w2 NULL: one layer),
+ * weights [cout][cin], act 0 none / 1 ReLU / 2 sigmoid, one CTA per image. */
+typedef struct cfb_bisenet cfb_bisenet;
+cfb_bisenet* cfb_bisenet_create(int32_t num_class);
+void         cfb_bisenet_destroy(cfb_bisenet* net);
+int          cfb_bisenet_set_param(cfb_bisenet* net, const char* name, const float* dev_ptr, int64_t numel);
+int          cfb_bisenet_prepare(cfb_bisenet* net, void* stream);
+int64_t      cfb_bisenet_workspace_bytes(cfb_bisenet* net, int32_t batch, int32_t h, int32_t w);
+int          cfb_bisenet_forward(cfb_bisenet* net, const float* x_nchw, float* out, float* out16, float* out32, int32_t batch,
+                                 int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int          cfb_bisenet_masks_u8(cfb_bisenet* net, const uint8_t* faces_bgr, uint8_t* classes, uint8_t* mask, int32_t batch,
+                                  int32_t h, int32_t w, void* workspace, int64_t workspace_bytes, void* stream);
+int          cfb_debug_bisenet_bilinear(const float* in_nhwc, int32_t pitch, int32_t n, int32_t h, int32_t w, int32_t c,
+                                        float* out_nchw, int32_t out_h, int32_t out_w, void* stream);
+int          cfb_debug_bisenet_attention(const float* feat_nhwc, int32_t n, int32_t hw, int32_t c, const float* w1, const float* b1,
+                                         int32_t c1, int32_t act1, const float* w2, const float* b2, int32_t c2, int32_t act2,
+                                         float* mean, float* att, void* stream);
+
 /* ---- ResNetArcFace('IRBlock', layers, use_se=False) identity embeddings (basicsr/archs/arcface_arch.py; arcface.cu + the
  * conv engine) ----
  * create: the four block counts of `layers` (each >= 1).  Parameters by the reference's state-dict names (BatchNorm folded at

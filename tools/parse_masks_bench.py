@@ -6,7 +6,13 @@ faces), three paths at batch 8 and 32:
 Device events, 3 warm-ups, median of --iters calls.  (a) and (b) must be byte-equal; the class-flip share of (c) against (b)
 is reported.
 
-    python tools/parse_masks_bench.py [--iters 20] [--batches 8,32]
+--model bisenet compares the two parsers in one process, masks per second at each batch:
+  ParseNet.masks_u8 in fp32 and fp16; BiSeNet(19).masks_u8 (seeded weights, oracle/bisenet_oracle.py); and the reference
+  BiSeNet's computation on cuDNN -- oracle.bisenet_oracle.forward (the reference's ops, bit-identical to the reference class
+  on the CPU) on CUDA tensors, with cudnn.allow_tf32 at its default (True) and False -- followed by face_parse_mask.  BiSeNet's
+  masks_u8 must be byte-equal to cfb_u8_to_input + BiSeNet.forward + face_parse_mask.
+
+    python tools/parse_masks_bench.py [--iters 20] [--batches 8,32] [--model parsenet|bisenet]
 """
 import argparse
 import os
@@ -44,13 +50,54 @@ def chain(net, faces):
     return PB.parse_masks(faces, lambda x: net(x))
 
 
+def bisenet_compare(parsenet, base, batches, iters, dev):
+    from oracle import bisenet_oracle as BO
+    sd = BO.random_bisenet_state_dict(1)
+    bise = cb.BiSeNet(num_class=19)
+    bise.load_state_dict(sd, strict=True)
+    bise = bise.to(dev).eval()
+    sd_dev = {k: v.to(dev) for k, v in sd.items()}
+
+    def cudnn(faces, tf32):
+        torch.backends.cudnn.allow_tf32 = tf32
+        return PB.parse_masks(faces, lambda x: BO.forward(sd_dev, x))
+
+    tf32_default = torch.backends.cudnn.allow_tf32
+    for b in batches:
+        faces = torch.from_numpy(np.ascontiguousarray(np.stack([np.roll(base[i % 4], 37 * (i // 4), axis=1)
+                                                                for i in range(b)]))).to(dev)
+        mask = bise.masks_u8(faces)[1]
+        assert torch.equal(mask, PB.parse_masks(faces, lambda x: bise(x))), 'BiSeNet masks_u8 differs from the unfused chain'
+        flip = float((cudnn(faces, False) != mask).float().mean()) * 100
+        t = {}
+        parsenet.set_precision('fp32')
+        t['ParseNet masks_u8 fp32'] = events(lambda: parsenet.masks_u8(faces), iters)
+        parsenet.set_precision('fp16')
+        t['ParseNet masks_u8 fp16'] = events(lambda: parsenet.masks_u8(faces), iters)
+        parsenet.set_precision('fp32')
+        t['BiSeNet masks_u8'] = events(lambda: bise.masks_u8(faces), iters)
+        t['BiSeNet reference on cuDNN (tf32 default)'] = events(lambda: cudnn(faces, tf32_default), iters)
+        t['BiSeNet reference on cuDNN (allow_tf32=False)'] = events(lambda: cudnn(faces, False), iters)
+        torch.backends.cudnn.allow_tf32 = tf32_default
+        print(f'B={b}: ' + ' | '.join(f'{k} {v:.2f} ms = {b * 1e3 / v:.0f} masks/s' for k, v in t.items()) +
+              f' | BiSeNet masks_u8 == unfused chain byte for byte; {flip:.3f} % of mask pixels differ from cuDNN fp32', flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--batches', default='8,32')
+    ap.add_argument('--model', choices=('parsenet', 'bisenet'), default='parsenet')
     args = ap.parse_args()
     torch.set_grad_enabled(False)
     dev = 'cuda:0'
+    if args.model == 'bisenet':
+        print(card(), '| ParseNet(512, 512, 19) and BiSeNet(19), seeded weights, 512x512 faces')
+        net = P.ParseNet(in_size=512, out_size=512, parsing_ch=19)
+        net.load_state_dict(P.random_parsenet_state_dict(P.parsenet_spec(512, 512, 32, 64, 19, 10, (32, 256)), 41), strict=True)
+        base = np.load(os.path.join(GOLDEN, 'faces.npz'))['faces'][..., ::-1]
+        bisenet_compare(net.to(dev).eval(), base, [int(v) for v in args.batches.split(',')], args.iters, dev)
+        return
     print(card(), '| ParseNet(512, 512, 19), seeded weights, 512x512 faces')
     net = P.ParseNet(in_size=512, out_size=512, parsing_ch=19)
     net.load_state_dict(P.random_parsenet_state_dict(P.parsenet_spec(512, 512, 32, 64, 19, 10, (32, 256)), 41), strict=True)

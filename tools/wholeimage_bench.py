@@ -5,7 +5,10 @@ path (resize, detect, warp, CodeFormer, parse, paste).
 Weights are seeded random (the numbers are about time, not quality).  The detector is RetinaFace-ResNet50 run in full;
 only its candidate rows are replaced by k fixed, well separated faces per frame so that every frame holds exactly k faces.
 
-    python tools/wholeimage_bench.py [--frames 8] [--reps 3] [--json out.json]
+--parser bisenet runs the paste-back's parse step with BiSeNet(19) (seeded weights, oracle/bisenet_oracle.py) instead of
+ParseNet, in both paths.
+
+    python tools/wholeimage_bench.py [--frames 8] [--reps 3] [--json out.json] [--parser parsenet|bisenet]
 """
 import argparse
 import json
@@ -39,7 +42,7 @@ class FixedFaces(cb.RetinaFace):
         return [r.to(loc.device) for _ in range(loc.shape[0])]
 
 
-def nets(k):
+def nets(k, parser_name='parsenet'):
     from codeformer_b200 import spec as S
     from codeformer_b200.detection import random_retinaface_state_dict
     from codeformer_b200.parsing import parsenet_spec, random_parsenet_state_dict
@@ -49,8 +52,12 @@ def nets(k):
     det = FixedFaces().cuda()
     det.load_state_dict(random_retinaface_state_dict(1), strict=True)
     det.k = k
-    parser = cb.init_parsing_model(device='cpu')
-    parser.load_state_dict(random_parsenet_state_dict(parsenet_spec(512, 512, 32, 64, 19, 10, (32, 256)), 41), strict=False)
+    parser = cb.init_parsing_model(parser_name, device='cpu')
+    if parser_name == 'bisenet':
+        from oracle.bisenet_oracle import random_bisenet_state_dict
+        parser.load_state_dict(random_bisenet_state_dict(1), strict=True)
+    else:
+        parser.load_state_dict(random_parsenet_state_dict(parsenet_spec(512, 512, 32, 64, 19, 10, (32, 256)), 41), strict=False)
     return net, det.eval(), parser.cuda().eval()
 
 
@@ -141,22 +148,24 @@ def main():
     ap.add_argument('--frames', type=int, default=8)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--json', default=None)
+    ap.add_argument('--parser', choices=('parsenet', 'bisenet'), default='parsenet')
     a = ap.parse_args()
     from oracle.pasteback_oracle import synthetic_background
     rows = []
+    print(f'parser: {a.parser}')
     print(f'{"frame":>10} {"faces":>5} {"loop img/s":>10} {"batch img/s":>11} {"loop face/s":>11} {"batch face/s":>12} '
           f'{"speed-up":>8}  stage shares (batched)', flush=True)
     for h, w in [(1080, 1920), (640, 853)]:
         imgs = [synthetic_background(h, w, s) for s in range(a.frames)]
         for k in (1, 3):
-            net, det, parser = nets(k)
+            net, det, parser = nets(k, a.parser)
             t_loop = timed(lambda: per_image_loop(imgs, net, det, parser), a.reps)
             t_batch = timed(lambda: cb.restore_images(imgs, net, det, parser=parser), a.reps)
             st = stages(imgs, net, det, parser)
             tot = sum(st.values())
             shares = {n: round(v / tot, 3) for n, v in st.items()}
             n = a.frames
-            row = dict(frame=f'{h}x{w}', faces_per_frame=k, frames=n, loop_s=t_loop, batch_s=t_batch,
+            row = dict(parser=a.parser, frame=f'{h}x{w}', faces_per_frame=k, frames=n, loop_s=t_loop, batch_s=t_batch,
                        loop_img_s=n / t_loop, batch_img_s=n / t_batch, loop_face_s=n * k / t_loop,
                        batch_face_s=n * k / t_batch, speedup=t_loop / t_batch, stage_shares=shares)
             rows.append(row)
