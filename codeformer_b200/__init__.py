@@ -17,6 +17,7 @@ from .pasteback import resize_area, warp_faces_multi, paste_faces_multi   # noqa
 from .pasteback import resize_lanczos4, gray_adain_faces, add_restored_face   # noqa: F401
 from .wholeimage import restore_images, restore_images_sweep, restore_aligned   # noqa: F401
 from .arcface import ResNetArcFace, identity_similarity   # noqa: F401
+from .metrics import calculate_psnr, calculate_ssim, psnr_ssim   # noqa: F401
 
 
 def check_async_status():
@@ -31,4 +32,4 @@ __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQua
            'warp_faces', 'paste_faces', 'align_warp_face', 'paste_faces_to_input_image', 'RetinaFace', 'init_detection_model',
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
-           'ResNetArcFace', 'identity_similarity', 'check_async_status']
+           'ResNetArcFace', 'identity_similarity', 'calculate_psnr', 'calculate_ssim', 'psnr_ssim', 'check_async_status']

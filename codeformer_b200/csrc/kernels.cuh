@@ -300,6 +300,17 @@ int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* ma
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);
 
+// Restoration metrics (metrics.cu; cfb_psnr_ssim): pair p compares a[p] with b[p / k], HWC images [h, w, c] of element type
+// `kind` (ImgKind); psnr_mode 0 none, 1 PSNR in dB, 2 the MSE; ssim (optional) the mean SSIM.  Outputs: device double [pairs].
+struct MetricArgs {
+  const void* a; const void* b; int kind;
+  int pairs, k, h, w, c, crop;
+  bool y;                           // test_y_channel
+  int psnr_mode; double* psnr; double* ssim;
+};
+size_t metrics_workspace_bytes(int pairs, int h, int w, int c, int crop, bool y);
+int psnr_ssim(const MetricArgs& a, void* ws, int64_t ws_bytes, cudaStream_t st);
+
 // weight re-layout: OIHW -> [taps][Cin][Cout]
 int relayout_oihw_to_tck(const float* oihw, float* out, int Cout, int Cin, int k, cudaStream_t st);
 

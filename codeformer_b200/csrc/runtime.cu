@@ -3161,6 +3161,31 @@ int cfb_yolov5face_candidates(const float* pred, int32_t batch, int32_t h, int32
   API_END(1)
 }
 
+int64_t cfb_psnr_ssim_workspace_bytes(int32_t pairs, int32_t h, int32_t w, int32_t c, int32_t crop_border, int32_t y_channel) {
+  if (pairs < 0 || h <= 0 || w <= 0 || c <= 0 || crop_border < 0) {
+    cfb::set_error("cfb_psnr_ssim_workspace_bytes: bad size");
+    return -1;
+  }
+  return (int64_t)cfb::metrics_workspace_bytes(pairs, h, w, c, crop_border, y_channel != 0);
+}
+int cfb_psnr_ssim(const void* a, const void* b, int32_t dtype, int32_t pairs, int32_t k, int32_t h, int32_t w, int32_t c,
+                  int32_t crop_border, int32_t y_channel, int32_t want_psnr, int32_t want_ssim, double* psnr_out, double* ssim_out,
+                  void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(dtype >= CFB_IMG_U8 && dtype <= CFB_IMG_F64, "cfb_psnr_ssim: dtype must be one of CFB_IMG_*");
+  CFB_REQUIRE(pairs >= 0 && pairs <= 65535 && k >= 1 && pairs % k == 0, "cfb_psnr_ssim: bad pair count");
+  CFB_REQUIRE(h > 0 && w > 0 && c > 0 && crop_border >= 0, "cfb_psnr_ssim: bad size");
+  CFB_REQUIRE(want_psnr >= 0 && want_psnr <= 2, "cfb_psnr_ssim: want_psnr must be 0, 1 or 2");
+  CFB_REQUIRE(!want_psnr || psnr_out, "cfb_psnr_ssim: NULL psnr_out");
+  CFB_REQUIRE(!want_ssim || ssim_out, "cfb_psnr_ssim: NULL ssim_out");
+  if (pairs == 0 || (!want_psnr && !want_ssim)) return 0;
+  CFB_REQUIRE(a && b, "cfb_psnr_ssim: NULL image");
+  const cfb::MetricArgs m{a, b, dtype, pairs, k, h, w, c, crop_border, y_channel != 0, want_psnr, want_psnr ? psnr_out : nullptr,
+                          want_ssim ? ssim_out : nullptr};
+  return cfb::psnr_ssim(m, workspace, workspace_bytes, (cudaStream_t)stream);
+  API_END(1)
+}
+
 int cfb_check_async_status(void) {
   API_BEGIN
   return cfb::async_status_check("cfb_check_async_status");

@@ -474,6 +474,24 @@ int             cfb_yolov5face_forward_u8(cfb_yolov5face* net, const uint8_t* im
 int             cfb_yolov5face_candidates(const float* pred, int32_t batch, int32_t h, int32_t w, float conf_threshold, float* rows,
                                           int32_t* counts, void* stream);
 
+/* ---- Restoration metrics: basicsr's calculate_psnr / calculate_ssim (basicsr/metrics/psnr_ssim.py) on the device ----
+ * Pair p compares a[p] with b[p / k] (a holds pairs images, b pairs / k: a sweep's K candidates per face against one ground
+ * truth each), HWC images [h, w, c] of element type dtype (CFB_IMG_U8 / _U16 / _F32 / _F64) read in place.  crop_border pixels
+ * are dropped from each edge.  y_channel: to_y_channel (metric_util.py:32-45) at load -- v = float32(x) / 255; for c == 3
+ * Y = (v0 * 24.966 + v1 * 128.553) + v2 * 65.481 + 16 in float64 (channel 0 blue), / 255 rounded to float32; then * 255 in float32.
+ * want_psnr: 0 none, 1 psnr_out[p] = 20 log10(255 / sqrt(mse)) (inf for mse == 0; peak 255 for every dtype), 2 psnr_out[p] =
+ *   mse, the mean of (a - b)^2 -- summed exactly in int64 for integer images without y_channel (so it equals numpy's mean), in
+ *   float64 otherwise, of float32 squares on the Y path.
+ * want_ssim: ssim_out[p] = the mean over channels of the mean SSIM map (Gaussian window 11, sigma 1.5, valid region only,
+ *   C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2), filtered in float64 (the 11 horizontal taps, then the 11 vertical ones).
+ * psnr_out / ssim_out: device double [pairs].  Needs at least one pixel (PSNR) or 11 x 11 (SSIM) after the crop;
+ * pairs <= 65535.  Every sum has a fixed order that depends on the image size only: the results are the same on every run and
+ * whatever the batch.  NaN or inf values give NaN / inf results.  workspace: cfb_psnr_ssim_workspace_bytes bytes. */
+int64_t cfb_psnr_ssim_workspace_bytes(int32_t pairs, int32_t h, int32_t w, int32_t c, int32_t crop_border, int32_t y_channel);
+int     cfb_psnr_ssim(const void* a, const void* b, int32_t dtype, int32_t pairs, int32_t k, int32_t h, int32_t w, int32_t c,
+                      int32_t crop_border, int32_t y_channel, int32_t want_psnr, int32_t want_ssim, double* psnr_out,
+                      double* ssim_out, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Asynchronous failures.  Kernels never trap and never leave a sticky CUDA error behind (the reference's callers catch
  * RuntimeError and fall back to the input face, inference_codeformer.py:209-211; web-demos/hugging_face/app.py:176): a
  * barrier time-out of the tensor-core pipeline or an activation outside the fp16 operand range (|x| > 65504) sets a bit
