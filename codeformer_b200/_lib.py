@@ -151,6 +151,17 @@ SIGNATURES = {
     'cfb_yolov5face_forward_u8': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32,
                                           _P, c_int64, _P]),
     'cfb_yolov5face_candidates': (c_int, [_P, c_int32, c_int32, c_int32, c_float, _P, _P, _P]),
+    'cfb_lpips_create': (c_void_p, []),
+    'cfb_lpips_destroy': (None, [_P]),
+    'cfb_lpips_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
+    'cfb_lpips_prepare': (c_int, [_P, _P]),
+    'cfb_lpips_workspace_bytes': (c_int64, [_P, c_int32, c_int32, c_int32, c_int32]),
+    'cfb_lpips_forward': (c_int, [_P, _P, _P] + [c_int32] * 5 + [_P, _P, _P, c_int64, _P]),
+    'cfb_lpips_forward_u8': (c_int, [_P, _P, _P] + [c_int32] * 5 + [_P, _P, _P, c_int64, _P]),
+    'cfb_lpips_u8_table': (c_int, [c_int32, _P, _P, _P]),
+    'cfb_debug_lpips_stem': (c_int, [_P, _P, _P, c_int32, c_int32, _P, c_int32, c_int32, c_int32, c_int32, _P]),
+    'cfb_debug_lpips_head_workspace_bytes': (c_int64, [c_int32] * 4),
+    'cfb_debug_lpips_head': (c_int, [_P, _P, _P, _P] + [c_int32] * 5 + [_P, c_int64, _P]),
     'cfb_psnr_ssim_workspace_bytes': (c_int64, [c_int32] * 6),
     'cfb_psnr_ssim': (c_int, [_P, _P] + [c_int32] * 10 + [_P, _P, _P, c_int64, _P]),
     'cfb_check_async_status': (c_int, []),

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.environ.get('CFB_BUILD_OUT') or os.path.join(HERE, 'libcfb200.so')
-SOURCES = ['simt_kernels.cu', 'conv_tc.cu', 'runtime.cu', 'pasteback.cu', 'detection.cu', 'yolo.cu', 'arcface.cu', 'bisenet.cu', 'metrics.cu']
+SOURCES = ['simt_kernels.cu', 'conv_tc.cu', 'runtime.cu', 'pasteback.cu', 'detection.cu', 'yolo.cu', 'arcface.cu', 'bisenet.cu', 'metrics.cu', 'lpips.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
          '-Wno-deprecated-gpu-targets', '-Xptxas', '-v' if os.environ.get('CFB_PTXAS_V') else '-O3'] + \

@@ -296,6 +296,29 @@ int bise_scale_add(const float* feat, const float* att, const float* add_vec, co
 int bise_bilinear(const float* in, int pitch, int h, int w, int C, float* out, int N, int H, int W, cudaStream_t st);
 int bise_bilinear_argmax(const float* in, int pitch, int h, int w, int C, unsigned char* cls, unsigned char* mask, int N, int H, int W,
                          cudaStream_t st);
+// LPIPS-VGG (lpips.cu): image i of a launch is image i % (1 + G) of group i / (1 + G), 0 the reference, j >= 1 candidate j - 1
+//   stem      conv1_1 + ReLU -> NHWC [M,H,W,64] from fp32 NCHW ref [groups] / cand [groups * G] through the LpipsXform chain, or
+//             from uint8 HWC BGR ref8 / cand8 through `table` ([3][256], RGB channel order) when table is set
+//   head      relu_k [M,H,W,C] -> pooled [M,H/2,W/2,C] (null: none) and partial [groups][G][lpips_head_blocks(H, W)]
+//   finalize  partials of L.n layers -> val [P] (the sum over the layers) and per_layer [P][L.n] (either may be null)
+enum { LPIPS_NORMALIZE = 1, LPIPS_RANGE_NORM = 2, LPIPS_INPUT_NORM = 4 };
+struct LpipsXform {                // applied in the order range_norm, input_norm, normalize, ScalingLayer
+  int flags = 0;
+  float mean[3] = {}, std[3] = {}, shift[3] = {}, scale[3] = {};
+};
+struct LpipsLayers {
+  static constexpr int kMax = 5;
+  int n = 0;
+  const float* part[kMax] = {};
+  int nblk[kMax] = {};
+  int64_t hw[kMax] = {};
+};
+int lpips_stem(const float* ref, const float* cand, const unsigned char* ref8, const unsigned char* cand8, const float* table,
+               const LpipsXform& xf, const float* wt, const float* bias, float* out, int groups, int G, int H, int W, cudaStream_t st);
+int lpips_head_blocks(int H, int W);
+int lpips_head(const float* feat, const float* lin, int groups, int G, int H, int W, int C, float* pooled, float* partial,
+               cudaStream_t st);
+int lpips_finalize(const LpipsLayers& L, int P, float* val, float* per_layer, cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

@@ -2384,6 +2384,182 @@ static int arc_forward(cfb_arcface* n, const float* x, const unsigned char* face
 }  // namespace cfb
 
 // =========================================================================================================
+// LPIPS(net='vgg', version='0.1'): the perceptual distance of restored faces (lpips 0.1; basicsr/losses/losses.py:257-282,
+// LPIPSLoss, the perceptual term of every CodeFormer training config).
+//   ScalingLayer -> torchvision vgg16().features cut after relu1_2, relu2_2, relu3_3, relu4_3, relu5_3 -> per layer k:
+//   f / (|f|_c + 1e-10) of both images, (f0 - f1)^2, lin_k (1x1, C -> 1, no bias), mean over H x W -> val = sum over k.
+// Engines:
+//   conv1_1 (3 -> 64) + ReLU                    SIMT stem (lpips.cu), the input transform fused into its load
+//   the 12 other 3x3 convs + ReLU               generalised halo engine (biases kept; no BatchNorm)
+//   head of relu_k + MaxPool2d(2, 2) into the next slice      one SIMT pass over relu_k (lpips.cu), then a finalize
+// A launch holds `groups` groups of one reference and G candidates; every relu_k is released after its head-and-pool pass, so
+// the workspace peaks at two relu1 maps of the launch's images.
+// =========================================================================================================
+struct cfb_lpips : cfb::NetCore {
+  cfb_lpips() : NetCore("LPIPS", "lpips") {}
+  cfb::GenConv convs[12];                  // conv1_2 .. conv5_3
+  float *stem_w = nullptr, *stem_b = nullptr;
+  float* lin[5] = {};
+  float* tables = nullptr;                 // [LPIPS_U8_CONVENTIONS][3][256] uint8 -> stem input, RGB channel order
+  float shift[3] = {}, scale[3] = {};      // ScalingLayer, read at prepare
+};
+namespace cfb {
+
+// torchvision vgg16().features: index, cin, cout of the 13 convs; the conv count that ends each LPIPS slice
+static const int kLpConv[13][3] = {{0, 3, 64},     {2, 64, 64},     {5, 64, 128},    {7, 128, 128},  {10, 128, 256},
+                                   {12, 256, 256}, {14, 256, 256},  {17, 256, 512},  {19, 512, 512}, {21, 512, 512},
+                                   {24, 512, 512}, {26, 512, 512},  {28, 512, 512}};
+static const int kLpSliceEnd[5] = {2, 4, 7, 10, 13};
+constexpr int LPIPS_U8_CONVENTIONS = 2;
+
+static std::string lp_conv_name(int i) {   // net.slice<s>.<index>. (lpips pretrained_networks.vgg16: features[x] in slice s)
+  const int idx = kLpConv[i][0];
+  const int s = idx < 4 ? 1 : idx < 9 ? 2 : idx < 16 ? 3 : idx < 23 ? 4 : 5;
+  return "net.slice" + std::to_string(s) + "." + std::to_string(idx) + ".";
+}
+
+// The per-channel table of a uint8 convention, on the host in each step's own precision (x86-64 SSE: IEEE single / double,
+// no contraction), RGB channel order:
+//   0 'lpips'       lpips.im2tensor: float32(u / 127.5 - 1) [numpy float64], then the ScalingLayer in fp32
+//   1 'codeformer'  float32(u / 255.) [float64 division] and normalize(0.5, 0.5) (the training pipeline's image tensors), then
+//                   LPIPSLoss(use_input_norm=True, range_norm=True): (x + 1) / 2, (x - mean) / std, then the ScalingLayer
+static int lp_u8_table(int convention, const float shift[3], const float scale[3], float* t) {
+  CFB_REQUIRE(convention >= 0 && convention < LPIPS_U8_CONVENTIONS, "LPIPS: unknown uint8 convention");
+  const float mean[3] = {(float)0.485, (float)0.456, (float)0.406}, stdv[3] = {(float)0.229, (float)0.224, (float)0.225};
+  for (int c = 0; c < 3; ++c)
+    for (int u = 0; u < 256; ++u) {
+      float x;
+      if (convention == 0) {
+        x = (float)((double)u / 127.5 - 1.0);
+      } else {
+        const float v = (float)((double)u / 255.0);
+        x = (v - 0.5f) / 0.5f;
+        x = (x + 1.f) / 2.f;
+        x = (x - mean[c]) / stdv[c];
+      }
+      t[c * 256 + u] = (x - shift[c]) / scale[c];
+    }
+  return 0;
+}
+
+static LpipsXform lp_xform(const cfb_lpips* n, int flags) {
+  LpipsXform x;
+  x.flags = flags;
+  const float mean[3] = {(float)0.485, (float)0.456, (float)0.406}, stdv[3] = {(float)0.229, (float)0.224, (float)0.225};
+  for (int c = 0; c < 3; ++c) { x.mean[c] = mean[c]; x.std[c] = stdv[c]; x.shift[c] = n->shift[c]; x.scale[c] = n->scale[c]; }
+  return x;
+}
+
+static int lp_prepare(cfb_lpips* n, cudaStream_t st) {
+  CFB_CHECK(n->begin_prepare(st));
+  SlabPlan plan;
+  for (int i = 0; i < 12; ++i) {
+    n->convs[i] = plan_conv(lp_conv_name(i + 1) + "weight", kLpConv[i + 1][1], kLpConv[i + 1][2]);
+    plan.add(n->convs[i]);
+  }
+  const size_t tbytes = (size_t)LPIPS_U8_CONVENTIONS * 3 * 256 * 4;
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256(64 * 27 * 4) + align256(64 * 4) + 5 * align256(512 * 4) + align256(tbytes)));
+  WeightPrep wp(*n, plan, st);
+  for (int i = 0; i < 12; ++i) {
+    GenConv& c = n->convs[i];
+    const std::string p = lp_conv_name(i + 1);
+    const float* w = n->param(p + "weight", (int64_t)c.cout * c.cin * 9);
+    const float* b = n->param(p + "bias", c.cout);
+    if (!w || !b) return 1;
+    CFB_CHECK(wp.conv(c, w, b));
+  }
+  const float* w0 = n->param("net.slice1.0.weight", 64 * 27);
+  const float* b0 = n->param("net.slice1.0.bias", 64);
+  const float* sh = n->param("scaling_layer.shift", 3);
+  const float* sc = n->param("scaling_layer.scale", 3);
+  if (!w0 || !b0 || !sh || !sc) return 1;
+  n->stem_w = (float*)wp.take(64 * 27 * 4); n->stem_b = (float*)wp.take(64 * 4);
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, w0, 64 * 27 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, b0, 64 * 4, cudaMemcpyDeviceToDevice, st));
+  for (int k = 0; k < 5; ++k) {
+    const int C = kLpConv[kLpSliceEnd[k] - 1][2];
+    const float* l = n->param("lin" + std::to_string(k) + ".model.1.weight", C);
+    if (!l) return 1;
+    n->lin[k] = (float*)wp.take(512 * 4);
+    CFB_CUDA(cudaMemcpyAsync(n->lin[k], l, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  CFB_CUDA(cudaMemcpyAsync(n->shift, sh, 12, cudaMemcpyDeviceToHost, st));
+  CFB_CUDA(cudaMemcpyAsync(n->scale, sc, 12, cudaMemcpyDeviceToHost, st));
+  CFB_CUDA(cudaStreamSynchronize(st));
+  std::vector<float> t((size_t)LPIPS_U8_CONVENTIONS * 768);
+  for (int c = 0; c < LPIPS_U8_CONVENTIONS; ++c) CFB_CHECK(lp_u8_table(c, n->shift, n->scale, t.data() + (size_t)c * 768));
+  n->tables = (float*)wp.take(tbytes);
+  CFB_CUDA(cudaMemcpyAsync(n->tables, t.data(), tbytes, cudaMemcpyHostToDevice, st));
+  CFB_CUDA(cudaStreamSynchronize(st));
+  n->prepared = true;
+  return 0;
+}
+
+// The inputs of a launch: fp32 NCHW ref [groups,3,H,W] / cand [groups*G,3,H,W] with the LpipsXform flags, or uint8 HWC BGR
+// ref8 [groups,H,W,3] / cand8 [groups*G,H,W,3] with a convention.
+struct LpIn {
+  const float* ref = nullptr; const float* cand = nullptr; int flags = 0;
+  const unsigned char* ref8 = nullptr; const unsigned char* cand8 = nullptr; int convention = -1;
+};
+
+static int lp_stem(cfb_lpips* n, const LpIn& in, float* out, int groups, int G, int H, int W, cudaStream_t st) {
+  const float* table = nullptr;
+  if (in.ref8) {
+    CFB_REQUIRE(in.convention >= 0 && in.convention < LPIPS_U8_CONVENTIONS, "LPIPS: unknown uint8 convention");
+    table = n->tables + (size_t)in.convention * 768;
+  }
+  CFB_REQUIRE(in.flags >= 0 && in.flags < 8, "LPIPS: unknown input transform flags");
+  return lpips_stem(in.ref, in.cand, in.ref8, in.cand8, table, lp_xform(n, in.flags), n->stem_w, n->stem_b, out, groups, G, H, W, st);
+}
+
+static int lp_forward(cfb_lpips* n, const LpIn& in, int groups, int G, int H, int W, float* val, float* per_layer, void* ws,
+                      int64_t ws_bytes, cudaStream_t st, bool dry) {
+  CFB_CHECK(n->begin_forward(dry));
+  CFB_REQUIRE(groups >= 0 && G >= 1, "LPIPS: a group needs at least one candidate");
+  CFB_REQUIRE(H >= 16 && W >= 16, "LPIPS: H and W must be at least 16 (relu5_3 is at 1/16 of the input)");
+  if (groups == 0) return 0;
+  const int64_t M = (int64_t)groups * (1 + G), P = (int64_t)groups * G;
+  CFB_REQUIRE(M <= 65535, "LPIPS: at most 65535 images per launch");
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  LpipsLayers L;
+  L.n = 5;
+  float* part[5] = {};
+  for (int k = 0, h = H, w = W; k < 5; ++k, h /= 2, w /= 2) {
+    L.nblk[k] = lpips_head_blocks(h, w);
+    L.hw[k] = (int64_t)h * w;
+    CFB_CHECK(n->alloc(&part[k], (size_t)P * L.nblk[k]));
+    L.part[k] = part[k];
+  }
+  float* cur = nullptr;
+  CFB_CHECK(n->alloc(&cur, (size_t)M * H * W * 64));
+  if (!dry) CFB_CHECK(lp_stem(n, in, cur, groups, G, H, W, st));
+  int h = H, w = W, ci = 1;
+  for (int s = 0; s < 5; ++s) {
+    for (; ci < kLpSliceEnd[s]; ++ci) {
+      const GenConv& c = n->convs[ci - 1];
+      float* y = nullptr;
+      CFB_CHECK(n->alloc(&y, (size_t)M * h * w * c.cout));
+      GenLaunch g{&c, cur, c.cin, h, w, (int)M, y, c.cout, 0, OUT_RELU};
+      if (!dry) CFB_CHECK(gen_conv(g, n->sm_count, st));
+      ar.release(cur);
+      cur = y;
+    }
+    const int C = kLpConv[ci - 1][2];
+    float* pooled = nullptr;
+    if (s < 4) CFB_CHECK(n->alloc(&pooled, (size_t)M * (h / 2) * (w / 2) * C));
+    if (!dry) CFB_CHECK(lpips_head(cur, n->lin[s], groups, G, h, w, C, pooled, part[s], st));
+    ar.release(cur);
+    cur = pooled; h /= 2; w /= 2;
+  }
+  if (!dry) CFB_CHECK(lpips_finalize(L, (int)P, val, per_layer, st));
+  for (float* p : part) ar.release(p);
+  return 0;
+}
+
+}  // namespace cfb
+
+// =========================================================================================================
 // YOLOv5l-face: the other large detector of whole-image mode (--detection_model YOLOv5l)
 //   facelib/detection/yolov5face/models/yolov5l.yaml, common.py (Conv, StemBlock, C3, Bottleneck, SPP), yolo.py (Detect).
 // Every Conv is conv (no bias) + BatchNorm2d (folded at prepare) + SiLU.  Engines per conv form:
@@ -3158,6 +3334,93 @@ int cfb_yolov5face_candidates(const float* pred, int32_t batch, int32_t h, int32
   const int64_t P = cfb_yolov5face_predictions(h, w);
   CFB_REQUIRE(P > 0 && batch >= 0 && P * batch < ((int64_t)1 << 31) / 16, "cfb_yolov5face_candidates: bad size");
   return cfb::yolo_candidates(pred, batch, (int)P, conf_threshold, rows, counts, (cudaStream_t)stream);
+  API_END(1)
+}
+
+cfb_lpips* cfb_lpips_create(void) {
+  API_BEGIN
+  return new cfb_lpips();
+  API_END(nullptr)
+}
+void cfb_lpips_destroy(cfb_lpips* n) { delete n; }
+int cfb_lpips_set_param(cfb_lpips* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_lpips_set_param: NULL argument");
+  return n->set_param(name, dev_ptr, numel);
+  API_END(1)
+}
+int cfb_lpips_prepare(cfb_lpips* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_lpips_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::lp_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_lpips_workspace_bytes(cfb_lpips* n, int32_t batch, int32_t h, int32_t w, int32_t group) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_lpips_workspace_bytes: NULL net"); return -1; }
+  cfb::LpIn in;
+  in.ref = in.cand = (const float*)0x1000;
+  return n->dry_run([&] { return cfb::lp_forward(n, in, batch, group, h, w, nullptr, nullptr, nullptr, 0, nullptr, true); });
+  API_END(-1)
+}
+int cfb_lpips_forward(cfb_lpips* n, const float* ref_nchw, const float* cand_nchw, int32_t batch, int32_t h, int32_t w, int32_t group,
+                      int32_t xform, float* val, float* per_layer, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (ref_nchw && cand_nchw && val && workspace)), "cfb_lpips_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  cfb::LpIn in;
+  in.ref = ref_nchw; in.cand = cand_nchw; in.flags = xform;
+  return cfb::lp_forward(n, in, batch, group, h, w, val, per_layer, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_lpips_forward_u8(cfb_lpips* n, const uint8_t* ref_bgr, const uint8_t* cand_bgr, int32_t batch, int32_t h, int32_t w,
+                         int32_t group, int32_t convention, float* val, float* per_layer, void* workspace, int64_t workspace_bytes,
+                         void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (ref_bgr && cand_bgr && val && workspace)), "cfb_lpips_forward_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  cfb::LpIn in;
+  in.ref8 = ref_bgr; in.cand8 = cand_bgr; in.convention = convention;
+  return cfb::lp_forward(n, in, batch, group, h, w, val, per_layer, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_lpips_u8_table(int32_t convention, const float* shift, const float* scale, float* table) {
+  API_BEGIN
+  CFB_REQUIRE(shift && scale && table, "cfb_lpips_u8_table: NULL argument");
+  return cfb::lp_u8_table(convention, shift, scale, table);
+  API_END(1)
+}
+int cfb_debug_lpips_stem(cfb_lpips* n, const void* ref, const void* cand, int32_t u8, int32_t mode, float* out, int32_t batch,
+                         int32_t h, int32_t w, int32_t group, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && ref && cand && out, "cfb_debug_lpips_stem: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  CFB_CHECK(n->begin_forward(false));
+  CFB_REQUIRE(batch >= 0 && group >= 1 && h >= 1 && w >= 1, "cfb_debug_lpips_stem: bad size");
+  cfb::LpIn in;
+  if (u8) { in.ref8 = (const uint8_t*)ref; in.cand8 = (const uint8_t*)cand; in.convention = mode; }
+  else { in.ref = (const float*)ref; in.cand = (const float*)cand; in.flags = mode; }
+  return cfb::lp_stem(n, in, out, batch, group, h, w, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_debug_lpips_head_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t group) {
+  if (batch < 0 || group < 1 || h < 1 || w < 1) return -1;
+  return (int64_t)batch * group * cfb::lpips_head_blocks(h, w) * 4 + 256;
+}
+int cfb_debug_lpips_head(const float* feat, const float* lin, float* pooled, float* res, int32_t batch, int32_t h, int32_t w,
+                         int32_t group, int32_t c, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(feat && lin && res && workspace, "cfb_debug_lpips_head: NULL argument");
+  const int64_t need = cfb_debug_lpips_head_workspace_bytes(batch, h, w, group);
+  CFB_REQUIRE(need >= 0 && workspace_bytes >= need, "cfb_debug_lpips_head: bad size or workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  CFB_CHECK(cfb::async_status_init(st));
+  float* part = (float*)(((uintptr_t)workspace + 255) / 256 * 256);
+  CFB_CHECK(cfb::lpips_head(feat, lin, batch, group, h, w, c, pooled, part, st));
+  cfb::LpipsLayers L;
+  L.n = 1; L.part[0] = part; L.nblk[0] = cfb::lpips_head_blocks(h, w); L.hw[0] = (int64_t)h * w;
+  return cfb::lpips_finalize(L, batch * group, nullptr, res, st);
   API_END(1)
 }
 

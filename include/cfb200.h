@@ -450,6 +450,44 @@ int          cfb_debug_arcface_conv(const float* in, const float* weight_oihw, c
                                     const float* in_shift, int32_t out_act, float prelu_slope, const float* residual,
                                     void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- LPIPS(net='vgg', version='0.1') perceptual distance (lpips 0.1; the perceptual term of basicsr's LPIPSLoss; lpips.cu +
+ * the conv engine) ----
+ * Parameters by lpips' state-dict names: scaling_layer.shift / .scale [3], net.slice<s>.<i>.weight / .bias (torchvision
+ * vgg16().features index i), lin<k>.model.1.weight [C_k].  A launch holds `batch` groups of one reference and `group` (>= 1)
+ * candidates: ref [batch], cand [batch * group] (candidate j of group q at q * group + j); pair p = q * group + j.  h, w >= 16.
+ * forward: fp32 NCHW RGB images; xform = flags applied to every element before the ScalingLayer, in this order: 2 range_norm
+ *   (x + 1) / 2, 4 input_norm (x - [0.485, 0.456, 0.406]) / [0.229, 0.224, 0.225], 1 normalize 2x - 1 (each a torch fp32 op).
+ * forward_u8: uint8 HWC BGR images; convention 0 'lpips' (im2tensor: u / 127.5 - 1) or 1 'codeformer' (float32(u / 255.),
+ *   normalize(0.5, 0.5), then LPIPSLoss's range_norm and input_norm), through the table cfb_lpips_u8_table gives; it equals
+ *   forward on those transformed images bit for bit.
+ * Outputs: val [P] float32 (the sum over the five layers, in order) and, when per_layer is set, per_layer [P][5].  Results do
+ * not depend on the batch or the group size.  Workspace: cfb_lpips_workspace_bytes(net, batch, h, w, group); it grows with
+ * batch * (1 + group) * h * w * 512 bytes (two relu1 maps).
+ * u8_table (host only): the [3][256] stem inputs of a convention by RGB channel, for ScalingLayer shift / scale [3].
+ * debug_stem (test entry point): conv1_1 + ReLU of the prepared net -> NHWC [batch * (1 + group), h, w, 64] in the launch's
+ *   image order; u8 selects the input form, mode is xform (fp32) or the convention (uint8).
+ * debug_head (test entry point): the head-and-pool pass of one layer on NHWC feat [batch * (1 + group), h, w, c] (c 64, 128,
+ *   256 or 512) with lin [c]: pooled (optional) [batch * (1 + group), h / 2, w / 2, c], res [P] the layer's values.  Workspace:
+ *   cfb_debug_lpips_head_workspace_bytes. */
+typedef struct cfb_lpips cfb_lpips;
+cfb_lpips* cfb_lpips_create(void);
+void       cfb_lpips_destroy(cfb_lpips* net);
+int        cfb_lpips_set_param(cfb_lpips* net, const char* name, const float* dev_ptr, int64_t numel);
+int        cfb_lpips_prepare(cfb_lpips* net, void* stream);
+int64_t    cfb_lpips_workspace_bytes(cfb_lpips* net, int32_t batch, int32_t h, int32_t w, int32_t group);
+int        cfb_lpips_forward(cfb_lpips* net, const float* ref_nchw, const float* cand_nchw, int32_t batch, int32_t h, int32_t w,
+                             int32_t group, int32_t xform, float* val, float* per_layer, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+int        cfb_lpips_forward_u8(cfb_lpips* net, const uint8_t* ref_bgr, const uint8_t* cand_bgr, int32_t batch, int32_t h, int32_t w,
+                                int32_t group, int32_t convention, float* val, float* per_layer, void* workspace,
+                                int64_t workspace_bytes, void* stream);
+int        cfb_lpips_u8_table(int32_t convention, const float* shift, const float* scale, float* table);
+int        cfb_debug_lpips_stem(cfb_lpips* net, const void* ref, const void* cand, int32_t u8, int32_t mode, float* out, int32_t batch,
+                                int32_t h, int32_t w, int32_t group, void* stream);
+int64_t    cfb_debug_lpips_head_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t group);
+int        cfb_debug_lpips_head(const float* feat, const float* lin, float* pooled, float* res, int32_t batch, int32_t h, int32_t w,
+                                int32_t group, int32_t c, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- YOLOv5l-face detector (facelib/detection/yolov5face, models/yolov5l.yaml; yolo.cu + the conv engine) ----
  * Parameters by the reference's state-dict names (BatchNorm folded at prepare; the Detect anchor_grid buffer gives the anchor
  * sizes in pixels).  h and w are multiples of 32; P = cfb_yolov5face_predictions(h, w) = 3 (hw/64 + hw/256 + hw/1024).
