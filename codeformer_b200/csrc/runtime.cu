@@ -4043,6 +4043,58 @@ int cfb_debug_conv_tc_prec_wv(const float* in, const float* in2, int32_t cin1, c
                        out_act, precision);
   API_END(1)
 }
+
+static size_t align1024(size_t b) { return (b + 1023) / 1024 * 1024; }
+int64_t cfb_debug_bmm_tc_workspace_bytes(int32_t n, int32_t heads, int32_t d) {
+  const size_t T = (size_t)n * 256, E = (size_t)heads * d;
+  return (int64_t)(1024 + 2 * align1024(T * 2 * E * 2) + 2 * align1024(T * E * 2) + align1024(T * heads * 256 * 4) +
+                   2 * align1024(T * heads * 256 * 2) + 2 * align1024(T * E * 2));
+}
+int cfb_debug_bmm_tc(const float* q, const float* k, const float* v, float* out, void* out_planes, int32_t n, int32_t heads,
+                     int32_t d, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(q && k && v && out && workspace, "cfb_debug_bmm_tc: NULL argument");
+  CFB_REQUIRE(n >= 0 && heads >= 1 && d >= 64 && d % 64 == 0, "cfb_debug_bmm_tc: d must be a positive multiple of 64");
+  CFB_REQUIRE(workspace_bytes >= cfb_debug_bmm_tc_workspace_bytes(n, heads, d), "cfb_debug_bmm_tc: workspace too small");
+  CFB_CHECK(cfb::async_status_init(nullptr));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int E = heads * d;
+  const int64_t T = (int64_t)n * 256, rows = T * heads;
+  char* p = (char*)workspace;
+  float* consts = (float*)p; p += 1024;
+  void* qk = p; p += 2 * align1024((size_t)T * 2 * E * 2);
+  void* vp = p; p += 2 * align1024((size_t)T * E * 2);
+  float* scores = (float*)p; p += align1024((size_t)rows * 256 * 4);
+  void* pp = p; p += 2 * align1024((size_t)rows * 256 * 2);
+  void* vt = p;
+  // the scale of each core as the forward holds it: C^-1/2 (AttnBlock, one head), head_dim^-1/2 (nn.MultiheadAttention)
+  const float hc[2] = {1.0f / sqrtf((float)d), 1.0f};
+  CFB_CUDA(cudaMemcpyAsync(consts, hc, sizeof(hc), cudaMemcpyHostToDevice, st));
+  // q | k and v as the operand planes their producing convs write (one [T][2E] plane pair, one [T][E])
+  CFB_CHECK(cfb::concat_planes(q, k, qk, T, E, E, st));
+  CFB_CHECK(cfb::concat_planes(v, nullptr, vp, T, E, 0, st));
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  // the launch sequence of Fwd::attnblock (heads 1) and of the Transformer layer (several heads), with an fp32 output added
+  cfb::BmmArgs g1;
+  g1.a_planes = qk; g1.a_pitch = 2 * E; g1.a_c0 = 0;
+  g1.b_planes = qk; g1.b_pitch = 2 * E; g1.b_c0 = E; g1.b_rows = 256;
+  g1.N = n; g1.K = d; g1.Cout = 256; g1.scale_dev = consts; g1.out = scores;
+  if (heads > 1) { g1.heads = heads; g1.a_c_head = d; g1.b_c_head = d; g1.out_per_head = true; }
+  CFB_CHECK(cfb::bmm_tc(g1, sms, st));
+  CFB_CHECK(cfb::softmax256_planes(scores, pp, rows, st));
+  CFB_CHECK(cfb::transpose_planes(vp, n, E, 0, E, vt, st));
+  cfb::BmmArgs g2;
+  g2.a_planes = pp; g2.a_pitch = 256; g2.a_c0 = 0;
+  g2.b_planes = vt; g2.b_pitch = 256; g2.b_c0 = 0; g2.b_rows = E;
+  g2.N = n; g2.K = 256; g2.Cout = heads > 1 ? d : E; g2.scale_dev = consts + 1; g2.out = out; g2.out_planes = out_planes;
+  if (heads > 1) { g2.heads = heads; g2.a_img_per_head = true; g2.b_r_head = d; g2.out_per_head = false; g2.o_c_head = d; }
+  CFB_CHECK(cfb::bmm_tc(g2, sms, st));
+  return 0;
+  API_END(1)
+}
+
 int cfb_debug_time_conv(const float* in, const float* weight_oihw, float* out, int32_t n, int32_t h, int32_t w, int32_t cin,
                         int32_t cout, int32_t ksize, int32_t mode, int32_t reps, void* workspace, int64_t workspace_bytes,
                         void* stream, const float* in_scale, const float* in_shift, int32_t in_act, float* ms_per_launch) {

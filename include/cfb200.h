@@ -253,6 +253,14 @@ int cfb_debug_conv_tc_prec_wv(const float* in, const float* in2, int32_t cin1, c
                               const float* sft_dec, const float* sft_scale, const float* sft_wv, void* out_planes,
                               float* gn_part, void* workspace, int64_t workspace_bytes, void* stream, int32_t* tile_n,
                               int32_t ksize, int32_t out_act, int32_t precision);
+/* diagnostics / tests: the attention core of the forward on the wgmma engine (bmm_tc: scores, softmax256_planes, bmm_tc: P v)
+ * from fp32 inputs.  q, k, v, out: [n][256 tokens][heads * d] (the 16x16 latent), out = softmax(q_h k_h^T d^-1/2) v_h per head h
+ * (channels [h*d, (h+1)*d)); out_planes (optional): fp16 hi | lo planes of out, each align1024(n*256*heads*d*2) bytes.  heads 1
+ * is the AttnBlock core (d = C), heads > 1 the Transformer's nn.MultiheadAttention core; d a multiple of 64.  q, k and v are
+ * split into operand planes as their producing convs write them.  workspace >= cfb_debug_bmm_tc_workspace_bytes(n, heads, d). */
+int64_t cfb_debug_bmm_tc_workspace_bytes(int32_t n, int32_t heads, int32_t d);
+int cfb_debug_bmm_tc(const float* q, const float* k, const float* v, float* out, void* out_planes, int32_t n, int32_t heads,
+                     int32_t d, void* workspace, int64_t workspace_bytes, void* stream);
 /* diagnostics / tests: the GroupNorm(32) finalize of the forward on partials in the layout cfb_debug_conv_tc writes (slots of
  * 32 pixels, [n][slots][32 groups][2] floats): scale[n,c] = rstd*gamma, shift[n,c] = beta - mean*rstd*gamma over hw pixels
  * of c channels.  The workspace (>= cfb_debug_gn_partials_workspace_bytes) holds the split-finalize scratch and the ticket

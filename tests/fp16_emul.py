@@ -19,12 +19,16 @@ def fp16_round(x):
     return x.float().half().double()
 
 
+def weight_exponent(w):
+    """e = frexp(max|w|) of the whole conv (tc_split_weights): the split scales the weights by 2^(14-e)."""
+    amax = float(w.float().abs().max()) if w.numel() else 0.0
+    return math.frexp(amax)[1] if amax > 0 and math.isfinite(amax) else 0
+
+
 def weight_hi(w):
     """Hi plane of the split weights as float64 values: fp16(w * 2^(14-e)) * 2^(e-14), e = frexp(max|w|) (tc_split_weights)."""
-    w = w.float()
-    amax = float(w.abs().max()) if w.numel() else 0.0
-    e = math.frexp(amax)[1] if amax > 0 and math.isfinite(amax) else 0
-    return (w * 2.0 ** (14 - e)).half().double() * 2.0 ** (e - 14)
+    e = weight_exponent(w)
+    return (w.float() * 2.0 ** (14 - e)).half().double() * 2.0 ** (e - 14)
 
 
 # rows (columns) of the 3x3 kernel a 2x2 parity tap d sums for output parity 0 / 1 (up4_range in conv_tc.cu)
