@@ -6,8 +6,11 @@
 //                 the same weights as exact dyadic floats, ((v0 w0 + v1 w1) + v2 w2) + v3 w3.  The parse mask's flags=3
 //                 is INTER_AREA, which warpAffine runs as INTER_LINEAR.
 //   resize        INTER_LINEAR, 11-bit weights (horizontal clamped, vertical not); an exact halving is the 2x2 mean.
+//                 float64 (the parse mask): double coordinates fma(d + 0.5, ssize / dsize, -0.5) and lerp FMAs.
 //   erode         rectangular k x k, anchor k/2, pixels outside the image never erode, k == 0 means 3x3.
-//   GaussianBlur  separable, BORDER_REFLECT_101, taps summed in order (the float kernel is cv2.getGaussianKernel).
+//   GaussianBlur  separable, BORDER_REFLECT_101, cv2 4.13's x86-64 AVX2 arithmetic: which outputs take fused multiply-adds
+//                 depends on the SIMD block of their column (k_blur_roi, k_blur_f64).  The float kernel is
+//                 cv2.getGaussianKernel; the parse mask's float64 kernel is cv2's own table (kParseKernelHalf).
 //
 // Every per-face step works on the face's ROI: the bounding box of the face square grown by 2 source pixels, mapped
 // to the canvas, grown by 2 pixels and clipped.  Outside it every warp of the face is exactly 0, so the soft mask is 0
@@ -27,7 +30,8 @@
 //   gray images   add_restored_face's adain_npy(bgr2gray(restored), cropped) in float64 (cfb_gray_adain_faces) and the paste
 //                 of float64 faces (cfb_paste_faces_f64): warpAffine on CV_64F blends with the float32 weight table in
 //                 double, and the canvas is float64 from the first face on.
-// Arithmetic that cv2 does unfused is written with _rn intrinsics so nvcc cannot contract it into FMAs.
+// Arithmetic that cv2 does unfused is written with _rn intrinsics so nvcc cannot contract it into FMAs; where cv2 fuses,
+// the kernels call __fmaf_rn / __fma_rn.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -46,6 +50,23 @@ namespace {
 constexpr int kParse = 512;           // the parsing network's resolution
 constexpr int kParseK = 101;          // GaussianBlur(parse_mask, (101, 101), 11), applied twice
 constexpr int kRoiPad = 2;
+static_assert(kParse % 8 == 0, "k_blur_f64 assumes no SIMD tail columns in cv2's filter");
+
+// cv2.getGaussianKernel(101, 11, CV_64F), taps 0 .. 50 (the rest mirror them).  cv2 exponentiates in its software double,
+// whose last bit std::exp does not always reproduce, so the parse mask's kernel is cv2's own values.
+constexpr double kParseKernelHalf[kParseK / 2 + 1] = {
+  0x1.3d9320997c25bp-20, 0x1.de17a7bf38417p-20, 0x1.64e8ed67fb58cp-19, 0x1.08402ac73792fp-18, 0x1.8412e6ca94be9p-18,
+  0x1.1a9d258b611acp-17, 0x1.983ce6e2d8b48p-17, 0x1.246cb61c4022cp-16, 0x1.9f7c2e4f210b2p-16, 0x1.24bcaeb80f233p-15,
+  0x1.991c4ec5d6f8ep-15, 0x1.1b85423e811abp-14, 0x1.85bc1908d022ep-14, 0x1.09aa455fcb2a8p-13, 0x1.673421a12de51p-13,
+  0x1.e1add23bf2656p-13, 0x1.404c85f10d7b6p-12, 0x1.a677dc2924522p-12, 0x1.1452178d2dfc5p-11, 0x1.667cb15ebc175p-11,
+  0x1.cd4230959cfabp-11, 0x1.264dd24853bf3p-10, 0x1.7477bd22f281bp-10, 0x1.d382d89d4adafp-10, 0x1.22fd1739f5a24p-9,
+  0x1.6740df70cfe47p-9, 0x1.b7e1e31cfeb7cp-9, 0x1.0b165029af448p-8, 0x1.41ab7619e5c97p-8, 0x1.8037efebc0c46p-8,
+  0x1.c727155fbb708p-8, 0x1.0b5f5ae5abc27p-7, 0x1.378ad7eba8e32p-7, 0x1.680578de9fdf6p-7, 0x1.9c9eb782d6717p-7,
+  0x1.d502d0b5254c3p-7, 0x1.085c4a7f64ae8p-6, 0x1.27904729ecf7bp-6, 0x1.47bada6c7b599p-6, 0x1.6867edea4945bp-6,
+  0x1.8913f51fae714p-6, 0x1.a92eec6952cc7p-6, 0x1.c82029c32f07fp-6, 0x1.e54ae009f9925p-6, 0x1.0009941ac006fp-5,
+  0x1.0bf1ac50126f9p-5, 0x1.1618b501c3bf9p-5, 0x1.1e421299af7d2p-5, 0x1.243bea305ece7p-5, 0x1.27e11b8751b9cp-5,
+  0x1.291ac05d51e68p-5,
+};
 
 struct PbFace {
   double A[6];        // destination (canvas / crop) -> source (face) map: cv2's inverse of the given matrix
@@ -111,7 +132,8 @@ __device__ __forceinline__ void warp_coord(const double* A, int x, int y, int& i
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(A[1], (double)y), A[2]), 1024.)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(A[4], (double)y), A[5]), 1024.)) + 16;
   const int X = (X0 + ad) >> 5, Y = (Y0 + bd) >> 5;
-  ix = X >> 5; iy = Y >> 5; fx = X & 31; fy = Y & 31;
+  ix = min(max(X >> 5, -32768), 32767); iy = min(max(Y >> 5, -32768), 32767);   // cv2 keeps them as int16 (saturate_cast)
+  fx = X & 31; fy = Y & 31;
 }
 
 __device__ __forceinline__ int border_idx(int p, int n, int mode) {
@@ -298,27 +320,30 @@ __global__ void k_warp_crop_multi(const uint8_t* __restrict__ src, int h, int w,
   o[0] = (uint8_t)v[0]; o[1] = (uint8_t)v[1]; o[2] = (uint8_t)v[2];
 }
 
+// float64 INTER_LINEAR tap (cv2.resize on CV_64F): source coordinate fma(d + 0.5, ssize / dsize, -0.5) in double, the two
+// clamped source indices and the fraction
+__device__ __forceinline__ void lin_tap_f64(int d, double scale, int n, int& i0, int& i1, double& t) {
+  const double f = __fma_rn((double)d + 0.5, scale, -0.5), fl = floor(f);
+  const int i = (int)fl;
+  t = __dsub_rn(f, fl);
+  i0 = min(max(i, 0), n - 1);
+  i1 = min(max(i + 1, 0), n - 1);
+}
+
+// rows first, each pass the lerp fma(b - a, t, a); scale = source size / destination size
 __global__ void k_resize_f64(const double* __restrict__ src, int h, int w, double* __restrict__ dst, int oh, int ow,
                              double sx_scale, double sy_scale) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
   if (x >= ow || y >= oh) return;
   src += (size_t)f * h * w;
-  int sx, sy;
-  float fx, fy;
-  lin_tap(x, sx_scale, sx, fx);
-  bool hi = false;
-  if (sx < 0) { sx = 0; fx = 0.f; }
-  if (sx >= w - 1) { sx = w - 1; fx = 0.f; hi = true; }
-  const double a0 = (double)__fsub_rn(1.f, fx), a1 = (double)fx;
-  lin_tap(y, sy_scale, sy, fy);
-  const double b0 = (double)__fsub_rn(1.f, fy), b1 = (double)fy;
-  const int yy[2] = {min(max(sy, 0), h - 1), min(max(sy + 1, 0), h - 1)};
-  double r[2];
-  for (int i = 0; i < 2; ++i) {
-    const double* row = src + (size_t)yy[i] * w;
-    r[i] = hi ? row[sx] : __dadd_rn(__dmul_rn(row[sx], a0), __dmul_rn(row[min(sx + 1, w - 1)], a1));
-  }
-  dst[((size_t)f * oh + y) * ow + x] = __dadd_rn(__dmul_rn(r[0], b0), __dmul_rn(r[1], b1));
+  int x0, x1, y0, y1;
+  double tx, ty;
+  lin_tap_f64(x, sx_scale, w, x0, x1, tx);
+  lin_tap_f64(y, sy_scale, h, y0, y1, ty);
+  const double* r0 = src + (size_t)y0 * w;
+  const double* r1 = src + (size_t)y1 * w;
+  const double a = __fma_rn(__dsub_rn(r0[x1], r0[x0]), tx, r0[x0]), b = __fma_rn(__dsub_rn(r1[x1], r1[x0]), tx, r1[x0]);
+  dst[((size_t)f * oh + y) * ow + x] = __fma_rn(__dsub_rn(b, a), ty, a);
 }
 
 // ones(S x S) warped to the ROI, f32 bilinear with constant 0: the in-bounds weights, exact multiples of 1/1024
@@ -376,7 +401,14 @@ __global__ void k_area(const PbFace* __restrict__ faces, const float* __restrict
   if (threadIdx.x == 0) area[blockIdx.x] = red[0];
 }
 
-// f32 Gaussian pass on the ROI planes: reflect-101 at the canvas border, 0 outside the ROI inside the canvas
+// f32 Gaussian pass on the ROI planes: reflect-101 at the canvas border, 0 outside the ROI inside the canvas.  cv2's
+// sepFilter2D (x86-64, AVX2) picks the arithmetic by the output's canvas column gx = F.x0 + x, so the ROI pass does too:
+//   rows, n >= 7   gx < W - W % 4: FMA chain in tap order from 0; the last W % 4 columns: k[0] v[0], then the first
+//                  4 * ((n - 1) / 4) taps as rounded products and sums, the rest FMA'd
+//   rows, n == 5   gx < W - W % 2: fma(v0, k[2], p1 k[3]) + p2 k[4]; an odd width's last column rounds every step
+//   rows, n == 3   v0 k[1] + p1 k[2]                                    (p_i = v[+i] + v[-i])
+//   columns        the centre product, then fma(p_i, k[r + i], acc); the last W % 8 columns round every step
+// The zeros outside the ROI change nothing in any form: fma(0, k, acc) = acc + 0 * k = acc and v + 0 = v exactly.
 __global__ void k_blur_roi(const PbFace* __restrict__ faces, float* __restrict__ ws, const float* __restrict__ gk, int in,
                            int out, bool cols, int H, int W) {
   const PbFace& F = faces[blockIdx.z];
@@ -385,18 +417,37 @@ __global__ void k_blur_roi(const PbFace* __restrict__ faces, float* __restrict__
   const size_t plane = (size_t)F.rw * F.rh;
   const float* src = ws + F.off + in * plane;
   const float* k = gk + F.goff;
-  const int r = F.r;
-  float acc = 0.f;
-  for (int t = 0; t <= 2 * r; ++t) {
-    float v = 0.f;
+  const int r = F.r, n = 2 * r + 1, gx = F.x0 + x;
+  auto tap = [&](int d) -> float {          // the value d taps away along the pass
     if (!cols) {
-      const int gx = border_idx(F.x0 + x + t - r, W, 4) - F.x0;
-      if (gx >= 0 && gx < F.rw) v = src[(size_t)y * F.rw + gx];
-    } else {
-      const int gy = border_idx(F.y0 + y + t - r, H, 4) - F.y0;
-      if (gy >= 0 && gy < F.rh) v = src[(size_t)gy * F.rw + x];
+      const int g = border_idx(gx + d, W, 4) - F.x0;
+      return g >= 0 && g < F.rw ? src[(size_t)y * F.rw + g] : 0.f;
     }
-    acc = t == 0 ? __fmul_rn(v, k[0]) : __fadd_rn(acc, __fmul_rn(v, k[t]));
+    const int g = border_idx(F.y0 + y + d, H, 4) - F.y0;
+    return g >= 0 && g < F.rh ? src[(size_t)g * F.rw + x] : 0.f;
+  };
+  float acc;
+  if (cols) {
+    const bool fused = gx < W - W % 8;
+    acc = __fmul_rn(tap(0), k[r]);
+    for (int i = 1; i <= r; ++i) {
+      const float p = __fadd_rn(tap(i), tap(-i));
+      acc = fused ? __fmaf_rn(p, k[r + i], acc) : __fadd_rn(acc, __fmul_rn(p, k[r + i]));
+    }
+  } else if (n == 3) {
+    acc = __fadd_rn(__fmul_rn(tap(0), k[1]), __fmul_rn(__fadd_rn(tap(-1), tap(1)), k[2]));
+  } else if (n == 5) {
+    const float c = tap(0), q1 = __fmul_rn(__fadd_rn(tap(-1), tap(1)), k[3]);
+    acc = gx < W - W % 2 ? __fmaf_rn(c, k[2], q1) : __fadd_rn(__fmul_rn(c, k[2]), q1);
+    acc = __fadd_rn(acc, __fmul_rn(__fadd_rn(tap(-2), tap(2)), k[4]));
+  } else if (gx < W - W % 4) {
+    acc = 0.f;
+    for (int t = 0; t < n; ++t) acc = __fmaf_rn(tap(t - r), k[t], acc);
+  } else {
+    const int unfused = 4 * ((n - 1) / 4);
+    acc = __fmul_rn(tap(-r), k[0]);
+    for (int t = 1; t < n; ++t)
+      acc = t <= unfused ? __fadd_rn(acc, __fmul_rn(tap(t - r), k[t])) : __fmaf_rn(tap(t - r), k[t], acc);
   }
   ws[F.off + out * plane + (size_t)y * F.rw + x] = acc;
 }
@@ -406,18 +457,25 @@ __global__ void k_u8_to_f64(const uint8_t* __restrict__ src, double* __restrict_
   if (i < n) dst[i] = (double)src[i];
 }
 
-// f64 Gaussian pass over whole 512 x 512 parse masks (blockIdx.z = face), reflect-101
+// f64 Gaussian pass over whole 512 x 512 parse masks (blockIdx.z = face), reflect-101, cv2's arithmetic: rows are an FMA
+// chain in tap order from 0 (512 is a multiple of cv2's 4-column blocks, so no column takes its scalar tail); columns take
+// the centre product, then acc + (v[+i] + v[-i]) k[r + i] with every step rounded
 __global__ void k_blur_f64(const double* __restrict__ src, double* __restrict__ dst, const double* __restrict__ k, int ks, bool cols) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= kParse || y >= kParse) return;
   const size_t base = (size_t)blockIdx.z * kParse * kParse;
   src += base;
   const int r = ks / 2;
-  double acc = 0.;
-  for (int t = 0; t < ks; ++t) {
-    const double v = cols ? src[(size_t)border_idx(y + t - r, kParse, 4) * kParse + x]
-                          : src[(size_t)y * kParse + border_idx(x + t - r, kParse, 4)];
-    acc = t == 0 ? __dmul_rn(v, k[0]) : __dadd_rn(acc, __dmul_rn(v, k[t]));
+  double acc;
+  if (!cols) {
+    acc = 0.;
+    for (int t = 0; t < ks; ++t) acc = __fma_rn(src[(size_t)y * kParse + border_idx(x + t - r, kParse, 4)], k[t], acc);
+  } else {
+    acc = __dmul_rn(src[(size_t)y * kParse + x], k[r]);
+    for (int i = 1; i <= r; ++i) {
+      const double p = __dadd_rn(src[(size_t)border_idx(y + i, kParse, 4) * kParse + x], src[(size_t)border_idx(y - i, kParse, 4) * kParse + x]);
+      acc = __dadd_rn(acc, __dmul_rn(p, k[r + i]));
+    }
   }
   dst[base + (size_t)y * kParse + x] = acc;
 }
@@ -632,7 +690,8 @@ int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int 
     if (use_parse) {                        // independent of the areas: enqueue before the read-back
       double* p0 = (double*)(ws + L.parse0);
       double* p1 = (double*)(ws + L.parse1);
-      gaussian_kernel(kParseK, 11., gk);
+      gk.assign(kParseK, 0.);
+      for (int t = 0; t <= kParseK / 2; ++t) gk[t] = gk[kParseK - 1 - t] = kParseKernelHalf[t];
       CFB_CUDA(cudaMemcpyAsync(dpk, gk.data(), kParseK * 8, cudaMemcpyHostToDevice, st));
       const size_t pn = (size_t)n * kParse * kParse;
       k_u8_to_f64<<<(unsigned)((pn + 255) / 256), 256, 0, st>>>(parse_u8, p0, pn);
@@ -649,7 +708,7 @@ int paste_impl(uint8_t* canvas_u8, int n_img, const int32_t* img_of, int H, int 
       parse_src = p0;
       if (S != kParse) {
         double* rs = (double*)(ws + L.parse_rs);
-        const double sc = 1. / ((double)S / kParse);
+        const double sc = (double)kParse / S;
         k_resize_f64<<<grid2(S, S, n, b), b, 0, st>>>(p0, kParse, kParse, rs, S, S, sc, sc);
         CFB_LAUNCH_CHECK();
         parse_src = rs;

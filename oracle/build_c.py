@@ -10,7 +10,7 @@ OUT = os.path.join(HERE, '_c', 'liboracle.so')
 def build(force=False):
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     if force or not os.path.exists(OUT) or os.path.getmtime(OUT) < os.path.getmtime(SRC):
-        subprocess.check_call(['gcc', '-O2', '-fPIC', '-shared', '-fopenmp', '-o', OUT, SRC, '-lm'])
+        subprocess.check_call(['gcc', '-O2', '-ffp-contract=off', '-fPIC', '-shared', '-fopenmp', '-o', OUT, SRC, '-lm'])
     return OUT
 
 

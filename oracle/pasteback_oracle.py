@@ -4,13 +4,28 @@ numpy restatement of ``FaceRestoreHelper.align_warp_face`` and ``paste_faces_to_
 (/root/reference/facelib/utils/face_restoration_helper.py:319-349, 372-516) and of the cv2 primitives they call:
 ``warpAffine`` (bilinear u8 / f32 / f64, fixed-point coordinates), ``resize(INTER_LINEAR)`` (u8 and f64),
 ``erode`` with a rectangular kernel, ``getGaussianKernel`` and ``GaussianBlur`` (separable, BORDER_REFLECT_101) and
-``invertAffineTransform``.  ``paste_faces`` returns the canvas BEFORE the final ``astype(uint8)`` so the tests can compare
+``invertAffineTransform``.  The float64 resize and the blurs are cv2's fused multiply-adds, so they call the C restatement in
+oracle/c/oracle_kernels.c (built by oracle/build_c.py).  ``paste_faces`` returns the canvas BEFORE the final ``astype(uint8)`` so the tests can compare
 continuously.  tests/test_oracle_pasteback.py pins every primitive against cv2 and the whole step against
 tests/golden/pasteback.npz, written from the UNMODIFIED reference by oracle/gen_golden_pasteback.py.
 """
+import ctypes
+import functools
+
 import numpy as np
 
 BORDER_CONSTANT, BORDER_REFLECT, BORDER_REFLECT101 = 0, 2, 4
+
+
+@functools.lru_cache(None)
+def _clib():
+    """The C restatements (oracle/build_c.py): numpy has no fused multiply-add, and cv2's filters use it."""
+    from oracle import build_c
+    return build_c.load()
+
+
+def _ptr(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
 MASK_COLORMAP = np.array([0, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 0, 255, 0, 0, 0], np.uint8)
 
 
@@ -42,7 +57,8 @@ def border_index(p, n, mode):
 
 
 def warp_coords(M, dsize):
-    """Fixed-point source coordinates of cv2.warpAffine (no WARP_INVERSE_MAP): integer part and 1/32 fraction."""
+    """Fixed-point source coordinates of cv2.warpAffine (no WARP_INVERSE_MAP): integer part and 1/32 fraction.  cv2 stores
+    the integer part as int16 (saturate_cast<short>), which a near-singular matrix reaches; the fraction keeps its bits."""
     dw, dh = dsize
     A = invert_affine(M)
     x = np.arange(dw, dtype=np.float64)
@@ -53,7 +69,7 @@ def warp_coords(M, dsize):
     Y0 = np.rint((A[1, 1] * y + A[1, 2]) * 1024).astype(np.int64) + 16
     X = (X0[:, None] + adelta[None, :]) >> 5
     Y = (Y0[:, None] + bdelta[None, :]) >> 5
-    return X >> 5, Y >> 5, X & 31, Y & 31
+    return np.clip(X >> 5, -32768, 32767), np.clip(Y >> 5, -32768, 32767), X & 31, Y & 31
 
 
 def _gather(src, ys, xs, mode, cval):
@@ -129,22 +145,16 @@ def resize_linear_u8(src, dsize):
 
 
 def resize_linear_f64(src, dsize):
-    """cv2.resize(src f64 2-D, dsize, INTER_LINEAR): float32 weights, double sums, same clamping as the u8 path."""
+    """cv2.resize(src f64 2-D, dsize, INTER_LINEAR), both sides >= 2: double coordinates and lerp FMAs (resize_linear_f64_ref
+    in oracle/c/oracle_kernels.c)."""
     dw, dh = dsize
     h, w = src.shape
     if (dw, dh) == (w, h):
         return src.copy()
-    sx, fx = _linear_taps(dw, w, np.float32)
-    lo, hi = sx < 0, sx >= w - 1
-    fx = np.where(lo | hi, np.float32(0), fx)
-    sx = np.where(lo, 0, np.where(hi, w - 1, sx))
-    a0 = (np.float32(1) - fx).astype(np.float64)
-    a1 = fx.astype(np.float64)
-    row = np.where(hi[None, :], src[:, sx], src[:, sx] * a0[None, :] + src[:, np.minimum(sx + 1, w - 1)] * a1[None, :])
-    sy, fy = _linear_taps(dh, h, np.float32)
-    b0 = (np.float32(1) - fy).astype(np.float64)
-    b1 = fy.astype(np.float64)
-    return row[np.clip(sy, 0, h - 1)] * b0[:, None] + row[np.clip(sy + 1, 0, h - 1)] * b1[:, None]
+    src = np.ascontiguousarray(src, np.float64)
+    out = np.empty((dh, dw), np.float64)
+    _clib().resize_linear_f64_ref(_ptr(src), h, w, _ptr(out), dh, dw)
+    return out
 
 
 def erode_rect(src, k):
@@ -172,10 +182,32 @@ _SMALL_GAUSS = {1: [1.0], 3: [0.25, 0.5, 0.25], 5: [0.0625, 0.25, 0.375, 0.25, 0
                 9: [0.015625, 0.05078125, 0.1171875, 0.19921875, 0.234375, 0.19921875, 0.1171875, 0.05078125, 0.015625]}
 
 
+# cv2.getGaussianKernel(101, 11, CV_64F), taps 0 .. 50 (the rest mirror them): cv2 exponentiates in its software double,
+# whose last bit numpy's exp does not always reproduce.  The parse mask's blur uses it; csrc/pasteback.cu holds the same table.
+PARSE_KERNEL_HALF = [float.fromhex(v) for v in (
+    '0x1.3d9320997c25bp-20', '0x1.de17a7bf38417p-20', '0x1.64e8ed67fb58cp-19', '0x1.08402ac73792fp-18',
+    '0x1.8412e6ca94be9p-18', '0x1.1a9d258b611acp-17', '0x1.983ce6e2d8b48p-17', '0x1.246cb61c4022cp-16',
+    '0x1.9f7c2e4f210b2p-16', '0x1.24bcaeb80f233p-15', '0x1.991c4ec5d6f8ep-15', '0x1.1b85423e811abp-14',
+    '0x1.85bc1908d022ep-14', '0x1.09aa455fcb2a8p-13', '0x1.673421a12de51p-13', '0x1.e1add23bf2656p-13',
+    '0x1.404c85f10d7b6p-12', '0x1.a677dc2924522p-12', '0x1.1452178d2dfc5p-11', '0x1.667cb15ebc175p-11',
+    '0x1.cd4230959cfabp-11', '0x1.264dd24853bf3p-10', '0x1.7477bd22f281bp-10', '0x1.d382d89d4adafp-10',
+    '0x1.22fd1739f5a24p-9', '0x1.6740df70cfe47p-9', '0x1.b7e1e31cfeb7cp-9', '0x1.0b165029af448p-8',
+    '0x1.41ab7619e5c97p-8', '0x1.8037efebc0c46p-8', '0x1.c727155fbb708p-8', '0x1.0b5f5ae5abc27p-7',
+    '0x1.378ad7eba8e32p-7', '0x1.680578de9fdf6p-7', '0x1.9c9eb782d6717p-7', '0x1.d502d0b5254c3p-7',
+    '0x1.085c4a7f64ae8p-6', '0x1.27904729ecf7bp-6', '0x1.47bada6c7b599p-6', '0x1.6867edea4945bp-6',
+    '0x1.8913f51fae714p-6', '0x1.a92eec6952cc7p-6', '0x1.c82029c32f07fp-6', '0x1.e54ae009f9925p-6',
+    '0x1.0009941ac006fp-5', '0x1.0bf1ac50126f9p-5', '0x1.1618b501c3bf9p-5', '0x1.1e421299af7d2p-5',
+    '0x1.243bea305ece7p-5', '0x1.27e11b8751b9cp-5', '0x1.291ac05d51e68p-5',
+)]
+
+
 def gaussian_kernel(n, sigma, dtype):
-    """cv2.getGaussianKernel(n, sigma, CV_32F / CV_64F)."""
+    """cv2.getGaussianKernel(n, sigma, CV_32F / CV_64F); the float64 kernel is exact for the parse mask's (101, 11) and within an
+    ulp otherwise."""
     if sigma <= 0 and n in _SMALL_GAUSS:
         return np.array(_SMALL_GAUSS[n], dtype)
+    if (n, sigma) == (101, 11) and np.dtype(dtype) == np.float64:
+        return np.array(PARSE_KERNEL_HALF + PARSE_KERNEL_HALF[-2::-1], np.float64)
     sig = sigma if sigma > 0 else n * 0.15 + 0.35
     scale2 = -0.125 / (sig * sig)
     n2 = (n - 1) // 2
@@ -191,21 +223,14 @@ def gaussian_kernel(n, sigma, dtype):
 
 
 def blur_reflect101(src, kern):
-    """sepFilter2D(src, kern, kern, BORDER_REFLECT_101) in src's dtype: row pass, then column pass, taps summed in order."""
-    k = len(kern)
-    r = k // 2
-    h, w = src.shape
-    dt = src.dtype
-    xs = border_index(np.arange(-r, w + r), w, BORDER_REFLECT101)
-    p = src[:, xs]
-    row = p[:, 0:w] * kern[0]
-    for j in range(1, k):
-        row = (row + p[:, j:j + w] * kern[j]).astype(dt)
-    ys = border_index(np.arange(-r, h + r), h, BORDER_REFLECT101)
-    p = row[ys]
-    out = p[0:h] * kern[0]
-    for i in range(1, k):
-        out = (out + p[i:i + h] * kern[i]).astype(dt)
+    """cv2.GaussianBlur(src, (n, n), ...) = sepFilter2D(src, kern, kern, BORDER_REFLECT_101) in src's dtype (float32 or
+    float64), both sides >= 2: cv2 4.13's x86-64 AVX2 arithmetic, restated in C with its fused multiply-adds
+    (gauss_blur_f32_ref / gauss_blur_f64_ref in oracle/c/oracle_kernels.c)."""
+    src = np.ascontiguousarray(src)
+    kern = np.ascontiguousarray(kern, src.dtype)
+    fn = {np.dtype(np.float32): 'gauss_blur_f32_ref', np.dtype(np.float64): 'gauss_blur_f64_ref'}[src.dtype]
+    out, tmp = np.empty_like(src), np.empty_like(src)
+    getattr(_clib(), fn)(_ptr(src), _ptr(out), _ptr(tmp), src.shape[0], src.shape[1], _ptr(kern), len(kern))
     return out
 
 
