@@ -342,6 +342,20 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// the same with an L2 cache policy (createpolicy): the weight slices every CTA of a conv streams stay resident in L2 while the
+// activations stream through it
+__device__ __forceinline__ void tma_load_3d_hint(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
+                                                 uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ uint64_t l2_evict_last_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
 // One leader lane of a fully converged warp (same lane every time).  Keeping the role warps converged and predicating
 // only the issue instructions lets ptxas hold descriptors / addresses in uniform registers.
 __device__ __forceinline__ bool elect_one() {
@@ -597,10 +611,41 @@ struct TcParams {
 #endif
 };
 // phase stamps of CTA 0: one lane per role writes the SM cycle counter
+// Wait counters of the 128 x 128 tiles (same build option): every CTA adds the cycles its roles spend in each wait to
+// dbg[TC_CNT0 + blockIdx.x * TC_NCNT + k], summed over the warps of the role (lane 0 of each warp adds):
+//   MMA warpgroups  0 weight `full`, 1 patch `afull`, 2 `cempty` before the tile hand-off, 3 whole role
+//   epilogue warps  4 `cfull`, 5 residual / SFT loads (issue until the last value of the batch has arrived), 6 stores
+//                   (output, operand planes, GroupNorm partials), 7 whole role
+// TC_T0 / TC_ADD expand to nothing in production builds.
 #if CFB_TC_STAMPS
+constexpr int TC_CNT0 = 32, TC_NCNT = 8;
 #define TC_STAMP(i) do { if (p.dbg != nullptr && blockIdx.x == 0) p.dbg[i] = clock64(); } while (0)
+#define TC_T0(t) const long long t = clock64()
+#define TC_ADD(k, t) do { if (WIDE && p.dbg != nullptr && lane == 0) \
+    atomicAdd(reinterpret_cast<unsigned long long*>(p.dbg + TC_CNT0 + blockIdx.x * TC_NCNT + (k)), \
+              (unsigned long long)(clock64() - (t))); } while (0)
 #else
 #define TC_STAMP(i) do { } while (0)
+#define TC_T0(t) do { } while (0)
+#define TC_ADD(k, t) do { } while (0)
+#endif
+// the same with a running sum in a register, added to counter k once per tile (TC_FLUSH)
+#if CFB_TC_STAMPS
+#define TC_VAR(v) long long v = 0
+#define TC_SUM(v, t) v += clock64() - (t)
+#define TC_FLUSH(k, v) do { if (WIDE && p.dbg != nullptr && lane == 0) \
+    atomicAdd(reinterpret_cast<unsigned long long*>(p.dbg + TC_CNT0 + blockIdx.x * TC_NCNT + (k)), (unsigned long long)(v)); \
+    v = 0; } while (0)
+#else
+#define TC_VAR(v) do { } while (0)
+#define TC_SUM(v, t) do { } while (0)
+#define TC_FLUSH(k, v) do { } while (0)
+#endif
+#if CFB_TC_STAMPS
+// diagnostics: a warp vote that reads `v`, so a clock read after it is taken once the load of `v` has completed
+__device__ __forceinline__ void tc_arrived(float v) {
+  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.eq.f32 p, %0, 0f00000000;\n\tvote.sync.any.pred q, p, 0xffffffff;\n\t}" ::"f"(v));
+}
 #endif
 
 // XF (fused operand transform): the warps after the epilogue warps transform the A patches, the warp after them loads the raw
@@ -647,6 +692,7 @@ struct TcCfg {
   static constexpr int H_A_SLOTS = 2;
   static constexpr int H_B_SLOT = 2 * B_BYTES;
   static constexpr int H_B_SLOTS = WIDE ? 2 : 4;           // 2 x 32 KB: a refill has one k-block (1536 MMA clocks) to land
+                                                           // (single pass: 4 x 16 KB hi-only slots in the same memory)
   static constexpr int H_SMEM_BYTES = H_A_SLOTS * H_A_SLOT + H_B_SLOTS * H_B_SLOT + TAIL_BYTES;
   // fused operand transform (XF, halo engine only): the A patches arrive as the RAW fp32 activation (two 32-channel planes per
   // slot) and the transform warps apply GroupNorm-affine + SiLU + the hi/lo split in place before the MMAs read them
@@ -700,8 +746,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   // ring "full/empty": per-tap engine = STAGES k-block stages; halo engine = weight (B) slots.  "afull/aempty": halo A slots.
-  constexpr int NRING = HALO ? (XF ? Cfg::X_B_SLOTS : Cfg::H_B_SLOTS) : STAGES;
-  constexpr int RING_BYTES = HALO ? Cfg::H_B_SLOT : STAGE_BYTES;
+  // single-pass 128-wide tiles load only the hi weight plane: the same ring memory holds twice as many slots of half the size,
+  // so a refill has two k-blocks of MMA time to land instead of one (their MMAs waited on `full` for 29-44 % of their cycles
+  // with the 2-slot ring, tools/epilogue_waits.py)
+  constexpr bool HALF_B = HALO && WIDE && P1;
+  constexpr int NRING = HALO ? (XF ? Cfg::X_B_SLOTS : Cfg::H_B_SLOTS) * (HALF_B ? 2 : 1) : STAGES;
+  constexpr int RING_BYTES = HALO ? (HALF_B ? Cfg::B_BYTES : Cfg::H_B_SLOT) : STAGE_BYTES;
   uint8_t* ring_base = HALO ? smem + A_SLOTS * Cfg::H_A_SLOT : smem;
   float* acc_slot = reinterpret_cast<float*>(ring_base + NRING * RING_BYTES);       // partial sums, [128][SLOT_PITCH]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring_base + NRING * RING_BYTES + Cfg::SLOT_BYTES);
@@ -799,8 +849,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 const uint32_t fb = smem_u32(full + stage);
                 const bool drop = p.fault && blockIdx.x == 0 && tile == first_tile && kb == 0 && tap == 0;   // injected fault
                 mbar_expect_tx(fb, (uint32_t)(P1 ? Cfg::B_BYTES : Cfg::H_B_SLOT));
-                if (!drop) tma_load_3d(sb, &tmB_hi, fb, kb * 64, nt * BN, btap);
-                if constexpr (!P1) tma_load_3d(sb + Cfg::B_BYTES, &tmB_lo, fb, kb * 64, nt * BN, btap);
+                if constexpr (WIDE && !P1) {
+                  // split 128 x 128 tiles: their 2-slot ring gives a refill one k-block to land, and their MMAs waited on
+                  // `full` for 32-56 % of their cycles, most with a residual / SFT epilogue streaming activations through L2
+                  // (tools/epilogue_waits.py).  The weights every CTA of the conv reads are marked evict_last so that stream
+                  // does not push them out.  The single-pass tiles (4 slots) measured slower with the hint.
+                  const uint64_t pol = l2_evict_last_policy();
+                  if (!drop) tma_load_3d_hint(sb, &tmB_hi, fb, kb * 64, nt * BN, btap, pol);
+                  tma_load_3d_hint(sb + Cfg::B_BYTES, &tmB_lo, fb, kb * 64, nt * BN, btap, pol);
+                } else {
+                  if (!drop) tma_load_3d(sb, &tmB_hi, fb, kb * 64, nt * BN, btap);
+                  if constexpr (!P1) tma_load_3d(sb + Cfg::B_BYTES, &tmB_lo, fb, kb * 64, nt * BN, btap);
+                }
               }
               __syncwarp();
               if (++stage == NRING) { stage = 0; phase ^= 1; }
@@ -852,6 +912,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // CM: the same descriptor is the B operand and spans the whole 128-pixel tile: its 16 core-matrix groups are the 16 patch
     // rows, PW*128 B apart, and the second 64-row half starts a_half = 8 groups in.
     if constexpr (WIDE) wg_regs_inc<160>();
+    TC_T0(t_mma);
     {
       constexpr bool N128 = WIDE || CM;                 // m64n128k16 issue: one accumulator of 64 fp32 per thread
       constexpr int MH = N128 ? 1 : 2;                  // 64-row halves issued by this warpgroup
@@ -880,8 +941,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         float run[64];                                               // BN = 128 only (CM never touches it)
         // run -> slot [row][SLOT_PITCH] -> epilogue warps; true when the wait for the slot was abandoned (abort)
         auto hand_off = [&]() -> bool {
+          TC_T0(t_h);
           mbar_wait(smem_u32(cempty + slot), slot_phase ^ 1, aborted);
           if (wg_any(aborted, bar_id)) return true;
+          TC_ADD(2, t_h);
           const int row = wg * 64 + wq * 16 + (lane >> 2);
           // this thread's first slot element, formed anew per hand-off (opaque move): otherwise the compiler keeps the 32
           // store addresses live across the tile loop and spills them; this way they are immediate offsets of one register
@@ -912,8 +975,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               const int kb = it / p.taps;
               const int tap = it - kb * p.taps;
               if (tap == 0) {
+                TC_T0(t_a);
                 mbar_wait(smem_u32(afull + aslot), aphase, aborted);
                 if (wg_any(aborted, bar_id)) { wg_wait_all(); aborted = true; goto teardown; }
+                TC_ADD(1, t_a);
               }
               int r = (p.taps == 9) ? tap / 3 : 0;
               int sft = (p.taps == 9) ? tap - r * 3 : 0;
@@ -922,8 +987,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                                      (uint32_t)wg * a_half;
               const uint32_t a_lo0 = a_hi0 + (uint32_t)(XF ? Cfg::X_A_PLANE2 : Cfg::H_A_PLANE);
               const uint32_t bsm = smem_u32(ring_base + stage * RING_BYTES);
+              TC_T0(t_b);
               mbar_wait(smem_u32(full + stage), phase, aborted);
               if (wg_any(aborted, bar_id)) { wg_wait_all(); aborted = true; goto teardown; }
+              TC_ADD(0, t_b);
               wg_fence();
 #pragma unroll
               for (int k = 0; k < 4; ++k) {
@@ -994,6 +1061,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
         if constexpr (WIDE) {
           if (first_tile < total_tiles && hand_off()) { aborted = true; goto teardown; }      // the last tile
+          TC_ADD(3, t_mma);
         }
       } else {
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
@@ -1235,6 +1303,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     int slot = 0;
     uint32_t slot_phase = 0;
     float omax = 0.f;                        // largest magnitude emitted into fp16 operand planes (range guard)
+    TC_T0(t_epi);
+    TC_VAR(c_ld);
+    TC_VAR(c_st);
     for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
       const int pm = tile / p.n_tiles, nt = tile - pm * p.n_tiles;
       const int mt = pm;
@@ -1271,7 +1342,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       float acc[WIDE ? 1 : HC];
       if constexpr (WIDE) {
         // the MMA warpgroups have stored the finished tile (every partial sum folded) into the slot; the store loop reads it
+        TC_T0(t_c);
         mbar_wait<250>(smem_u32(cfull + slot), slot_phase, aborted); if (aborted) goto teardown;
+        TC_ADD(4, t_c);
       } else {
 #pragma unroll
         for (int j = 0; j < HC; ++j) acc[j] = 0.f;
@@ -1391,10 +1464,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           offs[k] = off_tile + colq + hh * SH + ww * SW;
           inside[k] = whole_tiles || ((ty * BH + hh) * ts < p.Ho && (tx * BW + ww) * ts < p.Wo);
         }
+        TC_T0(t_l);
         float4 rres[RB];
 #pragma unroll
         for (int k = 0; k < RB; ++k)
           rres[k] = (p.residual && inside[k]) ? __ldg(reinterpret_cast<const float4*>(p.residual + offs[k])) : make_float4(0.f, 0.f, 0.f, 0.f);
+#if CFB_TC_STAMPS
+        if (WIDE && p.residual) { tc_arrived(rres[RB - 1].w); TC_SUM(c_ld, t_l); }
+#endif
 #pragma unroll
         for (int k = 0; k < RB; ++k) {
           const int it = ib + k;
@@ -1425,14 +1502,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             v.x = tc_silu_out(v.x); v.y = tc_silu_out(v.y); v.z = tc_silu_out(v.z); v.w = tc_silu_out(v.w);
           }
           if (p.sft_dec && inside[k]) {
+            TC_T0(t_s);
             const float4 d = __ldg(reinterpret_cast<const float4*>(p.sft_dec + off));
             const float4 sc = __ldg(reinterpret_cast<const float4*>(p.sft_scale + off));
+#if CFB_TC_STAMPS
+            if (WIDE) { tc_arrived(d.w); tc_arrived(sc.w); TC_SUM(c_ld, t_s); }
+#endif
             float sw = p.sft_w;     // per image (a tile never spans two): max(w, 0), so w <= 0 or NaN leaves dec unchanged
             if constexpr (!XF) { if (p.sft_wv) { const float t = __ldg(p.sft_wv + n); sw = t > 0.f ? t : 0.f; } }
             v.x = d.x + sw * (d.x * sc.x + v.x); v.y = d.y + sw * (d.y * sc.y + v.y);
             v.z = d.z + sw * (d.z * sc.z + v.z); v.w = d.w + sw * (d.w * sc.w + v.w);
           }
           if (!inside[k]) v = make_float4(0.f, 0.f, 0.f, 0.f);          // outside the image: no store, no statistics
+          TC_T0(t_st);
           if (p.out && inside[k]) *reinterpret_cast<float4*>(p.out + off) = v;      // null: only the operand planes are consumed
           if (p.pl_hi && inside[k]) {
             omax = fmaxf(omax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
@@ -1445,6 +1527,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             *reinterpret_cast<uint2*>(p.pl_hi + off) = ph;
             *reinterpret_cast<uint2*>(p.pl_lo + off) = pl;
           }
+          TC_SUM(c_st, t_st);
           if constexpr (CPG == 2) {
             if (it == 0) { k0 = v.x; k1 = v.z; }
             const float a = v.x - k0, b = v.y - k0, c = v.z - k1, d = v.w - k1;
@@ -1470,6 +1553,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           if constexpr (CPG >= 8) gn_merge_xor(s0, q0, 1, 4.f * NL);
           if constexpr (CPG >= 16) gn_merge_xor(s0, q0, 2, 8.f * NL);
           constexpr int CL = (CPG >= 4) ? CPG / 4 : 1;         // chunk-lanes per group
+          TC_T0(t_gs);
           if (rsub == 0 && (cch & (CL - 1)) == 0) {
             float* gp = p.gn_part + ((int64_t)mt * 4 + lg) * 64;
             if constexpr (CPG == 2) {
@@ -1478,6 +1562,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
               *reinterpret_cast<float2*>(gp + (colq / CPG) * 2) = make_float2(s0, q0);
             }
           }
+          TC_SUM(c_st, t_gs);
         }
         __syncwarp();
       }
@@ -1485,11 +1570,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       if constexpr (WIDE) {          // every read of the tile slot is done: the MMA warpgroups may store the next tile
         if (lane == 0) mbar_arrive(smem_u32(cempty + slot));
         if (++slot == Cfg::SLOTS) { slot = 0; slot_phase ^= 1; }
+        TC_FLUSH(5, c_ld);
+        TC_FLUSH(6, c_st);
       }
       if (warp == 2 && lane == 0 && tile == first_tile) TC_STAMP(16);
       if (warp == 2 && lane == 0 && tile == first_tile + tile_step) TC_STAMP(18);
     }
     if (omax > 65504.f) report_overflow();   // a value left the fp16 range of the operand planes: reported, never silent
+    TC_ADD(7, t_epi);
     if (warp == 2 && lane == 0) TC_STAMP(13);
   }
 

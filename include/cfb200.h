@@ -552,8 +552,11 @@ int cfb_debug_inject_fault(int32_t kind);
 /* diagnostics: while `stamps` (device memory, >= 32 int64) is non-NULL, CTA 0 of every wgmma conv launch
  * writes the SM cycle counter at its role hand-offs ([0] entry, [1] set-up done, [2] first TMA, [3] first MMA, [4] last MMA
  * issued, [5]/[6] first/last accumulator seen by the epilogue, [7] epilogue K loop done, [13] epilogue done, [8]/[9] tear-down,
- * [10..12] transform roles, [14]/[15] %globaltimer at entry / exit).  NULL switches it off.  The stamps exist only in builds of the
- * library with -DCFB_TC_STAMPS=1 (they slow every conv kernel); the production build accepts the call and ignores it. */
+ * [10..12] transform roles, [14]/[15] %globaltimer at entry / exit), and every CTA of a 128x128-tile conv adds the cycles its
+ * roles wait to stamps[32 + 8 * cta + k] (k: MMA weight / patch / tile hand-off waits and whole role, epilogue cfull wait,
+ * residual/SFT loads, stores and whole role; zero them first; the buffer then needs 32 + 8 * grid int64).  NULL switches it
+ * off.  The stamps exist only in builds of the library with -DCFB_TC_STAMPS=1 (they slow every conv kernel); the production
+ * build accepts the call and ignores it. */
 int cfb_debug_set_stamps(int64_t* stamps);
 /* layout plumbing */
 int cfb_nchw_to_nhwc(const float* in, float* out, int32_t n, int32_t c, int32_t hw, void* stream);
