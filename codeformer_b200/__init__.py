@@ -19,6 +19,7 @@ from .wholeimage import restore_images, restore_images_sweep, restore_aligned   
 from .arcface import ResNetArcFace, identity_similarity   # noqa: F401
 from .metrics import calculate_psnr, calculate_ssim, psnr_ssim   # noqa: F401
 from .lpips import LPIPS, LPIPSLoss, lpips_distance   # noqa: F401
+from .degradation import degrade_faces, sample_degradations, jpeg_roundtrip   # noqa: F401
 
 
 def check_async_status():
@@ -34,4 +35,5 @@ __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQua
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
            'ResNetArcFace', 'identity_similarity', 'calculate_psnr', 'calculate_ssim', 'psnr_ssim', 'LPIPS', 'LPIPSLoss', 'lpips_distance',
+           'degrade_faces', 'sample_degradations', 'jpeg_roundtrip',
            'check_async_status']

@@ -166,6 +166,11 @@ SIGNATURES = {
     'cfb_debug_lpips_head': (c_int, [_P, _P, _P, _P] + [c_int32] * 5 + [_P, c_int64, _P]),
     'cfb_psnr_ssim_workspace_bytes': (c_int64, [c_int32] * 6),
     'cfb_psnr_ssim': (c_int, [_P, _P] + [c_int32] * 10 + [_P, _P, _P, c_int64, _P]),
+    'cfb_degrade_workspace_bytes': (c_int64, [c_int32, c_int32, _P, _P]),
+    'cfb_degrade_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, c_int32, _P, _P, c_int64, _P]),
+    'cfb_debug_degrade_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, c_int32, _P, _P, c_int64, _P, _P, _P]),
+    'cfb_jpeg_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32]),
+    'cfb_jpeg_roundtrip': (c_int, [_P, _P, c_int32, c_int32, c_int32, _P, _P, c_int64, _P]),
     'cfb_check_async_status': (c_int, []),
     'cfb_debug_set_wait_limit': (c_int, [c_int64]),
     'cfb_debug_inject_fault': (c_int, [c_int32]),

@@ -538,6 +538,31 @@ int     cfb_psnr_ssim(const void* a, const void* b, int32_t dtype, int32_t pairs
                       int32_t crop_border, int32_t y_channel, int32_t want_psnr, int32_t want_ssim, double* psnr_out,
                       double* ssim_out, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- Synthetic degradations: FFHQBlindDataset's blur -> downsample -> noise -> JPEG -> resize chain on the device ----
+ * (basicsr/data/ffhq_blind_dataset.py:210-240) for gt uint8 BGR faces [batch, gt_size, gt_size, 3], one launch per stage.
+ * Per face b: kernels [batch, ksize, ksize] float64 (device; odd ksize <= 63) correlated with BORDER_REFLECT_101 in float64
+ * and rounded once to float32, only where the downsample reads; small_sizes[b] (host, 1..gt_size) the INTER_LINEAR
+ * downsample (cv2's float arithmetic); noise_offsets[b] (host; -1 = none) the float offset of its [s, s, 3] field in the
+ * packed device array noise, added before the clip to [0, 1]; qualities[b] (host; 0 = none, else 1..100) the cv2 JPEG
+ * round trip (libjpeg-turbo baseline 4:2:0, islow) of saturate_cast<uchar>(x * 255); then / 255, INTER_LINEAR to in_size
+ * (<= gt_size) and clip(round(x * 255)) -> lq uint8 BGR [batch, in_size, in_size, 3].  Workspace:
+ * cfb_degrade_workspace_bytes (-1 for bad arguments).
+ * debug_degrade_faces (test entry point): also stage_a float32, the image after the downsample, and pre_jpeg uint8, the JPEG
+ *   input (faces with a quality only), each packed as the faces' [s, s, 3] images one after another.
+ * jpeg_roundtrip: dst = cv2.imdecode(cv2.imencode('.jpg', src, [IMWRITE_JPEG_QUALITY, q]), 1) for n uint8 BGR images
+ *   [n, h, w, 3], qualities (host) 1..100 per image; src and dst must not alias.  Workspace: cfb_jpeg_workspace_bytes. */
+int64_t cfb_degrade_workspace_bytes(int32_t batch, int32_t gt_size, const int32_t* small_sizes, const int32_t* qualities);
+int     cfb_degrade_faces(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                          const int32_t* small_sizes, const int32_t* qualities, const float* noise, const int64_t* noise_offsets,
+                          int32_t in_size, uint8_t* lq, void* workspace, int64_t workspace_bytes, void* stream);
+int     cfb_debug_degrade_faces(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                                const int32_t* small_sizes, const int32_t* qualities, const float* noise,
+                                const int64_t* noise_offsets, int32_t in_size, uint8_t* lq, void* workspace,
+                                int64_t workspace_bytes, float* stage_a, uint8_t* pre_jpeg, void* stream);
+int64_t cfb_jpeg_workspace_bytes(int32_t n, int32_t h, int32_t w);
+int     cfb_jpeg_roundtrip(const uint8_t* src, uint8_t* dst, int32_t n, int32_t h, int32_t w, const int32_t* qualities,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Asynchronous failures.  Kernels never trap and never leave a sticky CUDA error behind (the reference's callers catch
  * RuntimeError and fall back to the input face, inference_codeformer.py:209-211; web-demos/hugging_face/app.py:176): a
  * barrier time-out of the tensor-core pipeline or an activation outside the fp16 operand range (|x| > 65504) sets a bit
