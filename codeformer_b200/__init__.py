@@ -20,6 +20,8 @@ from .arcface import ResNetArcFace, identity_similarity   # noqa: F401
 from .metrics import calculate_psnr, calculate_ssim, psnr_ssim   # noqa: F401
 from .lpips import LPIPS, LPIPSLoss, lpips_distance   # noqa: F401
 from .degradation import degrade_faces, sample_degradations, jpeg_roundtrip   # noqa: F401
+from .fid import (InceptionV3, inception_features, fid_statistics, frechet_distance, calculate_fid,   # noqa: F401
+                  fid_scores)
 
 
 def check_async_status():
@@ -35,5 +37,6 @@ __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQua
            'YOLOv5lFace', 'YoloDetector', 'resize_area', 'warp_faces_multi', 'paste_faces_multi', 'restore_images',
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
            'ResNetArcFace', 'identity_similarity', 'calculate_psnr', 'calculate_ssim', 'psnr_ssim', 'LPIPS', 'LPIPSLoss', 'lpips_distance',
-           'degrade_faces', 'sample_degradations', 'jpeg_roundtrip',
+           'degrade_faces', 'sample_degradations', 'jpeg_roundtrip', 'InceptionV3', 'inception_features', 'fid_statistics',
+           'frechet_distance', 'calculate_fid', 'fid_scores',
            'check_async_status']

@@ -164,6 +164,18 @@ SIGNATURES = {
     'cfb_debug_lpips_stem': (c_int, [_P, _P, _P, c_int32, c_int32, _P, c_int32, c_int32, c_int32, c_int32, _P]),
     'cfb_debug_lpips_head_workspace_bytes': (c_int64, [c_int32] * 4),
     'cfb_debug_lpips_head': (c_int, [_P, _P, _P, _P] + [c_int32] * 5 + [_P, c_int64, _P]),
+    'cfb_fid_create': (c_void_p, []),
+    'cfb_fid_destroy': (None, [_P]),
+    'cfb_fid_set_param': (c_int, [_P, c_char_p, _P, c_int64]),
+    'cfb_fid_prepare': (c_int, [_P, _P]),
+    'cfb_fid_workspace_bytes': (c_int64, [_P] + [c_int32] * 4),
+    'cfb_fid_forward': (c_int, [_P, _P] + [c_int32] * 5 + [_P, _P, c_int64, _P]),
+    'cfb_fid_forward_u8': (c_int, [_P, _P] + [c_int32] * 3 + [_P, _P, c_int64, _P]),
+    'cfb_fid_input': (c_int, [_P] + [c_int32] * 6 + [_P, _P]),
+    'cfb_fid_stats': (c_int, [_P, c_int64, c_int32, _P, _P, _P]),
+    'cfb_debug_fid_pool': (c_int, [_P, _P] + [c_int32] * 5 + [_P]),
+    'cfb_conv2d_pertap_window_workspace_bytes': (c_int64, [c_int32] * 10),
+    'cfb_conv2d_pertap_window_nhwc': (c_int, [_P, _P, _P, _P] + [c_int32] * 13 + [_P, c_int64, _P]),
     'cfb_psnr_ssim_workspace_bytes': (c_int64, [c_int32] * 6),
     'cfb_psnr_ssim': (c_int, [_P, _P] + [c_int32] * 10 + [_P, _P, _P, c_int64, _P]),
     'cfb_degrade_workspace_bytes': (c_int64, [c_int32, c_int32, _P, _P]),

@@ -60,17 +60,17 @@ __global__ void tc_absmax_kernel(const float* __restrict__ w, int64_t total, uns
 }
 
 __global__ void tc_split_weights_kernel(const float* __restrict__ w, __half* __restrict__ hi, __half* __restrict__ lo,
-                                        int Cout, int Cin, int k, float* __restrict__ slot) {
+                                        int Cout, int Cin, int taps, float* __restrict__ slot) {
   const float amax = __uint_as_float(reinterpret_cast<const unsigned*>(slot)[0]);
   int e = 0;
   if (amax > 0.f && isfinite(amax)) frexpf(amax, &e);
   const float scale = exp2f((float)(14 - e));
-  const int64_t total = (int64_t)Cout * Cin * k * k;
+  const int64_t total = (int64_t)Cout * Cin * taps;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int ci = (int)(i % Cin);
     const int co = (int)((i / Cin) % Cout);
     const int tap = (int)(i / ((int64_t)Cout * Cin));
-    const float v = w[((int64_t)co * Cin + ci) * k * k + tap] * scale;
+    const float v = w[((int64_t)co * Cin + ci) * taps + tap] * scale;
     const __half h = __float2half_rn(v);
     hi[i] = h;
     lo[i] = __float2half_rn(v - __half2float(h));
@@ -80,13 +80,18 @@ __global__ void tc_split_weights_kernel(const float* __restrict__ w, __half* __r
 
 int tc_split_weights(const float* oihw, __half* hi, __half* lo, int Cout, int Cin, int k, float* scale_slot,
                      cudaStream_t st) {
-  const int64_t total = (int64_t)Cout * Cin * k * k;
+  return tc_split_weights_taps(oihw, hi, lo, Cout, Cin, k * k, scale_slot, st);
+}
+
+int tc_split_weights_taps(const float* oihw, __half* hi, __half* lo, int Cout, int Cin, int taps, float* scale_slot,
+                          cudaStream_t st) {
+  const int64_t total = (int64_t)Cout * Cin * taps;
   const int64_t blocks = (total + 255) / 256;
   const unsigned g = (unsigned)(blocks > 1024 ? 1024 : blocks);
   CFB_CUDA(cudaMemsetAsync(scale_slot, 0, 2 * sizeof(float), st));
   tc_absmax_kernel<<<g, 256, 0, st>>>(oihw, total, reinterpret_cast<unsigned*>(scale_slot));
   CFB_LAUNCH_CHECK();
-  tc_split_weights_kernel<<<g, 256, 0, st>>>(oihw, hi, lo, Cout, Cin, k, scale_slot);
+  tc_split_weights_kernel<<<g, 256, 0, st>>>(oihw, hi, lo, Cout, Cin, taps, scale_slot);
   CFB_LAUNCH_CHECK();
   return 0;
 }
@@ -208,6 +213,30 @@ __global__ void __launch_bounds__(256) tc_prep_kernel(const float* __restrict__ 
     *reinterpret_cast<uint4*>(lo + pix * C + c) = *reinterpret_cast<const uint4*>(ll);
   }
   if (vmax > 65504.f) report_overflow();       // fp16 operand range guard: reported through the status word, never silent
+}
+
+// The raw split of activations whose channel count is a multiple of 64 but not 64 * 2^k (Inception-v3's 192, 320, 448, 768,
+// 1280): one thread per 8 channels of a pixel, the same values as tc_prep_kernel without an affine.
+__global__ void __launch_bounds__(256) tc_prep_raw_kernel(const float* __restrict__ in, int64_t items, __half* __restrict__ hi,
+                                                          __half* __restrict__ lo) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  float vmax = 0.f;
+  if (i < items) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(in + i * 8));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(in + i * 8 + 4));
+    const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    __align__(16) __half hh[8];
+    __align__(16) __half ll[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      vmax = fmaxf(vmax, fabsf(v[j]));
+      hh[j] = __float2half_rn(v[j]);
+      ll[j] = __float2half_rn(v[j] - __half2float(hh[j]));
+    }
+    *reinterpret_cast<uint4*>(hi + i * 8) = *reinterpret_cast<const uint4*>(hh);
+    *reinterpret_cast<uint4*>(lo + i * 8) = *reinterpret_cast<const uint4*>(ll);
+  }
+  if (vmax > 65504.f) report_overflow();
 }
 
 // torch.cat([enc_feat, dec], dim=1) of Fuse_sft_block (codeformer_arch.py:152) written directly as RAW fp16 hi/lo operand
@@ -558,6 +587,7 @@ __device__ __forceinline__ void xf_patch(uint32_t src_base, uint32_t hi_base, ui
 struct TcParams {
   int N, Ho, Wo, Cout;
   int taps, pad, stride;  // 9/1/1 (3x3 'same'), 1/0/1 (1x1), 9/0/2 (Downsample: pad right/bottom = TMA OOB zero fill)
+  int kw, pad_w;          // per-tap engine: taps per kernel row and the left padding (pad = the top padding); square: 3|1, pad
   int BW, BH;             // pixel tile = BH rows x BW cols = 128
   int tiles_x, tiles_y;   // per image
   int m_tiles, n_tiles;
@@ -871,7 +901,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             // source offset of this tap and its weight slice: 3x3 -> (r,s)-pad; 2x2 parity conv -> (dy+py-1, dx+px-1)
             int r, s, btap = tap;
             if (p.up4) { r = (tap >> 1) + par_y; s = (tap & 1) + par_x; btap = (mt & 3) * 4 + tap; }
-            else { r = (p.taps == 9) ? tap / 3 : 0; s = (p.taps == 9) ? tap - r * 3 : 0; }
+            else { r = tap / p.kw; s = tap - r * p.kw; }          // kh x kw window, row-major taps (OIHW order)
             for (int kb = 0; kb < p.kblocks; ++kb) {
               mbar_wait<500>(smem_u32(empty + stage), phase ^ 1, aborted); if (aborted) goto teardown;
               if (elect_one()) {
@@ -886,8 +916,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                 const uint32_t fb = smem_u32(full + stage);
                 const bool drop = p.fault && blockIdx.x == 0 && tile == first_tile && kb == 0 && tap == 0;   // injected fault
                 mbar_expect_tx(fb, (uint32_t)(P1 ? TC_A_BYTES + Cfg::B_BYTES : Cfg::STAGE_BYTES));
-                tma_load_4d(sa, &tmA_hi, fb, ac, x0 + s - p.pad, y0 + r - p.pad, a_img);
-                if constexpr (!P1) tma_load_4d(sa + TC_A_BYTES, &tmA_lo, fb, ac, x0 + s - p.pad, y0 + r - p.pad, a_img);
+                tma_load_4d(sa, &tmA_hi, fb, ac, x0 + s - p.pad_w, y0 + r - p.pad, a_img);
+                if constexpr (!P1) tma_load_4d(sa + TC_A_BYTES, &tmA_lo, fb, ac, x0 + s - p.pad_w, y0 + r - p.pad, a_img);
                 if (!drop) tma_load_3d(sa + 2 * TC_A_BYTES, &tmB_hi, fb, bc, brow, b3);
                 if constexpr (!P1) tma_load_3d(sa + 2 * TC_A_BYTES + Cfg::B_BYTES, &tmB_lo, fb, bc, brow, b3);
               }
@@ -1515,7 +1545,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           }
           if (!inside[k]) v = make_float4(0.f, 0.f, 0.f, 0.f);          // outside the image: no store, no statistics
           TC_T0(t_st);
-          if (p.out && inside[k]) *reinterpret_cast<float4*>(p.out + off) = v;      // null: only the operand planes are consumed
+          // per-tap engine: the zero-padded weight columns from cout_valid on are not stored (a channel slice of a concatenation)
+          const bool col_in = HALO || colq < p.cout_valid;
+          if (p.out && inside[k] && col_in) *reinterpret_cast<float4*>(p.out + off) = v;      // null: only the operand planes are consumed
           if (p.pl_hi && inside[k]) {
             omax = fmaxf(omax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
             const __half2 h01 = __floats2half2_rn(v.x, v.y), h23 = __floats2half2_rn(v.z, v.w);
@@ -1673,7 +1705,7 @@ struct TcGeom { int BW, BH; bool halo; };
 static TcGeom tc_geometry(const ConvArgs& a) {
   TcGeom g;
   const int Wt = a.mode == CONV_UP ? a.W : a.Wo, Ht = a.mode == CONV_UP ? a.H : a.Ho;   // grid the tiles live on
-  g.halo = halo_enabled() && (a.ksize == 3 || (a.ksize == 1 && a.halo1x1 && a.mode == CONV_SAME)) &&
+  g.halo = halo_enabled() && a.kh == 0 && (a.ksize == 3 || (a.ksize == 1 && a.halo1x1 && a.mode == CONV_SAME)) &&
            (a.mode == CONV_SAME || a.mode == CONV_UP) &&
            ((Wt % 8 == 0 && Ht % 16 == 0) || a.gen);      // gen: ragged tiles, stores are bounds-checked
   if (g.halo) { g.BW = 8; g.BH = 16; }
@@ -1687,11 +1719,29 @@ int tc_tiles_per_image(const ConvArgs& a) {
   return ((a.Wo + g.BW - 1) / g.BW) * ((a.Ho + g.BH - 1) / g.BH);
 }
 
+// the window of a conv: the explicit kh x kw form (ConvArgs::kh > 0) or the square ksize forms
+struct TcWin { int kh, kw, ph, pw, stride; };
+static TcWin tc_window(const ConvArgs& a) {
+  const int s = a.mode == CONV_DOWN ? 2 : 1;
+  if (a.kh > 0) return {a.kh, a.kw, a.pad_h, a.pad_w, s};
+  const int p = a.mode == CONV_DOWN ? a.down_pad : a.ksize / 2;
+  return {a.ksize, a.ksize, p, p, s};
+}
+
 bool tc_supported(const ConvArgs& a) {
   if (a.Cin % 64 != 0 || a.Cout % 64 != 0) return false;
-  if (!(a.ksize == 1 || a.ksize == 3)) return false;
-  if (a.mode == CONV_DOWN && a.ksize != 3 && !(a.ksize == 1 && a.down_pad == 0 && a.Ho == (a.H + 1) / 2)) return false;
-  if (a.mode == CONV_DOWN && a.down_pad != 0 && !(a.down_pad == 1 && a.ksize == 3)) return false;
+  if (a.kh > 0) {
+    // explicit window: per-tap engine, raw input, stride 1 or 2, Ho = (H + 2 pad_h - kh) / stride + 1 (likewise Wo)
+    const int s = a.mode == CONV_DOWN ? 2 : 1;
+    if (a.gen || a.xform || a.mode == CONV_UP || a.kh > 7 || a.kw < 1 || a.kw > 7) return false;
+    if (a.pad_h < 0 || a.pad_w < 0 || a.pad_h >= a.kh || a.pad_w >= a.kw) return false;
+    if (a.H + 2 * a.pad_h < a.kh || a.W + 2 * a.pad_w < a.kw) return false;
+    if (a.Ho != (a.H + 2 * a.pad_h - a.kh) / s + 1 || a.Wo != (a.W + 2 * a.pad_w - a.kw) / s + 1) return false;
+  } else {
+    if (!(a.ksize == 1 || a.ksize == 3)) return false;
+    if (a.mode == CONV_DOWN && a.ksize != 3 && !(a.ksize == 1 && a.down_pad == 0 && a.Ho == (a.H + 1) / 2)) return false;
+    if (a.mode == CONV_DOWN && a.down_pad != 0 && !(a.down_pad == 1 && a.ksize == 3)) return false;
+  }
   if (a.Wo < 1 || a.Ho < 1) return false;
   const TcGeom g = tc_geometry(a);
   if (a.gen) return g.halo && a.ksize == 3;
@@ -1722,7 +1772,8 @@ bool tc_can_xform(const ConvArgs& a) {
 
 size_t tc_scratch_bytes(const ConvArgs& a) {
   if (!tc_supported(a)) return 0;
-  const int Hp = a.mode == CONV_SAME ? a.Ho : a.H, Wp = a.mode == CONV_SAME ? a.Wo : a.W;   // operand plane = input resolution
+  const bool same = a.mode == CONV_SAME && a.kh == 0;
+  const int Hp = same ? a.Ho : a.H, Wp = same ? a.Wo : a.W;   // operand plane = input resolution
   const size_t plane = ((size_t)a.N * Hp * Wp * a.Cin * 2 + 1023) / 1024 * 1024;
   return 2 * plane;
 }
@@ -1867,13 +1918,19 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   CFB_REQUIRE(a.wgt_hi && a.wgt_lo && a.wscale_inv, "conv_tc: split weights missing");
   const int64_t M = (int64_t)a.N * a.Ho * a.Wo;
   if (M == 0) return 0;
-  // ---- operand planes (fp16 hi/lo NHWC; at the output resolution, or the input resolution for Downsample)
-  const int Hp = a.mode == CONV_SAME ? a.Ho : a.H, Wp = a.mode == CONV_SAME ? a.Wo : a.W;
+  // ---- operand planes (fp16 hi/lo NHWC; at the output resolution, or the input resolution for Downsample / explicit windows)
+  const bool same = a.mode == CONV_SAME && a.kh == 0;
+  const int Hp = same ? a.Ho : a.H, Wp = same ? a.Wo : a.W;
   const int64_t Mp = (int64_t)a.N * Hp * Wp;
   const size_t plane = ((size_t)Mp * a.Cin * 2 + 1023) / 1024 * 1024;
   __half* hi = (__half*)scratch;
   __half* lo = (__half*)((char*)scratch + plane);
-  if (!a.skip_prep) {
+  if (!a.skip_prep && a.kh > 0 && (a.Cin / 8 > 256 || 256 % (a.Cin / 8) != 0)) {
+    CFB_REQUIRE(!a.in_scale && a.in_act == IN_NONE, "conv_tc: an input affine needs Cin = 64 * 2^k (<= 2048)");
+    const int64_t items = Mp * (a.Cin / 8);
+    tc_prep_raw_kernel<<<(unsigned)((items + 255) / 256), 256, 0, st>>>(a.in, items, hi, lo);
+    CFB_LAUNCH_CHECK();
+  } else if (!a.skip_prep) {
     const int C8 = a.Cin / 8;
     CFB_REQUIRE(C8 <= 256 && 256 % C8 == 0, "conv_tc: Cin must be 64 * 2^k (<= 2048)");
     const int64_t img_px = (int64_t)Hp * Wp;
@@ -1927,8 +1984,9 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_CHECK(make_map(&mA_hi, hi, 4, dims, str, box, sp));
     CFB_CHECK(make_map(&mA_lo, lo, 4, dims, str, box, sp));
   }
+  const TcWin win = tc_window(a);
   {
-    const int taps = a.mode == CONV_UP ? 16 : a.ksize * a.ksize;
+    const int taps = a.mode == CONV_UP ? 16 : win.kh * win.kw;
     const uint64_t dims[3] = {(uint64_t)a.Cin, (uint64_t)a.Cout, (uint64_t)taps};
     const uint64_t str[2] = {(uint64_t)a.Cin * 2, (uint64_t)a.Cout * a.Cin * 2};
     const uint32_t box[3] = {64, (uint32_t)BN, 1};
@@ -1937,11 +1995,11 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
   }
   TcParams p;
   p.N = a.N; p.Ho = a.Ho; p.Wo = a.Wo; p.Cout = a.Cout;
-  p.taps = a.ksize * a.ksize; p.pad = a.mode == CONV_DOWN ? a.down_pad : a.ksize / 2; p.stride = a.mode == CONV_DOWN ? 2 : 1;
+  p.taps = win.kh * win.kw; p.kw = win.kw; p.pad = win.ph; p.pad_w = win.pw; p.stride = win.stride;
   p.up4 = a.mode == CONV_UP ? 1 : 0;
   p.a_c0 = 0; p.b_c0 = 0; p.b_batched = 0;
   p.heads = 1; p.a_c_head = 0; p.b_c_head = 0; p.a_img_per_head = 0; p.b_r_head = 0; p.out_per_head = 1; p.o_c_head = 0;
-  if (p.up4) { p.taps = 4; p.pad = 1; }
+  if (p.up4) { p.taps = 4; p.pad = 1; p.pad_w = 1; }
   p.chunk = tc_chunk_kblocks();
   p.PW = PW; p.PH = PH;
   p.BW = BW; p.BH = BH;
@@ -1963,11 +2021,13 @@ int conv_tc(const ConvArgs& a, void* scratch, int sm_count, cudaStream_t st) {
     CFB_REQUIRE(a.out_act == OUT_NONE || a.out_act == OUT_LRELU || a.out_act == OUT_RELU || a.out_act == OUT_SILU ||
                     a.out_act == OUT_PRELU,
                 "conv_tc: generalised variant has bias / residual / LeakyReLU / ReLU / SiLU / PReLU epilogues");
-  } else if (p.out_pitch != a.Cout || p.out_c0 != 0) {
-    // per-tap engine writing a channel slice: the tile offsets use the destination pitch, which only the plain store follows
-    CFB_REQUIRE(!geo.halo && p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.out_c0 + a.Cout <= p.out_pitch,
+  } else if (p.out_pitch != a.Cout || p.out_c0 != 0 || a.cout_valid != 0) {
+    // per-tap engine writing a channel slice: the tile offsets use the destination pitch, which only the plain store follows;
+    // cout_valid < Cout leaves the destination channels after the slice's real ones untouched
+    CFB_REQUIRE(!geo.halo && p.out_pitch % 4 == 0 && p.out_c0 % 4 == 0 && p.cout_valid % 4 == 0 && p.cout_valid <= a.Cout &&
+                    p.out_c0 + p.cout_valid <= p.out_pitch,
                 "conv_tc: a destination slice needs the per-tap engine, 4-aligned and inside the pitch");
-    CFB_REQUIRE(!a.residual && !a.sft_dec && !a.out_planes && !a.gn_part && !a.residual2 && a.cout_valid == 0,
+    CFB_REQUIRE(!a.residual && !a.sft_dec && !a.out_planes && !a.gn_part && !a.residual2,
                 "conv_tc: a destination slice of the per-tap engine takes bias and activation only");
   }
   if (p.taps * p.kblocks <= 12) p.chunk = p.taps * p.kblocks;   // short K (Cin = 64): one partial sum, no 8+1 split
@@ -2052,7 +2112,7 @@ int bmm_tc(const BmmArgs& g, int sm_count, cudaStream_t st) {
   CFB_REQUIRE(g.heads == 1 || g.out_per_head || g.o_c_head == g.Cout, "bmm_tc: a head's column slice must equal its Cout");
   TcParams p;
   p.N = g.N * g.heads; p.Ho = 16; p.Wo = 16; p.Cout = out_pitch;
-  p.taps = 1; p.pad = 0; p.stride = 1; p.up4 = 0;
+  p.taps = 1; p.kw = 1; p.pad = 0; p.pad_w = 0; p.stride = 1; p.up4 = 0;
   p.a_c0 = g.a_c0; p.b_c0 = g.b_c0; p.b_batched = 1;
   p.heads = g.heads; p.a_c_head = g.a_c_head; p.b_c_head = g.b_c_head; p.a_img_per_head = g.a_img_per_head ? 1 : 0;
   p.b_r_head = g.b_r_head; p.out_per_head = g.out_per_head ? 1 : 0; p.o_c_head = g.o_c_head;

@@ -10,6 +10,8 @@ constexpr int TC_TILE_N = 64;                 // output channels of one n-tile o
 // OIHW fp32 -> [taps][Cout][Cin] fp16 hi / lo of w*2^k (hi = fp16(.), lo = fp16(. - hi)); scale_slot = 2 device floats,
 // [1] receives 2^-k for the epilogue
 int tc_split_weights(const float* oihw, __half* hi, __half* lo, int Cout, int Cin, int k, float* scale_slot, cudaStream_t st);
+// the same for a kh x kw window: OIHW fp32 -> [taps = kh * kw][Cout][Cin], taps in row-major (r, s) order
+int tc_split_weights_taps(const float* oihw, __half* hi, __half* lo, int Cout, int Cin, int taps, float* scale_slot, cudaStream_t st);
 // Upsample convs: pre-summed 2x2 parity weights [16][Cout][Cin] (hi/lo) -- pass these as wgt_hi/wgt_lo/wscale_inv with mode CONV_UP
 int tc_split_weights_up4(const float* oihw3x3, __half* hi, __half* lo, int Cout, int Cin, float* scale_slot, cudaStream_t st);
 bool tc_supported(const ConvArgs& a);

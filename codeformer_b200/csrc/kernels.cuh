@@ -139,6 +139,10 @@ struct ConvArgs {
   int mode = CONV_SAME;
   int down_pad = 0;                 // CONV_DOWN (per-tap engine): zero padding before the window; 0 = the Downsample's (0,1,0,1)
                                     // padding (Ho = H/2), 1 = a torchvision-style 3x3 stride-2 pad-1 conv (Ho = ceil(H/2))
+  // per-tap engine, explicit window (kh > 0; ksize and down_pad are then not read): a kh x kw kernel (1..7 each) with zero
+  // padding pad_h / pad_w on both sides, stride 1 (CONV_SAME) or 2 (CONV_DOWN); Ho = (H + 2 pad_h - kh) / stride + 1, likewise Wo.
+  // Weights [kh * kw][Cout][Cin] (tc_split_weights_taps).  Inception-v3's 1x7 / 7x1 / 1x3 / 3x1 / 5x5 and valid 3x3 convs
+  int kh = 0, kw = 0, pad_h = 0, pad_w = 0;
   const float* wgt_f32 = nullptr;   // [taps][Cin][Cout] fp32 (CUDA-core engine)
   const void* wgt_hi = nullptr;     // [taps][Cout][Cin] fp16 hi   (tensor-core engine)
   const void* wgt_lo = nullptr;     // [taps][Cout][Cin] fp16 lo
@@ -175,6 +179,7 @@ struct ConvArgs {
   bool subsample = false;       // keep the even output positions only: out is [N, Ho/2, Wo/2, ...] (Ho, Wo even)
   int out_pitch = 0, out_c0 = 0;   // destination channels per pixel (0: Cout) and channel offset
   int cout_valid = 0;           // real output channels (0: Cout); Cout itself is the 64-aligned padded count of the weights
+                                // (also read by the per-tap engine: columns from cout_valid on are not stored)
   int res_pitch = 0;            // channels per pixel of `residual` (0: out_pitch)
   const float* residual2 = nullptr;   // out = act(conv + bias + residual) * post_scale + residual2
   int res2_pitch = 0;
@@ -319,6 +324,27 @@ int lpips_head_blocks(int H, int W);
 int lpips_head(const float* feat, const float* lin, int groups, int G, int H, int W, int C, float* pooled, float* partial,
                cudaStream_t st);
 int lpips_finalize(const LpipsLayers& L, int P, float* val, float* per_layer, cudaStream_t st);
+// Inception-v3 for FID (fid.cu).  The input stage: fp32 NCHW RGB (f32) or uint8 HWC BGR (u8, read as RGB v / 255) of H x W;
+// resize: bilinear (align_corners=False) to FID_SIZE x FID_SIZE, else the source size; normalize: 2x - 1 afterwards
+constexpr int FID_SIZE = 299;
+struct FidInput {
+  const float* f32 = nullptr;
+  const unsigned char* u8 = nullptr;
+  int H = 0, W = 0;
+  int resize = 0, normalize = 0;
+};
+int fid_input(const FidInput& in, float* out_nchw, int N, cudaStream_t st);
+// Conv2d_1a_3x3 (3x3 stride 2 valid, weights [32][27] with the BatchNorm folded) + ReLU on the input stage's values -> NHWC
+// [N, Ho, Wo, pitch], channels [32, pitch) zero; nan_flag[n] (zero on entry) is set when a stem output of image n is NaN
+int fid_stem(const FidInput& in, const float* wt, const float* bias, float* out, int* nan_flag, int pitch, int N, cudaStream_t st);
+// 3x3 max pool, stride 2 valid or stride 1 pad 1, of channels [0, C) into channels [out_c0, out_c0 + C) of the destination
+int fid_maxpool(const float* in, int in_pitch, float* out, int out_pitch, int out_c0, int N, int H, int W, int C, int stride,
+                cudaStream_t st);
+int fid_avgpool(const float* in, int in_pitch, float* out, int out_pitch, int N, int H, int W, int C, cudaStream_t st);
+// -> [N, C]; NaN for the images whose nan_flag is set (nan_flag may be null)
+int fid_global_pool(const float* in, int pitch, const int* nan_flag, float* out, int N, int H, int W, int C, cudaStream_t st);
+// float64 mean mu [D] and covariance sigma [D, D] (np.cov(x, rowvar=False)) of x [N, D]; D a multiple of 64, N >= 2
+int fid_stats(const float* x, int64_t N, int D, double* mu, double* sigma, cudaStream_t st);
 int parse_argmax(const float* logits_nchw, unsigned char* cls, unsigned char* mask, int N, int C, int64_t HW, cudaStream_t st);
 int scale_scalar(float* p, float f, cudaStream_t st);
 int scale_vec(float* p, int n, float f, cudaStream_t st);

@@ -1252,7 +1252,9 @@ struct GenConv {
   std::string bn;                   // detectors: prefix of the BatchNorm folded into the weights ("": none)
   float out_scale = 1.f;            // constant folded into 2^-k and the bias
   bool up = false;                  // nearest x2 + conv (four parity convs)
+  int kh = 0, kw = 0, pad_h = 0, pad_w = 0;   // explicit kh x kw window (kh > 0, per-tap engine; k is then not read)
   __half* w_hi = nullptr; __half* w_lo = nullptr; float* bias = nullptr; float* wscale = nullptr;
+  int taps() const { return kh > 0 ? kh * kw : k * k; }
 };
 
 static GenConv plan_conv(const std::string& name, int cin, int cout, int k = 3, int stride = 1) {
@@ -1268,9 +1270,9 @@ struct SlabPlan {
   size_t convs = 0, padmax = 0;
   int cout_max = 0;
   void add(const GenConv& c) {
-    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : c.k * c.k);
+    const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : c.taps());
     convs += 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256;
-    padmax = std::max(padmax, (size_t)c.cout_p * c.cin_p * c.k * c.k * 4);
+    padmax = std::max(padmax, (size_t)c.cout_p * c.cin_p * c.taps() * 4);
     cout_max = std::max(cout_max, c.cout_p);
   }
   size_t bytes() const { return convs + 2 * align256(padmax) + align256((size_t)cout_max * 4); }
@@ -1281,7 +1283,7 @@ struct SlabPlan {
 // out_scale into 2^-k and the bias.
 static int prepare_conv(GenConv& c, const float* w, const float* b, float* pad, char*& p, cudaStream_t st) {
   auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
-  const int taps = c.k * c.k;
+  const int taps = c.taps();
   const size_t wn = (size_t)c.cout_p * c.cin_p * (c.up ? 16 : taps);
   c.w_hi = (__half*)take(wn * 2); c.w_lo = (__half*)take(wn * 2);
   c.bias = (float*)take((size_t)c.cout_p * 4); c.wscale = (float*)take(8);
@@ -1289,7 +1291,7 @@ static int prepare_conv(GenConv& c, const float* w, const float* b, float* pad, 
   CFB_CUDA(cudaMemcpy2DAsync(pad, (size_t)c.cin_p * taps * 4, w, (size_t)c.cin * taps * 4, (size_t)c.cin * taps * 4, c.cout,
                              cudaMemcpyDeviceToDevice, st));
   if (c.up) CFB_CHECK(tc_split_weights_up4(pad, c.w_hi, c.w_lo, c.cout_p, c.cin_p, c.wscale, st));
-  else CFB_CHECK(tc_split_weights(pad, c.w_hi, c.w_lo, c.cout_p, c.cin_p, c.k, c.wscale, st));
+  else CFB_CHECK(tc_split_weights_taps(pad, c.w_hi, c.w_lo, c.cout_p, c.cin_p, taps, c.wscale, st));
   CFB_CUDA(cudaMemsetAsync(c.bias, 0, (size_t)c.cout_p * 4, st));
   if (b) CFB_CUDA(cudaMemcpyAsync(c.bias, b, (size_t)c.cout * 4, cudaMemcpyDeviceToDevice, st));
   if (c.out_scale != 1.f) {
@@ -1312,14 +1314,14 @@ struct WeightPrep {
   }
   char* take(size_t bytes) { char* r = p; p += align256(bytes); return r; }
   // eval-mode BatchNorm `bn` (weight, bias, running_mean, running_var) folded into the conv weight `w_name` -> fold_w, fold_b
-  int fold(const std::string& w_name, const std::string& bn, int cout, int per_out) {
+  int fold(const std::string& w_name, const std::string& bn, int cout, int per_out, float eps = 1e-5f) {
     const float* w = net.param(w_name, (int64_t)cout * per_out);
     const float* g = net.param(bn + "weight", cout);
     const float* be = net.param(bn + "bias", cout);
     const float* mu = net.param(bn + "running_mean", cout);
     const float* var = net.param(bn + "running_var", cout);
     if (!w || !g || !be || !mu || !var) return 1;
-    return fold_bn(w, g, be, mu, var, 1e-5f, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps
+    return fold_bn(w, g, be, mu, var, eps, fold_w, fold_b, cout, per_out, st);     // nn.BatchNorm2d default eps 1e-5
   }
   int conv(GenConv& c, const float* w, const float* b) { return prepare_conv(c, w, b, pad, p, st); }
 };
@@ -1417,6 +1419,19 @@ static ConvArgs pertap_args(const float* in, int N, int h, int w, int cin, int c
   a.mode = stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = (stride == 2 && k == 3) ? 1 : 0;
   a.residual = res; a.out_act = act; a.out = out;
   a.out_pitch = out_pitch == cout ? 0 : out_pitch; a.out_c0 = out_c0;
+  return a;
+}
+
+// A conv with an explicit kh x kw window (GenConv::kh > 0) on the per-tap engine, weights not set: zero padding (pad_h, pad_w),
+// stride c.stride, written at channel out_c0 of a destination with out_pitch channels per pixel; into a slice (out_pitch != cout_p
+// or out_c0 != 0) only the c.cout real channels are stored.
+static ConvArgs pertap_window_args(const float* in, int N, int h, int w, const GenConv& c, float* out, int out_pitch, int out_c0,
+                                   int act) {
+  ConvArgs a = pertap_args(in, N, h, w, c.cin_p, c.cout_p, 1, 1, out, out_pitch, out_c0, act, nullptr);
+  a.kh = c.kh; a.kw = c.kw; a.pad_h = c.pad_h; a.pad_w = c.pad_w;
+  a.mode = c.stride == 2 ? CONV_DOWN : CONV_SAME; a.down_pad = 0;
+  a.Ho = (h + 2 * c.pad_h - c.kh) / c.stride + 1; a.Wo = (w + 2 * c.pad_w - c.kw) / c.stride + 1;
+  if (out_pitch != c.cout_p || out_c0 != 0) a.cout_valid = c.cout;
   return a;
 }
 
@@ -2795,6 +2810,258 @@ static int yo_forward(cfb_yolov5face* n, const float* x, const unsigned char* im
 // =========================================================================================================
 // C ABI
 // =========================================================================================================
+// =========================================================================================================
+// InceptionV3 for FID: pytorch-fid's InceptionV3(output_blocks=[3]) with use_fid_inception=True (basicsr/archs/inception.py),
+// the pool3 features of restored faces.  torchvision's Inception3 with the FID blocks: Mixed_5b..5d FIDInceptionA (pool
+// features 32 / 64 / 64), Mixed_6b..6e FIDInceptionC (channels_7x7 128 / 160 / 160 / 192), Mixed_7b FIDInceptionE_1, Mixed_7c
+// FIDInceptionE_2; the pool branches of A, C and E_1 are avg_pool2d(3, 1, 1, count_include_pad=False), that of E_2
+// max_pool2d(3, 1, 1).  Every BasicConv2d is conv (no bias) + BatchNorm(eps 1e-3, folded at prepare) + ReLU.  Engines:
+//   Conv2d_1a_3x3 (3x3 s2 valid, 3 -> 32)        SIMT stem (fid.cu), the input stage (bilinear to 299, 2x - 1) fused into its load
+//   3x3 pad 1 stride 1                            generalised halo engine
+//   1x1, 3x3 valid (stride 1 and 2), 5x5, 1x7, 7x1, 1x3, 3x1     per-tap engine, explicit windows
+//   max / avg pools, global average pool         SIMT (fid.cu)
+// Maps are NHWC with a 64-aligned channel pitch whose pad channels are zero (zero weights and bias + ReLU, or a memset).  Each
+// block's branches write their channel slices of one concatenation buffer, in torchvision's order.
+// =========================================================================================================
+struct cfb_fid : cfb::NetCore {
+  cfb_fid() : NetCore("InceptionV3", "fid") {}
+  std::vector<cfb::GenConv> convs;        // the 93 convs after the stem, in plan order
+  float *stem_w = nullptr, *stem_b = nullptr;
+};
+namespace cfb {
+
+constexpr float FID_BN_EPS = 1e-3f;
+constexpr int FID_FEATURES = 2048;
+
+// block prefixes of the wrapper's state dict (blocks.<i>.<j>.) for the convs after the stem
+static void fid_build(cfb_fid* n) {
+  std::vector<GenConv>& v = n->convs;
+  v.clear();
+  auto add = [&](const std::string& name, int cin, int cout, int kh, int kw, int ph, int pw, int stride) {
+    GenConv c = plan_conv(name, cin, cout, kh == kw ? kh : 1, stride);
+    c.gen = kh == 3 && kw == 3 && ph == 1 && pw == 1 && stride == 1;
+    if (!c.gen) { c.kh = kh; c.kw = kw; c.pad_h = ph; c.pad_w = pw; }
+    v.push_back(c);
+  };
+  add("blocks.0.1.", 32, 32, 3, 3, 0, 0, 1);          // Conv2d_2a_3x3
+  add("blocks.0.2.", 32, 64, 3, 3, 1, 1, 1);          // Conv2d_2b_3x3
+  add("blocks.1.0.", 64, 80, 1, 1, 0, 0, 1);          // Conv2d_3b_1x1
+  add("blocks.1.1.", 80, 192, 3, 3, 0, 0, 1);         // Conv2d_4a_3x3
+  const int pf[3] = {32, 64, 64};
+  int cin = 192;
+  for (int i = 0; i < 3; ++i) {                       // Mixed_5b..5d (InceptionA)
+    const std::string p = "blocks.2." + std::to_string(i) + ".";
+    add(p + "branch1x1.", cin, 64, 1, 1, 0, 0, 1);
+    add(p + "branch5x5_1.", cin, 48, 1, 1, 0, 0, 1);
+    add(p + "branch5x5_2.", 48, 64, 5, 5, 2, 2, 1);
+    add(p + "branch3x3dbl_1.", cin, 64, 1, 1, 0, 0, 1);
+    add(p + "branch3x3dbl_2.", 64, 96, 3, 3, 1, 1, 1);
+    add(p + "branch3x3dbl_3.", 96, 96, 3, 3, 1, 1, 1);
+    add(p + "branch_pool.", cin, pf[i], 1, 1, 0, 0, 1);
+    cin = 224 + pf[i];
+  }
+  add("blocks.2.3.branch3x3.", 288, 384, 3, 3, 0, 0, 2);           // Mixed_6a (InceptionB)
+  add("blocks.2.3.branch3x3dbl_1.", 288, 64, 1, 1, 0, 0, 1);
+  add("blocks.2.3.branch3x3dbl_2.", 64, 96, 3, 3, 1, 1, 1);
+  add("blocks.2.3.branch3x3dbl_3.", 96, 96, 3, 3, 0, 0, 2);
+  const int c7s[4] = {128, 160, 160, 192};
+  for (int i = 0; i < 4; ++i) {                       // Mixed_6b..6e (InceptionC)
+    const std::string p = "blocks.2." + std::to_string(4 + i) + ".";
+    const int c7 = c7s[i];
+    add(p + "branch1x1.", 768, 192, 1, 1, 0, 0, 1);
+    add(p + "branch7x7_1.", 768, c7, 1, 1, 0, 0, 1);
+    add(p + "branch7x7_2.", c7, c7, 1, 7, 0, 3, 1);
+    add(p + "branch7x7_3.", c7, 192, 7, 1, 3, 0, 1);
+    add(p + "branch7x7dbl_1.", 768, c7, 1, 1, 0, 0, 1);
+    add(p + "branch7x7dbl_2.", c7, c7, 7, 1, 3, 0, 1);
+    add(p + "branch7x7dbl_3.", c7, c7, 1, 7, 0, 3, 1);
+    add(p + "branch7x7dbl_4.", c7, c7, 7, 1, 3, 0, 1);
+    add(p + "branch7x7dbl_5.", c7, 192, 1, 7, 0, 3, 1);
+    add(p + "branch_pool.", 768, 192, 1, 1, 0, 0, 1);
+  }
+  add("blocks.3.0.branch3x3_1.", 768, 192, 1, 1, 0, 0, 1);         // Mixed_7a (InceptionD)
+  add("blocks.3.0.branch3x3_2.", 192, 320, 3, 3, 0, 0, 2);
+  add("blocks.3.0.branch7x7x3_1.", 768, 192, 1, 1, 0, 0, 1);
+  add("blocks.3.0.branch7x7x3_2.", 192, 192, 1, 7, 0, 3, 1);
+  add("blocks.3.0.branch7x7x3_3.", 192, 192, 7, 1, 3, 0, 1);
+  add("blocks.3.0.branch7x7x3_4.", 192, 192, 3, 3, 0, 0, 2);
+  cin = 1280;
+  for (int i = 0; i < 2; ++i) {                       // Mixed_7b, 7c (InceptionE)
+    const std::string p = "blocks.3." + std::to_string(1 + i) + ".";
+    add(p + "branch1x1.", cin, 320, 1, 1, 0, 0, 1);
+    add(p + "branch3x3_1.", cin, 384, 1, 1, 0, 0, 1);
+    add(p + "branch3x3_2a.", 384, 384, 1, 3, 0, 1, 1);
+    add(p + "branch3x3_2b.", 384, 384, 3, 1, 1, 0, 1);
+    add(p + "branch3x3dbl_1.", cin, 448, 1, 1, 0, 0, 1);
+    add(p + "branch3x3dbl_2.", 448, 384, 3, 3, 1, 1, 1);
+    add(p + "branch3x3dbl_3a.", 384, 384, 1, 3, 0, 1, 1);
+    add(p + "branch3x3dbl_3b.", 384, 384, 3, 1, 1, 0, 1);
+    add(p + "branch_pool.", cin, 192, 1, 1, 0, 0, 1);
+    cin = 2048;
+  }
+}
+
+static int fid_prepare(cfb_fid* n, cudaStream_t st) {
+  CFB_CHECK(n->begin_prepare(st));
+  SlabPlan plan;
+  for (const GenConv& c : n->convs) plan.add(c);
+  CFB_CHECK(n->reserve_slab(plan.bytes() + align256(32 * 27 * 4) + align256(32 * 4)));
+  WeightPrep wp(*n, plan, st);
+  for (GenConv& c : n->convs) {
+    CFB_CHECK(wp.fold(c.name + "conv.weight", c.name + "bn.", c.cout, c.cin * c.taps(), FID_BN_EPS));
+    CFB_CHECK(wp.conv(c, wp.fold_w, wp.fold_b));
+  }
+  CFB_CHECK(wp.fold("blocks.0.0.conv.weight", "blocks.0.0.bn.", 32, 27, FID_BN_EPS));
+  n->stem_w = (float*)wp.take(32 * 27 * 4); n->stem_b = (float*)wp.take(32 * 4);
+  CFB_CUDA(cudaMemcpyAsync(n->stem_w, wp.fold_w, 32 * 27 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaMemcpyAsync(n->stem_b, wp.fold_b, 32 * 4, cudaMemcpyDeviceToDevice, st));
+  CFB_CUDA(cudaStreamSynchronize(st));
+  n->prepared = true;
+  return 0;
+}
+
+static int pad64(int c) { return (c + 63) / 64 * 64; }
+
+// pool3 features [N, 2048] of N images through the input stage `in`
+static int fid_forward(cfb_fid* n, const FidInput& in, int N, float* feat, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
+  CFB_CHECK(n->begin_forward(dry));
+  const int OH = in.resize ? FID_SIZE : in.H, OW = in.resize ? FID_SIZE : in.W;
+  CFB_REQUIRE(N >= 0 && in.H >= 1 && in.W >= 1, "InceptionV3: bad input size");
+  CFB_REQUIRE(OH >= 75 && OW >= 75, "InceptionV3: the network input must be at least 75 x 75 (resize_input=True gives 299 x 299)");
+  if (N == 0) return 0;
+  Arena& ar = n->arena;
+  ar.reset(ws, (size_t)ws_bytes, dry);
+  struct Map { float* p; int h, w, c, pitch; };       // c real channels, pitch >= c (pad channels zero)
+  auto alloc = [&](Map& m, int h, int w, int c, int pitch) -> int {
+    m.h = h; m.w = w; m.c = c; m.pitch = pitch;
+    CFB_CHECK(n->alloc(&m.p, (size_t)N * h * w * pitch));
+    if (!dry && (pitch != c)) CFB_CUDA(cudaMemsetAsync(m.p, 0, (size_t)N * h * w * pitch * 4, st));
+    return 0;
+  };
+  auto out_hw = [](const GenConv& c, int h, int w, int& oh, int& ow) {
+    if (c.gen) { oh = h; ow = w; return; }
+    oh = (h + 2 * c.pad_h - c.kh) / c.stride + 1; ow = (w + 2 * c.pad_w - c.kw) / c.stride + 1;
+  };
+  // conv + ReLU of x into channels [c0, c0 + cout) of `o` (o.pitch channels per pixel)
+  auto conv = [&](const GenConv& c, const Map& x, const Map& o, int c0) -> int {
+    CFB_REQUIRE(x.c == c.cin, "InceptionV3: channel mismatch at " + c.name);
+    if (c.gen) {
+      GenLaunch g{&c, x.p, x.pitch, x.h, x.w, N, o.p, o.pitch, c0, OUT_RELU};
+      return dry ? 0 : gen_conv(g, n->sm_count, st);
+    }
+    CFB_REQUIRE(x.pitch == c.cin_p, "InceptionV3: per-tap input pitch at " + c.name);
+    return pertap_conv(*n, pertap_window_args(x.p, N, x.h, x.w, c, o.p, o.pitch, c0, OUT_RELU), c, dry, st);
+  };
+  // conv into a new map of its own (pitch cout_p; the generalised engine stores only the real channels, so the pad is zeroed)
+  auto conv_new = [&](const GenConv& c, const Map& x, Map& o) -> int {
+    int oh = 0, ow = 0;
+    out_hw(c, x.h, x.w, oh, ow);
+    CFB_CHECK(alloc(o, oh, ow, c.cout, c.cout_p));
+    return conv(c, x, o, 0);
+  };
+  auto pool_conv = [&](const GenConv& c, const Map& x, bool max_pool, const Map& o, int c0) -> int {
+    Map pm;
+    CFB_CHECK(alloc(pm, x.h, x.w, x.c, x.pitch));
+    if (!dry) {
+      if (max_pool) CFB_CHECK(fid_maxpool(x.p, x.pitch, pm.p, x.pitch, 0, N, x.h, x.w, x.pitch, 1, st));
+      else CFB_CHECK(fid_avgpool(x.p, x.pitch, pm.p, x.pitch, N, x.h, x.w, x.pitch, st));
+    }
+    CFB_CHECK(conv(c, pm, o, c0));
+    ar.release(pm.p);
+    return 0;
+  };
+  // a chain of convs from x, the last one into channels [c0, ..) of o
+  auto chain = [&](std::initializer_list<const GenConv*> cs, const Map& x, const Map& o, int c0) -> int {
+    Map cur = x;
+    size_t i = 0;
+    for (const GenConv* c : cs) {
+      if (++i == cs.size()) { CFB_CHECK(conv(*c, cur, o, c0)); break; }
+      Map nx;
+      CFB_CHECK(conv_new(*c, cur, nx));
+      if (cur.p != x.p) ar.release(cur.p);
+      cur = nx;
+    }
+    if (cur.p != x.p) ar.release(cur.p);
+    return 0;
+  };
+  const std::vector<GenConv>& C = n->convs;
+  // stem: Conv2d_1a (SIMT, input stage fused), 2a, 2b, max pool, 3b, 4a, max pool
+  Map x, y;
+  // per-image NaN flags of the stem, read by the global pool (the engine's ReLU epilogue maps NaN to 0, torch's keeps it)
+  int* nan_flag = (int*)ar.alloc((size_t)N * sizeof(int));
+  CFB_REQUIRE(nan_flag != nullptr, n->ws_error());
+  if (!dry) CFB_CUDA(cudaMemsetAsync(nan_flag, 0, (size_t)N * sizeof(int), st));
+  CFB_CHECK(alloc(x, (OH - 3) / 2 + 1, (OW - 3) / 2 + 1, 32, 64));
+  if (!dry) CFB_CHECK(fid_stem(in, n->stem_w, n->stem_b, x.p, nan_flag, 64, N, st));
+  CFB_CHECK(conv_new(C[0], x, y)); ar.release(x.p); x = y;
+  CFB_CHECK(conv_new(C[1], x, y)); ar.release(x.p); x = y;
+  CFB_CHECK(alloc(y, (x.h - 3) / 2 + 1, (x.w - 3) / 2 + 1, x.c, x.pitch));
+  if (!dry) CFB_CHECK(fid_maxpool(x.p, x.pitch, y.p, y.pitch, 0, N, x.h, x.w, x.pitch, 2, st));
+  ar.release(x.p); x = y;
+  CFB_CHECK(conv_new(C[2], x, y)); ar.release(x.p); x = y;
+  CFB_CHECK(conv_new(C[3], x, y)); ar.release(x.p); x = y;
+  CFB_CHECK(alloc(y, (x.h - 3) / 2 + 1, (x.w - 3) / 2 + 1, x.c, x.pitch));
+  if (!dry) CFB_CHECK(fid_maxpool(x.p, x.pitch, y.p, y.pitch, 0, N, x.h, x.w, x.pitch, 2, st));
+  ar.release(x.p); x = y;
+  size_t k = 4;
+  for (int i = 0; i < 3; ++i, k += 7) {               // Mixed_5b..5d: [1x1 64 | 5x5 64 | 3x3dbl 96 | pool pf]
+    const int c = 224 + C[k + 6].cout;
+    CFB_CHECK(alloc(y, x.h, x.w, c, pad64(c)));
+    CFB_CHECK(conv(C[k], x, y, 0));
+    CFB_CHECK(chain({&C[k + 1], &C[k + 2]}, x, y, 64));
+    CFB_CHECK(chain({&C[k + 3], &C[k + 4], &C[k + 5]}, x, y, 128));
+    CFB_CHECK(pool_conv(C[k + 6], x, false, y, 224));
+    ar.release(x.p); x = y;
+  }
+  {                                                   // Mixed_6a: [3x3 s2 384 | 3x3dbl s2 96 | max pool 288]
+    const int h = (x.h - 3) / 2 + 1, w = (x.w - 3) / 2 + 1;
+    CFB_CHECK(alloc(y, h, w, 768, 768));
+    CFB_CHECK(conv(C[k], x, y, 0));
+    CFB_CHECK(chain({&C[k + 1], &C[k + 2], &C[k + 3]}, x, y, 384));
+    if (!dry) CFB_CHECK(fid_maxpool(x.p, x.pitch, y.p, y.pitch, 480, N, x.h, x.w, x.c, 2, st));
+    ar.release(x.p); x = y; k += 4;
+  }
+  for (int i = 0; i < 4; ++i, k += 10) {              // Mixed_6b..6e: [1x1 192 | 7x7 192 | 7x7dbl 192 | pool 192]
+    CFB_CHECK(alloc(y, x.h, x.w, 768, 768));
+    CFB_CHECK(conv(C[k], x, y, 0));
+    CFB_CHECK(chain({&C[k + 1], &C[k + 2], &C[k + 3]}, x, y, 192));
+    CFB_CHECK(chain({&C[k + 4], &C[k + 5], &C[k + 6], &C[k + 7], &C[k + 8]}, x, y, 384));
+    CFB_CHECK(pool_conv(C[k + 9], x, false, y, 576));
+    ar.release(x.p); x = y;
+  }
+  {                                                   // Mixed_7a: [3x3 s2 320 | 7x7x3 s2 192 | max pool 768]
+    const int h = (x.h - 3) / 2 + 1, w = (x.w - 3) / 2 + 1;
+    CFB_CHECK(alloc(y, h, w, 1280, 1280));
+    CFB_CHECK(chain({&C[k], &C[k + 1]}, x, y, 0));
+    CFB_CHECK(chain({&C[k + 2], &C[k + 3], &C[k + 4], &C[k + 5]}, x, y, 320));
+    if (!dry) CFB_CHECK(fid_maxpool(x.p, x.pitch, y.p, y.pitch, 512, N, x.h, x.w, x.c, 2, st));
+    ar.release(x.p); x = y; k += 6;
+  }
+  for (int i = 0; i < 2; ++i, k += 9) {               // Mixed_7b, 7c: [1x1 320 | 3x3 2a 2b 768 | 3x3dbl 3a 3b 768 | pool 192]
+    CFB_CHECK(alloc(y, x.h, x.w, 2048, 2048));
+    CFB_CHECK(conv(C[k], x, y, 0));
+    Map t, u;
+    CFB_CHECK(conv_new(C[k + 1], x, t));
+    CFB_CHECK(conv(C[k + 2], t, y, 320));
+    CFB_CHECK(conv(C[k + 3], t, y, 704));
+    ar.release(t.p);
+    CFB_CHECK(conv_new(C[k + 4], x, t));
+    CFB_CHECK(conv_new(C[k + 5], t, u));
+    ar.release(t.p);
+    CFB_CHECK(conv(C[k + 6], u, y, 1088));
+    CFB_CHECK(conv(C[k + 7], u, y, 1472));
+    ar.release(u.p);
+    CFB_CHECK(pool_conv(C[k + 8], x, i == 1, y, 1856));     // FIDInceptionE_2 pools with max_pool2d(3, 1, 1)
+    ar.release(x.p); x = y;
+  }
+  if (!dry) CFB_CHECK(fid_global_pool(x.p, x.pitch, nan_flag, feat, N, x.h, x.w, FID_FEATURES, st));
+  ar.release(x.p);
+  ar.release(nan_flag);
+  return 0;
+}
+
+}  // namespace cfb
+
 #define API_BEGIN try {
 #define API_END(ret)                                                             \
   } catch (const std::exception& e) { cfb::set_error(std::string("exception: ") + e.what()); return ret; } \
@@ -4212,4 +4479,126 @@ int cfb_nhwc_to_nchw(const float* in, float* out, int32_t n, int32_t c, int32_t 
   API_END(1)
 }
 
+
+cfb_fid* cfb_fid_create(void) {
+  API_BEGIN
+  cfb_fid* n = new cfb_fid();
+  cfb::fid_build(n);           // the plan: workspace queries need no prepared weights
+  return n;
+  API_END(nullptr)
+}
+void cfb_fid_destroy(cfb_fid* n) { delete n; }
+int cfb_fid_set_param(cfb_fid* n, const char* name, const float* dev_ptr, int64_t numel) {
+  API_BEGIN
+  CFB_REQUIRE(n && name && dev_ptr, "cfb_fid_set_param: NULL argument");
+  return n->set_param(name, dev_ptr, numel);
+  API_END(1)
+}
+int cfb_fid_prepare(cfb_fid* n, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_fid_prepare: NULL net");
+  std::lock_guard<std::mutex> lk(n->mu);
+  return cfb::fid_prepare(n, (cudaStream_t)stream);
+  API_END(1)
+}
+int64_t cfb_fid_workspace_bytes(cfb_fid* n, int32_t batch, int32_t h, int32_t w, int32_t resize) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_fid_workspace_bytes: NULL net"); return -1; }
+  cfb::FidInput in;
+  in.f32 = (const float*)0x1000; in.H = h; in.W = w; in.resize = resize != 0;
+  return n->dry_run([&] { return cfb::fid_forward(n, in, batch, nullptr, nullptr, 0, nullptr, true); });
+  API_END(-1)
+}
+int cfb_fid_forward(cfb_fid* n, const float* x_nchw, int32_t batch, int32_t h, int32_t w, int32_t resize, int32_t normalize,
+                    float* feat, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (x_nchw && feat && workspace)), "cfb_fid_forward: NULL argument");
+  CFB_REQUIRE(((uintptr_t)feat & 15) == 0, "cfb_fid_forward: feat must be 16-byte aligned");
+  std::lock_guard<std::mutex> lk(n->mu);
+  cfb::FidInput in;
+  in.f32 = x_nchw; in.H = h; in.W = w; in.resize = resize != 0; in.normalize = normalize != 0;
+  return cfb::fid_forward(n, in, batch, feat, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_fid_forward_u8(cfb_fid* n, const uint8_t* faces_bgr, int32_t batch, int32_t h, int32_t w, float* feat, void* workspace,
+                       int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n && (batch == 0 || (faces_bgr && feat && workspace)), "cfb_fid_forward_u8: NULL argument");
+  CFB_REQUIRE(((uintptr_t)feat & 15) == 0, "cfb_fid_forward_u8: feat must be 16-byte aligned");
+  std::lock_guard<std::mutex> lk(n->mu);
+  cfb::FidInput in;
+  in.u8 = faces_bgr; in.H = h; in.W = w; in.resize = 1; in.normalize = 1;
+  return cfb::fid_forward(n, in, batch, feat, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  API_END(1)
+}
+int cfb_fid_input(const void* src, int32_t u8, int32_t batch, int32_t h, int32_t w, int32_t resize, int32_t normalize, float* out,
+                  void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(batch == 0 || (src && out), "cfb_fid_input: NULL argument");
+  CFB_REQUIRE(batch >= 0 && h >= 1 && w >= 1, "cfb_fid_input: bad size");
+  cfb::FidInput in;
+  if (u8) in.u8 = (const uint8_t*)src; else in.f32 = (const float*)src;
+  in.H = h; in.W = w; in.resize = resize != 0; in.normalize = normalize != 0;
+  return cfb::fid_input(in, out, batch, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_fid_stats(const float* feat, int64_t n, int32_t d, double* mu, double* sigma, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(feat && mu && sigma, "cfb_fid_stats: NULL argument");
+  return cfb::fid_stats(feat, n, d, mu, sigma, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_debug_fid_pool(const float* in, float* out, int32_t n, int32_t h, int32_t w, int32_t c, int32_t kind, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(in && out, "cfb_debug_fid_pool: NULL argument");
+  CFB_REQUIRE(n >= 0 && h >= 1 && w >= 1 && c >= 4 && kind >= 0 && kind <= 2, "cfb_debug_fid_pool: bad size or kind");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (kind == 2) return cfb::fid_avgpool(in, c, out, c, n, h, w, c, st);
+  return cfb::fid_maxpool(in, c, out, c, 0, n, h, w, c, kind == 0 ? 2 : 1, st);
+  API_END(1)
+}
+
+int64_t cfb_conv2d_pertap_window_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw,
+                                                 int32_t stride, int32_t pad_h, int32_t pad_w) {
+  if (n < 0 || h < 1 || w < 1 || cin < 1 || cout < 1 || kh < 1 || kw < 1 || kh > 7 || kw > 7 || !(stride == 1 || stride == 2) ||
+      pad_h < 0 || pad_w < 0)
+    return -1;
+  cfb::GenConv c = cfb::plan_conv("", cin, cout, 1, stride);
+  c.kh = kh; c.kw = kw; c.pad_h = pad_h; c.pad_w = pad_w;
+  if (h + 2 * pad_h < kh || w + 2 * pad_w < kw) return -1;
+  const cfb::ConvArgs a = cfb::pertap_window_args(nullptr, n, h, w, c, nullptr, c.cout_p, 0, cfb::OUT_NONE);
+  const size_t wn = (size_t)c.cout_p * c.cin_p * c.taps();
+  return (int64_t)(align256(wn * 4) + 2 * align256(wn * 2) + align256((size_t)c.cout_p * 4) + 256 + cfb::tc_scratch_bytes(a) + 8192);
+}
+
+int cfb_conv2d_pertap_window_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h,
+                                  int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad_h,
+                                  int32_t pad_w, int32_t out_act, int32_t out_pitch, int32_t out_c0, void* workspace,
+                                  int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  const char* fn = "cfb_conv2d_pertap_window_nhwc";
+  CFB_REQUIRE(in && weight_oihw && out && workspace, std::string(fn) + ": NULL argument");
+  CFB_REQUIRE(cin % 64 == 0 && cout % 4 == 0, std::string(fn) + ": cin must be a multiple of 64 and cout of 4");
+  CFB_REQUIRE(out_act == cfb::OUT_NONE || out_act == cfb::OUT_RELU, std::string(fn) + ": activation must be none or ReLU");
+  const int64_t need = cfb_conv2d_pertap_window_workspace_bytes(n, h, w, cin, cout, kh, kw, stride, pad_h, pad_w);
+  CFB_REQUIRE(need > 0 && workspace_bytes >= need, std::string(fn) + ": bad shape or workspace too small");
+  CFB_REQUIRE(out_pitch >= cout && out_c0 >= 0 && out_c0 + cout <= out_pitch, std::string(fn) + ": slice outside the pitch");
+  cudaStream_t st = (cudaStream_t)stream;
+  CFB_CHECK(cfb::async_status_init(st));
+  int dev = 0, sms = 148;
+  CFB_CUDA(cudaGetDevice(&dev));
+  CFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  cfb::GenConv c = cfb::plan_conv("", cin, cout, 1, stride);
+  c.kh = kh; c.kw = kw; c.pad_h = pad_h; c.pad_w = pad_w;
+  char* p = (char*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+  float* pad = (float*)p; p += align256((size_t)c.cout_p * c.cin_p * c.taps() * 4);
+  CFB_CHECK(cfb::prepare_conv(c, weight_oihw, bias, pad, p, st));
+  p = (char*)(((uintptr_t)p + 1023) / 1024 * 1024);
+  cfb::ConvArgs a = cfb::pertap_window_args(in, n, h, w, c, out, out_pitch, out_c0, out_act);
+  if (out_pitch == c.cout_p && out_c0 == 0 && cout != c.cout_p) a.cout_valid = cout;
+  a.wgt_hi = c.w_hi; a.wgt_lo = c.w_lo; a.wscale_inv = c.wscale + 1; a.bias = c.bias;
+  CFB_REQUIRE(cfb::tc_supported(a), std::string(fn) + ": shape not supported by the wgmma engine");
+  return cfb::conv_tc(a, p, sms, st);
+  API_END(1)
+}
 }  // extern "C"

@@ -496,6 +496,47 @@ int64_t    cfb_debug_lpips_head_workspace_bytes(int32_t batch, int32_t h, int32_
 int        cfb_debug_lpips_head(const float* feat, const float* lin, float* pooled, float* res, int32_t batch, int32_t h, int32_t w,
                                 int32_t group, int32_t c, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- InceptionV3 for the Fréchet Inception Distance (pytorch-fid InceptionV3(output_blocks=[3]), use_fid_inception=True;
+ * fid.cu + the conv engine) ----
+ * Parameters by the state-dict names of pytorch-fid's wrapper (blocks.<i>.<j>.conv.weight, .bn.weight / bias / running_mean /
+ * running_var; BatchNorm eps 1e-3 folded at prepare).
+ * forward: x fp32 NCHW [batch,3,h,w] RGB -> feat [batch,2048] float32, the pool3 features; resize: bilinear (align_corners=False,
+ *   torch's CPU arithmetic) to 299 x 299 first, normalize: 2x - 1 after it.  The network input must be at least 75 x 75.
+ *   An image with a NaN in a value the first conv reads gets NaN features, as in torch.  feat is 16-byte aligned.
+ * forward_u8: uint8 HWC BGR faces [batch,h,w,3] through pytorch-fid's path (RGB v / 255, resize, 2x - 1), fused into the stem;
+ *   equal to cfb_fid_input followed by forward with both flags off, bit for bit.  Workspace: cfb_fid_workspace_bytes.
+ * input: the input stage alone, fp32 NCHW [batch,3,h,w] or (u8) uint8 HWC BGR [batch,h,w,3] -> out fp32 NCHW [batch,3,299,299]
+ *   (resize) or [batch,3,h,w].
+ * stats: float64 mu [d] and sigma [d,d] = np.cov(feat, rowvar=False) of feat [n,d] (n >= 2, d a multiple of 64, feat 16-byte
+ *   aligned); every sum runs
+ *   over the rows in order, so the result depends only on the matrix.
+ * debug_fid_pool (test entry point): NHWC [n,h,w,c] -> 3x3 max pool stride 2 valid (kind 0), max pool stride 1 pad 1 (1), or avg
+ *   pool stride 1 pad 1 with count_include_pad=False (2); c a multiple of 4. */
+typedef struct cfb_fid cfb_fid;
+cfb_fid* cfb_fid_create(void);
+void     cfb_fid_destroy(cfb_fid* net);
+int      cfb_fid_set_param(cfb_fid* net, const char* name, const float* dev_ptr, int64_t numel);
+int      cfb_fid_prepare(cfb_fid* net, void* stream);
+int64_t  cfb_fid_workspace_bytes(cfb_fid* net, int32_t batch, int32_t h, int32_t w, int32_t resize);
+int      cfb_fid_forward(cfb_fid* net, const float* x_nchw, int32_t batch, int32_t h, int32_t w, int32_t resize, int32_t normalize,
+                         float* feat, void* workspace, int64_t workspace_bytes, void* stream);
+int      cfb_fid_forward_u8(cfb_fid* net, const uint8_t* faces_bgr, int32_t batch, int32_t h, int32_t w, float* feat, void* workspace,
+                            int64_t workspace_bytes, void* stream);
+int      cfb_fid_input(const void* src, int32_t u8, int32_t batch, int32_t h, int32_t w, int32_t resize, int32_t normalize, float* out,
+                       void* stream);
+int      cfb_fid_stats(const float* feat, int64_t n, int32_t d, double* mu, double* sigma, void* stream);
+int      cfb_debug_fid_pool(const float* in, float* out, int32_t n, int32_t h, int32_t w, int32_t c, int32_t kind, void* stream);
+/* Test entry point of the per-tap engine's explicit windows: a kh x kw conv (1..7 each), zero padding (pad_h, pad_w), stride 1
+ * or 2, of NHWC in [n,h,w,cin] (cin a multiple of 64) with OIHW weights [cout,cin,kh,kw] and bias [cout] (may be NULL), into
+ * channels [out_c0, out_c0 + cout) of out [n,ho,wo,out_pitch], ho = (h + 2 pad_h - kh) / stride + 1; the other channels are
+ * not written.  Workspace: cfb_conv2d_pertap_window_workspace_bytes. */
+int64_t  cfb_conv2d_pertap_window_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw,
+                                                  int32_t stride, int32_t pad_h, int32_t pad_w);
+int      cfb_conv2d_pertap_window_nhwc(const float* in, const float* weight_oihw, const float* bias, float* out, int32_t n, int32_t h,
+                                       int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad_h,
+                                       int32_t pad_w, int32_t out_act, int32_t out_pitch, int32_t out_c0, void* workspace,
+                                       int64_t workspace_bytes, void* stream);
+
 /* ---- YOLOv5l-face detector (facelib/detection/yolov5face, models/yolov5l.yaml; yolo.cu + the conv engine) ----
  * Parameters by the reference's state-dict names (BatchNorm folded at prepare; the Detect anchor_grid buffer gives the anchor
  * sizes in pixels).  h and w are multiples of 32; P = cfb_yolov5face_predictions(h, w) = 3 (hw/64 + hw/256 + hw/1024).
