@@ -181,6 +181,11 @@ SIGNATURES = {
     'cfb_degrade_workspace_bytes': (c_int64, [c_int32, c_int32, _P, _P]),
     'cfb_degrade_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, c_int32, _P, _P, c_int64, _P]),
     'cfb_debug_degrade_faces': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, c_int32, _P, _P, c_int64, _P, _P, _P]),
+    'cfb_degrade_color_workspace_bytes': (c_int64, [c_int32, c_int32, _P, _P, _P, c_int32]),
+    'cfb_degrade_faces_color': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, c_int32, _P, _P, c_int64,
+                                        _P]),
+    'cfb_debug_degrade_faces_color': (c_int, [_P, c_int32, c_int32, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, c_int32, _P, _P,
+                                              c_int64, _P, _P]),
     'cfb_jpeg_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32]),
     'cfb_jpeg_roundtrip': (c_int, [_P, _P, c_int32, c_int32, c_int32, _P, _P, c_int64, _P]),
     'cfb_check_async_status': (c_int, []),

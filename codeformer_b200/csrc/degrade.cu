@@ -36,6 +36,7 @@ struct DegFace {
   int64_t noise;    // offset of the face's noise field in floats, -1 = no noise
   int64_t grid;     // offset of the blur grid [n][n][3] in floats
   int64_t img;      // offset of the small image [s][s][3] in elements
+  int64_t fstate;   // offset of the face's float result [in][in][3] for the colour stages, -1 = round to lq here
 };
 
 struct JpgImg {
@@ -366,7 +367,8 @@ __global__ void __launch_bounds__(kThreads) jpeg_color_kernel(const JpgImg* __re
 
 // --------------------------------------------------------------------------------------------------- final resize
 __global__ void __launch_bounds__(kThreads) final_kernel(const DegFace* __restrict__ faces, const float* __restrict__ fimg,
-                                                         const uint8_t* __restrict__ dimg, int in_size, uint8_t* __restrict__ lq) {
+                                                         const uint8_t* __restrict__ dimg, int in_size, uint8_t* __restrict__ lq,
+                                                         float* __restrict__ fstate) {
   const int b = blockIdx.y;
   const DegFace f = faces[b];
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -379,6 +381,7 @@ __global__ void __launch_bounds__(kThreads) final_kernel(const DegFace* __restri
   const int64_t p00 = f.img + ((int64_t)y0 * f.s + x0) * 3, p01 = f.img + ((int64_t)y0 * f.s + x1) * 3;
   const int64_t p10 = f.img + ((int64_t)y1 * f.s + x0) * 3, p11 = f.img + ((int64_t)y1 * f.s + x1) * 3;
   uint8_t* o = lq + ((int64_t)b * in_size * in_size + idx) * 3;
+  float* fo = f.fstate >= 0 ? fstate + f.fstate + idx * 3 : nullptr;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     float a, bb, cc, dd;
@@ -391,7 +394,10 @@ __global__ void __launch_bounds__(kThreads) final_kernel(const DegFace* __restri
       a = fimg[p00 + c], bb = fimg[p01 + c], cc = fimg[p10 + c], dd = fimg[p11 + c];
     }
     const float v = lerp(lerp(a, bb, tx), lerp(cc, dd, tx), ty);
-    o[c] = sat_u8(__fmul_rn(v, 255.f));
+    if (fo)
+      fo[c] = v;
+    else
+      o[c] = sat_u8(__fmul_rn(v, 255.f));
   }
 }
 
@@ -409,7 +415,8 @@ struct DegPlan {
   int64_t max_grid, max_small, max_blocks, max_px;
 };
 
-DegPlan plan_degrade(int batch, int S, const int32_t* sizes, const int32_t* qualities, const int64_t* noise_offsets) {
+DegPlan plan_degrade(int batch, int S, const int32_t* sizes, const int32_t* qualities, const int64_t* noise_offsets,
+                     const int64_t* fstate = nullptr) {
   DegPlan P;
   P.faces.resize(batch);
   int64_t grid = 0, img = 0, planes = 0;
@@ -421,6 +428,7 @@ DegPlan plan_degrade(int batch, int S, const int32_t* sizes, const int32_t* qual
     f.q = qualities ? qualities[b] : 0;
     f.pad = 0;
     f.noise = noise_offsets ? noise_offsets[b] : -1;
+    f.fstate = fstate ? fstate[b] : -1;
     f.grid = grid;
     f.img = img;
     grid += (int64_t)f.n * f.n * 3;
@@ -459,7 +467,8 @@ int launch_jpeg(const JpgImg* djpg, int n, int64_t max_blocks, int64_t max_px, c
 
 int degrade(const uint8_t* gt, int batch, int S, const double* kernels, int ks, const int32_t* sizes, const int32_t* qualities,
             const float* noise, const int64_t* noise_offsets, int in_size, uint8_t* lq, void* ws, int64_t ws_bytes,
-            float* cap_a, uint8_t* cap_u8, cudaStream_t st) {
+            float* cap_a, uint8_t* cap_u8, cudaStream_t st, const int64_t* fstate_offsets = nullptr,
+            float* fstate = nullptr) {
   CFB_REQUIRE(batch >= 0 && batch <= 65535, "cfb_degrade_faces: batch must be 0..65535");
   CFB_REQUIRE(S >= 1 && in_size >= 1 && in_size <= S, "cfb_degrade_faces: need 1 <= in_size <= gt_size");
   CFB_REQUIRE(ks >= 1 && ks % 2 == 1 && ks <= kMaxKsize, "cfb_degrade_faces: the kernel size must be odd and at most 63");
@@ -470,7 +479,7 @@ int degrade(const uint8_t* gt, int batch, int S, const double* kernels, int ks, 
     CFB_REQUIRE(!qualities || (qualities[b] >= 0 && qualities[b] <= 100), "cfb_degrade_faces: quality must be 0 (none) or 1..100");
     CFB_REQUIRE(!noise_offsets || noise_offsets[b] < 0 || noise, "cfb_degrade_faces: noise offsets without a noise field");
   }
-  const DegPlan P = plan_degrade(batch, S, sizes, qualities, noise_offsets);
+  const DegPlan P = plan_degrade(batch, S, sizes, qualities, noise_offsets, fstate_offsets);
   CFB_REQUIRE(ws && ws_bytes >= P.total, "cfb_degrade_faces: workspace too small (cfb_degrade_workspace_bytes)");
   char* w = static_cast<char*>(ws);
   DegFace* dfaces = reinterpret_cast<DegFace*>(w + P.desc);
@@ -492,7 +501,287 @@ int degrade(const uint8_t* gt, int batch, int S, const double* kernels, int ks, 
   CFB_LAUNCH_CHECK();
   CFB_CHECK(launch_jpeg(djpg, (int)P.jpg.size(), P.max_blocks, P.max_px, uimg, planes, dimg, st));
   final_kernel<<<dim3((unsigned)(((int64_t)in_size * in_size + kThreads - 1) / kThreads), batch), kThreads, 0, st>>>(
-      dfaces, fimg, dimg, in_size, lq);
+      dfaces, fimg, dimg, in_size, lq, fstate);
+  CFB_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------ colour stages
+// FFHQBlindDataset.__getitem__:253-273 on the float image before its clip(round(x * 255)): the shift, cv2's gray, then
+// BGR -> RGB and torchvision's adjust_* ops in the drawn order, each with torch's float32 op sequence (separate mul and add
+// kernels, so nothing is contracted) and clamps.  adjust_contrast blends with the mean gray of the whole face, so a face's
+// ops split there: color_pre_kernel runs the ops before it and writes per-block float64 sums of the gray, color_mean_kernel
+// adds them in block order, color_post_kernel runs the rest and rounds.  Mask faces (inpainting) are where(mask, 255, gt).
+constexpr int kShift = 1, kGray = 2, kMask = 4;
+constexpr int kBrightness = 0, kContrast = 1, kSaturation = 2, kHue = 3;   // color_jitter_pt's fn_id
+
+struct ColorFace {
+  int flags;        // kShift | kGray | kMask
+  int nops;         // torchvision ops, 0..4
+  int pre;          // ops before the contrast mean: the position of contrast, or nops
+  int pad;
+  int op[4];
+  float jit[3];     // the shift, BGR
+  float fac[4];     // each op's factor
+  float omf[4];     // float32(1.0 - factor), as _blend's Python double cast to float32
+  int64_t state;    // offset of the face's float state [n][3] (RGB after the first kernel) in floats, -1 = no colour stage
+};
+
+__device__ __forceinline__ float clamp01(float x) { return fminf(fmaxf(x, 0.f), 1.f); }
+
+// rgb_to_grayscale: (0.2989 r + 0.587 g) + 0.114 b
+__device__ __forceinline__ float tv_gray(float r, float g, float b) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(0.2989f, r), __fmul_rn(0.587f, g)), __fmul_rn(0.114f, b));
+}
+
+// _blend: (ratio * x + (1.0 - ratio) * y).clamp(0, 1)
+__device__ __forceinline__ float blend(float x, float y, float f, float omf) {
+  return clamp01(__fadd_rn(__fmul_rn(f, x), __fmul_rn(omf, y)));
+}
+
+// adjust_hue: _rgb2hsv, (h + f) % 1.0, _hsv2rgb
+__device__ __forceinline__ void hue_shift(float& r, float& g, float& b, float f) {
+  const float maxc = fmaxf(fmaxf(r, g), b), minc = fminf(fminf(r, g), b);
+  const bool eqc = maxc == minc;
+  const float cr = __fsub_rn(maxc, minc);
+  const float s = __fdiv_rn(cr, eqc ? 1.f : maxc);
+  const float crd = eqc ? 1.f : cr;
+  const float rc = __fdiv_rn(__fsub_rn(maxc, r), crd), gc = __fdiv_rn(__fsub_rn(maxc, g), crd);
+  const float bc = __fdiv_rn(__fsub_rn(maxc, b), crd);
+  const float hr = __fmul_rn(maxc == r ? 1.f : 0.f, __fsub_rn(bc, gc));
+  const float hg = __fmul_rn(maxc == g && maxc != r ? 1.f : 0.f, __fsub_rn(__fadd_rn(2.f, rc), bc));
+  const float hb = __fmul_rn(maxc != g && maxc != r ? 1.f : 0.f, __fsub_rn(__fadd_rn(4.f, gc), rc));
+  float h = fmodf(__fadd_rn(__fdiv_rn(__fadd_rn(__fadd_rn(hr, hg), hb), 6.f), 1.f), 1.f);
+  h = fmodf(__fadd_rn(h, f), 1.f);            // torch.remainder: fmod, plus the divisor when the signs differ
+  if (h < 0.f) h = __fadd_rn(h, 1.f);
+  const float v = maxc, h6 = __fmul_rn(h, 6.f), fi = floorf(h6), fr = __fsub_rn(h6, fi);
+  const float p = clamp01(__fmul_rn(v, __fsub_rn(1.f, s)));
+  const float q = clamp01(__fmul_rn(v, __fsub_rn(1.f, __fmul_rn(s, fr))));
+  const float t = clamp01(__fmul_rn(v, __fsub_rn(1.f, __fmul_rn(s, __fsub_rn(1.f, fr)))));
+  switch ((int)fi % 6) {
+    case 0: r = v, g = t, b = p; break;
+    case 1: r = q, g = v, b = p; break;
+    case 2: r = p, g = v, b = t; break;
+    case 3: r = p, g = q, b = v; break;
+    case 4: r = t, g = p, b = v; break;
+    default: r = v, g = p, b = q; break;
+  }
+}
+
+__device__ __forceinline__ void apply_op(const ColorFace& c, int k, float& r, float& g, float& b, float mean) {
+  const float f = c.fac[k], omf = c.omf[k];
+  switch (c.op[k]) {
+    case kBrightness:
+      r = blend(r, 0.f, f, omf), g = blend(g, 0.f, f, omf), b = blend(b, 0.f, f, omf);
+      break;
+    case kContrast:
+      r = blend(r, mean, f, omf), g = blend(g, mean, f, omf), b = blend(b, mean, f, omf);
+      break;
+    case kSaturation: {
+      const float y = tv_gray(r, g, b);
+      r = blend(r, y, f, omf), g = blend(g, y, f, omf), b = blend(b, y, f, omf);
+      break;
+    }
+    default:
+      hue_shift(r, g, b, f);
+  }
+}
+
+// fixed-order block sum: lanes by shuffle, then the warps' sums in warp order
+__device__ __forceinline__ double block_sum(double v) {
+  __shared__ double warp_sums[kThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, warp_sums[w]);
+  return s;
+}
+
+// the shift, gray, BGR -> RGB and the ops before contrast; the gray of the result summed per block when contrast follows.
+// gt is the uint8 source of faces without corruption (state then starts as gt / 255), NULL when final_kernel wrote it.
+__global__ void __launch_bounds__(kThreads) color_pre_kernel(const ColorFace* __restrict__ faces, const uint8_t* __restrict__ gt,
+                                                             int n_px, float* __restrict__ state, double* __restrict__ partials) {
+  const int b = blockIdx.y;
+  const ColorFace& c = faces[b];       // read in place: the ops are indexed at run time
+  if (c.state < 0) return;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  double gsum = 0.;
+  if (idx < n_px) {
+    float* st = state + c.state + idx * 3;
+    float x[3];
+    if (gt) {
+      const uint8_t* p = gt + ((int64_t)b * n_px + idx) * 3;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) x[k] = __fdiv_rn((float)p[k], 255.f);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) x[k] = st[k];
+    }
+    if (c.flags & kShift) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) x[k] = clamp01(__fadd_rn(x[k], c.jit[k]));
+    }
+    if (c.flags & kGray)     // cv2.cvtColor(float32, COLOR_BGR2GRAY): fma(r, 0.299, fma(b, 0.114, g * 0.587))
+      x[0] = x[1] = x[2] = __fmaf_rn(x[2], 0.299f, __fmaf_rn(x[0], 0.114f, __fmul_rn(x[1], 0.587f)));
+    float r = x[2], g = x[1], bl = x[0];
+    for (int k = 0; k < c.pre; ++k) apply_op(c, k, r, g, bl, 0.f);
+    if (c.pre < c.nops) gsum = (double)tv_gray(r, g, bl);
+    st[0] = r, st[1] = g, st[2] = bl;
+  }
+  if (c.pre < c.nops) {
+    const double s = block_sum(gsum);
+    if (threadIdx.x == 0) partials[(int64_t)b * gridDim.x + blockIdx.x] = s;
+  }
+}
+
+// per face, the block sums in block order, / n_px in float64, rounded once to float32 (NaN for faces without contrast)
+__global__ void __launch_bounds__(kThreads) color_mean_kernel(const ColorFace* __restrict__ faces, const double* __restrict__ partials,
+                                                              int nblk, int n_px, float* __restrict__ means) {
+  const int b = blockIdx.x;
+  const ColorFace& c = faces[b];
+  if (c.state < 0 || c.pre >= c.nops) {
+    if (threadIdx.x == 0) means[b] = __int_as_float(0x7fc00000);
+    return;
+  }
+  double v = 0.;
+  for (int i = threadIdx.x; i < nblk; i += kThreads) v = __dadd_rn(v, partials[(int64_t)b * nblk + i]);
+  const double s = block_sum(v);
+  if (threadIdx.x == 0) means[b] = __double2float_rn(s / n_px);
+}
+
+// contrast and the ops after it, RGB -> BGR, round half to even, clip; mask faces and faces without colour stages
+__global__ void __launch_bounds__(kThreads) color_post_kernel(const ColorFace* __restrict__ faces, const uint8_t* __restrict__ gt,
+                                                              const uint8_t* __restrict__ masks, int n_px,
+                                                              const float* __restrict__ state, const float* __restrict__ means,
+                                                              uint8_t* __restrict__ lq) {
+  const int b = blockIdx.y;
+  const ColorFace& c = faces[b];       // read in place: the ops are indexed at run time
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_px) return;
+  uint8_t* o = lq + ((int64_t)b * n_px + idx) * 3;
+  if (c.state < 0) {       // without corruption: clip(round(float32(k / 255) * 255)) = k; corrupted faces: lq is written
+    if (!gt) return;
+    const uint8_t* p = gt + ((int64_t)b * n_px + idx) * 3;
+    const bool m = (c.flags & kMask) && masks[(int64_t)b * n_px + idx];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) o[k] = m ? 255 : p[k];
+    return;
+  }
+  const float* st = state + c.state + idx * 3;
+  float r = st[0], g = st[1], bl = st[2];
+  if (c.pre < c.nops) {
+    const float mean = means[b];
+    for (int k = c.pre; k < c.nops; ++k) apply_op(c, k, r, g, bl, mean);
+  }
+  o[0] = sat_u8(__fmul_rn(bl, 255.f));
+  o[1] = sat_u8(__fmul_rn(g, 255.f));
+  o[2] = sat_u8(__fmul_rn(r, 255.f));
+}
+
+struct ColorPlan {
+  std::vector<ColorFace> faces;
+  std::vector<int64_t> fstate;
+  int64_t deg, desc, state, partials, means, total;
+  int nblk;
+};
+
+// ops: [batch][6] int32 (flags, nops, op[4]); factors: [batch][7] float32 (jit[3], factor[4]); NULL = no colour stages
+ColorPlan plan_color(int batch, int S, const int32_t* sizes, const int32_t* qualities, int in_size, const int32_t* ops,
+                     const float* factors) {
+  ColorPlan P;
+  P.faces.resize(batch);
+  P.fstate.assign(batch, -1);
+  const int64_t n_px = (int64_t)in_size * in_size;
+  int64_t state = 0;
+  for (int b = 0; b < batch; ++b) {
+    ColorFace& c = P.faces[b];
+    c = ColorFace{};
+    c.state = -1;
+    if (ops) {
+      c.flags = ops[b * 6];
+      c.nops = ops[b * 6 + 1];
+      c.pre = c.nops;
+      for (int k = 0; k < c.nops; ++k) {
+        c.op[k] = ops[b * 6 + 2 + k];
+        c.fac[k] = factors[b * 7 + 3 + k];
+        c.omf[k] = (float)(1.0 - (double)c.fac[k]);
+        if (c.op[k] == kContrast) c.pre = k;
+      }
+      for (int k = 0; k < 3; ++k) c.jit[k] = factors[b * 7 + k];
+    }
+    if ((c.flags & (kShift | kGray)) || c.nops > 0) {
+      c.state = P.fstate[b] = state;
+      state += n_px * 3;
+    }
+  }
+  P.nblk = (int)((n_px + kThreads - 1) / kThreads);
+  P.deg = sizes ? align256(plan_degrade(batch, S, sizes, qualities, nullptr).total) : 0;
+  P.desc = P.deg;
+  P.state = P.desc + align256((int64_t)batch * sizeof(ColorFace));
+  P.partials = P.state + align256(state * 4);
+  P.means = P.partials + align256((int64_t)batch * P.nblk * 8);
+  P.total = P.means + align256((int64_t)batch * 4);
+  return P;
+}
+
+bool valid_color(int batch, bool corrupt, const int32_t* ops, const float* factors, const uint8_t* masks) {
+  if (!ops) return true;
+  if (!factors) return false;
+  for (int b = 0; b < batch; ++b) {
+    const int flags = ops[b * 6], nops = ops[b * 6 + 1];
+    if (flags & ~(kShift | kGray | kMask) || nops < 0 || nops > 4) return false;
+    if ((flags & kMask) && (corrupt || !masks || (flags & ~kMask) || nops)) return false;
+    int seen = 0;
+    for (int k = 0; k < nops; ++k) {
+      const int op = ops[b * 6 + 2 + k];
+      const float f = factors[b * 7 + 3 + k];
+      if (op < 0 || op > 3 || (seen >> op & 1) || !isfinite(f)) return false;
+      if (op == kHue ? !(f >= -0.5f && f <= 0.5f) : !(f >= 0.f)) return false;
+      seen |= 1 << op;
+    }
+    for (int k = 0; k < 3; ++k)
+      if ((flags & kShift) && !isfinite(factors[b * 7 + k])) return false;
+  }
+  return true;
+}
+
+int degrade_color(const uint8_t* gt, int batch, int S, const double* kernels, int ks, const int32_t* sizes, const int32_t* qualities,
+                  const float* noise, const int64_t* noise_offsets, const int32_t* ops, const float* factors, const uint8_t* masks,
+                  int in_size, uint8_t* lq, void* ws, int64_t ws_bytes, float* means_out, cudaStream_t st) {
+  const bool corrupt = kernels != nullptr;
+  CFB_REQUIRE(batch >= 0 && batch <= 65535, "cfb_degrade_faces_color: batch must be 0..65535");
+  CFB_REQUIRE(S >= 1 && in_size >= 1 && in_size <= S, "cfb_degrade_faces_color: need 1 <= in_size <= gt_size");
+  CFB_REQUIRE(corrupt || in_size == S, "cfb_degrade_faces_color: without corruption in_size must equal gt_size");
+  CFB_REQUIRE(corrupt == (sizes != nullptr), "cfb_degrade_faces_color: give kernels and small sizes together, or neither");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(gt && lq, "cfb_degrade_faces_color: NULL argument");
+  CFB_REQUIRE(valid_color(batch, corrupt, ops, factors, masks),
+              "cfb_degrade_faces_color: bad colour descriptor (flags, op codes, repeated ops, factors, or a mask with "
+              "corruption or colour stages)");
+  if (corrupt)
+    for (int b = 0; b < batch; ++b)
+      CFB_REQUIRE(sizes[b] >= 1 && sizes[b] <= S, "cfb_degrade_faces_color: small sizes must be 1..gt_size");
+  const ColorPlan P = plan_color(batch, S, sizes, qualities, in_size, ops, factors);
+  CFB_REQUIRE(ws && ws_bytes >= P.total, "cfb_degrade_faces_color: workspace too small (cfb_degrade_color_workspace_bytes)");
+  char* w = static_cast<char*>(ws);
+  ColorFace* dfaces = reinterpret_cast<ColorFace*>(w + P.desc);
+  float* state = reinterpret_cast<float*>(w + P.state);
+  double* partials = reinterpret_cast<double*>(w + P.partials);
+  float* means = means_out ? means_out : reinterpret_cast<float*>(w + P.means);
+  if (corrupt)
+    CFB_CHECK(degrade(gt, batch, S, kernels, ks, sizes, qualities, noise, noise_offsets, in_size, lq, ws, P.deg, nullptr, nullptr,
+                      st, P.fstate.data(), state));
+  CFB_CUDA(cudaMemcpyAsync(dfaces, P.faces.data(), P.faces.size() * sizeof(ColorFace), cudaMemcpyHostToDevice, st));
+  const int64_t n_px = (int64_t)in_size * in_size;
+  const uint8_t* src = corrupt ? nullptr : gt;
+  color_pre_kernel<<<dim3((unsigned)P.nblk, batch), kThreads, 0, st>>>(dfaces, src, (int)n_px, state, partials);
+  CFB_LAUNCH_CHECK();
+  color_mean_kernel<<<batch, kThreads, 0, st>>>(dfaces, partials, P.nblk, (int)n_px, means);
+  CFB_LAUNCH_CHECK();
+  color_post_kernel<<<dim3((unsigned)P.nblk, batch), kThreads, 0, st>>>(dfaces, src, masks, (int)n_px, state, means, lq);
   CFB_LAUNCH_CHECK();
   return 0;
 }
@@ -533,6 +822,40 @@ int cfb_debug_degrade_faces(const uint8_t* gt, int32_t batch, int32_t gt_size, c
   DEG_API_BEGIN
   return cfb::degrade(gt, batch, gt_size, kernels, ksize, small_sizes, qualities, noise, noise_offsets, in_size, lq, workspace,
                       workspace_bytes, stage_a, pre_jpeg, (cudaStream_t)stream);
+  DEG_API_END
+}
+
+int64_t cfb_degrade_color_workspace_bytes(int32_t batch, int32_t gt_size, const int32_t* small_sizes, const int32_t* qualities,
+                                          const int32_t* color_ops, int32_t in_size) {
+  if (batch < 0 || gt_size < 1 || in_size < 1 || in_size > gt_size || (!small_sizes && in_size != gt_size)) return -1;
+  for (int b = 0; b < batch; ++b) {
+    if (small_sizes && (small_sizes[b] < 1 || small_sizes[b] > gt_size || (qualities && (qualities[b] < 0 || qualities[b] > 100))))
+      return -1;
+    if (color_ops && (color_ops[b * 6 + 1] < 0 || color_ops[b * 6 + 1] > 4)) return -1;
+  }
+  std::vector<float> zeros(color_ops ? (size_t)batch * 7 : 0, 0.f);
+  return cfb::plan_color(batch, gt_size, small_sizes, qualities, in_size, color_ops, color_ops ? zeros.data() : nullptr).total;
+}
+
+int cfb_degrade_faces_color(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                            const int32_t* small_sizes, const int32_t* qualities, const float* noise, const int64_t* noise_offsets,
+                            const int32_t* color_ops, const float* color_factors, const uint8_t* masks, int32_t in_size,
+                            uint8_t* lq, void* workspace, int64_t workspace_bytes, void* stream) {
+  DEG_API_BEGIN
+  return cfb::degrade_color(gt, batch, gt_size, kernels, ksize, small_sizes, qualities, noise, noise_offsets, color_ops,
+                            color_factors, masks, in_size, lq, workspace, workspace_bytes, nullptr, (cudaStream_t)stream);
+  DEG_API_END
+}
+
+int cfb_debug_degrade_faces_color(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                                  const int32_t* small_sizes, const int32_t* qualities, const float* noise,
+                                  const int64_t* noise_offsets, const int32_t* color_ops, const float* color_factors,
+                                  const uint8_t* masks, int32_t in_size, uint8_t* lq, void* workspace, int64_t workspace_bytes,
+                                  float* contrast_means, void* stream) {
+  DEG_API_BEGIN
+  CFB_REQUIRE(contrast_means || batch == 0, "cfb_debug_degrade_faces_color: NULL contrast_means");
+  return cfb::degrade_color(gt, batch, gt_size, kernels, ksize, small_sizes, qualities, noise, noise_offsets, color_ops,
+                            color_factors, masks, in_size, lq, workspace, workspace_bytes, contrast_means, (cudaStream_t)stream);
   DEG_API_END
 }
 

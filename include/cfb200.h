@@ -600,6 +600,38 @@ int     cfb_debug_degrade_faces(const uint8_t* gt, int32_t batch, int32_t gt_siz
                                 const int32_t* small_sizes, const int32_t* qualities, const float* noise,
                                 const int64_t* noise_offsets, int32_t in_size, uint8_t* lq, void* workspace,
                                 int64_t workspace_bytes, float* stage_a, uint8_t* pre_jpeg, void* stream);
+/* ---- Colorization and inpainting inputs: FFHQBlindDataset's colour and mask stages (ffhq_blind_dataset.py:242-273) ----
+ * applied to the dataset's float32 image before its clip(round(x * 255)), so each face rounds once, as the dataset does.
+ * With kernels and small_sizes (both or neither), that image is the corruption chain's final INTER_LINEAR (arguments as
+ * cfb_degrade_faces); without them it is gt / 255 and in_size must equal gt_size (the dataset does not resize then).
+ * color_ops (host; NULL = no colour stages) [batch][6] int32: flags (1 shift, 2 gray, 4 mask), the number of torchvision ops
+ * n (0..4), then n op codes in application order (0 brightness, 1 contrast, 2 saturation, 3 hue; each at most once).
+ * color_factors (host) [batch][7] float32: the shift in BGR order, then the n factors (>= 0; hue in [-0.5, 0.5]).  Per face:
+ *   shift   x + shift[c] in float32, clip to [0, 1]
+ *   gray    cv2.cvtColor(float32, COLOR_BGR2GRAY) bit for bit, fma(r, 0.299f, fma(b, 0.114f, g * 0.587f)), on 3 channels
+ *   ops     on RGB, torchvision's adjust_brightness / _contrast / _saturation / _hue with torch's float32 op sequence:
+ *           _blend = clamp(f * x + float32(1.0 - f) * y, 0, 1) without contraction, gray = (0.2989 r + 0.587 g) + 0.114 b,
+ *           hue = _rgb2hsv, (h + f) % 1.0, _hsv2rgb
+ *   output  round half to even of x * 255, clip -> lq uint8 BGR [batch, in_size, in_size, 3]
+ * The contrast mean is the mean gray of the whole face just before the contrast op: float64 sums per 256-pixel block, added
+ * in block order, / n in float64, rounded once to float32 -- the same whatever the batch and on every run.
+ * Mask faces (flags 4 alone, no corruption): masks is a device uint8 [batch, gt_size, gt_size] array, and lq is 255 where
+ * the face's mask is nonzero and gt elsewhere.  Faces without any stage give cfb_degrade_faces' bytes (with corruption)
+ * or gt (without).  Mixed stages and op orders run in the same four launches after the chain, without host synchronisation.
+ * Workspace: cfb_degrade_color_workspace_bytes (-1 for bad arguments).
+ * debug_degrade_faces_color (test entry point): also each face's contrast mean (device float32 [batch]; NaN without one). */
+int64_t cfb_degrade_color_workspace_bytes(int32_t batch, int32_t gt_size, const int32_t* small_sizes, const int32_t* qualities,
+                                          const int32_t* color_ops, int32_t in_size);
+int     cfb_degrade_faces_color(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                                const int32_t* small_sizes, const int32_t* qualities, const float* noise,
+                                const int64_t* noise_offsets, const int32_t* color_ops, const float* color_factors,
+                                const uint8_t* masks, int32_t in_size, uint8_t* lq, void* workspace, int64_t workspace_bytes,
+                                void* stream);
+int     cfb_debug_degrade_faces_color(const uint8_t* gt, int32_t batch, int32_t gt_size, const double* kernels, int32_t ksize,
+                                      const int32_t* small_sizes, const int32_t* qualities, const float* noise,
+                                      const int64_t* noise_offsets, const int32_t* color_ops, const float* color_factors,
+                                      const uint8_t* masks, int32_t in_size, uint8_t* lq, void* workspace,
+                                      int64_t workspace_bytes, float* contrast_means, void* stream);
 int64_t cfb_jpeg_workspace_bytes(int32_t n, int32_t h, int32_t w);
 int     cfb_jpeg_roundtrip(const uint8_t* src, uint8_t* dst, int32_t n, int32_t h, int32_t w, const int32_t* qualities,
                            void* workspace, int64_t workspace_bytes, void* stream);
