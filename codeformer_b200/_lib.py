@@ -81,6 +81,8 @@ SIGNATURES = {
                                          c_int32, c_int32]),
     'cfb_debug_bmm_tc_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32]),
     'cfb_debug_bmm_tc': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_debug_layer_norm_planes': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, c_int32, _P]),
+    'cfb_debug_code_lookup': (c_int, [_P, _P, _P, _P, c_int32, c_int32, c_int32, _P]),
     'cfb_debug_gn_partials_workspace_bytes': (c_int64, [c_int32, c_int32]),
     'cfb_debug_gn_coef_from_partials': (c_int, [_P, c_int32, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_float, _P, c_int64, _P]),
     'cfb_debug_gn_cat_partials': (c_int, [_P, _P, _P, c_int64, c_int32, _P]),

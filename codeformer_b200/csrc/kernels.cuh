@@ -46,6 +46,9 @@ void set_error(const std::string& msg);
 #define CFB_STATUS_OVERFLOW 2u
 int async_status_init(cudaStream_t st);      // per-device one-time setup (idempotent)
 int async_status_check(const char* where);   // non-zero + set_error() when a kernel reported a failure since the last check
+// device pointer of the current device's status word (bound on first use), for kernels outside conv_tc.cu: they take it as
+// an argument (the library is linked without -rdc, so conv_tc.cu's device symbols are not visible to them)
+int async_status_word(unsigned** dev_word);
 int tc_bind_status_word(unsigned* host_mapped_dev_ptr, long long wait_limit_cycles);   // conv_tc.cu: device symbols of this device
 int tc_clear_abort();
 int tc_set_stamps(long long* dev_ptr);     // diagnostics: phase stamps of CTA 0 (cfb_debug_set_stamps)

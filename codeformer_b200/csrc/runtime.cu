@@ -48,6 +48,7 @@ void reset_launch_count() { g_launches.store(0); }
 // (SURVEY.md section 8(b) "Errors"; /root/reference/inference_codeformer.py:209-211).
 static std::mutex g_status_mu;
 static unsigned* g_status_words = nullptr;            // host pointer of a mapped, portable allocation: [64] words
+static unsigned* g_status_dev_word[64] = {};          // device pointer of word `dev`, as bound on device `dev`
 static uint64_t g_status_bound = 0;                   // devices whose symbols are bound
 static long long g_wait_limit_cycles = 4000000000LL;
 
@@ -63,8 +64,18 @@ int async_status_init(cudaStream_t) {
   }
   unsigned* dptr = nullptr;
   CFB_CUDA(cudaHostGetDevicePointer((void**)&dptr, g_status_words, 0));
+  g_status_dev_word[dev] = dptr + dev;
   CFB_CHECK(tc_bind_status_word(dptr + dev, g_wait_limit_cycles));
   g_status_bound |= 1ull << dev;
+  return 0;
+}
+
+int async_status_word(unsigned** dev_word) {
+  CFB_CHECK(async_status_init(nullptr));      // after the first call per device: a lock and a bit test, no CUDA call
+  int dev = 0;
+  CFB_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(g_status_mu);
+  *dev_word = g_status_dev_word[dev];
   return 0;
 }
 
@@ -4461,6 +4472,21 @@ int cfb_layer_norm(const float* x, const float* gamma, const float* beta, float*
                    int32_t pos_rows, int32_t rows, int32_t c, void* stream) {
   API_BEGIN
   return cfb::layer_norm(x, gamma, beta, y, y2, pos, pos_rows, rows, c, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_debug_layer_norm_planes(const float* x, const float* gamma, const float* beta, void* y_planes, void* y2_planes,
+                                const float* pos, int32_t pos_rows, int32_t rows, int32_t c, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(x && gamma && beta && (y_planes || y2_planes), "cfb_debug_layer_norm_planes: NULL argument");
+  CFB_REQUIRE(!y2_planes || (pos && pos_rows > 0), "cfb_debug_layer_norm_planes: y2_planes needs pos and pos_rows > 0");
+  return cfb::layer_norm_planes(x, gamma, beta, y_planes, y2_planes, pos, pos_rows, rows, c, (cudaStream_t)stream);
+  API_END(1)
+}
+int cfb_debug_code_lookup(const float* logits, const float* codebook, int64_t* idx, float* quant, int32_t T, int32_t K,
+                          int32_t D, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(logits && codebook && (idx || quant) && T >= 0 && K > 0 && D > 0, "cfb_debug_code_lookup: bad argument");
+  return cfb::argmax_gather(logits, codebook, idx, quant, T, K, D, (cudaStream_t)stream);
   API_END(1)
 }
 int cfb_adain_nhwc(const float* content, const float* style, float* out, int32_t batch, int32_t hw, int32_t c, void* stream) {

@@ -960,12 +960,14 @@ __device__ __forceinline__ void split_store4(__half* __restrict__ hi, __half* __
 
 // PLANES: y / y2 are written as fp16 hi/lo operand planes (hi = rn(v), lo = rn(v - hi)) for the tensor-core linears that
 // consume them -- the LayerNorm output of a TransformerSALayer is only ever a GEMM operand (codeformer_arch.py:124-131),
-// so no fp32 copy and no separate operand-preparation pass exist on that path.  |LN output| is O(10): inside the fp16 range.
+// so no fp32 copy and no separate operand-preparation pass exist on that path.  |LN output| reaches |gamma| sqrt(C - 1) + |beta|:
+// a value past the fp16 range (65504) sets the overflow bit of the status word (`status`, host-mapped), as every other
+// producer of operand planes does -- never a silent inf / NaN operand.
 template <int C, bool PLANES>
 __global__ void __launch_bounds__(256) layer_norm_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, float* __restrict__ y,
                                                          float* __restrict__ y2, const float* __restrict__ pos,
-                                                         int pos_rows, int rows, int64_t plane_elems) {
+                                                         int pos_rows, int rows, int64_t plane_elems, unsigned* status) {
   constexpr int V = C / 128;  // float4 per lane
   pdl_launch_dependents();
   pdl_wait();
@@ -992,6 +994,7 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const float* __restrict
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
   const float rstd = rsqrtf(sq * (1.f / C) + 1e-5f);
+  float vmax = 0.f;                          // PLANES: largest |value| written to the operand planes
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     const int c = (i * 32 + l) * 4;
@@ -1002,24 +1005,32 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const float* __restrict
     o.z = (v[i].z - mean) * rstd * g.z + bb.z; o.w = (v[i].w - mean) * rstd * g.w + bb.w;
     const int64_t off = (int64_t)row * C + c;
     if (PLANES) {
-      if (y) split_store4(reinterpret_cast<__half*>(y), reinterpret_cast<__half*>(y) + plane_elems, off, o);
+      if (y) {
+        split_store4(reinterpret_cast<__half*>(y), reinterpret_cast<__half*>(y) + plane_elems, off, o);
+        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
+      }
     } else {
       *reinterpret_cast<float4*>(y + off) = o;
     }
     if (y2) {
       const float4 p = __ldg(reinterpret_cast<const float4*>(pos + (int64_t)(row % pos_rows) * C + c));
       const float4 o2 = make_float4(o.x + p.x, o.y + p.y, o.z + p.z, o.w + p.w);
-      if (PLANES) split_store4(reinterpret_cast<__half*>(y2), reinterpret_cast<__half*>(y2) + plane_elems, off, o2);
-      else *reinterpret_cast<float4*>(y2 + off) = o2;
+      if (PLANES) {
+        split_store4(reinterpret_cast<__half*>(y2), reinterpret_cast<__half*>(y2) + plane_elems, off, o2);
+        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(o2.x), fabsf(o2.y)), fmaxf(fabsf(o2.z), fabsf(o2.w))));
+      } else {
+        *reinterpret_cast<float4*>(y2 + off) = o2;
+      }
     }
   }
+  if (PLANES && vmax > 65504.f && status) { atomicOr_system(status, CFB_STATUS_OVERFLOW); __threadfence_system(); }
 }
 int layer_norm(const float* x, const float* gamma, const float* beta, float* y, float* y2, const float* pos,
                int pos_rows, int rows, int C, cudaStream_t st) {
   CFB_REQUIRE(C == 512, "layer_norm: only dim_embd=512 is built");
   if (rows == 0) return 0;
   CFB_LAUNCH_PDL((layer_norm_kernel<512, false>), dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, st, x, gamma, beta, y, y2, pos,
-                 pos_rows > 0 ? pos_rows : 1, rows, (int64_t)0);
+                 pos_rows > 0 ? pos_rows : 1, rows, (int64_t)0, (unsigned*)nullptr);
   return 0;
 }
 // outputs as fp16 hi/lo operand planes: [hi plane | lo plane], each align1024(rows*C*2) bytes (the conv engine's layout)
@@ -1027,9 +1038,11 @@ int layer_norm_planes(const float* x, const float* gamma, const float* beta, voi
                       int pos_rows, int rows, int C, cudaStream_t st) {
   CFB_REQUIRE(C == 512, "layer_norm: only dim_embd=512 is built");
   if (rows == 0) return 0;
+  unsigned* status = nullptr;
+  CFB_CHECK(async_status_word(&status));
   const int64_t plane_elems = (int64_t)((((size_t)rows * C * 2 + 1023) / 1024 * 1024) / 2);
   CFB_LAUNCH_PDL((layer_norm_kernel<512, true>), dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, st, x, gamma, beta, (float*)y_planes,
-                 (float*)y2_planes, pos, pos_rows > 0 ? pos_rows : 1, rows, plane_elems);
+                 (float*)y2_planes, pos, pos_rows > 0 ? pos_rows : 1, rows, plane_elems, status);
   return 0;
 }
 

@@ -261,6 +261,17 @@ int cfb_debug_conv_tc_prec_wv(const float* in, const float* in2, int32_t cin1, c
 int64_t cfb_debug_bmm_tc_workspace_bytes(int32_t n, int32_t heads, int32_t d);
 int cfb_debug_bmm_tc(const float* q, const float* k, const float* v, float* out, void* out_planes, int32_t n, int32_t heads,
                      int32_t d, void* workspace, int64_t workspace_bytes, void* stream);
+/* diagnostics / tests: the LayerNorm of the forward on the wgmma engine (cfb_layer_norm's arithmetic, eps 1e-5), which writes
+ * its outputs only as fp16 operand planes: y_planes (optional) of y, y2_planes (optional; needs pos, pos_rows > 0) of
+ * y + pos[t % pos_rows].  Each is hi | lo, hi = fp16(v), lo = fp16(v - hi), each plane align1024(rows * c * 2) bytes, as
+ * cfb_debug_bmm_tc's out_planes.  A value past 65504 sets the fp16 overflow bit of the status word (cfb_check_async_status). */
+int cfb_debug_layer_norm_planes(const float* x, const float* gamma, const float* beta, void* y_planes, void* y2_planes,
+                                const float* pos, int32_t pos_rows, int32_t rows, int32_t c, void* stream);
+/* diagnostics / tests: the code lookup of the forward (codeformer_arch.py:257-259): idx[t] (optional) = the first maximum of
+ * logits[t] ([T][K]), quant[t] (optional, [T][D]) = codebook[idx[t]] ([K][D]; D a multiple of 4).  NaN logits never win; a row
+ * without a maximum (all NaN or -inf) gives index 0. */
+int cfb_debug_code_lookup(const float* logits, const float* codebook, int64_t* idx, float* quant, int32_t T, int32_t K,
+                          int32_t D, void* stream);
 /* diagnostics / tests: the GroupNorm(32) finalize of the forward on partials in the layout cfb_debug_conv_tc writes (slots of
  * 32 pixels, [n][slots][32 groups][2] floats): scale[n,c] = rstd*gamma, shift[n,c] = beta - mean*rstd*gamma over hw pixels
  * of c channels.  The workspace (>= cfb_debug_gn_partials_workspace_bytes) holds the split-finalize scratch and the ticket
