@@ -22,6 +22,7 @@ from .lpips import LPIPS, LPIPSLoss, lpips_distance   # noqa: F401
 from .degradation import degrade_faces, sample_degradations, jpeg_roundtrip   # noqa: F401
 from .fid import (InceptionV3, inception_features, fid_statistics, frechet_distance, calculate_fid,   # noqa: F401
                   fid_scores)
+from .latent import generate_latent_gt, code_scores   # noqa: F401
 
 
 def check_async_status():
@@ -38,5 +39,5 @@ __all__ = ['ARCH_REGISTRY', 'install', 'CodeFormer', 'VQAutoEncoder', 'VectorQua
            'resize_lanczos4', 'gray_adain_faces', 'add_restored_face', 'restore_aligned', 'restore_images_sweep',
            'ResNetArcFace', 'identity_similarity', 'calculate_psnr', 'calculate_ssim', 'psnr_ssim', 'LPIPS', 'LPIPSLoss', 'lpips_distance',
            'degrade_faces', 'sample_degradations', 'jpeg_roundtrip', 'InceptionV3', 'inception_features', 'fid_statistics',
-           'frechet_distance', 'calculate_fid', 'fid_scores',
+           'frechet_distance', 'calculate_fid', 'fid_scores', 'generate_latent_gt', 'code_scores',
            'check_async_status']

@@ -52,6 +52,11 @@ SIGNATURES = {
     'cfb_u8_to_input': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_output_to_u8': (c_int, [_P, _P, c_int32, c_int32, _P]),
     'cfb_vqae_forward': (c_int, [_P, _P, _P, _P, _P, _P, c_int32, _P, c_int64, _P]),
+    'cfb_encoder_workspace_bytes': (c_int64, [_P, c_int32]),
+    'cfb_encoder_forward': (c_int, [_P, _P, _P, c_int32, _P, c_int64, _P]),
+    'cfb_latent_codes_u8': (c_int, [_P, _P, _P, _P, c_int32, c_int32, _P, c_int64, _P]),
+    'cfb_codeformer_code_only_u8': (c_int, [_P, _P, _P, _P, _P, c_int32, _P, c_int64, _P]),
+    'cfb_code_scores': (c_int, [_P, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P]),
     'cfb_vq_workspace_bytes': (c_int64, [c_int32, c_int32, c_int32, c_int32]),
     'cfb_vq_nearest': (c_int, [_P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_float, _P, _P, _P, _P, _P, c_int64, _P]),
     'cfb_vq_fast_supported': (c_int32, [c_int32] * 5),

@@ -21,6 +21,7 @@ import ctypes
 import math
 import os
 import threading
+import weakref
 from typing import Dict, Optional
 
 import numpy as np
@@ -130,6 +131,23 @@ class _BlockStack(_ParamsOnly):
             elif kind == 'norm':
                 blocks.append(_Norm(cin))
         self.blocks = nn.ModuleList(blocks)
+
+
+class _Encoder(_BlockStack):
+    """``Encoder`` of vqgan_arch.py:229-273: the parameters of its ``blocks``, and a ``forward`` that runs the owning network's
+    encoder alone (``cfb_encoder_forward``).  The blocks stay parameter holders."""
+
+    def forward(self, x):
+        """``Encoder.forward`` (vqgan_arch.py:269-273): fp32 CUDA [B,3,S,S] in [-1,1] -> a fresh NCHW latent
+        [B,emb_dim,S/2^(n-1),S/2^(n-1)], bit for bit the latent the network's forward quantizes (VQAutoEncoder) or returns as
+        ``lq_feat`` (CodeFormer).  Only the encoder runs, on a workspace sized for it.  Like the reference it takes one
+        argument: scripts/generate_latent_gt.py:55 calls ``encoder(img, True)``, which raises ``TypeError`` in the reference as
+        well (its ``feat_dict`` return does not exist there either)."""
+        owner = self.__dict__.get('_cfb_owner')
+        net = owner() if owner is not None else None
+        if net is None:
+            raise RuntimeError('Encoder.forward: the encoder is not attached to a VQAutoEncoder / CodeFormer')
+        return net._encode(x)
 
 
 class _Embedding(_ParamsOnly):
@@ -268,7 +286,8 @@ class VQAutoEncoder(Precision, NativeHandle):
         self.resolution = img_size
         self.attn_resolutions = list(attn_resolutions)
         self.quantizer_type = quantizer
-        self.encoder = _BlockStack(S.encoder_plan(nf, ch_mult, res_blocks, img_size, attn_resolutions, 3, emb_dim))
+        self.encoder = _Encoder(S.encoder_plan(nf, ch_mult, res_blocks, img_size, attn_resolutions, 3, emb_dim))
+        object.__setattr__(self.encoder, '_cfb_owner', weakref.ref(self))
         self.beta = beta
         self.quantize = VectorQuantizer(codebook_size, emb_dim, beta)
         self.generator = _BlockStack(S.generator_plan(nf, ch_mult, res_blocks, img_size, attn_resolutions, emb_dim))
@@ -359,6 +378,64 @@ class VQAutoEncoder(Precision, NativeHandle):
     @property
     def last_launch_count(self) -> int:
         return 0 if self._net is None else int(_lib.load().cfb_last_launch_count(self._net))
+
+    # ---- the encoder alone: Encoder.forward (vqgan_arch.py:269-273) and the latent codes of generate_latent_gt.py ----------
+    @property
+    def latent_hw(self) -> int:
+        """Side of the latent grid: img_size / 2^(len(ch_mult)-1) (16 for the 512-pixel nets)."""
+        return self.resolution >> (len(self.ch_mult) - 1)
+
+    def _encoder_workspace(self, device, n_img):
+        """The module's workspace of the encoder-only path at ``n_img`` encoded images (cfb_encoder_workspace_bytes)."""
+        need = _lib.load().cfb_encoder_workspace_bytes(self._net, n_img)
+        if need < 0:
+            _lib.check(1, 'cfb_encoder_workspace_bytes')
+        key = ('enc', device.index, torch.cuda.current_stream(device).cuda_stream)
+        ws = self._cfb_ws.get(key)
+        if ws is None or ws.numel() < need:
+            self._cfb_ws.pop(key, None)
+            ws = None
+            ws = torch.empty(int(need), dtype=torch.uint8, device=device)
+            self._cfb_ws[key] = ws
+        return ws
+
+    def _encode(self, x):
+        x = self._check_input(x)
+        lib = _lib.load()
+        B, dev, h = x.shape[0], x.device, self.latent_hw
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            z = torch.empty((B, self.embed_dim, h, h), dtype=torch.float32, device=dev)
+            if B:
+                ws = self._encoder_workspace(dev, B)
+                _lib.check(lib.cfb_encoder_forward(self._net, _lib.ptr(x), _lib.ptr(z), B, _lib.ptr(ws), ws.numel(),
+                                                   _lib.stream(dev)), 'cfb_encoder_forward')
+        return z
+
+    def latent_codes_u8(self, faces, hflip=False):
+        """The latent codes of scripts/generate_latent_gt.py for DEVICE uint8 [B,S,S,3] HWC BGR faces (``cv2.imread`` as it is)
+        -> int64 [B,h,h] (h = ``latent_hw``): ``quantize(encoder(x))[2]['min_encoding_indices']`` of the script's chain
+        ``img2tensor(img / 255., bgr2rgb=True, float32=True)`` + ``normalize(0.5, 0.5)``, bit for bit (``cfb_latent_codes_u8``).
+        The input conversion is fused into the first conv and the decoder never runs.  ``hflip=True`` returns ``(orig, hflip)``,
+        the second the codes of ``cv2.flip(img, 1)``: both come from ONE encoder pass at batch 2B in which the mirrored images
+        are read mirrored, so the flipped copy never exists in memory."""
+        if not torch.is_tensor(faces) or not faces.is_cuda or faces.dtype != torch.uint8:
+            raise RuntimeError('latent_codes_u8 expects a CUDA uint8 tensor; there is no CPU fallback')
+        R = self.resolution
+        if faces.dim() != 4 or tuple(faces.shape[1:]) != (R, R, 3):
+            raise RuntimeError(f'latent_codes_u8 expects [B,{R},{R},3] HWC BGR faces, got {tuple(faces.shape)}')
+        faces = faces.contiguous()
+        B, dev, h = faces.shape[0], faces.device, self.latent_hw
+        n_img = 2 * B if hflip else B
+        lib = _lib.load()
+        with self._lock, torch.cuda.device(dev):
+            self._prepare(dev)
+            idx = torch.empty((n_img, h, h), dtype=torch.int64, device=dev)
+            if B:
+                ws = self._encoder_workspace(dev, n_img)
+                _lib.check(lib.cfb_latent_codes_u8(self._net, _lib.ptr(faces), _lib.ptr(idx), None, B, B if hflip else 0,
+                                                   _lib.ptr(ws), ws.numel(), _lib.stream(dev)), 'cfb_latent_codes_u8')
+        return (idx[:B], idx[B:]) if hflip else idx
 
     # ---- VQAutoEncoder.forward  vqgan_arch.py:385-389 -------------------------------------------
     def forward(self, x, return_min_encodings=True):

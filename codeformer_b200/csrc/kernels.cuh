@@ -44,6 +44,7 @@ void set_error(const std::string& msg);
 // of trapping; the host turns it into an error without poisoning the context (runtime.cu)
 #define CFB_STATUS_TIMEOUT 1u
 #define CFB_STATUS_OVERFLOW 2u
+#define CFB_STATUS_INDEX 4u      // a code index outside the codebook was given (cfb_code_scores)
 int async_status_init(cudaStream_t st);      // per-device one-time setup (idempotent)
 int async_status_check(const char* where);   // non-zero + set_error() when a kernel reported a failure since the last check
 // device pointer of the current device's status word (bound on first use), for kernels outside conv_tc.cu: they take it as
@@ -204,8 +205,9 @@ int conv_last(const float* in, const float* in_scale, const float* in_shift, con
               float* out_nchw, int N, int H, int W, int Cin, cudaStream_t st);
 // the same two kernels with the caller's image plumbing fused in (inference_codeformer.py:199-206,
 // basicsr/utils/img_util.py:9-35,38-94): uint8 HWC BGR face in, uint8 HWC BGR restored face out
+// n_orig in (0, N): images n >= n_orig are face n - n_orig mirrored left-right (cv2.flip(face, 1)); 0 = no mirror
 int conv_first_u8(const unsigned char* x_bgr_hwc, const float* wgt, const float* bias, float* out, int N, int H, int W,
-                  int Cout, cudaStream_t st, float* gn_part = nullptr);
+                  int Cout, cudaStream_t st, float* gn_part = nullptr, int n_orig = 0);
 int conv_last_u8(const float* in, const float* in_scale, const float* in_shift, const float* wgt, const float* bias,
                  unsigned char* out_bgr_hwc, int N, int H, int W, int Cin, cudaStream_t st);
 // conv_last_u8 with the inpainting blend of inference_inpainting.py:68-75 before the conversion: where the normalised input
@@ -392,6 +394,11 @@ int add_pos(const float* x, const float* pos, float* y, int rows, int pos_rows, 
 int argmax_gather(const float* logits, const float* codebook, int64_t* idx, float* quant, int T, int K, int D,
                   cudaStream_t st);
 int gather_rows(const int64_t* idx, const float* codebook, float* out, int T, int K, int D, cudaStream_t st);
+// code-prediction scores per image of S tokens, in float64 (cfb_code_scores): out[b] = {mean CE, tokens with top_idx == gt, mean
+// squared distance of lq [B*S,D] (NHWC) to E[gt]}.  A gt index outside [0,K) is not read: it sets CFB_STATUS_INDEX, and that
+// image's three values are NaN.
+int code_scores(const float* logits, const int64_t* top_idx, const int64_t* gt, const float* lq, const float* codebook, int B,
+                int S, int K, int D, double* out, cudaStream_t st);
 int adain_nhwc(const float* content, const float* style, float* out, int B, int HW, int C, cudaStream_t st);
 int nchw_to_nhwc(const float* in, float* out, int N, int C, int HW, cudaStream_t st);
 int nhwc_to_nchw(const float* in, float* out, int N, int C, int HW, cudaStream_t st);

@@ -92,6 +92,7 @@ int async_status_check(const char* where) {
   std::string msg = std::string(where) + ": a kernel of an earlier launch on this device reported";
   if (bits & CFB_STATUS_TIMEOUT) msg += " [barrier time-out: the tensor-core pipeline was aborted, results of that launch are invalid]";
   if (bits & CFB_STATUS_OVERFLOW) msg += " [fp16 operand overflow: an activation exceeded 65504 on the fp16 tensor-core operand path]";
+  if (bits & CFB_STATUS_INDEX) msg += " [code index out of range: a ground-truth code given to cfb_code_scores is outside [0, codebook_size)]";
   if (bits & CFB_STATUS_TIMEOUT) {
     if (cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();   // the aborted launch has drained; the context is healthy
     tc_clear_abort();
@@ -600,6 +601,7 @@ struct Fwd {
   int engine;   // 0 auto, 1 f32, 2 tc
   // caller-side image plumbing fused into the first / last conv (cfb_codeformer_forward_u8): uint8 HWC BGR faces
   const unsigned char* in_u8 = nullptr;
+  int in_u8_orig = 0;         // in (0, N): images n >= in_u8_orig are face n - in_u8_orig mirrored (cfb_latent_codes_u8)
   unsigned char* out_u8 = nullptr;
   bool inpaint = false;       // conv_last blends out_u8 with in_u8 as inference_inpainting.py does (cfb_codeformer_inpaint_u8)
   bool single_pass = false;   // the convs issued now run single-pass fp16 (ConvArgs::single_pass): set by generator()
@@ -928,7 +930,9 @@ struct Fwd {
       CFB_CHECK(alloc_raw((void**)&x.gn_part, (size_t)B * x.gn_slots * 64 * sizeof(float)));
     }
     if (!dry) {
-      if (in_u8) CFB_CHECK(conv_first_u8(in_u8, n->enc[0].conv.w_f32, n->enc[0].conv.bias, x.p, B, c.img_size, c.img_size, c.nf, st, x.gn_part));
+      if (in_u8)
+        CFB_CHECK(conv_first_u8(in_u8, n->enc[0].conv.w_f32, n->enc[0].conv.bias, x.p, B, c.img_size, c.img_size, c.nf, st, x.gn_part,
+                                in_u8_orig));
       else CFB_CHECK(conv_first(x_nchw, n->enc[0].conv.w_f32, n->enc[0].conv.bias, x.p, B, c.img_size, c.img_size, c.nf, st, x.gn_part));
     }
     CFB_CHECK(capture("enc.0", x));
@@ -1236,6 +1240,51 @@ static int vqae_forward_impl(cfb_net* n, const float* x, float* out, int64_t* id
   }
   f.release(z);
   CFB_CHECK(f.generator(zq, out, nullptr, {}, 0.f));
+  return 0;
+}
+
+// Encoder.forward alone (vqgan_arch.py:269-273) for either network kind; the generator and, for CodeFormer, the Transformer
+// never run.  B images are encoded.  x_u8 (uint8 HWC BGR faces) replaces x; with n_orig in (0, B), images b >= n_orig are face
+// b - n_orig mirrored (conv_first_u8).  latent_nchw [B,D,h,w] is optional when idx is given.  idx [B*h*w]: the code selection
+// of VectorQuantizer.forward on that latent, through the same library entry that module calls (cfb_vq_nearest_fast where
+// cfb_vq_fast_supported, else cfb_vq_nearest), so the indices equal quantize(encoder(x)) bit for bit.
+static int encoder_impl(cfb_net* n, const float* x, const unsigned char* x_u8, int n_orig, float* latent_nchw, int64_t* idx,
+                        int B, void* ws, int64_t ws_bytes, cudaStream_t st, bool dry) {
+  CFB_REQUIRE(dry || n->prepared, "cfb_net_prepare has not been called");
+  CFB_REQUIRE(B >= 0, "negative batch");
+  if (B == 0) return 0;
+  if (!dry) CFB_CHECK(check_device(n));
+  n->arena.reset(ws, (size_t)ws_bytes, dry);
+  Fwd f{n, st, n->arena, dry, n->engine};
+  f.in_u8 = x_u8;
+  f.in_u8_orig = n_orig;
+  const cfb_config& c = n->cfg;
+  Tensor z;
+  CFB_CHECK(f.encoder(x, B, z, nullptr, {}));
+  const int H = z.H, W = z.W, D = z.C, K = c.codebook_size;
+  float* zn = latent_nchw;
+  if (!zn) CFB_CHECK(f.alloc_raw((void**)&zn, (size_t)B * D * H * W * 4));
+  if (!dry) CFB_CHECK(nhwc_to_nchw(z.p, zn, B, D, H * W, st));
+  f.release(z);
+  if (!idx) return 0;
+  // the quantizer's z_q and statistics are scratch here; the workspace holds either selection path
+  const size_t zq_b = ((size_t)B * D * H * W * 4 + 1023) / 1024 * 1024;
+  const size_t prep_b = ((size_t)cfb_vq_prepared_bytes(K, D) + 1023) / 1024 * 1024;
+  const size_t fast_b = prep_b + (size_t)cfb_vq_fast_workspace_bytes(B, H * W, D, K);
+  const size_t slow_b = (size_t)cfb_vq_workspace_bytes(B, H * W, D, K);
+  char* scratch = nullptr;
+  CFB_CHECK(f.alloc_raw((void**)&scratch, zq_b + 1024 + std::max(fast_b, slow_b)));
+  if (dry) return 0;
+  float* zq = (float*)scratch;
+  float* stats = (float*)(scratch + zq_b);
+  char* vws = scratch + zq_b + 1024;
+  if (cfb_vq_fast_supported(B, H, W, D, K)) {
+    CFB_CHECK(cfb_vq_prepare(n->codebook, K, D, vws, (int64_t)prep_b, st));
+    CFB_CHECK(cfb_vq_nearest_fast(zn, n->codebook, vws, B, H, W, D, K, c.beta, zq, idx, stats, nullptr, vws + prep_b,
+                                  (int64_t)(fast_b - prep_b), st));
+  } else {
+    CFB_CHECK(cfb_vq_nearest(zn, n->codebook, B, H, W, D, K, c.beta, zq, idx, stats, nullptr, vws, (int64_t)slow_b, st));
+  }
   return 0;
 }
 
@@ -4041,6 +4090,78 @@ int cfb_vqae_forward(cfb_net* n, const float* x, float* out, int64_t* idx, float
                                         (cudaStream_t)stream, false);
   n->last_launches = cfb::launch_count() - before;
   return rc;
+  API_END(1)
+}
+
+int64_t cfb_encoder_workspace_bytes(cfb_net* n, int32_t batch) {
+  API_BEGIN
+  if (!n) { cfb::set_error("cfb_encoder_workspace_bytes: NULL net"); return -1; }
+  std::lock_guard<std::mutex> lk(n->mu);
+  // the worst of the call forms: latent out alone, codes alone, both (host-only dry runs of the encoder)
+  size_t high = 0;
+  for (int m = 1; m < 4; ++m) {
+    if (cfb::encoder_impl(n, (const float*)0x1000, nullptr, 0, (m & 1) ? (float*)0x1000 : nullptr, (m & 2) ? (int64_t*)0x1000 : nullptr,
+                          batch, nullptr, 0, nullptr, true) != 0)
+      return -1;
+    if (n->arena.high() > high) high = n->arena.high();
+  }
+  return (int64_t)high + 4096;
+  API_END(-1)
+}
+
+int cfb_encoder_forward(cfb_net* n, const float* x, float* latent, int32_t batch, void* workspace, int64_t workspace_bytes,
+                        void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_encoder_forward: NULL net");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(x && latent, "cfb_encoder_forward: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  const int64_t before = cfb::launch_count();
+  const int rc = cfb::encoder_impl(n, x, nullptr, 0, latent, nullptr, batch, workspace, workspace_bytes, (cudaStream_t)stream, false);
+  n->last_launches = cfb::launch_count() - before;
+  return rc;
+  API_END(1)
+}
+
+int cfb_latent_codes_u8(cfb_net* n, const uint8_t* faces_bgr, int64_t* idx, float* latent, int32_t batch, int32_t mirror,
+                        void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_latent_codes_u8: NULL net");
+  CFB_REQUIRE(batch >= 0 && mirror >= 0 && mirror <= batch, "cfb_latent_codes_u8: needs 0 <= mirror <= batch");
+  CFB_REQUIRE((int64_t)batch + mirror <= INT32_MAX / 2, "cfb_latent_codes_u8: batch too large");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(faces_bgr && idx, "cfb_latent_codes_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  const int64_t before = cfb::launch_count();
+  const int rc = cfb::encoder_impl(n, nullptr, faces_bgr, mirror ? batch : 0, latent, idx, batch + mirror, workspace,
+                                   workspace_bytes, (cudaStream_t)stream, false);
+  n->last_launches = cfb::launch_count() - before;
+  return rc;
+  API_END(1)
+}
+
+int cfb_codeformer_code_only_u8(cfb_net* n, const uint8_t* faces_bgr, float* logits, float* lq_feat, int64_t* top_idx,
+                                int32_t batch, void* workspace, int64_t workspace_bytes, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(n, "cfb_codeformer_code_only_u8: NULL net");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(faces_bgr && logits, "cfb_codeformer_code_only_u8: NULL argument");
+  std::lock_guard<std::mutex> lk(n->mu);
+  const int64_t before = cfb::launch_count();
+  const int rc = cfb::codeformer_forward_impl(n, nullptr, nullptr, logits, lq_feat, top_idx, batch, 0.f, 0, 1, workspace,
+                                              workspace_bytes, (cudaStream_t)stream, false, faces_bgr);
+  n->last_launches = cfb::launch_count() - before;
+  return rc;
+  API_END(1)
+}
+
+int cfb_code_scores(const float* logits, const int64_t* top_idx, const int64_t* gt_idx, const float* lq_feat_nhwc,
+                    const float* codebook, int32_t batch, int32_t tokens, int32_t codes, int32_t dim, double* scores, void* stream) {
+  API_BEGIN
+  CFB_REQUIRE(batch >= 0 && tokens > 0 && codes > 0 && dim > 0, "cfb_code_scores: bad shape");
+  if (batch == 0) return 0;
+  CFB_REQUIRE(logits && top_idx && gt_idx && lq_feat_nhwc && codebook && scores, "cfb_code_scores: NULL argument");
+  return cfb::code_scores(logits, top_idx, gt_idx, lq_feat_nhwc, codebook, batch, tokens, codes, dim, scores, (cudaStream_t)stream);
   API_END(1)
 }
 

@@ -237,10 +237,13 @@ __device__ __forceinline__ unsigned model_output_to_u8(float v) {
 }
 
 // U8 = true: x is the caller's uint8 HWC BGR face [N][H][W][3]; the normalisation above is a 256-entry table.
-template <int COUT, bool U8>
+// MIRROR (with U8): images n >= n_orig of the launch are face n - n_orig flipped left-right (cv2.flip(img, 1)): they read column
+// W-1-x, so the mirrored copy never exists in memory.  The other instantiations ignore n_orig.
+template <int COUT, bool U8, bool MIRROR = false>
 __global__ void __launch_bounds__(256) conv_first_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
                                                          const float* __restrict__ bias, float* __restrict__ out,
-                                                         int N, int H, int W, float* __restrict__ gn_part) {
+                                                         int N, int H, int W, float* __restrict__ gn_part, int n_orig) {
+  static_assert(U8 || !MIRROR, "conv_first: the mirror reads uint8 faces");
   __shared__ __align__(16) float ws[27 * COUT];
   __shared__ float bs[COUT];
   __shared__ float lut[U8 ? 256 : 1];
@@ -272,11 +275,13 @@ __global__ void __launch_bounds__(256) conv_first_kernel(const float* __restrict
     for (int c = 0; c < 3; ++c) {
       float v[6];
       if constexpr (U8) {
-        const unsigned char* rp8 = reinterpret_cast<const unsigned char*>(x) + ((int64_t)n * HW + (int64_t)iy * W) * 3 + (2 - c);
+        const bool flip = MIRROR && n >= n_orig;
+        const int src = flip ? n - n_orig : n;
+        const unsigned char* rp8 = reinterpret_cast<const unsigned char*>(x) + ((int64_t)src * HW + (int64_t)iy * W) * 3 + (2 - c);
 #pragma unroll
         for (int q = 0; q < 6; ++q) {
           const int ix = x0 + q - 1;
-          v[q] = (rowok && ix >= 0 && ix < W) ? lut[__ldg(rp8 + ix * 3)] : 0.f;
+          v[q] = (rowok && ix >= 0 && ix < W) ? lut[__ldg(rp8 + (flip ? W - 1 - ix : ix) * 3)] : 0.f;
         }
       } else {
         const float* rp = x + ((int64_t)n * 3 + c) * HW + (int64_t)iy * W;
@@ -346,18 +351,24 @@ int conv_first(const float* x, const float* wgt, const float* bias, float* out, 
   const int64_t quads = (int64_t)N * H * W / 4;
   if (quads == 0) return 0;
   CFB_REQUIRE(gn_part == nullptr || ((int64_t)H * W) % 256 == 0, "conv_first: GroupNorm partials need H*W % 256 == 0");
-  CFB_LAUNCH_PDL((conv_first_kernel<64, false>), dim3((unsigned)((quads + 63) / 64)), dim3(256), 0, st, x, wgt, bias, out, N, H, W, gn_part);
+  CFB_LAUNCH_PDL((conv_first_kernel<64, false>), dim3((unsigned)((quads + 63) / 64)), dim3(256), 0, st, x, wgt, bias, out, N, H, W, gn_part,
+                 N);
   return 0;
 }
 int conv_first_u8(const unsigned char* x_bgr_hwc, const float* wgt, const float* bias, float* out, int N, int H, int W,
-                  int Cout, cudaStream_t st, float* gn_part) {
+                  int Cout, cudaStream_t st, float* gn_part, int n_orig) {
   CFB_REQUIRE(Cout == 64, "conv_first: only nf=64 is built");
   CFB_REQUIRE(W % 4 == 0, "conv_first: W must be a multiple of 4");
+  CFB_REQUIRE(n_orig <= 0 || 2 * n_orig >= N, "conv_first: more mirrored images than faces");
   const int64_t quads = (int64_t)N * H * W / 4;
   if (quads == 0) return 0;
   CFB_REQUIRE(gn_part == nullptr || ((int64_t)H * W) % 256 == 0, "conv_first: GroupNorm partials need H*W % 256 == 0");
-  CFB_LAUNCH_PDL((conv_first_kernel<64, true>), dim3((unsigned)((quads + 63) / 64)), dim3(256), 0, st,
-                 reinterpret_cast<const float*>(x_bgr_hwc), wgt, bias, out, N, H, W, gn_part);
+  if (n_orig > 0 && n_orig < N)
+    CFB_LAUNCH_PDL((conv_first_kernel<64, true, true>), dim3((unsigned)((quads + 63) / 64)), dim3(256), 0, st,
+                   reinterpret_cast<const float*>(x_bgr_hwc), wgt, bias, out, N, H, W, gn_part, n_orig);
+  else
+    CFB_LAUNCH_PDL((conv_first_kernel<64, true>), dim3((unsigned)((quads + 63) / 64)), dim3(256), 0, st,
+                   reinterpret_cast<const float*>(x_bgr_hwc), wgt, bias, out, N, H, W, gn_part, N);
   return 0;
 }
 
@@ -1102,6 +1113,79 @@ __global__ void gather_rows_kernel(const int64_t* __restrict__ idx, const float*
 int gather_rows(const int64_t* idx, const float* codebook, float* out, int T, int K, int D, cudaStream_t st) {
   if (T == 0) return 0;
   gather_rows_kernel<<<(T + 7) / 8, 256, 0, st>>>(idx, codebook, out, T, K, D);
+  CFB_LAUNCH_CHECK();
+  return 0;
+}
+
+// =====================================================================================================
+// Code-prediction scores of CodeFormer's stage 2 (codeformer_idx_model.py:100-115), per image, in float64
+// =====================================================================================================
+// One CTA per image, one warp per token (tokens warp, warp + CS_WARPS, ...).  A lane sums its columns in column order, the
+// lanes meet in a butterfly, a warp adds its tokens in token order and thread 0 adds the warps in warp order: every sum has a
+// fixed order that depends on neither the batch nor the grid.  The row maximum is taken with fmaxf, which skips NaN; a NaN
+// logit then makes exp(NaN - m) and so the row's cross-entropy NaN.
+constexpr int CS_WARPS = 16;
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);   // x + y == y + x: every lane ends equal
+  return v;
+}
+__global__ void __launch_bounds__(CS_WARPS * 32, 1) code_scores_kernel(const float* __restrict__ logits,
+                                                                    const int64_t* __restrict__ top_idx,
+                                                                    const int64_t* __restrict__ gt, const float* __restrict__ lq,
+                                                                    const float* __restrict__ codebook, int S, int K, int D,
+                                                                    double* __restrict__ out, unsigned* status) {
+  __shared__ double s_ce[CS_WARPS], s_se[CS_WARPS];
+  __shared__ int s_hit[CS_WARPS], s_bad[CS_WARPS];
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, l = threadIdx.x & 31;
+  double ce = 0.0, se = 0.0;
+  int hit = 0, bad = 0;
+  for (int t = warp; t < S; t += CS_WARPS) {
+    const int64_t tok = (int64_t)b * S + t;
+    const int64_t g = __ldg(gt + tok);
+    if (g < 0 || g >= K) { bad = 1; continue; }
+    const float* lr = logits + tok * K;
+    float m = -INFINITY;
+    for (int i = l; i < K; i += 32) m = fmaxf(m, __ldg(lr + i));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    double s = 0.0;
+    for (int i = l; i < K; i += 32) s += exp((double)__ldg(lr + i) - (double)m);
+    s = warp_sum_f64(s);
+    ce += ((double)m + log(s)) - (double)__ldg(lr + g);       // logsumexp(logits_t) - logits_t[gt_t]
+    hit += __ldg(top_idx + tok) == g;
+    const float* e = codebook + g * D;
+    const float* q = lq + tok * D;
+    double d2 = 0.0;
+    for (int c = l; c < D; c += 32) {
+      const double d = (double)__ldg(e + c) - (double)__ldg(q + c);
+      d2 += d * d;
+    }
+    se += warp_sum_f64(d2);
+  }
+  if (l == 0) { s_ce[warp] = ce; s_se[warp] = se; s_hit[warp] = hit; s_bad[warp] = bad; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double c = 0.0, q = 0.0;
+    int h = 0, nb = 0;
+    for (int w = 0; w < CS_WARPS; ++w) { c += s_ce[w]; q += s_se[w]; h += s_hit[w]; nb |= s_bad[w]; }
+    if (nb) {
+      out[3 * b] = out[3 * b + 1] = out[3 * b + 2] = __longlong_as_double(0x7ff8000000000000LL);
+      if (status) { atomicOr_system(status, CFB_STATUS_INDEX); __threadfence_system(); }
+    } else {
+      out[3 * b] = c / (double)S;
+      out[3 * b + 1] = (double)h;
+      out[3 * b + 2] = q / ((double)S * (double)D);
+    }
+  }
+}
+int code_scores(const float* logits, const int64_t* top_idx, const int64_t* gt, const float* lq, const float* codebook, int B,
+                int S, int K, int D, double* out, cudaStream_t st) {
+  CFB_REQUIRE(B >= 0 && S > 0 && K > 0 && D > 0, "code_scores: bad shape");
+  if (B == 0) return 0;
+  unsigned* status = nullptr;
+  CFB_CHECK(async_status_word(&status));
+  code_scores_kernel<<<B, CS_WARPS * 32, 0, st>>>(logits, top_idx, gt, lq, codebook, S, K, D, out, status);
   CFB_LAUNCH_CHECK();
   return 0;
 }

@@ -155,6 +155,37 @@ int cfb_vqae_forward(cfb_net* net, const float* x, float* out, int64_t* idx, flo
                      float* min_encodings, int32_t batch,
                      void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- Encoder.forward alone (vqgan_arch.py:269-273), for both network kinds: the generator, the fusion and the Transformer
+ * never run, and the workspace is that of the encoder (cfb_encoder_workspace_bytes(net, n) for n ENCODED images; <0 on error).
+ * The latent equals the one the fused forwards quantize (VQAutoEncoder) or return as lq_feat (CodeFormer), bit for bit.
+ * cfb_encoder_forward: x [batch,3,S,S] NCHW in [-1,1] -> latent [batch,emb_dim,S/2^(n-1),S/2^(n-1)] NCHW. */
+int64_t cfb_encoder_workspace_bytes(cfb_net* net, int32_t batch);
+int cfb_encoder_forward(cfb_net* net, const float* x, float* latent, int32_t batch, void* workspace, int64_t workspace_bytes,
+                        void* stream);
+/* Latent codes of uint8 faces (scripts/generate_latent_gt.py): faces_bgr DEVICE uint8 [batch,S,S,3] HWC BGR, read with the
+ * input arithmetic of cfb_codeformer_forward_u8.  The encoder runs once at batch + mirror images: images 0..batch-1 are the
+ * faces, images batch + j (j < mirror <= batch) face j flipped left-right (cv2.flip(face, 1)), read mirrored by the first conv.
+ * idx [(batch+mirror)*h*w] int64 gets the code selection of VectorQuantizer.forward on each latent -- the same entry that module
+ * calls (cfb_vq_nearest_fast where cfb_vq_fast_supported, else cfb_vq_nearest) -- so the indices equal quantize(encoder(x)) of
+ * the fp32 chain bit for bit.  latent [(batch+mirror),emb_dim,h,w] NCHW is optional.  Workspace: cfb_encoder_workspace_bytes(net,
+ * batch + mirror). */
+int cfb_latent_codes_u8(cfb_net* net, const uint8_t* faces_bgr, int64_t* idx, float* latent, int32_t batch, int32_t mirror,
+                        void* workspace, int64_t workspace_bytes, void* stream);
+/* CodeFormer.forward(code_only=True) from uint8 faces (codeformer_arch.py:247-249) with no restored-image buffer: logits
+ * [batch,256,K] (required), lq_feat [batch,256,16,16] NCHW and top_idx [batch,256] int64 (the argmax of the logits) optional.
+ * Equal, bit for bit, to cfb_codeformer_forward on the fp32 chain of the faces with code_only = 1.  Workspace: cfb_workspace_bytes. */
+int cfb_codeformer_code_only_u8(cfb_net* net, const uint8_t* faces_bgr, float* logits, float* lq_feat, int64_t* top_idx,
+                                int32_t batch, void* workspace, int64_t workspace_bytes, void* stream);
+/* Code-prediction scores of CodeFormer's stage 2 (codeformer_idx_model.py:100-115), per image, in float64: logits [batch,tokens,
+ * codes], top_idx [batch,tokens] int64 (the net's argmax, not recomputed), gt_idx [batch,tokens] int64, lq_feat_nhwc
+ * [batch,tokens,dim], codebook [codes,dim]; all DEVICE.  scores [batch][3] double: the mean over tokens of
+ * logsumexp(logits_t) - logits_t[gt_t], the number of tokens with top_idx == gt, and the mean over tokens x dim of
+ * (codebook[gt_t] - lq_feat_t)^2.  Every sum runs in a fixed order that does not depend on the batch.  A NaN logit makes that
+ * image's cross-entropy NaN.  A gt index outside [0, codes) is never read: that image's three scores are NaN and the status word
+ * reports it (cfb_check_async_status, or the next forward). */
+int cfb_code_scores(const float* logits, const int64_t* top_idx, const int64_t* gt_idx, const float* lq_feat_nhwc,
+                    const float* codebook, int32_t batch, int32_t tokens, int32_t codes, int32_t dim, double* scores, void* stream);
+
 /* ---- VectorQuantizer.forward (vqgan_arch.py:33-70), standalone (config 3 microbench) ----
  * z [B,D,H,W] NCHW, codebook [K,D]; z_q [B,D,H,W] NCHW (= z + (E[idx]-z), :57); idx [B*H*W] int64;
  * stats[4] as above; min_encodings optional.  workspace >= cfb_vq_workspace_bytes. */
@@ -649,8 +680,8 @@ int     cfb_jpeg_roundtrip(const uint8_t* src, uint8_t* dst, int32_t n, int32_t 
 
 /* Asynchronous failures.  Kernels never trap and never leave a sticky CUDA error behind (the reference's callers catch
  * RuntimeError and fall back to the input face, inference_codeformer.py:209-211; web-demos/hugging_face/app.py:176): a
- * barrier time-out of the tensor-core pipeline or an activation outside the fp16 operand range (|x| > 65504) sets a bit
- * in a host-mapped status word.  It is reported (status 1 + cfb_last_error) by the NEXT forward on that device, by the
+ * barrier time-out of the tensor-core pipeline, an activation outside the fp16 operand range (|x| > 65504) or a code index
+ * outside the codebook given to cfb_code_scores sets a bit in a host-mapped status word.  It is reported (status 1 + cfb_last_error) by the NEXT forward on that device, by the
  * *_host entry points right after their stream synchronisation, and by this call -- use it after synchronising the stream
  * of an asynchronous forward.  The context stays usable; the reporting call clears the condition. */
 int cfb_check_async_status(void);
